@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — pairs/s of RoMa dense match() (+ sample()) at 560 -> 864 on B200s.
+"""bench.py — pairs/s of RoMa dense match() (+ sample()) at 560 -> 864 on H100s.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision fp32|fp32_simt|fp16|bf16]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--precision fp32|fp32_simt|fp16|bf16] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 A "step" is one pass of the hot path over one batch of synthetic input: `roma_outdoor(...).match()` on
@@ -12,15 +12,16 @@ no data-path collective — pairs are independent, SURVEY §8e).  Prints ONE JSO
   value      whole-job pairs/s, inputs resident in HBM, CUDA-event timed per step, max over ranks
   e2e        the same through the public API with HOST buffers: pinned inputs -> H2D inside match(), and the
              step's results (warp, certainty, sampled matches) read back D2H inside the timed region
-  roofline   the dominant kernel (the GEMM back-end: tcgen05 in the 16-bit modes), algorithmic FLOPs of every
+  roofline   the dominant kernel (the GEMM back-end: wgmma in the 16-bit modes), algorithmic FLOPs of every
              launch / its CUDA-event time, both collected live during the timed steps
   parity     max-abs error of this run's warp / certainty against tests/golden/full_sym_up.npz (the UNMODIFIED reference's
              fp32 output for the seed-1 pair, every 8th pixel), computed live; the default precision is the one that meets
-             the 1e-4 bar: "fp32" = fp32-class GEMMs on tcgen05 from split-fp16 operand pairs (DESIGN.md §2)
+             the 1e-4 bar: "fp32" = fp32-class GEMMs on the tensor cores from split-fp16 operand pairs (DESIGN.md §2)
   fast_mode  the same workload in the reference's CUDA autocast regime (fp16 operands), reported beside it with its error
   cpu_baseline  the CPU oracle (a port of the reference's fp32 CPU path) on this box's host cores, one pair
---impl reference times that CPU path alone (the reference itself is pure Python/PyTorch and does not travel
-to the GPU box; `oracle/` is its validated restatement, bit-exact against it in the build container).
+--impl reference times that CPU path alone (`oracle/` is a validated restatement of the reference, which is pure Python/PyTorch).
+--dump-outputs DIR writes what the last headline step returned (warp, certainty, sampled matches and their certainties) as
+float32 .npy files; inputs and sampler seeds are fixed, so two builds can be compared output for output.
 """
 import argparse
 import json
@@ -35,6 +36,32 @@ sys.path.insert(0, ROOT)
 
 COARSE, UPSAMPLE = 560, 864
 FLOP_PER_PAIR = 6.58e12          # SURVEY §6 (FlopCounterMode + analytic attention/solves)
+FP32_PEAK = 67.0                 # TFLOP/s, non-tensor fp32 of the H100 SXM data sheet
+DUMP_BUDGET = 64 << 20           # bytes of --dump-outputs in all
+
+
+def write_outputs(out_dir, match_out, samples):
+    """--dump-outputs: warp / certainty of the step's match() and every pair's sample() as float32 .npy files.  When they exceed
+    DUMP_BUDGET, every array keeps the same fixed, seeded choice of flat elements (written as <name>.npy) and their flat indices
+    (<name>_index.npy, float64)."""
+    import numpy as np
+    import torch
+    warp, cert = match_out
+    arrays = {"warp": warp, "certainty": cert}
+    if samples:
+        arrays["sample_matches"] = torch.stack([m for m, _ in samples])
+        arrays["sample_certainty"] = torch.stack([c for _, c in samples])
+    arrays = {k: v.detach().float().cpu().numpy() for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    for name, a in arrays.items():
+        if total > DUMP_BUDGET:
+            keep = max(1, int(a.size * DUMP_BUDGET / total / 3))          # values (4 B) + float64 indices (8 B)
+            idx = np.sort(rng.choice(a.size, size=min(keep, a.size), replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(a, dtype=np.float32))
 
 
 def load_peaks():
@@ -43,7 +70,7 @@ def load_peaks():
         d = json.load(open(path))
         return dict(hbm_gbs=d["hbm_gbs"], bf16_burst=d["bf16_tflops"], bf16_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_burst=1590.0, bf16_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_burst=989.0, bf16_sustained=989.0, source="fallback: NVIDIA H100 SXM data sheet (dense bf16, HBM3), not measured")
 
 
 class ClockSampler(threading.Thread):
@@ -86,8 +113,7 @@ def cpu_reference_time(steps, warmup, budget_s=240.0, with_sample=True):
     import torch
     from oracle.roma_oracle import RomaOracle
     from roma_b200 import synthetic
-    # measured on the 128-core GPU box (scripts/cpu_threads_probe.py): 16 thr 40 s, 32 thr 28 s, 64 thr 32 s, 128 thr 59 s for
-    # the coarse pass -> the oracle (like the reference: torch CPU ops) is fastest at ~32 threads; more only add contention
+    # the oracle (like the reference: torch CPU ops) stops scaling at a few dozen threads; more only add contention
     threads = int(os.environ.get("ROMA_CPU_THREADS", "0")) or min(os.cpu_count() or 1, 32)
     torch.set_num_threads(threads)
     mw, dw = synthetic.make_weights(0)
@@ -115,7 +141,7 @@ def local_corr_flow_sweep(dev, precision, mode="engine"):
     """The local-correlation prologue launches alone, on smooth flow (identity + 0.5 pixel of noise: neighbouring pixels share their
     windows) and on random flow (uniform over the image: no sharing, what the seeded synthetic weights produce): ms per launch and the
     compulsory HBM bytes of SURVEY 8d (read f0 + f1 + flow, write the window) per second, for the five launches of one direction pair.
-    mode "engine" = what the parity mode runs (stride 16: split + two all-pairs tcgen05 GEMMs + the gathering prologue, replayed from a
+    mode "engine" = what the parity mode runs (stride 16: split + two all-pairs tensor-core GEMMs + the gathering prologue, replayed from a
     CUDA graph; stride 4: tile-cooperative pass + per-pixel kernel for the tiles it declines; stride 8: per-pixel kernel);
     "per_pixel" = the per-pixel kernel everywhere; "tile_all" = the tile-cooperative pass at every scale."""
     import torch
@@ -169,7 +195,7 @@ def local_corr_flow_sweep(dev, precision, mode="engine"):
                             "romab200_gemm", "rb_gemm_args", A=hi[i0 * n:], A_lo=lo[i0 * n:], B=hi[y0 * n:], B_lo=lo[y0 * n:], C=table[i0], M=n, N=n, K=cf, lda=cf,
                             ldb=cf, ldc=ldt, dtype_ab=cabi.RB_F16S, dtype_c=cabi.RB_F32, batch0=1, batch1=1, ntaps=1, alpha=float(cf) ** -0.5))
                     kw.update(corr_table=table, ld_corr_table=ldt)
-                    how = "split + 2 all-pairs tcgen05 GEMMs + gathering prologue (CUDA graph of the 4 launches)"
+                    how = "split + 2 all-pairs tensor-core GEMMs + gathering prologue (CUDA graph of the 4 launches)"
 
                 def launches():
                     for f in pre:
@@ -203,7 +229,7 @@ def local_corr_flow_sweep(dev, precision, mode="engine"):
 
 def allpairs_kernel_leg(dev, reps=20):
     """The all-pairs CosKernel launches of one pair exactly as the engine issues them (K_AA | K_BB batched into the Cholesky workspace,
-    K_AB and K_BA as split pairs for mu = K_xy alpha; 1600 x 1600 x 512 each, split-fp16 operands on tcgen05), `reps` times in ONE CUDA
+    K_AB and K_BA as split pairs for mu = K_xy alpha; 1600 x 1600 x 512 each, split-fp16 operands on the tensor cores), `reps` times in ONE CUDA
     graph so that host launch latency (3 launches of ~30 us each) is not in the timed region; inputs are L2-resident as in the step
     (the split kernel that produces them runs right before)."""
     import torch
@@ -378,8 +404,8 @@ def run_ours(args):
         # more, and communicator creation (init + first collective) runs with fd 1 pointed at stderr
         if os.environ.get("NCCL_DEBUG", "VERSION").upper() == "VERSION":
             os.environ["NCCL_DEBUG"] = "WARN"
-        # the data path is point-to-point (scatter of inputs, gather of results): measured at N=2 with NCCL's default one or two P2P
-        # channels it moved 17-49 GB/s; more channels per peer use the NVLink bandwidth (770 GB/s per direction measured)
+        # the data path is point-to-point (scatter of inputs, gather of results): NCCL's default one or two P2P channels per peer
+        # leave most of the NVLink bandwidth unused
         os.environ.setdefault("NCCL_MIN_P2P_NCHANNELS", "16")
         os.environ.setdefault("NCCL_MAX_P2P_NCHANNELS", "32")
         sys.stdout.flush()
@@ -415,18 +441,21 @@ def run_ours(args):
     host = [t.pin_memory() for t in src_pairs] if src_pairs is not None else None
     devt = [t.to(dev) for t in src_pairs] if src_pairs is not None else None
     del src_pairs
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)        # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)        # > 50 MB L2
     out_host = None
     d2h_samples = [0]
     sample_calls = [0]
 
     sample_host = {}                                  # pinned read-back buffers of the samples, per pair slot of a step
+    dump = {"armed": False, "samples": [], "out": None}   # --dump-outputs: what the last headline step returned
 
     def sample_batch(warp, cert, to_host=False):
         if args.no_sample:
             return
         for i in range(warp.shape[0]):
             m, c = model.sample(warp[i], cert[i], num=10000)
+            if dump["armed"]:
+                dump["samples"].append((m.clone(), c.clone()))      # the sampler's output buffers are reused by the next call
             if to_host:
                 # asynchronous read-back into pinned memory on the step's stream: no host synchronisation inside a step, so the host
                 # queues the next step while this one runs (a blocking .cpu() here exposed ~0.2 ms of launch latency per step)
@@ -548,6 +577,7 @@ def run_ours(args):
             out[-1] += max(0.0, ev[-1][1].elapsed_time(last))   # the last step's read-back ends after its stream-side end event
         return out
 
+    torch.manual_seed(0)                                      # the sampler's seeds come from torch's CPU generator
     for _ in range(max(args.warmup, 3)):
         step_device()
     torch.cuda.synchronize()
@@ -556,8 +586,19 @@ def run_ours(args):
     sampler.start()
     time.sleep(0.3)
     launches0 = cabi.kernel_launches() + model.graph_launches
-    ms = timed(step_device, args.steps)                       # headline: device side replayed as a CUDA graph
+    headline_steps = [0]
+
+    def headline_step():
+        headline_steps[0] += 1
+        last = headline_steps[0] == args.steps
+        dump["armed"] = bool(args.dump_outputs) and last
+        out = step_device()
+        if dump["armed"]:
+            dump["out"], dump["armed"] = out, False
+    ms = timed(headline_step, args.steps)                     # headline: device side replayed as a CUDA graph
     launches = cabi.kernel_launches() + model.graph_launches - launches0
+    if args.dump_outputs and dump["out"] is not None:
+        write_outputs(args.dump_outputs, dump["out"], dump["samples"])
     # second timed region, same workload, eager launches with a CUDA-event pair around every GEMM launch and every
     # pipeline stage (events cannot be read back from inside a replayed graph): feeds `roofline` and the stage table
     eng.gemm_profile, eng.profile = [], {}
@@ -654,25 +695,16 @@ def run_ours(args):
         if dom:
             fl, t_ms, n = by[dom]
             ach = fl / (t_ms / 1e3) / 1e12
-            # dram__bytes_read+write of one named launch of this kernel, measured by `ncu --set full` on this same command
-            # (scripts/gpu_profile.sh writes the side-car next to the ncu summary it comes from); null when not captured
-            traffic = None
-            tpath = os.path.join(ROOT, "profiles", "r02_traffic.json")
-            if os.path.exists(tpath):
-                traffic = json.load(open(tpath)).get(dom)
             passes = 3.0 if dom == "tcgen05-split" else 1.0
             roofline = {"kernel": f"romab200_gemm[{dom}]", "bound": "tensor", "achieved": ach * passes, "peak": peaks["bf16_sustained"],
                         "unit": "TFLOP/s", "frac": ach * passes / peaks["bf16_sustained"],
                         "flops_definition": ("tensor-core FLOPs of the algorithm as it runs on the f16 pipe: an fp32-class product from split-fp16 operand pairs is THREE "
                                              "f16 MMAs per k-step (hi.hi, hi.lo, lo.hi; 22 significand bits), i.e. 3 x 2MNK per launch - each term is needed, none is a "
-                                             "recomputation; ncu's sm__pipe_tensor_cycles_active of the same kernel (profiles/r02_ncu_gemm_fc1_qkv_tcgen05_split_final.txt: "
-                                             "46-53 %) is the independent check" if passes > 1 else "2MNK per launch"),
+                                             "recomputation" if passes > 1 else "2MNK per launch"),
                         "fp32_equivalent": {"achieved": ach, "frac": ach / peaks["bf16_sustained"],
                                             "note": "2MNK per launch (the FLOPs of the fp32 contraction the reference performs) against the same bf16 peak: "
                                                     "bounded by 1/3 in the split mode"} if passes > 1 else None,
                         "passes": passes,
-                        "traffic": traffic["dram_bytes"] if traffic else None,
-                        "traffic_launch": traffic["launch"] if traffic else None,
                         "peak_source": peaks["source"] + ", sustained bf16 cuBLAS figure (kernel timed inside a long step)",
                         "launches_timed": n, "share_of_step": t_ms / sum(ms_prof),
                         "measured_in": "second timed region of the same K steps, eager launches (per-kernel events cannot be read "
@@ -690,12 +722,12 @@ def run_ours(args):
             split = 3.0 if cos_backend == "tcgen05" else 1.0
             executed = 3.0 if cos_backend == "tcgen05-split" else 1.0
             ach = cos_flops / split / (cos_ms / 1e3) / 1e12
-            pk = peaks["bf16_sustained"] if cos_backend.startswith("tcgen05") else 72.0
+            pk = peaks["bf16_sustained"] if cos_backend.startswith("tcgen05") else FP32_PEAK
             entry = {"kernel": f"all-pairs CosKernel (romab200_gemm, RB_EPI_COSKERNEL, {cos_backend})", "bound": "tensor" if cos_backend.startswith("tcgen05") else "fp32",
                      "achieved": ach, "achieved_executed": cos_flops * executed / (cos_ms / 1e3) / 1e12, "peak": pk, "unit": "TFLOP/s", "frac": ach / pk,
                      "launches_per_step": cos_n / args.steps, "ms_per_step": cos_ms / args.steps,
                      "measured_in": "eager launches of the step, CUDA events around each launch (includes the host's launch latency: ~100 us for a ~30 us kernel)",
-                     "note": "four 1600x1600x512 problems per pair (2.6 GFLOP each, 1.5 us at peak): size-limited, see DESIGN.md"}
+                     "note": "four 1600x1600x512 problems per pair (2.6 GFLOP each): size-limited, see DESIGN.md"}
             if cos_backend == "tcgen05-split" and world == 1:
                 try:
                     leg = allpairs_kernel_leg(dev)
@@ -732,23 +764,23 @@ def run_ours(args):
             except Exception as exc:
                 lc_pp = {"error": f"{type(exc).__name__}: {exc}"[:200]}
         if lc_ms > 0:
-            extra.append({"kernel": "local correlation (stride 16: all-pairs tcgen05 table + gather; stride 8: refiner_prologue_kernel<3>; stride 4: "
+            extra.append({"kernel": "local correlation (stride 16: all-pairs tensor-core table + gather; stride 8: refiner_prologue_kernel<3>; stride 4: "
                                     "refiner_prologue_tile_kernel<2> + refiner_prologue_kernel<2>) incl. the x / grid_sample / embedding part of the prologue",
                           "bound": "hbm", "achieved": lc_bytes / (lc_ms / 1e3) / 1e9, "peak": peaks["hbm_gbs"], "unit": "GB/s", "frac": lc_bytes / (lc_ms / 1e3) / 1e9 / peaks["hbm_gbs"],
-                          "fp32_fma_tflops": 2 * lc_fma / (lc_ms / 1e3) / 1e12, "fp32_fma_frac_of_nominal_72": 2 * lc_fma / (lc_ms / 1e3) / 1e12 / 72.0,
+                          "fp32_fma_tflops": 2 * lc_fma / (lc_ms / 1e3) / 1e12, "fp32_fma_frac_of_nominal": 2 * lc_fma / (lc_ms / 1e3) / 1e12 / FP32_PEAK,
                           "ms_per_step": lc_ms, "measured_in": "eager launches of the step (the flow of the seeded synthetic weights is random: no window sharing)",
                           "flow_sweep": lc_sweep, "flow_sweep_hbm_frac": ({k: round(v["hbm_gbs"] / peaks["hbm_gbs"], 4) for k, v in lc_sweep.items()} if lc_sweep and "error" not in lc_sweep else None),
                           "flow_sweep_other_kernels": lc_pp,
                           "note": "algorithmic bytes = SURVEY 8d (f0 + f1 + flow read once, window written once).  The windows of neighbouring pixels overlap, so f1 "
                                   "is served from L1/L2, not HBM; the CUDA-core kernels are bound by the 4 bytes of L1/shared-memory bandwidth each fp32 FMA "
-                                  "needs (floor 0.29 ms per pair = 0.24 of the HBM roofline, DESIGN.md 4); only stride 16, where the table is small, goes "
+                                  "needs (DESIGN.md 4); only stride 16, where the table is small, goes "
                                   "through the tensor cores"})
         cpu = None
         if world == 1 and not args.no_cpu_baseline:
             times, threads = cpu_reference_time(1, 1, with_sample=not args.no_sample)
             cpu = {"value": 1.0 / (sum(times) / len(times)), "unit": "pairs/s", "cores": threads, "kind": "port",
                    "sample": f"{len(times)} symmetric pair 560->864 match()" + ("" if args.no_sample else "+sample(10000)") +
-                             " through oracle/roma_oracle.py (fp32 restatement of the reference, bit-exact vs it in the build container)"}
+                             " through oracle/roma_oracle.py (fp32 restatement of the reference, pinned against its outputs by tests/test_oracle_golden.py)"}
         prep = None
         if world == 1:
             try:
@@ -771,7 +803,7 @@ def run_ours(args):
             "steps": args.steps, "warmup": max(args.warmup, 3), "ms_per_step": total_ms / args.steps, "higher_is_better": True,
             "scaling": "strong" if args.global_pairs else "weak", "vs_baseline": None,
             "dtype": {"fp16": "f16 operands / f32 accumulate (reference CUDA autocast regime)", "bf16": "bf16 operands / f32 accumulate",
-                      "fp32": "f32 (activations f32; GEMM operands as split-f16 pairs hi + 2^-11 lo on tcgen05, f32 accumulate: fp32-class)",
+                      "fp32": "f32 (activations f32; GEMM operands as split-f16 pairs hi + 2^-11 lo on wgmma, f32 accumulate: fp32-class)",
                       "fp32_simt": "f32 (CUDA-core FFMA GEMMs)"}[args.precision],
             "data": "synthetic",
             "config": {"workload": workload,
@@ -781,7 +813,7 @@ def run_ours(args):
                                        (f"dp{world} (every rank on its own resident pairs, no collective)" if world > 1 else "1 GPU")),
                        "nccl_bytes_per_step": {"scatter": wire[0], "gather": wire[1]} if sharded else None,
                        "precision": args.precision, "weights": "seeded synthetic (no network)",
-                       "l2": "256 MiB buffer written between timed steps; per-step activations also exceed the 126 MB L2"},
+                       "l2": "256 MiB buffer written between timed steps; per-step activations also exceed the 50 MB L2"},
             "e2e": {"value": e2e_value, "unit": "pairs/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h_box[0],
                     "ms_per_step": total_ms_e2e / args.steps,
                     "how": ("every step's inputs go from pinned host memory to the device and its warp, certainty and samples back into pinned host memory, "
@@ -820,6 +852,8 @@ def main():
     ap.add_argument("--no-scatter", action="store_true", help="N > 1: every rank on its own resident pairs (no NCCL scatter / gather in the timed region)")
     ap.add_argument("--no-sample", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's warp, certainty and samples to DIR/<name>.npy (float32, at most 64 MB in all)")
     args = ap.parse_args()
     if args.impl == "torch_cuda":
         import torch

@@ -1,5 +1,5 @@
 /*
- * romab200.h — C ABI of the B200-native RoMa dense-matching kernels (libromab200.so).
+ * romab200.h — C ABI of the H100-native RoMa dense-matching kernels (libromab200.so).
  *
  * Drop-in boundary for ONE path: RoMa's dense match()/sample() inference.  The reference
  * (Parskatt/RoMa) is pure Python/PyTorch; the only native operator boundary it has on this path is
@@ -16,7 +16,7 @@
  *   - RB_F16S ("split fp16 pair") is the storage format of the tensor-core parity mode: a matrix is held as TWO fp16
  *     planes of the same pitch, hi = fp16(x) and lo = fp16((x - hi) * 2^11), value = hi + lo * 2^-11: 22 significand bits
  *     with the exponent range of fp16 (the reference's own CUDA autocast range).  romab200_gemm contracts such operands
- *     with three tcgen05 MMAs per k-step (hi.hi + 2^-11 (hi.lo + lo.hi), fp32 accumulation in TMEM), which reproduces an
+ *     with three wgmma MMAs per k-step (hi.hi + 2^-11 (hi.lo + lo.hi), fp32 accumulation in registers), which reproduces an
  *     fp32 GEMM to ~2^-22 relative; arguments named *_lo carry the second plane.
  */
 #ifndef ROMAB200_H
@@ -40,7 +40,7 @@ int romab200_abi_version(void);
 const char* romab200_last_error(void);
 /* number of CUDA kernels this library has launched so far in this process */
 unsigned long long romab200_launch_count(void);
-/* 1 if the running device is sm_100 (B200) and the tcgen05/TMA kernels may be launched */
+/* 1 if the running device is sm_90 (H100) and the wgmma/TMA kernels may be launched */
 int romab200_device_ok(void);
 
 /* ------------------------------------------------------------------------------------------------
@@ -66,8 +66,9 @@ int romab200_device_ok(void);
  * Row map of the store: NONE; PAD_KEEP (m indexes a zero-padded [*,pad_h,pad_w] grid; border rows are not
  * computed: they are left alone or rewritten with zeros, the value they hold in every map of the path); PAD_TO_COMPACT (same, interior rows are written to the un-padded row index);
  * SEGMENT (row m -> (m / seg_in) * seg_out + m % seg_in + seg_off).
- * Output pitch: the tcgen05 back-end stores tiles with TMA when ldc (and the batch strides) are multiples of 16 bytes; TMA clips at
- * 16-byte granules, so the pad columns N .. roundup(N, 16 bytes) of a written row receive zeros (columns beyond are untouched).
+ * Output pitch: when ldc (and the batch strides) are multiples of 16 bytes, the row map is NONE or PAD_KEEP and there is no
+ * residual operand, the tensor-core back-end also writes zeros into the pad columns N .. roundup(N, 16 bytes) of every written row
+ * (columns beyond are untouched).
  * ------------------------------------------------------------------------------------------------ */
 typedef struct {
     const void* A; const void* B; void* C;
@@ -90,7 +91,7 @@ typedef struct {
     /* second planes of RB_F16S operands / output (dtype_ab == RB_F16S: A_lo and B_lo, same geometry as A and B;
        dtype_c == RB_F16S: C_lo, same pitch as C); NULL otherwise */
     const void* A_lo; const void* B_lo; void* C_lo;
-    /* tcgen05 back-end: upper bound on the persistent grid (0 = one CTA per SM).  A GEMM running on a side stream beside a chain of short
+    /* tensor-core back-end: upper bound on the persistent grid (0 = one CTA per SM).  A GEMM running on a side stream beside a chain of short
        dependent kernels (the GP solve) leaves the remaining SMs free, so that those kernels start without waiting for a whole GEMM. */
     int32_t max_ctas;
 } rb_gemm_args;
@@ -263,7 +264,7 @@ typedef struct {
 int romab200_refiner_block_small(const rb_refiner_block_small_args* args, void* stream);
 
 /* Fused ConvRefiner block for the stride-2 maps (C = 144): depthwise 5x5 + BN + ReLU on the CUDA cores feeding a
- * tcgen05 pointwise GEMM whose weights stay resident in shared memory; one read + one write of the map.
+ * wgmma pointwise GEMM whose weights stay resident in shared memory; one read + one write of the map.
  * in/out [batch, h, w, ld] 16-bit (in != out); dw_weight [25][ldw] fp32 (BN folded), pw_weight [144][ld_pw] 16-bit. */
 typedef struct {
     const void* in; void* out; int64_t ld; const float* dw_weight; int64_t ldw; const float* dw_bias;
@@ -350,10 +351,6 @@ typedef struct {
     int64_t ss0, ss1, sd0, sd1; int32_t dtype;
 } rb_transpose_args;
 int romab200_transpose(const rb_transpose_args* args, void* stream);
-
-/* debug: role-time counters of the tcgen05 GEMM kernels, collected when the environment variable ROMAB200_TC_CLK=1 is set before
- * the first GEMM (16 x uint64: MMA-thread / TMA-producer / epilogue wait and total cycles, tiles, k-blocks; scripts/gemm_clk.py) */
-int romab200_debug_tc_clk(unsigned long long* out, int reset);
 
 #ifdef __cplusplus
 }

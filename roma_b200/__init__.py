@@ -1,4 +1,4 @@
-"""roma_b200 — B200-native implementation of RoMa's dense `match()` / `sample()` path.
+"""roma_b200 — H100-native implementation of RoMa's dense `match()` / `sample()` path.
 
 Drop-in for `romatch`'s public surface on that path (`romatch/__init__.py:2`):
 

@@ -3,7 +3,7 @@
 The argument structs are generated from `include/romab200.h` itself at import time, so the Python side
 cannot drift from the header.  Every wrapper passes raw device pointers (`tensor.data_ptr()`) and the
 current CUDA stream; a non-zero return code becomes a `RuntimeError` carrying `romab200_last_error()`.
-There is no fallback: if the library is missing or the device is not a B200, calls fail loudly.
+There is no fallback: if the library is missing or the device is not an H100 (sm_90), calls fail loudly.
 """
 from __future__ import annotations
 

@@ -38,7 +38,7 @@ extern "C" int romab200_device_ok(void) {
         cudaGetLastError();
         return 0;
     }
-    return prop.major == 10 ? 1 : 0;
+    return prop.major == 9 && prop.minor == 0 ? 1 : 0;
 }
 
 extern "C" int romab200_gemm(const rb_gemm_args* a, void* stream) {

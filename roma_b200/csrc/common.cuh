@@ -1,4 +1,4 @@
-// Shared helpers for libromab200 kernels (sm_100a only).
+// Shared helpers for libromab200 kernels (sm_90a only).
 #pragma once
 #include <cstdlib>
 #include <cuda_runtime.h>
@@ -82,11 +82,14 @@ __device__ __forceinline__ float warp_max(float v) {
     return v;
 }
 
+// two independent fp32 FMAs on a channel pair (c + a * b per component, round-to-nearest)
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+
 // exact-erf GELU (nn.GELU default, mlp.py:26)
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
 
 // ------------------------------------------------------------------------------------------------
-// GEMM epilogue shared by the SIMT and tcgen05 back-ends
+// GEMM epilogue shared by the SIMT and tensor-core back-ends
 // ------------------------------------------------------------------------------------------------
 struct Epilogue {
     void* C; void* C_lo; int64_t ldc; int dtype_c;
@@ -140,8 +143,8 @@ struct Epilogue {
 // starts with pdl_wait(), so that its launch latency and per-CTA set-up overlap the tail of the previous kernel in the
 // stream (the ~680 launches of one match() are otherwise separated by a few microseconds each).
 // ------------------------------------------------------------------------------------------------
-// No early griddepcontrol.launch_dependents: measured on B200 it costs 5 % of a match() (the next grid's CTAs take SM
-// slots and issue bandwidth while they spin in their wait); the implicit trigger at grid exit already hides the launch.
+// No early griddepcontrol.launch_dependents: the next grid's CTAs would take SM slots and issue bandwidth while they spin in
+// their wait; the implicit trigger at grid exit already hides the launch.
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 // ROMAB200_NO_PDL=1 launches every kernel fully serialised (debugging knob; griddepcontrol.* are no-ops then)
 inline int pdl_mode() { static const int m = [] { const char* e = getenv("ROMAB200_NO_PDL"); return e ? atoi(e) : 0; }(); return m; }

@@ -148,7 +148,7 @@ __global__ void __launch_bounds__(DwCfg<TIN>::THREADS) dwconv5x5_relu_tma_kernel
 #pragma unroll
                         for (int kx = 0; kx < 5; ++kx) {
                             const int ox = px - kx;
-                            if (ox >= 0 && ox < DT_TW) acc[rr][ox] = __ffma2_rn(wv[ky * 5 + kx], v, acc[rr][ox]);
+                            if (ox >= 0 && ox < DT_TW) acc[rr][ox] = rb::fma2(wv[ky * 5 + kx], v, acc[rr][ox]);
                         }
                     }
                 }
@@ -247,7 +247,7 @@ int dwconv_tma(const rb_dwconv_args* a, cudaStream_t st) {
     p.total_tiles = (int)total;
     const int groups = (a->c + DT_CH - 1) / DT_CH;
     RB_REQUIRE(groups <= 65535, "dwconv: too many channel groups");
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, current_device());
     int per_group = (f32 ? 1 : 2) * sms / groups;              // resident CTAs per SM (one for the fp32 ring), never more CTAs than fit at once
     if (per_group < 1) per_group = 1;

@@ -358,7 +358,7 @@ __global__ void transpose_kernel(const T* __restrict__ src, T* __restrict__ dst,
     }
 }
 
-static inline int grid_for(int64_t total, int block, int cap = 148 * 32) {
+static inline int grid_for(int64_t total, int block, int cap = 132 * 32) {
     int64_t g = (total + block - 1) / block;
     return (int)(g < cap ? (g > 0 ? g : 1) : cap);
 }
@@ -369,7 +369,7 @@ int split_f16s_batched(const float* x, void* hi, void* lo, int64_t rows, int col
     RB_REQUIRE(cols % 4 == 0 && ldx % 4 == 0 && ldd % 4 == 0 && sx % 4 == 0 && sd % 4 == 0 && ((uintptr_t)x) % 16 == 0 && ((uintptr_t)hi) % 8 == 0 && ((uintptr_t)lo) % 8 == 0,
                "split_f16s_batched: alignment");
     RB_REQUIRE(batch > 0 && batch <= 65535 && rows > 0, "split_f16s_batched: bad shape");
-    dim3 grid(grid_for(rows * (cols / 4), 256, 148 * 8), batch);
+    dim3 grid(grid_for(rows * (cols / 4), 256, 132 * 8), batch);
     rb::launch_pdl(split_f16s_batched_kernel, grid, dim3(256), 0, st, x, (__half*)hi, (__half*)lo, rows, cols / 4, ldx, ldd, sx, sd);
     return check_launch("split_f16s_batched");
 }

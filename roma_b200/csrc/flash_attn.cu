@@ -3,16 +3,30 @@
 // embedding decoder (8 heads x d=128, N=1600).  softmax(Q K^T / sqrt(d)) V without ever writing the N x N
 // scores to HBM (the un-fused path moves 2 x 164 MB per layer).
 //
-// One CTA = one (image, head, 128-query tile).  Warp roles:
-//   warp 0     TMA producer: Q tile once, then K/V tiles of 128 keys through a 2-3 stage smem ring
-//   warp 1     MMA issuer:   S_j = Q K_j^T (tcgen05, M=128,N=128,K=d) into a double-buffered TMEM score tile, and
-//              O += P_j V_j (M=128,N=d,K=128; V is the MN-major B operand straight from the qkv buffer)
-//   warps 2-5  one thread per query row: tcgen05.ld the scores, online softmax in the exp2 domain, rescale the
-//              fp32 O accumulator in TMEM when the running max moved (tcgen05.ld/st), write P_j as the 16-bit
-//              K-major 128B-swizzled A operand into shared memory; finally O / l -> global.
-// The score MMA of tile j+1 overlaps the softmax of tile j; the PV MMA of tile j overlaps the softmax of j+1.
+// One CTA = one (image, head, 128-query tile), 384 threads:
+//   warps 0-7   two consumer warpgroups, 64 query rows each.  Per key tile: S = Q K_j^T with wgmma (A = Q, B = K_j, both
+//               K-major from shared memory) into registers, online softmax in the exp2 domain on the accumulator fragments
+//               (a row lives in the 4 lanes of a quad), rescale of the fp32 O accumulator, then O += P_j V_j with P_j as the
+//               register A operand (the S fragment of 16 keys is exactly the A fragment of one k-step) and V_j the MN-major
+//               B operand straight from the qkv buffer; finally O / l -> global.
+//   warps 8-11  TMA producer (one lane): Q once, then K/V tiles through a STAGES-deep shared-memory ring.  Its registers go
+//               to the consumers (setmaxnreg).
+// The two warpgroups run independently, so one's softmax overlaps the other's MMAs.
+//
+// Split-fp16 (RB_F16S) variant for the parity mode, head_dim 64 (DINOv2 ViT-L): fp32-class attention on the f16 tensor pipe.
+//   q, k, v arrive as (hi, lo') plane pairs (value = hi + lo' * 2^-11, written by the qkv GEMM epilogue).
+//   S_j = Q K_j^T with three MMAs per k-step into TWO accumulators (main: hi.hi; cross: hi.lo' + lo'.hi), score = main +
+//         cross * 2^-11; key tiles of 64.
+//   P V : the probabilities are written in an exponent-shifted form so that ONE accumulator suffices:
+//         O' = sum_j (Pt_hi + Pt_lo) V_hi + P_hi V_lo'      with Pt = 2048 p, Pt_hi = fp16(Pt), Pt_lo = fp16(Pt - Pt_hi),
+//         P_hi = fp16(p) = Pt_hi / 2048, i.e. O' = 2048 * sum p (V_hi + V_lo' / 2048) up to a 2^-22 relative term.  p <= 1, so
+//         Pt <= 2048 never overflows; the unscaled low part Pt_lo only underflows for p < 6e-5, where its absolute error
+//         (1.5e-11 in units of p) is irrelevant.
+//   out  = O' / (2048 l) written as an RB_F16S pair for the projection GEMM.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
+#include <type_traits>
 
 namespace rb {
 
@@ -46,576 +60,248 @@ __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* m
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])), "r"(__float_as_uint(v[3])),
-          "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])), "r"(__float_as_uint(v[7])),
-          "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])), "r"(__float_as_uint(v[11])),
-          "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])), "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])),
-          "r"(__float_as_uint(v[16])), "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-          "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])), "r"(__float_as_uint(v[23])),
-          "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])), "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])),
-          "r"(__float_as_uint(v[28])), "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
-    asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-}
 __device__ __forceinline__ float ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
     return y;
 }
-// K-major / MN-major 128B-swizzle matrix descriptor
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
+template <typename T> __device__ __forceinline__ uint32_t pack2(float a, float b) {
+    T h[2] = {from_f<T>(a), from_f<T>(b)};
+    return *reinterpret_cast<uint32_t*>(h);
+}
+template <typename T> __device__ __forceinline__ float2 unpack2(uint32_t w) {
+    const T* h = reinterpret_cast<const T*>(&w);
+    return make_float2(to_f(h[0]), to_f(h[1]));
+}
+// keeps registers that an in-flight wgmma reads alive (and unmodified) until after the wait
+template <int R> __device__ __forceinline__ void keep_regs(const uint32_t (&a)[R][4]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" ::"r"(a[i][0]), "r"(a[i][1]), "r"(a[i][2]), "r"(a[i][3]) : "memory");
 }
 }  // namespace fa
 
 struct FaParams {
-    void* out; int64_t ldo;          // [Bn, N, dim] rows of pitch ldo (elements)
-    int N, heads, dim, is_bf16;
-    float scale_log2;                // log2(e) / sqrt(d)
-};
-
-template <int D> struct FaCfg {
-    static constexpr int BQ = 128, BKV = 128;
-    static constexpr int STAGES = D == 64 ? 3 : 2;
-    static constexpr int Q_BYTES = BQ * D * 2;
-    static constexpr int KV_BYTES = BKV * D * 2;            // one of K, V
-    static constexpr int P_BYTES = BQ * BKV * 2;
-    static constexpr int SMEM = Q_BYTES + STAGES * 2 * KV_BYTES + 2 * P_BYTES + 1024 + 256;   // two probability buffers
-    static constexpr int TMEM_COLS = 512;                   // S: 2 x 128, O: D  (power of two >= 256 + D)
-};
-
-template <int D, typename T>
-__global__ void __launch_bounds__(192, 1) flash_attn_kernel(const __grid_constant__ CUtensorMap map_qkv, const FaParams p) {
-    rb::pdl_wait();
-    using namespace fa;
-    using Cfg = FaCfg<D>;
-    constexpr int STAGES = Cfg::STAGES, BQ = Cfg::BQ, BKV = Cfg::BKV, DB = D / 64;
-    extern __shared__ uint8_t smem_raw[];
-    uint8_t* smem = smem_raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);   // offset on the array: keeps ld/st.shared
-    uint8_t* sQ = smem;
-    uint8_t* sK = sQ + Cfg::Q_BYTES;
-    uint8_t* sV = sK + STAGES * Cfg::KV_BYTES;
-    uint8_t* sP = sV + STAGES * Cfg::KV_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * Cfg::P_BYTES);
-    uint64_t* q_full = bars;                  // [1]
-    uint64_t* kv_full = bars + 1;             // [STAGES]
-    uint64_t* kv_empty = kv_full + STAGES;    // [STAGES]
-    uint64_t* s_full = kv_empty + STAGES;     // [2]
-    uint64_t* s_empty = s_full + 2;           // [2]
-    uint64_t* p_ready = s_empty + 2;          // [2]  one per probability buffer (tile j uses buffer j & 1)
-    uint64_t* pv_done = p_ready + 2;          // [2]  PV_j retired, committed on pv_done[j & 1]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int q0 = blockIdx.x * BQ, head = blockIdx.y, img = blockIdx.z;
-    const int ntiles = (p.N + BKV - 1) / BKV;
-
-    if (warp == 0 && lane == 0) {
-        mbar_init(q_full, 1);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], 4); mbar_init(&p_ready[s], 4); mbar_init(&pv_done[s], 1); }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_S = tmem_base;              // columns [0, 256): two score tiles
-    const uint32_t tmem_O = tmem_base + 256;        // columns [256, 256 + D)
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            const int cq = head * D, ck = p.dim + head * D, cv = 2 * p.dim + head * D;
-            mbar_expect_tx(q_full, Cfg::Q_BYTES);
-#pragma unroll
-            for (int b = 0; b < DB; ++b) tma_load_3d(sQ + b * (BQ * 128), &map_qkv, q_full, cq + 64 * b, q0, img);
-            for (int j = 0; j < ntiles; ++j) {
-                const int s = j % STAGES;
-                const uint32_t u = j / STAGES;
-                mbar_wait(&kv_empty[s], (u & 1) ^ 1);
-                mbar_expect_tx(&kv_full[s], 2 * Cfg::KV_BYTES);
-#pragma unroll
-                for (int b = 0; b < DB; ++b) {
-                    tma_load_3d(sK + s * Cfg::KV_BYTES + b * (BKV * 128), &map_qkv, &kv_full[s], ck + 64 * b, j * BKV, img);
-                    tma_load_3d(sV + s * Cfg::KV_BYTES + b * (BKV * 128), &map_qkv, &kv_full[s], cv + 64 * b, j * BKV, img);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            const uint32_t fmt = p.is_bf16 ? 1u : 0u;
-            // S = Q K^T : A, B K-major, N = 128;   O += P V : A K-major, B MN-major, N = D
-            const uint32_t idesc_s = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(BKV >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-            const uint32_t idesc_o = (1u << 4) | (fmt << 7) | (fmt << 10) | (1u << 16) | ((uint32_t)(D >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-            const uint32_t q_addr = smem_u32(sQ), p_addr = smem_u32(sP);
-            auto issue_s = [&](int j) {
-                const int s = j % STAGES;
-                mbar_wait(&kv_full[s], (j / STAGES) & 1);
-                const uint32_t u = j >> 1;                       // previous uses of this score buffer
-                mbar_wait(&s_empty[j & 1], (u & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t k_addr = smem_u32(sK + s * Cfg::KV_BYTES);
-#pragma unroll
-                for (int k = 0; k < D / 16; ++k) {
-                    const uint32_t off = (k >> 2) * (128 * 128) + (k & 3) * 32;     // 64-element block, 32 B per K step
-                    umma_f16(tmem_S + (j & 1) * 128, smem_desc(q_addr + off, 16, 1024), smem_desc(k_addr + off, 16, 1024), idesc_s, k != 0);
-                }
-                umma_commit(&s_full[j & 1]);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < ntiles; ++j) {
-                if (j + 1 < ntiles) issue_s(j + 1);
-                mbar_wait(&p_ready[j & 1], (j >> 1) & 1);
-                tc_fence_after();
-                const int s = j % STAGES;
-                const uint32_t v_addr = smem_u32(sV + s * Cfg::KV_BYTES);
-#pragma unroll
-                for (int k = 0; k < BKV / 16; ++k) {
-                    const uint32_t a_off = (j & 1) * Cfg::P_BYTES + (k >> 2) * (BQ * 128) + (k & 3) * 32;    // P buffer j & 1: two 64-key blocks
-                    // V tile: D/64 boxes of [128 keys x 128 B]; 16 keys = 2 swizzle row-groups = 2048 B
-                    umma_f16(tmem_O, smem_desc(p_addr + a_off, 16, 1024), smem_desc(v_addr + k * 2048, BKV * 128, 1024), idesc_o, (j | k) != 0);
-                }
-                umma_commit(&kv_empty[s]);
-                umma_commit(&pv_done[j & 1]);
-            }
-        }
-    } else {
-        // ===== softmax / correction / epilogue: one thread per query row =====
-        // The probabilities are double-buffered, so this loop runs one tile ahead of the PV products: it only waits for PV_{j-2} (its
-        // buffer is free again) and, when a running maximum moved, for PV_{j-1} before rescaling O in TMEM.
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        float m_run = -INFINITY, l_run = 0.f;
-        for (int j = 0; j < ntiles; ++j) {
-            mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            float sc[128];
-#pragma unroll
-            for (int c = 0; c < 4; ++c) tmem_ld32(tmem_S + lane_addr + (j & 1) * 128 + c * 32, sc + c * 32);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_empty[j & 1]);
-            const int valid = min(BKV, p.N - j * BKV);
-            float m_new = m_run;
-#pragma unroll
-            for (int i = 0; i < 128; ++i) {
-                sc[i] = i < valid ? sc[i] * p.scale_log2 : -INFINITY;
-                m_new = fmaxf(m_new, sc[i]);
-            }
-            const float alpha = ex2(m_run - m_new);           // 0 on the first tile (m_run = -inf)
-            if (j > 0 && __any_sync(0xffffffffu, m_new > m_run)) {
-                mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);   // PV_{j-1} (and all before it) retired: O is stable
-                tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < D / 32; ++c) {
-                    float o[32];
-                    tmem_ld32(tmem_O + lane_addr + c * 32, o);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o[i] *= alpha;
-                    tmem_st32(tmem_O + lane_addr + c * 32, o);
-                }
-            }
-            if (j >= 2) mbar_wait(&pv_done[j & 1], ((j >> 1) - 1) & 1);   // PV_{j-2} retired: probability buffer j & 1 is free
-            float lsum = 0.f;
-            // P row -> K-major SW128: block kb = key/64, 16-byte chunk c' = (key%64)/8 XOR (row%8)
-            uint8_t* prow = sP + (j & 1) * Cfg::P_BYTES + row * 128;
-#pragma unroll
-            for (int c = 0; c < 16; ++c) {
-                T pk[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const float pv = ex2(sc[c * 8 + e] - m_new);
-                    pk[e] = from_f<T>(pv);
-                    lsum += to_f(pk[e]);                       // sum what the MMA will actually see
-                }
-                const int kb = c >> 3, cc = (c & 7) ^ (row & 7);
-                *reinterpret_cast<uint4*>(prow + kb * (BQ * 128) + cc * 16) = *reinterpret_cast<uint4*>(pk);
-            }
-            l_run = l_run * alpha + lsum;
-            m_run = m_new;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to UMMA
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_ready[j & 1]);
-        }
-        mbar_wait(&pv_done[(ntiles - 1) & 1], ((ntiles - 1) >> 1) & 1);
-        tc_fence_after();
-        const int qi = q0 + row;
-        const float inv = 1.0f / l_run;
-        T* orow = (T*)p.out + ((int64_t)img * p.N + qi) * p.ldo + head * D;
-#pragma unroll
-        for (int c = 0; c < D / 32; ++c) {
-            float o[32];
-            tmem_ld32(tmem_O + lane_addr + c * 32, o);
-            if (qi < p.N) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    T pk[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) pk[e] = from_f<T>(o[g * 8 + e] * inv);
-                    *reinterpret_cast<uint4*>(orow + c * 32 + g * 8) = *reinterpret_cast<uint4*>(pk);
-                }
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, Cfg::TMEM_COLS); }
-}
-
-
-// ================================================================================================================
-// Split-fp16 (RB_F16S) variant for the parity mode, head_dim 64 (DINOv2 ViT-L): fp32-class attention on the f16 tensor pipe.
-//   q, k, v arrive as (hi, lo') plane pairs (value = hi + lo' * 2^-11, written by the qkv GEMM epilogue).
-//   S_j = Q K_j^T with three MMAs per k-step into TWO accumulators (main: hi.hi; cross: hi.lo' + lo'.hi), score = main +
-//         cross * 2^-11; key tiles of 64 so that two score stages (2 x 128 columns) + O fit the 512 TMEM columns.
-//   P V : the probabilities are written in an exponent-shifted form so that ONE accumulator suffices:
-//         O' = sum_j (Pt_hi + Pt_lo) V_hi + P_hi V_lo'      with Pt = 2048 p, Pt_hi = fp16(Pt), Pt_lo = fp16(Pt - Pt_hi),
-//         P_hi = fp16(p) = Pt_hi / 2048, i.e. O' = 2048 * sum p (V_hi + V_lo' / 2048) up to a 2^-22 relative term.  p <= 1, so
-//         Pt <= 2048 never overflows; the unscaled low part Pt_lo only underflows for p < 6e-5, where its absolute error
-//         (1.5e-11 in units of p) is irrelevant.
-//   out  = O' / (2048 l) written as an RB_F16S pair for the projection GEMM.
-// Warp roles and barriers are those of flash_attn_kernel above.
-//
-// HALVES = 2 runs the softmax with TWO threads per query row (8 softmax warps, two per scheduler instead of one): thread h of a row owns
-// keys [32h, 32h + 32) of every key tile with its own running maximum / sum AND its own output accumulator O_h (the PV MMAs of k-steps
-// 0-1 go to O_0, of k-steps 2-3 to O_1: same MMA count), so no per-tile exchange between the two threads is needed; the two partial
-// results are merged once at the end, out = (O_0 2^(m_0 - m) + O_1 2^(m_1 - m)) / (2048 (l_0 2^(m_0 - m) + l_1 2^(m_1 - m))).
-// ================================================================================================================
-struct FaSplitParams {
-    void* out_hi; void* out_lo; int64_t ldo;
+    void* out; void* out_lo; int64_t ldo;     // [Bn, N, dim] rows of pitch ldo (elements); out_lo: low plane of the split variant
     int N, heads, dim;
-    float scale_log2;
+    float scale_log2;                         // log2(e) / sqrt(d)
 };
 
-struct FaSplitCfg {
-    static constexpr int D = 64, BQ = 128, BKV = 64, STAGES = 3;
-    static constexpr int Q_BYTES = BQ * D * 2;              // one plane
-    static constexpr int KV_BYTES = BKV * D * 2;            // one plane of one of K, V
-    static constexpr int STAGE_BYTES = 4 * KV_BYTES;        // K_hi, K_lo, V_hi, V_lo
-    static constexpr int P_BYTES = BQ * BKV * 2;            // one of the three probability operands
-    static constexpr int SMEM = 2 * Q_BYTES + STAGES * STAGE_BYTES + 2 * 3 * P_BYTES + 1024 + 256;   // two sets of the three probability operands
-    static constexpr int TMEM_COLS = 512;                   // S: 2 stages x (64 main + 64 cross), O: 64 per key half  (power of two >= 384)
+// D = head dim; SPLIT: RB_F16S planes (D = 64, T = __half)
+template <int D, bool SPLIT> struct FaCfg {
+    static constexpr int BQ = 128, BKV = SPLIT ? 64 : 128;
+    static constexpr int NP = SPLIT ? 2 : 1;                // operand planes
+    static constexpr int Q_BYTES = BQ * D * 2;              // one plane: D / 64 blocks of [BQ rows x 128 B]
+    static constexpr int KV_BYTES = BKV * D * 2;            // one plane of one of K, V: D / 64 blocks of [BKV rows x 128 B]
+    static constexpr int STAGE_BYTES = 2 * NP * KV_BYTES;   // K planes, then V planes
+    static constexpr int STAGES = (200 * 1024 - NP * Q_BYTES) / STAGE_BYTES > 4 ? 4 : (200 * 1024 - NP * Q_BYTES) / STAGE_BYTES;
+    static constexpr int SMEM = NP * Q_BYTES + STAGES * STAGE_BYTES + 1024 + 256;
+    static_assert(STAGES >= 2, "shared memory budget");
 };
 
-template <int HALVES>
-__global__ void __launch_bounds__(64 + 128 * HALVES, 1) flash_attn_split_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
-                                                                                 const FaSplitParams p) {
+template <int D, typename T, bool SPLIT>
+__global__ void __launch_bounds__(384, 1) flash_attn_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo,
+                                                            const FaParams p) {
     rb::pdl_wait();
     using namespace fa;
-    using Cfg = FaSplitCfg;
-    constexpr int STAGES = Cfg::STAGES, BQ = Cfg::BQ, BKV = Cfg::BKV, D = Cfg::D;
+    using Cfg = FaCfg<D, SPLIT>;
+    constexpr int STAGES = Cfg::STAGES, BQ = Cfg::BQ, BKV = Cfg::BKV, NP = Cfg::NP, DB = D / 64;
+    constexpr bool BF16 = std::is_same<T, __nv_bfloat16>::value;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);   // offset on the array: keeps ld/st.shared
-    uint8_t* sQh = smem;
-    uint8_t* sQl = sQh + Cfg::Q_BYTES;
-    uint8_t* sKV = sQl + Cfg::Q_BYTES;                        // per stage: K_hi | K_lo | V_hi | V_lo
-    uint8_t* sP = sKV + STAGES * Cfg::STAGE_BYTES;            // two buffers of Pt_hi | Pt_lo | P_hi (tile j uses buffer j & 1)
-    constexpr int PSET = 3 * Cfg::P_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(sP + 2 * PSET);
+    uint8_t* sQ = smem;                                       // plane q at sQ + q * Q_BYTES
+    uint8_t* sKV = sQ + NP * Cfg::Q_BYTES;                    // stage s: K planes, V planes
+    uint64_t* bars = reinterpret_cast<uint64_t*>(sKV + STAGES * Cfg::STAGE_BYTES);
     uint64_t* q_full = bars;                  // [1]
     uint64_t* kv_full = bars + 1;             // [STAGES]
-    uint64_t* kv_empty = kv_full + STAGES;    // [STAGES]
-    uint64_t* s_full = kv_empty + STAGES;     // [2]
-    uint64_t* s_empty = s_full + 2;           // [2]
-    uint64_t* p_ready = s_empty + 2;          // [2]  one per probability buffer
-    uint64_t* pv_done = p_ready + 2;          // [2]  PV_j retired, committed on pv_done[j & 1]
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(pv_done + 2);
+    uint64_t* kv_empty = kv_full + STAGES;    // [STAGES]  one arrival per consumer warpgroup
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int q0 = blockIdx.x * BQ, head = blockIdx.y, img = blockIdx.z;
     const int ntiles = (p.N + BKV - 1) / BKV;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         mbar_init(q_full, 1);
-        for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 1); }
-        for (int s = 0; s < 2; ++s) {
-            mbar_init(&s_full[s], 1); mbar_init(&s_empty[s], 4 * HALVES); mbar_init(&p_ready[s], 4 * HALVES); mbar_init(&pv_done[s], 1);
-        }
+        for (int s = 0; s < STAGES; ++s) { mbar_init(&kv_full[s], 1); mbar_init(&kv_empty[s], 2); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::TMEM_COLS);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_S = tmem_base;              // stage s: main at s * 128, cross at s * 128 + 64
-    const uint32_t tmem_O = tmem_base + 256;        // columns [256, 320): O (HALVES = 1) or O_0; [320, 384): O_1
 
-    if (warp == 0) {
-        // ===== TMA producer (boxes of 64 rows x 64 columns; the 128-query tile is two boxes per plane) =====
-        if (lane == 0) {
+    if (warp >= 8) {
+        // ===== TMA producer: boxes of 64 rows x 64 columns (128 B) =====
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+        if (warp == 8 && lane == 0) {
+            const CUtensorMap* maps[2] = {&map_hi, &map_lo};
             const int cq = head * D, ck = p.dim + head * D, cv = 2 * p.dim + head * D;
-            mbar_expect_tx(q_full, 2 * Cfg::Q_BYTES);
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-                tma_load_3d(sQh + h * (64 * 128), &map_hi, q_full, cq, q0 + 64 * h, img);
-                tma_load_3d(sQl + h * (64 * 128), &map_lo, q_full, cq, q0 + 64 * h, img);
-            }
+            mbar_expect_tx(q_full, NP * Cfg::Q_BYTES);
+            for (int pl = 0; pl < NP; ++pl)
+                for (int b = 0; b < DB; ++b)
+                    for (int h = 0; h < BQ / 64; ++h)
+                        tma_load_3d(sQ + pl * Cfg::Q_BYTES + b * (BQ * 128) + h * (64 * 128), maps[pl], q_full, cq + 64 * b, q0 + 64 * h, img);
             for (int j = 0; j < ntiles; ++j) {
                 const int s = j % STAGES;
-                const uint32_t u = j / STAGES;
-                mbar_wait(&kv_empty[s], (u & 1) ^ 1);
+                mbar_wait(&kv_empty[s], ((j / STAGES) & 1) ^ 1);
                 mbar_expect_tx(&kv_full[s], Cfg::STAGE_BYTES);
                 uint8_t* st = sKV + s * Cfg::STAGE_BYTES;
-                tma_load_3d(st, &map_hi, &kv_full[s], ck, j * BKV, img);
-                tma_load_3d(st + Cfg::KV_BYTES, &map_lo, &kv_full[s], ck, j * BKV, img);
-                tma_load_3d(st + 2 * Cfg::KV_BYTES, &map_hi, &kv_full[s], cv, j * BKV, img);
-                tma_load_3d(st + 3 * Cfg::KV_BYTES, &map_lo, &kv_full[s], cv, j * BKV, img);
+                for (int pl = 0; pl < NP; ++pl)
+                    for (int b = 0; b < DB; ++b)
+                        for (int h = 0; h < BKV / 64; ++h) {
+                            const int off = b * (BKV * 128) + h * (64 * 128);
+                            tma_load_3d(st + pl * Cfg::KV_BYTES + off, maps[pl], &kv_full[s], ck + 64 * b, j * BKV + 64 * h, img);
+                            tma_load_3d(st + (NP + pl) * Cfg::KV_BYTES + off, maps[pl], &kv_full[s], cv + 64 * b, j * BKV + 64 * h, img);
+                        }
             }
         }
-    } else if (warp == 1) {
-        // ===== MMA issuer =====
-        if (lane == 0) {
-            // S = Q K^T : A, B K-major fp16, N = 64;   O' += P V : A K-major, B MN-major, N = 64
-            const uint32_t idesc_s = (1u << 4) | ((uint32_t)(BKV >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-            const uint32_t idesc_o = (1u << 4) | (1u << 16) | ((uint32_t)(D >> 3) << 17) | ((uint32_t)(BQ >> 4) << 24);
-            const uint32_t qh_addr = smem_u32(sQh), ql_addr = smem_u32(sQl), p_addr = smem_u32(sP);
-            auto issue_s = [&](int j) {
-                const int s = j % STAGES;
-                mbar_wait(&kv_full[s], (j / STAGES) & 1);
-                const uint32_t u = j >> 1;                       // previous uses of this score stage
-                mbar_wait(&s_empty[j & 1], (u & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t kh_addr = smem_u32(sKV + s * Cfg::STAGE_BYTES), kl_addr = kh_addr + Cfg::KV_BYTES;
-                const uint32_t t_main = tmem_S + (j & 1) * 128, t_cross = t_main + 64;
-#pragma unroll
-                for (int k = 0; k < D / 16; ++k) {
-                    const uint32_t off = k * 32;                 // 32 B per K step inside the 128-byte swizzle atom
-                    const uint64_t qh = smem_desc(qh_addr + off, 16, 1024), ql = smem_desc(ql_addr + off, 16, 1024);
-                    const uint64_t kh = smem_desc(kh_addr + off, 16, 1024), kl = smem_desc(kl_addr + off, 16, 1024);
-                    umma_f16(t_main, qh, kh, idesc_s, k != 0);
-                    umma_f16(t_cross, qh, kl, idesc_s, k != 0);
-                    umma_f16(t_cross, ql, kh, idesc_s, 1u);
-                }
-                umma_commit(&s_full[j & 1]);
-            };
-            mbar_wait(q_full, 0);
-            issue_s(0);
-            for (int j = 0; j < ntiles; ++j) {
-                if (j + 1 < ntiles) issue_s(j + 1);
-                mbar_wait(&p_ready[j & 1], (j >> 1) & 1);
-                tc_fence_after();
-                const int s = j % STAGES;
-                const uint32_t pj_addr = p_addr + (j & 1) * PSET;
-                const uint32_t vh_addr = smem_u32(sKV + s * Cfg::STAGE_BYTES + 2 * Cfg::KV_BYTES), vl_addr = vh_addr + Cfg::KV_BYTES;
-#pragma unroll
-                for (int k = 0; k < BKV / 16; ++k) {
-                    // P operands: 128 rows x 64 keys (one swizzle atom wide), 16 keys = 32 B; V tile [64 keys x 128 B]: 16 keys = 2048 B
-                    const uint64_t pth = smem_desc(pj_addr + k * 32, 16, 1024), ptl = smem_desc(pj_addr + Cfg::P_BYTES + k * 32, 16, 1024);
-                    const uint64_t ph = smem_desc(pj_addr + 2 * Cfg::P_BYTES + k * 32, 16, 1024);
-                    const uint64_t vh = smem_desc(vh_addr + k * 2048, BKV * 128, 1024), vl = smem_desc(vl_addr + k * 2048, BKV * 128, 1024);
-                    // HALVES = 2: keys [0, 32) of the tile (k-steps 0, 1) accumulate into O_0, keys [32, 64) into O_1
-                    const uint32_t t_o = HALVES == 2 ? tmem_O + (uint32_t)(k >> 1) * 64 : tmem_O;
-                    const uint32_t acc = HALVES == 2 ? (uint32_t)((j != 0) || (k & 1)) : (uint32_t)((j | k) != 0);
-                    umma_f16(t_o, pth, vh, idesc_o, acc);
-                    umma_f16(t_o, ptl, vh, idesc_o, 1u);
-                    umma_f16(t_o, ph, vl, idesc_o, 1u);
-                }
-                umma_commit(&kv_empty[s]);
-                umma_commit(&pv_done[j & 1]);
-            }
-        }
-    } else {
-        // ===== softmax / correction / epilogue: HALVES threads per query row, each on KW = 64 / HALVES keys of every tile =====
-        constexpr int KW = BKV / HALVES;
-        const int q = warp & 3;                                  // TMEM lane quadrant of this warp
-        const int half = HALVES == 2 ? (warp - 2) >> 2 : 0;
-        const int row = q * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(q * 32) << 16;
-        const uint32_t my_O = tmem_O + (uint32_t)half * 64;
-        float m_run = -INFINITY, l_run = 0.f;
-        for (int j = 0; j < ntiles; ++j) {
-            mbar_wait(&s_full[j & 1], (j >> 1) & 1);
-            tc_fence_after();
-            float sc[KW];
-            {
-                float cr[32];
-#pragma unroll
-                for (int c = 0; c < KW / 32; ++c) {
-                    tmem_ld32(tmem_S + lane_addr + (j & 1) * 128 + half * KW + c * 32, sc + c * 32);
-                    tmem_ld32(tmem_S + lane_addr + (j & 1) * 128 + 64 + half * KW + c * 32, cr);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) sc[c * 32 + i] = fmaf(cr[i], 1.0f / 2048.0f, sc[c * 32 + i]);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&s_empty[j & 1]);
-            const int valid = min(BKV, p.N - j * BKV) - half * KW;
-            float m_new = m_run;
-#pragma unroll
-            for (int i = 0; i < KW; ++i) {
-                sc[i] = i < valid ? sc[i] * p.scale_log2 : -INFINITY;
-                m_new = fmaxf(m_new, sc[i]);
-            }
-            // a key half that has not seen a valid key yet (N < 33 only) keeps m = -inf: use 0 as the reference so that p = 0, alpha = 0
-            const float m_ref = m_new == -INFINITY ? 0.f : m_new;
-            const float alpha = ex2(m_run - m_ref);           // 0 on the first tile (m_run = -inf)
-            // the probability operands are double-buffered, so this loop runs one tile ahead of the PV products: it only waits for
-            // PV_{j-2} (its buffer is free again) and, when a running maximum moved, for PV_{j-1} before rescaling O in TMEM
-            if (j > 0 && __any_sync(0xffffffffu, m_new > m_run)) {
-                mbar_wait(&pv_done[(j - 1) & 1], ((j - 1) >> 1) & 1);   // PV_{j-1} (and all before it) retired: O is stable
-                tc_fence_after();
-#pragma unroll
-                for (int c = 0; c < D / 32; ++c) {
-                    float o[32];
-                    tmem_ld32(my_O + lane_addr + c * 32, o);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) o[i] *= alpha;
-                    tmem_st32(my_O + lane_addr + c * 32, o);
-                }
-            }
-            if (j >= 2) mbar_wait(&pv_done[j & 1], ((j >> 1) - 1) & 1);   // PV_{j-2} retired: probability buffer j & 1 is free
-            float lsum = 0.f;
-            // P rows -> K-major SW128 (one 64-key atom): 16-byte chunk c' = (key / 8) XOR (row % 8)
-            uint8_t* prow = sP + (j & 1) * PSET + row * 128;
-#pragma unroll
-            for (int c = 0; c < KW / 8; ++c) {
-                __half pth[8], ptl[8], ph[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const float pv = ex2(sc[c * 8 + e] - m_ref);
-                    lsum += pv;
-                    const float pt = pv * 2048.0f;
-                    pth[e] = __float2half_rn(pt);
-                    ptl[e] = __float2half_rn(pt - __half2float(pth[e]));
-                    ph[e] = __float2half_rn(pv);
-                }
-                const int cc = (c + half * (KW / 8)) ^ (row & 7);
-                *reinterpret_cast<uint4*>(prow + cc * 16) = *reinterpret_cast<uint4*>(pth);
-                *reinterpret_cast<uint4*>(prow + Cfg::P_BYTES + cc * 16) = *reinterpret_cast<uint4*>(ptl);
-                *reinterpret_cast<uint4*>(prow + 2 * Cfg::P_BYTES + cc * 16) = *reinterpret_cast<uint4*>(ph);
-            }
-            l_run = l_run * alpha + lsum;
-            m_run = m_new;
-            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy smem writes -> visible to UMMA
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&p_ready[j & 1]);
-        }
-        mbar_wait(&pv_done[(ntiles - 1) & 1], ((ntiles - 1) >> 1) & 1);
-        tc_fence_after();
-        const int qi = q0 + row;
-        const int64_t o_off = ((int64_t)img * p.N + qi) * p.ldo + head * D;
-        if constexpr (HALVES == 1) {
-            const float inv = 1.0f / (l_run * 2048.0f);
-#pragma unroll
-            for (int c = 0; c < D / 32; ++c) {
-                float o[32];
-                tmem_ld32(tmem_O + lane_addr + c * 32, o);
-                if (qi < p.N) {
-#pragma unroll
-                    for (int g = 0; g < 4; ++g) {
-                        __half hi[8], lo[8];
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) split_f16s(o[g * 8 + e] * inv, hi[e], lo[e]);
-                        *reinterpret_cast<uint4*>((__half*)p.out_hi + o_off + c * 32 + g * 8) = *reinterpret_cast<uint4*>(hi);
-                        *reinterpret_cast<uint4*>((__half*)p.out_lo + o_off + c * 32 + g * 8) = *reinterpret_cast<uint4*>(lo);
-                    }
-                }
-            }
-        } else {
-            // merge the two key halves: (m, l) of both through shared memory (the P buffers are free after the last PV), then thread h of a
-            // row writes output columns [32h, 32h + 32) from O_0 and O_1
-            float2* ml = reinterpret_cast<float2*>(sP);
-            ml[half * BQ + row] = make_float2(m_run, l_run);
-            asm volatile("bar.sync 1, 256;" ::: "memory");                 // the 8 softmax warps only
-            const float2 a0 = ml[row], a1 = ml[BQ + row];
-            const float m = fmaxf(a0.x, a1.x);                             // finite: key half 0 always holds a valid key
-            const float w0 = ex2(a0.x - m), w1 = ex2(a1.x - m);
-            const float inv = 1.0f / ((a0.y * w0 + a1.y * w1) * 2048.0f);
-            const float s0 = w0 * inv, s1 = w1 * inv;
-            float o0[32], o1[32];
-            tmem_ld32(tmem_O + lane_addr + half * 32, o0);
-            tmem_ld32(tmem_O + 64 + lane_addr + half * 32, o1);
-            if (qi < p.N) {
-#pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    __half hi[8], lo[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) split_f16s(fmaf(o0[g * 8 + e], s0, o1[g * 8 + e] * s1), hi[e], lo[e]);
-                    *reinterpret_cast<uint4*>((__half*)p.out_hi + o_off + half * 32 + g * 8) = *reinterpret_cast<uint4*>(hi);
-                    *reinterpret_cast<uint4*>((__half*)p.out_lo + o_off + half * 32 + g * 8) = *reinterpret_cast<uint4*>(lo);
-                }
-            }
-        }
-        tc_fence_before();
+        return;
     }
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, Cfg::TMEM_COLS); }
+
+    // ===== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64); this thread rows r and r + 8 of them =====
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    const int quad = t & 3;
+    float o[D / 2];
+#pragma unroll
+    for (int i = 0; i < D / 2; ++i) o[i] = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};     // l_run: this thread's part of the row sums
+    const uint32_t q_addr = smem_u32(sQ) + wg * (64 * 128);
+    mbar_wait(q_full, 0);
+    for (int j = 0; j < ntiles; ++j) {
+        const int s = j % STAGES;
+        mbar_wait(&kv_full[s], (j / STAGES) & 1);
+        const uint32_t k_addr = smem_u32(sKV + s * Cfg::STAGE_BYTES), v_addr = k_addr + NP * Cfg::KV_BYTES;
+        float sc[BKV / 2];
+        float cr[SPLIT ? BKV / 2 : 1];
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < D / 16; ++k) {
+            const uint32_t qoff = (k >> 2) * (BQ * 128) + (k & 3) * 32, koff = (k >> 2) * (BKV * 128) + (k & 3) * 32;   // 64-element blocks, 32 B per k-step
+            const uint64_t qh = gmma_desc(q_addr + qoff, 16, 1024), kh = gmma_desc(k_addr + koff, 16, 1024);
+            Wgmma<BKV, BF16>::template ss<0>(sc, qh, kh, k != 0);
+            if constexpr (SPLIT) {
+                const uint64_t ql = gmma_desc(q_addr + Cfg::Q_BYTES + qoff, 16, 1024), kl = gmma_desc(k_addr + Cfg::KV_BYTES + koff, 16, 1024);
+                Wgmma<BKV, BF16>::template ss<0>(cr, qh, kl, k != 0);
+                Wgmma<BKV, BF16>::template ss<0>(cr, ql, kh, 1);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(sc);
+        if constexpr (SPLIT) {
+            wgmma_fence_regs(cr);
+#pragma unroll
+            for (int i = 0; i < BKV / 2; ++i) sc[i] = fmaf(cr[i], 1.0f / RB_SPLIT_SCALE, sc[i]);
+        }
+        // scale, mask the keys beyond N, row maxima over the quad
+        const int valid = min(BKV, p.N - j * BKV);
+        float mx[2] = {m_run[0], m_run[1]};
+#pragma unroll
+        for (int i = 0; i < BKV / 2; ++i) {
+            const int col = 8 * (i >> 2) + 2 * quad + (i & 1);
+            sc[i] = col < valid ? sc[i] * p.scale_log2 : -INFINITY;
+            mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sc[i]);
+        }
+        float m_ref[2], alpha[2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+            m_ref[h] = mx[h] == -INFINITY ? 0.f : mx[h];
+            alpha[h] = ex2(m_run[h] - m_ref[h]);          // 0 on the first tile (m_run = -inf)
+            l_run[h] *= alpha[h];
+            m_run[h] = mx[h];
+        }
+#pragma unroll
+        for (int i = 0; i < D / 2; ++i) o[i] *= alpha[(i >> 1) & 1];
+        // probabilities -> A fragments: k-step kk covers accumulator columns [16 kk, 16 kk + 16) = sc[8 kk .. 8 kk + 7]
+        constexpr int KS = BKV / 16;
+        uint32_t ph[KS][4];
+        uint32_t pl[SPLIT ? KS : 1][4], pp[SPLIT ? KS : 1][4];
+#pragma unroll
+        for (int kk = 0; kk < KS; ++kk) {
+#pragma unroll
+            for (int r = 0; r < 4; ++r) {
+                const int i = 8 * kk + 2 * r, h = r & 1;
+                const float p0 = ex2(sc[i] - m_ref[h]), p1 = ex2(sc[i + 1] - m_ref[h]);
+                if constexpr (SPLIT) {
+                    l_run[h] += p0 + p1;
+                    const uint32_t th = pack2<__half>(p0 * RB_SPLIT_SCALE, p1 * RB_SPLIT_SCALE);
+                    const float2 thf = unpack2<__half>(th);
+                    ph[kk][r] = th;
+                    pl[kk][r] = pack2<__half>(p0 * RB_SPLIT_SCALE - thf.x, p1 * RB_SPLIT_SCALE - thf.y);
+                    pp[kk][r] = pack2<__half>(p0, p1);
+                } else {
+                    ph[kk][r] = pack2<T>(p0, p1);
+                    const float2 q = unpack2<T>(ph[kk][r]);
+                    l_run[h] += q.x + q.y;                   // sum what the MMA will actually see
+                }
+            }
+        }
+        // O += P V: V tile = D / 64 blocks of [BKV keys x 128 B], MN-major; 16 keys = 2048 B, the next 64 columns BKV * 128 B further
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < KS; ++kk) {
+            const uint64_t vh = gmma_desc(v_addr + kk * 2048, BKV * 128, 1024);
+            Wgmma<D, BF16>::template rs<1>(o, ph[kk], vh, 1);
+            if constexpr (SPLIT) {
+                const uint64_t vl = gmma_desc(v_addr + Cfg::KV_BYTES + kk * 2048, BKV * 128, 1024);
+                Wgmma<D, BF16>::template rs<1>(o, pl[kk], vh, 1);
+                Wgmma<D, BF16>::template rs<1>(o, pp[kk], vl, 1);
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
+        keep_regs(ph);
+        if constexpr (SPLIT) { keep_regs(pl); keep_regs(pp); }
+        if (t == 0) mbar_arrive(&kv_empty[s]);          // this warpgroup no longer reads stage s
+    }
+    // ===== O / l -> global (16-bit rows, or an RB_F16S pair) =====
+    float inv[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        float l = l_run[h];
+        l += __shfl_xor_sync(0xffffffffu, l, 1);
+        l += __shfl_xor_sync(0xffffffffu, l, 2);
+        inv[h] = 1.0f / (SPLIT ? l * RB_SPLIT_SCALE : l);
+    }
+    const int row0 = q0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int qi = row0 + 8 * h;
+        if (qi >= p.N) continue;
+        const int64_t off = ((int64_t)img * p.N + qi) * p.ldo + head * D + 2 * quad;
+#pragma unroll
+        for (int c = 0; c < D / 8; ++c) {
+            const float v0 = o[4 * c + 2 * h] * inv[h], v1 = o[4 * c + 2 * h + 1] * inv[h];
+            if constexpr (SPLIT) {
+                const uint32_t hi = pack2<__half>(v0, v1);
+                const float2 hf = unpack2<__half>(hi);
+                *reinterpret_cast<uint32_t*>((__half*)p.out + off + 8 * c) = hi;
+                *reinterpret_cast<uint32_t*>((__half*)p.out_lo + off + 8 * c) = pack2<__half>((v0 - hf.x) * RB_SPLIT_SCALE, (v1 - hf.y) * RB_SPLIT_SCALE);
+            } else {
+                *reinterpret_cast<uint32_t*>((T*)p.out + off + 8 * c) = pack2<T>(v0, v1);
+            }
+        }
+    }
 }
 
 typedef CUresult (*EncodeTiledFnFa)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                     CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 
-template <int D, typename T>
-static int launch_fa(const CUtensorMap& map, const FaParams& p, int batch, cudaStream_t st) {
-    using Cfg = FaCfg<D>;
+template <int D, typename T, bool SPLIT>
+static int launch_fa(const CUtensorMap& map_hi, const CUtensorMap& map_lo, const FaParams& p, int batch, cudaStream_t st) {
+    using Cfg = FaCfg<D, SPLIT>;
+    auto kernel = flash_attn_kernel<D, T, SPLIT>;
     static bool configured[64] = {};      // function attributes are per device
     const int dev = current_device() & 63;
     if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(flash_attn_kernel<D, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
+        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
         RB_REQUIRE(e == cudaSuccess, "flash_attn: cannot set %d bytes of dynamic shared memory: %s", Cfg::SMEM, cudaGetErrorString(e));
         configured[dev] = true;
     }
     dim3 grid((p.N + Cfg::BQ - 1) / Cfg::BQ, p.heads, batch);
-    rb::launch_pdl(flash_attn_kernel<D, T>, dim3(grid), dim3(192), Cfg::SMEM, st, map, p);
-    return check_launch("flash_attn");
+    rb::launch_pdl(kernel, dim3(grid), dim3(384), Cfg::SMEM, st, map_hi, map_lo, p);
+    return check_launch(SPLIT ? "flash_attn_split" : "flash_attn");
 }
 
 }  // namespace rb
@@ -640,47 +326,27 @@ extern "C" int romab200_flash_attn(const rb_flash_attn_args* a, void* stream) {
                    "flash_attn: cuTensorMapEncodeTiled not available");
         enc = (EncodeTiledFnFa)ptr;
     }
-    CUtensorMap map;
+    // [batch, tokens, 3 * dim] with boxes of 64 tokens x 64 columns, 128B-swizzled: one plane (hi) or two (hi, lo)
     cuuint64_t dims[3] = {(cuuint64_t)(3 * dim), (cuuint64_t)a->n_tokens, (cuuint64_t)a->batch};
     cuuint64_t strides[2] = {(cuuint64_t)a->ld_qkv * 2, (cuuint64_t)a->ld_qkv * 2 * (cuuint64_t)a->n_tokens};
-    cuuint32_t box[3] = {64, 128, 1};
+    cuuint32_t box[3] = {64, 64, 1};
     cuuint32_t estr[3] = {1, 1, 1};
-    CUresult r = enc(&map, a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv),
+    CUtensorMap map_hi, map_lo;
+    CUresult r = enc(&map_hi, a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv),
                      dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     RB_REQUIRE(r == CUDA_SUCCESS, "flash_attn: cuTensorMapEncodeTiled failed with %d", (int)r);
+    map_lo = map_hi;
     if (a->dtype == RB_F16S) {
-        CUtensorMap map_hi, map_lo;
-        cuuint32_t box64[3] = {64, 64, 1};
-        r = enc(&map_hi, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv), dims, strides, box64, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RB_REQUIRE(r == CUDA_SUCCESS, "flash_attn: cuTensorMapEncodeTiled (hi plane) failed with %d", (int)r);
-        r = enc(&map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv_lo), dims, strides, box64, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+        r = enc(&map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv_lo), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                 CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         RB_REQUIRE(r == CUDA_SUCCESS, "flash_attn: cuTensorMapEncodeTiled (lo plane) failed with %d", (int)r);
-        // ROMAB200_FA_HALVES = 1 | 2: softmax threads per query row of the split kernel (see the kernel's header)
-        const char* halves_env = getenv("ROMAB200_FA_HALVES");      // read per call: tests switch it inside one process
-        const int halves = halves_env && atoi(halves_env) == 2 ? 2 : 1;
-        static bool configured[64] = {};
-        const int dev = current_device() & 63;
-        if (!configured[dev]) {
-            cudaError_t e = cudaFuncSetAttribute(flash_attn_split_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSplitCfg::SMEM);
-            if (e == cudaSuccess) e = cudaFuncSetAttribute(flash_attn_split_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, FaSplitCfg::SMEM);
-            RB_REQUIRE(e == cudaSuccess, "flash_attn: cannot set %d bytes of dynamic shared memory: %s", FaSplitCfg::SMEM, cudaGetErrorString(e));
-            configured[dev] = true;
-        }
-        FaSplitParams sp;
-        sp.out_hi = a->out; sp.out_lo = a->out_lo; sp.ldo = a->ld_out; sp.N = a->n_tokens; sp.heads = a->heads; sp.dim = dim;
-        sp.scale_log2 = 1.4426950408889634f / sqrtf((float)a->head_dim);
-        dim3 grid((a->n_tokens + FaSplitCfg::BQ - 1) / FaSplitCfg::BQ, a->heads, a->batch);
-        if (halves == 2) rb::launch_pdl(flash_attn_split_kernel<2>, dim3(grid), dim3(320), FaSplitCfg::SMEM, st, map_hi, map_lo, sp);
-        else rb::launch_pdl(flash_attn_split_kernel<1>, dim3(grid), dim3(192), FaSplitCfg::SMEM, st, map_hi, map_lo, sp);
-        return check_launch("flash_attn_split");
     }
     FaParams p;
-    p.out = a->out; p.ldo = a->ld_out; p.N = a->n_tokens; p.heads = a->heads; p.dim = dim; p.is_bf16 = a->dtype == RB_BF16;
+    p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ld_out; p.N = a->n_tokens; p.heads = a->heads; p.dim = dim;
     p.scale_log2 = 1.4426950408889634f / sqrtf((float)a->head_dim);
+    if (a->dtype == RB_F16S) return launch_fa<64, __half, true>(map_hi, map_lo, p, a->batch, st);
     if (a->head_dim == 64)
-        return a->dtype == RB_F16 ? launch_fa<64, __half>(map, p, a->batch, st) : launch_fa<64, __nv_bfloat16>(map, p, a->batch, st);
-    return a->dtype == RB_F16 ? launch_fa<128, __half>(map, p, a->batch, st) : launch_fa<128, __nv_bfloat16>(map, p, a->batch, st);
+        return a->dtype == RB_F16 ? launch_fa<64, __half, false>(map_hi, map_lo, p, a->batch, st) : launch_fa<64, __nv_bfloat16, false>(map_hi, map_lo, p, a->batch, st);
+    return a->dtype == RB_F16 ? launch_fa<128, __half, false>(map_hi, map_lo, p, a->batch, st) : launch_fa<128, __nv_bfloat16, false>(map_hi, map_lo, p, a->batch, st);
 }

@@ -181,13 +181,13 @@ __global__ void __launch_bounds__(256) gemm_simt_kernel(const SimtParams p) {
             *reinterpret_cast<float4*>(&b[0]) = *reinterpret_cast<const float4*>(&Bs[buf][k][tx * 4]);
             if constexpr (TN == 8)
                 *reinterpret_cast<float4*>(&b[4]) = *reinterpret_cast<const float4*>(&Bs[buf][k][BN / 2 + tx * 4]);
-            // packed fp32 FMA (FFMA2, sm_100): two accumulator columns per instruction
+            // two accumulator columns per step (a channel pair of fp32 FMAs)
 #pragma unroll
             for (int i = 0; i < TM; ++i) {
                 const float2 ai = make_float2(a[i], a[i]);
 #pragma unroll
                 for (int j = 0; j < TN; j += 2) {
-                    float2 r = __ffma2_rn(ai, make_float2(b[j], b[j + 1]), make_float2(acc[i][j], acc[i][j + 1]));
+                    float2 r = rb::fma2(ai, make_float2(b[j], b[j + 1]), make_float2(acc[i][j], acc[i][j + 1]));
                     acc[i][j] = r.x; acc[i][j + 1] = r.y;
                 }
             }

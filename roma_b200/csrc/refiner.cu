@@ -487,7 +487,7 @@ __global__ void __launch_bounds__(256) refiner_block_small_kernel(const T* __res
 #pragma unroll
                 for (int kx = 0; kx < 5; ++kx) {
                     const int ox = px - kx;
-                    if (ox >= 0 && ox < TS) acc[ox] = __ffma2_rn(wv[ky * 5 + kx], v, acc[ox]);
+                    if (ox >= 0 && ox < TS) acc[ox] = rb::fma2(wv[ky * 5 + kx], v, acc[ox]);
                 }
             }
         }
@@ -589,7 +589,7 @@ __global__ void __launch_bounds__(256) refiner_block_small_f32_kernel(const floa
 #pragma unroll
                 for (int kx = 0; kx < 5; ++kx) {
                     const int ox = px - kx;
-                    if (ox >= 0 && ox < TS) acc[ox] = __ffma2_rn(wv[ky * 5 + kx], v, acc[ox]);
+                    if (ox >= 0 && ox < TS) acc[ox] = rb::fma2(wv[ky * 5 + kx], v, acc[ox]);
                 }
             }
         }
@@ -790,7 +790,7 @@ using namespace rb;
 
 static inline unsigned grid1d(int64_t total, int block) {
     int64_t g = (total + block - 1) / block;
-    int64_t cap = 148 * 64;
+    int64_t cap = 132 * 64;
     return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
 }
 

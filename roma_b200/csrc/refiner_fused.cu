@@ -4,13 +4,14 @@
 // of their time in per-tile overheads; here
 //   * 1 thread TMA-loads the 12x20 pixel input window of an 8x16 tile (4-D tensor map over [B,H,W,C]: the image border
 //     is the map's out-of-bounds zero fill, no address arithmetic, no registers);
-//   * 9 depthwise warps run the 5x5 stage on the CUDA cores (channel pairs, packed FFMA2) and write the ReLU'd
-//     128 x 144 result straight into the 128B-swizzled K-major layout of a UMMA A operand;
-//   * 1 thread issues 9 tcgen05.mma (M=128, N=144, K=16) against the pointwise weights, which were TMA-loaded into
-//     shared memory once and stay resident;
-//   * 4 epilogue warps read the fp32 accumulator from TMEM (double-buffered), add the bias and store 16-bit rows.
+//   * 9 depthwise warps run the 5x5 stage on the CUDA cores (channel pairs) and write the ReLU'd 128 x 144 result
+//     straight into the 128B-swizzled K-major layout of a wgmma A operand;
+//   * 1 warpgroup multiplies it with the pointwise weights (TMA-loaded into shared memory once, resident for the whole
+//     persistent kernel): per 64-pixel half 9 wgmma (M=64, N=144, K=16) into registers, then + bias -> 16-bit rows.
 #include "common.cuh"
+#include "wgmma.cuh"
 #include <cuda.h>
+#include <type_traits>
 
 namespace rb {
 namespace fz {
@@ -48,51 +49,6 @@ __device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* m
         ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
         : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-          "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-          "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-          "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr));
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
 }  // namespace fz
 
 #ifdef RB_FZ_CLK
@@ -110,7 +66,7 @@ struct FusedParams {
 
 constexpr int FZ_C = 144, FZ_CP = 72, FZ_TH = 8, FZ_TW = 16, FZ_IH = 12, FZ_IW = 20;
 constexpr int FZ_DW_THREADS = 288;                    // 72 channel pairs x 4 row groups
-constexpr int FZ_THREADS = 32 + 128 + FZ_DW_THREADS + 32;  // warp 0: weights + MMA, warps 1-4: epilogue, warps 5-13: depthwise, warp 14: input TMA
+constexpr int FZ_THREADS = 128 + 32 + FZ_DW_THREADS;  // warps 0-3: weights + MMA + epilogue, warp 4: input TMA, warps 5-13: depthwise
 constexpr int FZ_IN_BYTES = FZ_IH * FZ_IW * FZ_C * 2;              // 69120
 constexpr int FZ_A_BYTES = 3 * 128 * 128;                          // 49152: 3 k-blocks of 64 channels, 128 pixel rows
 constexpr int FZ_B_KB = FZ_C * 128;                                // 18432 per k-block
@@ -132,90 +88,68 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const
     uint64_t* w_full = bars;            // weights landed
     uint64_t* a_full = bars + 1;        // depthwise tile written (9 warp arrivals)
     uint64_t* a_empty = bars + 2;       // MMAs that read it retired
-    uint64_t* t_full = bars + 3;        // [2] accumulator ready
-    uint64_t* t_empty = bars + 5;       // [2] accumulator drained (4 warp arrivals)
-    uint64_t* in_full = bars + 7;       // input window landed (TMA transaction bytes)
-    uint64_t* in_empty = bars + 8;      // depthwise warps have read it (9 warp arrivals)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 9);
-    float* s_bias = reinterpret_cast<float*>(bars + 10);    // [144]
+    uint64_t* in_full = bars + 3;       // input window landed (TMA transaction bytes)
+    uint64_t* in_empty = bars + 4;      // depthwise warps have read it (9 warp arrivals)
+    float* s_bias = reinterpret_cast<float*>(bars + 6);     // [144]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     if (threadIdx.x == 0) {
         mbar_init(w_full, 1); mbar_init(a_full, FZ_DW_THREADS / 32); mbar_init(a_empty, 1);
-        for (int s = 0; s < 2; ++s) { mbar_init(&t_full[s], 1); mbar_init(&t_empty[s], 4); }
         mbar_init(in_full, 1); mbar_init(in_empty, FZ_DW_THREADS / 32);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
     for (int i = threadIdx.x; i < FZ_C; i += FZ_THREADS) s_bias[i] = p.pw_b[i];
     for (int i = threadIdx.x; i < 25 * FZ_C; i += FZ_THREADS) s_dw[i] = p.dw_w[(int64_t)(i / FZ_C) * p.ldw + (i % FZ_C)];
     for (int i = threadIdx.x; i < FZ_A_BYTES / 16; i += FZ_THREADS) reinterpret_cast<uint4*>(sA)[i] = make_uint4(0u, 0u, 0u, 0u);   // K padding stays 0
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     const int tiles_per_img = p.tiles_x * p.tiles_y;
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (warp < 4) {
+        // ===== pointwise GEMM + epilogue: the warpgroup takes the 128-pixel tile in two halves of 64 rows =====
+        const int t = threadIdx.x;
+        if (t == 0) {
             // pointwise weights [144 x 144] -> three K-major k-blocks, loaded once for the whole persistent kernel
             mbar_expect_tx(w_full, FZ_B_BYTES);
             for (int kb = 0; kb < 3; ++kb) tma_load_2d(sB + kb * FZ_B_KB, &map_w, w_full, kb * 64, 0);
-            const uint32_t fmt = p.is_bf16 ? 1u : 0u;
-            const uint32_t idesc = (1u << 4) | (fmt << 7) | (fmt << 10) | ((uint32_t)(FZ_C >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-            mbar_wait(w_full, 0);
-            const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
-            uint32_t it = 0;
-            for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
-                const uint32_t acc = it & 1;
-                mbar_wait(&t_empty[acc], ((it >> 1) & 1) ^ 1);
-                mbar_wait(a_full, it & 1);
-                tc_fence_after();
-#pragma unroll
-                for (int k = 0; k < FZ_C / 16; ++k) {
-                    const uint32_t aoff = (k >> 2) * (128 * 128) + (k & 3) * 32, boff = (k >> 2) * FZ_B_KB + (k & 3) * 32;
-                    umma_f16(tmem_base + acc * FZ_C, smem_desc(a_addr + aoff, 16, 1024), smem_desc(b_addr + boff, 16, 1024), idesc, k != 0);
-                }
-                umma_commit(a_empty);
-                umma_commit(&t_full[acc]);
-            }
         }
-    } else if (warp <= 4) {
-        // ===== epilogue: TMEM -> + bias -> 16-bit rows (one pixel per thread, 288 contiguous bytes) =====
-        const int q = warp & 3;
-        const int m = q * 32 + lane;                       // pixel of the tile
-        const int py = m / FZ_TW, px = m - py * FZ_TW;
+        mbar_wait(w_full, 0);
+        const uint32_t a_addr = smem_u32(sA), b_addr = smem_u32(sB);
         uint32_t it = 0;
         for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x, ++it) {
             const int img = tile / tiles_per_img, r = tile - img * tiles_per_img;
             const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
-            const int yy = ty * FZ_TH + py, xx = tx * FZ_TW + px;
-            const bool live = yy < p.H && xx < p.W;
-            T* orow = (T*)p.out + (((int64_t)img * p.H + yy) * p.W + xx) * p.ld;
-            const uint32_t acc = it & 1;
-            mbar_wait(&t_full[acc], (it >> 1) & 1);
-            tc_fence_after();
+            mbar_wait(a_full, it & 1);
 #pragma unroll 1
-            for (int cb = 0; cb < FZ_C; cb += 32) {
-                float v[32];
-                tmem_ld32(tmem_base + ((uint32_t)(q * 32) << 16) + acc * FZ_C + cb, v);
-                if (!live) continue;
+            for (int half = 0; half < 2; ++half) {
+                float acc[FZ_C / 2];
+                wgmma_fence();
 #pragma unroll
-                for (int g = 0; g < 4; ++g) {
-                    if (cb + 8 * g < FZ_C) {
-                        T pk[8];
+                for (int k = 0; k < FZ_C / 16; ++k) {
+                    const uint32_t aoff = (k >> 2) * (128 * 128) + half * (64 * 128) + (k & 3) * 32, boff = (k >> 2) * FZ_B_KB + (k & 3) * 32;
+                    Wgmma<FZ_C, std::is_same<T, __nv_bfloat16>::value>::template ss<0>(acc, gmma_desc(a_addr + aoff, 16, 1024), gmma_desc(b_addr + boff, 16, 1024), k != 0);
+                }
+                wgmma_commit();
+                wgmma_wait<0>();
+                wgmma_fence_regs(acc);
+                if (half == 1 && t == 0) mbar_arrive(a_empty);     // the depthwise warps may overwrite sA
+                // accumulator fragment: pixels m and m + 8 of this half, channel pairs 8 i + 2 (t % 4)
+                const int m0 = half * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
 #pragma unroll
-                        for (int e = 0; e < 8; ++e) pk[e] = from_f<T>(v[8 * g + e] + s_bias[cb + 8 * g + e]);
-                        *reinterpret_cast<uint4*>(orow + cb + 8 * g) = *reinterpret_cast<uint4*>(pk);
+                for (int h = 0; h < 2; ++h) {
+                    const int m = m0 + 8 * h;
+                    const int yy = ty * FZ_TH + m / FZ_TW, xx = tx * FZ_TW + m % FZ_TW;
+                    if (yy >= p.H || xx >= p.W) continue;
+                    T* orow = (T*)p.out + (((int64_t)img * p.H + yy) * p.W + xx) * p.ld + 2 * (t & 3);
+#pragma unroll
+                    for (int i = 0; i < FZ_C / 8; ++i) {
+                        T pr[2] = {from_f<T>(acc[4 * i + 2 * h] + s_bias[8 * i + 2 * (t & 3)]), from_f<T>(acc[4 * i + 2 * h + 1] + s_bias[8 * i + 2 * (t & 3) + 1])};
+                        *reinterpret_cast<uint32_t*>(orow + 8 * i) = *reinterpret_cast<uint32_t*>(pr);
                     }
                 }
             }
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&t_empty[acc]);
         }
-    } else if (warp == 14) {
+    } else if (warp == 4) {
         // ===== input loader: one TMA box per tile, re-armed as soon as the depthwise warps have read the previous window =====
         if (lane == 0) {
             uint32_t it = 0;
@@ -262,7 +196,7 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const
 #pragma unroll
                             for (int kx = 0; kx < 5; ++kx) {
                                 const int ox = ix - kx;
-                                if (ox >= 0 && ox < FZ_TW) acc2[rr][ox] = __ffma2_rn(wv[ky * 5 + kx], v, acc2[rr][ox]);
+                                if (ox >= 0 && ox < FZ_TW) { const float2 w2 = wv[ky * 5 + kx]; acc2[rr][ox].x = fmaf(w2.x, v.x, acc2[rr][ox].x); acc2[rr][ox].y = fmaf(w2.y, v.y, acc2[rr][ox].y); }
                             }
                         }
                     }
@@ -290,9 +224,6 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const
 #endif
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, 512); }
 }
 
 typedef CUresult (*EncodeTiledFnFz)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -350,7 +281,7 @@ extern "C" int romab200_refiner_block_c144(const rb_refiner_block_c144_args* a, 
     const long long total = (long long)p.tiles_x * p.tiles_y * a->batch;
     RB_REQUIRE(total > 0 && total < (1ll << 31), "refiner_block_c144: bad tile count");
     p.total_tiles = (int)total; p.is_bf16 = a->dtype == RB_BF16;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = p.total_tiles < sms ? p.total_tiles : sms;

@@ -9,7 +9,9 @@
 //            no intermediate tensor is materialised; the histogram of bits [31:21] is accumulated on the way;
 //   select   (one CTA per batch item, three times) radix select of the k-th smallest key over bits [31:21], [20:10], [9:0] of
 //            the (order-preserving) bit pattern of the positive float keys; `hist` re-histograms the surviving candidates;
-//   compact  indices of all keys below the threshold and as many ties as are still needed (in no particular order).
+//            then three more times over the bits of the INDICES of the keys equal to the k-th one, so that ties at the cut are
+//            resolved by index (smallest first) and the drawn set does not depend on thread timing;
+//   compact  indices of all keys below the k-th one and of the tied keys up to the selected index (in no particular order).
 // The keys of a 1.5 M-pixel certainty map are 6 MB: L2-resident across the passes.  Items of zero weight have key = +inf and are
 // only drawn when fewer than k positive weights exist.
 #include "common.cuh"
@@ -46,8 +48,10 @@ __device__ __forceinline__ float sample_weight(float v, int transform, float par
 
 constexpr int SMP_THREADS = 256;
 constexpr int SMP_BINS = 2048;
-// scratch layout per batch item (int32 words): [0, 2048) histogram, 2048: prefix, 2049: need, 2050: mask, 2051: taken, 2052: ties
+// scratch layout per batch item (int32 words): [0, 2048) histogram, 2048: prefix, 2049: need, 2050: mask, 2051: output count,
+// 2053: the k-th smallest key (set by the last key pass).  Passes 0-2 select over key bits, passes 3-5 over index bits of the ties.
 constexpr int SMP_SCRATCH = SMP_BINS + 8;
+constexpr int SMP_PASSES = 6;
 
 __device__ __forceinline__ void flush_hist(uint32_t* smem_hist, uint32_t* gh, int bins) {
     __syncthreads();
@@ -86,7 +90,8 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_select_kernel(uint32_t* __
     __shared__ uint32_t part[SMP_THREADS];
     uint32_t* sc = scratch + (int64_t)blockIdx.x * SMP_SCRATCH;
     const int shifts[3] = {21, 10, 0}, nbits[3] = {11, 11, 10};
-    const int sh = shifts[pass], bins = 1 << nbits[pass];
+    const int sh = shifts[pass % 3], bins = 1 << nbits[pass % 3];
+    const bool first = pass % 3 == 0;                  // a new radix select starts: empty prefix / mask
     const uint32_t need = pass == 0 ? (uint32_t)k : sc[SMP_BINS + 1];
     // 8 consecutive bins per thread: local sums, scan of the 256 partial sums, then the thread that holds the crossing finds the bin
     constexpr int PER = SMP_BINS / SMP_THREADS;
@@ -106,9 +111,10 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_select_kernel(uint32_t* __
 #pragma unroll
         for (int j = 0; j < PER; ++j) {
             if (cum + local[j] >= need) {
-                const uint32_t prefix = (pass == 0 ? 0u : sc[SMP_BINS]) | ((uint32_t)(threadIdx.x * PER + j) << sh);
-                const uint32_t mask = (pass == 0 ? 0u : sc[SMP_BINS + 2]) | ((uint32_t)(bins - 1) << sh);
+                const uint32_t prefix = (first ? 0u : sc[SMP_BINS]) | ((uint32_t)(threadIdx.x * PER + j) << sh);
+                const uint32_t mask = (first ? 0u : sc[SMP_BINS + 2]) | ((uint32_t)(bins - 1) << sh);
                 sc[SMP_BINS] = prefix; sc[SMP_BINS + 1] = need - cum; sc[SMP_BINS + 2] = mask;
+                if (pass == 2) sc[SMP_BINS + 5] = prefix;     // the k-th smallest key; need - cum of its ties are drawn
                 break;
             }
             cum += local[j];
@@ -116,10 +122,11 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_select_kernel(uint32_t* __
     }
     __syncthreads();
     for (int i = threadIdx.x; i < SMP_BINS; i += SMP_THREADS) sc[i] = 0;
-    if (threadIdx.x == 0) { sc[SMP_BINS + 3] = 0; sc[SMP_BINS + 4] = 0; }
+    if (threadIdx.x == 0) sc[SMP_BINS + 3] = 0;
 }
 
-// passes 1, 2: histogram of the next bits over the candidates (keys whose masked bits equal the prefix)
+// passes 1, 2: histogram of the next key bits over the candidates (keys whose masked bits equal the prefix); passes 3-5: histogram
+// of the index bits of the keys equal to the k-th one (whose masked index bits equal the prefix; none masked in pass 3)
 __global__ void __launch_bounds__(SMP_THREADS) sample_hist_kernel(const float* __restrict__ keys_ws, int64_t n, uint32_t* __restrict__ scratch, int pass) {
     rb::pdl_wait();
     __shared__ uint32_t hist[SMP_BINS];
@@ -127,30 +134,35 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_hist_kernel(const float* _
     uint32_t* sc = scratch + (int64_t)b * SMP_SCRATCH;
     for (int i = threadIdx.x; i < SMP_BINS; i += SMP_THREADS) hist[i] = 0;
     __syncthreads();
-    const uint32_t prefix = sc[SMP_BINS], mask = sc[SMP_BINS + 2];
-    const int sh = pass == 1 ? 10 : 0, bins = pass == 1 ? 2048 : 1024;
+    const bool ties = pass >= 3;
+    const uint32_t prefix = pass == 3 ? 0u : sc[SMP_BINS], mask = pass == 3 ? 0u : sc[SMP_BINS + 2], kth = sc[SMP_BINS + 5];
+    const int shifts[3] = {21, 10, 0};
+    const int sh = shifts[pass % 3], bins = pass % 3 == 2 ? 1024 : 2048;
     const float* keys = keys_ws + (int64_t)b * n;
     for (int64_t i = (int64_t)blockIdx.x * SMP_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * SMP_THREADS) {
         const uint32_t x = __float_as_uint(keys[i]);
-        if ((x & mask) == prefix) atomicAdd(&hist[(x >> sh) & (bins - 1)], 1u);
+        if (!ties) {
+            if ((x & mask) == prefix) atomicAdd(&hist[(x >> sh) & (bins - 1)], 1u);
+        } else if (x == kth && ((uint32_t)i & mask) == prefix) {
+            atomicAdd(&hist[((uint32_t)i >> sh) & (bins - 1)], 1u);
+        }
     }
     flush_hist(hist, sc, bins);
 }
 
-// compaction: every key below the k-th smallest, and as many ties as are still needed
+// compaction: every key below the k-th smallest, and the ties up to the selected index
 __global__ void __launch_bounds__(SMP_THREADS) sample_compact_kernel(const float* __restrict__ values, const float* __restrict__ keys_ws, int64_t n, int k, int64_t stride,
                                                                      int transform, float param, uint32_t* __restrict__ scratch, int32_t* __restrict__ out_idx,
                                                                      float* __restrict__ out_w) {
     rb::pdl_wait();
     const int b = blockIdx.y;
     uint32_t* sc = scratch + (int64_t)b * SMP_SCRATCH;
-    const uint32_t kth = sc[SMP_BINS], need = sc[SMP_BINS + 1];
+    const uint32_t kth = sc[SMP_BINS + 5], last_tie = sc[SMP_BINS];
     const float* keys = keys_ws + (int64_t)b * n;
     const float* v = values + (int64_t)b * stride;
     for (int64_t i = (int64_t)blockIdx.x * SMP_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * SMP_THREADS) {
         const uint32_t x = __float_as_uint(keys[i]);
-        bool take = x < kth;
-        if (x == kth) take = atomicAdd(&sc[SMP_BINS + 4], 1u) < need;
+        const bool take = x < kth || (x == kth && (uint32_t)i <= last_tie);
         if (take) {
             const uint32_t pos = atomicAdd(&sc[SMP_BINS + 3], 1u);
             if (pos < (uint32_t)k) {
@@ -180,10 +192,10 @@ extern "C" int romab200_weighted_sample(const rb_sample_args* a, void* stream) {
     const dim3 grid(gx, a->batch);
     rb::launch_pdl(sample_keys_kernel, grid, dim3(SMP_THREADS), 0, st, a->values, a->n, stride, a->seed, a->seed_dev, a->transform, a->param, a->keys, scratch);
     if (check_launch("weighted_sample(keys)")) return 1;
-    for (int pass = 0; pass < 3; ++pass) {
+    for (int pass = 0; pass < SMP_PASSES; ++pass) {
         rb::launch_pdl(sample_select_kernel, dim3(a->batch), dim3(SMP_THREADS), 0, st, scratch, pass, a->k);
         if (check_launch("weighted_sample(select)")) return 1;
-        if (pass < 2) {
+        if (pass < SMP_PASSES - 1) {
             rb::launch_pdl(sample_hist_kernel, grid, dim3(SMP_THREADS), 0, st, (const float*)a->keys, a->n, scratch, pass + 1);
             if (check_launch("weighted_sample(hist)")) return 1;
         }

@@ -176,7 +176,7 @@ extern "C" int romab200_maxpool2x2_padded(const rb_maxpool_args* a, void* stream
         else rb::launch_pdl(maxpool2x2_padded_vec_kernel<__nv_bfloat162>, dim3((unsigned)gv), dim3(256), 0, st, (const uint4*)a->in, (uint4*)a->out, a->batch, a->height, a->width, a->channels / 8);
         return check_launch("maxpool2x2_padded");
     }
-    int64_t g = (total + 255) / 256; if (g > 148 * 64) g = 148 * 64;
+    int64_t g = (total + 255) / 256; if (g > 132 * 64) g = 132 * 64;
     if (a->dtype == RB_F32) rb::launch_pdl(maxpool2x2_padded_kernel<float>, dim3((unsigned)g), dim3(256), 0, st, (const float*)a->in, (float*)a->out, a->batch, a->height, a->width, a->channels);
     else if (a->dtype == RB_F16) rb::launch_pdl(maxpool2x2_padded_kernel<__half>, dim3((unsigned)g), dim3(256), 0, st, (const __half*)a->in, (__half*)a->out, a->batch, a->height, a->width, a->channels);
     else rb::launch_pdl(maxpool2x2_padded_kernel<__nv_bfloat16>, dim3((unsigned)g), dim3(256), 0, st, (const __nv_bfloat16*)a->in, (__nv_bfloat16*)a->out, a->batch, a->height, a->width, a->channels);

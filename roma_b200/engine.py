@@ -8,12 +8,12 @@ and enqueues the whole of `forward_symmetric` / `forward` (`romatch/models/match
 Precision regimes (`precision=`):
   "fp32"        parity mode on the tensor cores: activations stay fp32 in HBM, every GEMM operand is carried as an
                 RB_F16S pair (fp16 hi plane + 2^11-scaled fp16 lo plane, 22 significand bits) and contracted by
-                three tcgen05 MMAs per k-step with fp32 accumulation in TMEM (gemm_tc.cu, SPLIT variant) — fp32-class
+                three wgmma MMAs per k-step with fp32 accumulation in registers (gemm_tc.cu, SPLIT variant) — fp32-class
                 results, comparable to the reference's CPU fp32 path at the 1e-4 level
                 (tests/test_e2e_gpu.py::test_match_full_vs_reference_golden);
   "fp32_simt"   the same arithmetic regime with CUDA-core FFMA GEMMs (gemm_simt.cu): the slow cross-check of "fp32";
   "fp16"/"bf16" fast mode, mirrors the reference's CUDA autocast regime (`utils.py:639-653`): 16-bit GEMM
-                operands on the tcgen05 tensor pipe with fp32 accumulation, fp32 residual stream,
+                operands on the wgmma tensor pipe with fp32 accumulation, fp32 residual stream,
                 LayerNorm, softmax statistics, GP solve, local-correlation accumulation, heads and
                 flow/certainty state.
 
@@ -51,7 +51,7 @@ class Engine:
         self.precision = precision
         self.dtype = PRECISIONS[precision]
         self.dt = cabi.DTYPE_CODE[self.dtype]
-        self.split = precision == "fp32"         # fp32-class GEMMs on tcgen05 from RB_F16S operand pairs
+        self.split = precision == "fp32"         # fp32-class GEMMs on the tensor cores from RB_F16S operand pairs
         self._lane = "main"                      # scratch buffers are per stream ("main" / "side")
         with torch.cuda.device(self.device):
             self.w = PackedWeights(matcher_sd, dino_sd, self.device, self.dtype, split=self.split)
@@ -59,13 +59,13 @@ class Engine:
         self.generation = 0
         self._const: Dict[tuple, torch.Tensor] = {}
         self.debug: Optional[dict] = None        # set to {} to keep stage tensors (tests)
-        self.use_flash_attn = True               # fused tcgen05 attention in the 16-bit modes (else QK^T / softmax / PV GEMMs)
+        self.use_flash_attn = True               # fused tensor-core attention in the 16-bit modes (else QK^T / softmax / PV GEMMs)
         self.gp_algo = 2 if precision == "fp32_simt" else 3   # 3: 128-wide blocks factored in shared memory + explicit block inverses, the
                                                  # K=128 GEMMs (13 dependent steps) on the tensor cores as split-fp16 pairs; 2: the same with
                                                  # CUDA-core GEMMs; 0: 32-wide launch chain (50 steps); 1: one cooperative persistent kernel.
         self.overlap_cnn = True                  # VGG/proj branch on a side stream, overlapping ViT / GP / decoder
-        self.gp_tensor_core = True               # all-pairs CosKernel on tcgen05 (split-fp16 operands) in the 16-bit modes
-        self.fused_c144 = True                   # stride-2 refiner blocks as one fused DW + tcgen05-PW kernel
+        self.gp_tensor_core = True               # all-pairs CosKernel on the tensor cores (split-fp16 operands) in the 16-bit modes
+        self.fused_c144 = True                   # stride-2 refiner blocks as one fused DW + wgmma-PW kernel
         self.lc_table16 = os.environ.get("ROMAB200_LC_TABLE16", "1") != "0"   # parity mode: stride-16 local correlation gathered from an all-pairs tensor-core table
         self.side_ctas = int(os.environ.get("ROMAB200_SIDE_CTAS", "0"))   # persistent-grid cap of the side stream's GEMMs (0: none)
         self.kde_symmetric = os.environ.get("ROMAB200_KDE_SYM", "1") != "0"   # sample(): KDE over the upper triangle of the pair matrix
@@ -368,7 +368,7 @@ class Engine:
         tc_kernel = False                 # (the K' = 3K operand trick of round 1 is superseded by the split back-end)
         xs = None
         if gp_split:
-            # all-pairs CosKernel on tcgen05 with fp32-class accuracy: the L2-normalised rows as an RB_F16S pair
+            # all-pairs CosKernel on the tensor cores with fp32-class accuracy: the L2-normalised rows as an RB_F16S pair
             with self.stage("  gp.split"):
                 xs = self.split_pair(p16, E * n, cf, cf, name="gp.xs", row_norm=norms)
         elif tc_kernel:
@@ -382,7 +382,7 @@ class Engine:
         self._corr16 = None
         if self.split and self.lc_table16:
             # the stride-16 refiner's local correlation (r = 7: 256 dot products of 512 channels per pixel) from ONE all-pairs
-            # contraction per direction on tcgen05: table[i, p, q] = <x_i[p], y_i[q]> / sqrt(512), gathered by the prologue
+            # contraction per direction on the tensor cores: table[i, p, q] = <x_i[p], y_i[q]> / sqrt(512), gathered by the prologue
             with self.stage("  gp.corr16"):
                 ps = self.split_pair(p16, E * n, cf, cf, name="gp.p16s")
                 tab = self.buf("ref.corr16", (D, n, ldw), dtype=torch.float32)
@@ -480,13 +480,13 @@ class Engine:
                   eps=arch.GP_COS_EPS, inv_t=1.0 / arch.GP_TEMPERATURE, diag_add=diag, cos_normalized=0)
 
     def gp_kernel_matrix_split(self, A: Split, B: Split, na, nb, C, n, cf, ldc, batch, sa, sb, sc, sna, snb, diag):
-        """Same contraction on tcgen05 from RB_F16S pairs of the L2-normalised rows (cos_normalized=1); C fp32 or a pair."""
+        """Same contraction on the tensor cores from RB_F16S pairs of the L2-normalised rows (cos_normalized=1); C fp32 or a pair."""
         self.gemm(A, B, C, n, n, cf, cf, cf, ldc, dtype_c=cabi.RB_F32, batch0=batch,
                   sa0=sa, sb0=sb, sc0=sc, epi=cabi.EPI_COSKERNEL, norm_a=na, norm_b=nb, sna0=sna, snb0=snb,
                   eps=arch.GP_COS_EPS, inv_t=1.0 / arch.GP_TEMPERATURE, diag_add=diag, cos_normalized=1)
 
     def gp_kernel_matrix_tc(self, A, B, na, nb, C, n, cf, ldc, batch, sa, sb, sc, sna, snb, diag):
-        """Same contraction on tcgen05 from the split fp16 operands (pre-normalised rows: cos_normalized=1)."""
+        """Same contraction on the tensor cores from the split fp16 operands (pre-normalised rows: cos_normalized=1)."""
         self.gemm(A, B, C, n, n, 3 * cf, 3 * cf, 3 * cf, ldc, dtype_ab=cabi.RB_F16, dtype_c=cabi.RB_F32, batch0=batch,
                   sa0=sa, sb0=sb, sc0=sc, epi=cabi.EPI_COSKERNEL, norm_a=na, norm_b=nb, sna0=sna, snb0=snb,
                   eps=arch.GP_COS_EPS, inv_t=1.0 / arch.GP_TEMPERATURE, diag_add=diag, cos_normalized=1)
@@ -524,7 +524,7 @@ class Engine:
                      ldw=cp, dw_bias=blk["dw_b"], pw_weight_host=blk["pw_w_host"].data_ptr(), pw_bias_host=blk["pw_b_host"].data_ptr(), batch=D, h=h, w=w, c=c, dtype=self.dt)
                 d, t = t, d
         elif c == 144 and self.dtype != torch.float32 and self.fused_c144:
-            # stride-2 maps: depthwise stage on the CUDA cores feeding a tcgen05 pointwise GEMM inside one kernel
+            # stride-2 maps: depthwise stage on the CUDA cores feeding a wgmma pointwise GEMM inside one kernel
             for blk in R["blocks"]:
                 call("romab200_refiner_block_c144", "rb_refiner_block_c144_args", **{"in": d}, out=t, ld=cp, dw_weight=blk["dw_w"], ldw=cp,
                      dw_bias=blk["dw_b"], pw_weight=blk["pw_w"], ld_pw=cp, pw_bias=blk["pw_b"], batch=D, h=h, w=w, c=c, dtype=self.dt)

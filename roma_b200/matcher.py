@@ -1,4 +1,4 @@
-"""`RegressionMatcher`: the reference's public matcher API on top of the B200 engine.
+"""`RegressionMatcher`: the reference's public matcher API on top of the H100 engine.
 
 Mirrors `romatch.models.matcher.RegressionMatcher` (`romatch/models/matcher.py:550-986`): same
 constructor-level attributes (mutable, as the reference's README documents), same method names,

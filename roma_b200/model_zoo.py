@@ -29,7 +29,8 @@ weight_urls = {
 }
 
 _PRECISION = {torch.float16: "fp16", torch.bfloat16: "bf16", torch.float32: "fp32"}
-# GEMM back-end of the amp_dtype=float32 parity mode: "tcgen05" (default) = split-fp16 operand pairs on the tensor cores
+# GEMM back-end of the amp_dtype=float32 parity mode: "tcgen05" (default; the name of the tensor-core back-end, wgmma on
+# sm_90a) = split-fp16 operand pairs on the tensor cores
 # (fp32-class results); "simt" = CUDA-core FFMA GEMMs, kept as the slow cross-check.  Also settable with the environment
 # variable ROMA_B200_FP32_BACKEND (the factories keep the reference's signatures, so this is not a keyword argument).
 fp32_backend = None

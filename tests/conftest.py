@@ -15,7 +15,7 @@ def pytest_configure(config):
         torch.backends.cuda.matmul.allow_tf32 = False
     except Exception:
         pass
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device, an H100 (run with -m gpu)")
     config.addinivalue_line("markers", "slow: takes more than ~30 s on 8 CPU cores")
 
 

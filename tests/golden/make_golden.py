@@ -1,14 +1,15 @@
 """Generate the golden fixtures in this directory FROM THE UNMODIFIED REFERENCE.
 
-Run in the build container only (the GPU box has no /root/reference):
+Run where the reference is importable (it is not needed by any test):
 
-    PYTHONPATH=/root/reference PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
+    PYTHONPATH=<reference tree> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden.py
 
 The reference (`romatch.roma_outdoor`, model_zoo/__init__.py:31-61) is built on CPU (fp32,
 `use_custom_corr=False` because the fused-local-corr wheel is absent) with the seeded synthetic weights of
 `roma_b200.synthetic`, which load with strict=True, and run on seeded N(0,1) tensors / seeded PIL images.
-Stage tensors are captured with forward hooks on the reference's own modules.  Large tensors are stored
-sub-sampled (`[::step]`) together with float64 checksums of the full tensor.
+Stage tensors are captured with forward hooks on the reference's own modules and stored in `<name>_stages.npz`,
+sub-sampled as `x[:, ::cs, ::ss, ::ss]` with `<key>__step = [cs, ss]` beside each tensor.  Large outputs are stored
+sub-sampled (`[::step]`) together with float64 checksums of the full tensor, so that no fixture exceeds 1 MB.
 """
 import os
 import sys
@@ -21,6 +22,11 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
 
 from roma_b200 import synthetic  # noqa: E402
 from romatch import roma_indoor, roma_outdoor  # noqa: E402  (the reference)
+
+
+# channel / pixel steps of the stored stage tensors
+STAGE_STEPS = {"proj16": (8, 1), "gp_mu": (8, 1), "cls_and_cert": (16, 1), "delta16": (1, 1), "proj8": (8, 1), "delta8": (1, 1),
+               "proj4": (16, 1), "delta4": (1, 1), "proj2": (16, 1), "delta2": (1, 1), "proj1": (1, 2), "delta1": (1, 2)}
 
 
 def checksum(t):
@@ -70,6 +76,13 @@ def run(name, coarse, up, symmetric=True, upsample_preds=True, batch=1, seed=1, 
         torch.manual_seed(123)
         m, c = model.sample(warp[0], cert[0], num=500)
         out["sample_matches"], out["sample_certainty"] = m.numpy(), c.numpy()
+    stages = {}
+    for key, (cs, ss) in STAGE_STEPS.items():
+        if key in out:
+            stages[key] = np.ascontiguousarray(out.pop(key)[:, ::cs, ::ss, ::ss])
+            stages[key + "__step"] = np.array([cs, ss])
+    if stages:
+        np.savez(os.path.join(HERE, f"{name}_stages.npz"), **stages)
     np.savez_compressed(os.path.join(HERE, f"{name}.npz"), **out)
     print(name, {k: v.shape for k, v in out.items()})
 
@@ -83,7 +96,7 @@ if __name__ == "__main__":
     run("small_sym_up", 112, 168)
     run("small_nosym_up", 112, 168, symmetric=False, hooks=False)
     run("small_sym_noup", 112, None, upsample_preds=False, hooks=False)
-    run("small_b2_sym_up", 112, 168, batch=2, seed=7, hooks=False)
+    run("small_b2_sym_up", 112, 168, batch=2, seed=7, step=2, hooks=False)
     run("small_pil_sym_up", 112, 168, pil=True, hooks=False, seed=3)
     run("rect_sym_up", (112, 168), (168, 224), hooks=False, seed=5)
     run("full_sym_up", 560, 864, step=8, hooks=False)

@@ -1,8 +1,8 @@
 """Golden vectors for the pure-Python API helpers of the path (SURVEY §8 a14), FROM THE UNMODIFIED REFERENCE.
 
-Run in the build container only:
+Run where the reference is importable (it is not needed by any test):
 
-    PYTHONPATH=/root/reference PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_helpers.py
+    PYTHONPATH=<reference tree> PYTHONDONTWRITEBYTECODE=1 python tests/golden/make_golden_helpers.py
 
 `RegressionMatcher.to_pixel_coordinates / to_normalized_coordinates / match_keypoints / conf_from_fb_consistency`
 (romatch/models/matcher.py:672-773) use nothing of the model but `self`, so they are called unbound on a bare

@@ -1,4 +1,4 @@
-"""tcgen05 / TMA back-end of romab200_gemm against torch matmul on the same 16-bit-rounded operands."""
+"""Tensor-core (wgmma) / TMA back-end of romab200_gemm against torch matmul on the same 16-bit-rounded operands."""
 import math
 
 import pytest
@@ -171,7 +171,7 @@ def test_flash_attn(dt, H, d, N, Bn):
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("B,H,W", [(2, 37, 50), (1, 8, 16), (2, 84, 84)])
 def test_refiner_block_c144_fused(dt, B, H, W):
-    """Fused stride-2 block (DW5x5+ReLU on CUDA cores -> tcgen05 PW 144x144) against conv2d on the same rounded tensors."""
+    """Fused stride-2 block (DW5x5+ReLU on CUDA cores -> wgmma PW 144x144) against conv2d on the same rounded tensors."""
     C = 144
     x = rnd(B, C, H, W, seed=1, dtype=dt)
     dw, db = rnd(C, 1, 5, 5, seed=2, scale=0.3, dtype=torch.float32), rnd(C, seed=3, dtype=torch.float32)

@@ -647,7 +647,7 @@ def test_cls_to_flow_refine_16bit(dt):
 # ----------------------------------------------------------------------------------------------- device-side sampling
 def test_weighted_sample_kernel_is_a_draw_without_replacement():
     """romab200_weighted_sample: k distinct indices, never an item of zero weight while positive ones remain, inclusion frequencies
-    proportional to the weights (for k << n), the three weight transforms, batching, determinism under the seed."""
+    proportional to the weights (for k << n), the three weight transforms, batching, determinism under the seed (ties included)."""
     n, k, B = 20000, 500, 3
     g = torch.Generator().manual_seed(0)
     vals = torch.rand(B, n, generator=g)
@@ -689,3 +689,7 @@ def test_weighted_sample_kernel_is_a_draw_without_replacement():
     assert sorted(all_idx[0].tolist()) == [0, 1, 2, 3, 4]
     three, _ = draw(6, values=small, kk=3)
     assert sorted(three[0].tolist()) == [1, 2, 4]
+    # ties at the cut (here the +inf keys of the zero weights) are drawn by index, so a draw depends on the seed only
+    for s in range(20):
+        assert sorted(draw(7 + s, values=small, kk=4)[0][0].tolist()) == [0, 1, 2, 4]
+    assert all(torch.equal(draw(3, cabi.SAMPLE_THRESHOLD, 0.05)[0].sort(-1).values, idx_t.sort(-1).values) for _ in range(5))
