@@ -352,6 +352,64 @@ typedef struct {
 } rb_transpose_args;
 int romab200_transpose(const rb_transpose_args* args, void* stream);
 
+/* ---- TinyRoMa (romatch/models/tiny.py), fp32 throughout like the reference ------------------------ */
+/* Direct convolution on channels-last fp32 maps, CUDA-core FFMA (the XFeat backbone convs, tiny.py:87-97, and the
+ * BasicLayer / 1x1 heads of the coarse and fine matchers, tiny.py:47-61,208-215):
+ *   out[b,y,x,n] = epi( sum_{ky,kx,c} in[b, y*stride+ky-k/2, x*stride+kx-k/2, c] * weight[(ky*k+kx)*cin + c][n] ),
+ * zero padding k/2, epi(v) = ((v + bias[n]) -> ReLU if relu) * col_scale[n] + R[b,y,x,n]  (bias / col_scale / R optional: NULL).
+ * weight [k*k*cin][ldw] fp32 (BN folded), ldw a multiple of 4 >= cout with zero columns beyond cout; k in {1,3}, stride in {1,2}.
+ * in [B,hi,wi,ldi], out / R [B,ho,wo,ldo / ldr]; ho = (hi - 1) / stride + 1, wo = (wi - 1) / stride + 1 (nn.Conv2d with padding k/2). */
+typedef struct {
+    const float* in; float* out; const float* weight; const float* bias; const float* col_scale; const float* R;
+    int64_t ldi, ldo, ldw, ldr;
+    int32_t batch, hi, wi, ho, wo, cin, cout, ksize, stride, relu;
+} rb_tiny_conv_args;
+int romab200_tiny_conv(const rb_tiny_conv_args* args, void* stream);
+
+/* Channel mean of an NCHW fp32 image batch (x.mean(dim=1), tiny.py:85) followed, when instance_norm != 0, by the
+ * per-image InstanceNorm2d(1) without affine or running statistics (biased variance, eps; tiny.py:86):
+ * in [B,C,H,W] -> out [B,H,W] (a 1-channel channels-last map). */
+typedef struct { const float* in; float* out; int32_t batch, channels, h, w, instance_norm; float eps; } rb_tiny_gray_args;
+int romab200_tiny_gray(const rb_tiny_gray_args* args, void* stream);
+
+/* AvgPool2d(4, 4) on a channels-last fp32 map (XFeat skip1, tiny.py:89): [B,hi,wi,c] -> [B,hi/4,wi/4,c], pitch = c */
+typedef struct { const float* in; float* out; int32_t batch, hi, wi, c; } rb_tiny_avgpool_args;
+int romab200_tiny_avgpool4(const rb_tiny_avgpool_args* args, void* stream);
+
+/* out[i] = (a[i] + b[i]) + c[i] over n floats: x3 + x4 + x5 in front of block_fusion (tiny.py:95-97) */
+typedef struct { const float* a; const float* b; const float* c; float* out; int64_t n; } rb_tiny_add3_args;
+int romab200_tiny_add3(const rb_tiny_add3_args* args, void* stream);
+
+/* Fused coarse-match embedding: correlation + first-index argmax + low-resolution softmax + expectation
+ * (corr_volume + pos_embed, tiny.py:115-140,178-191), without materialising the [h1*w1, h0*w0] volume.
+ * For pixel i of image 0: s_j = <f1[b,j,:], f0[b,i,:]> / scale for every pixel j of image 1, best = first argmax_j s_j;
+ *   exact == 0: P = softmax over {s_j : j on the stride-4 lattice (y % 4 == 0, x % 4 == 0)} U {(float)best}  (the extra logit is the
+ *               argmax INDEX, as the reference computes it), pos = sum_k P_k grid_lr[k] + P_last * grid[best];
+ *   exact != 0: pos = sum_j softmax(s)_j grid[j].
+ * f0 [B, h0*w0, c], f1 [B, h1*w1, c] fp32 contiguous, c == 64; state [B, h0*w0, 3] receives (pos_x, pos_y, 0).
+ * grid_x / grid_y: linspace(-1+1/w1, 1-1/w1, w1), linspace(-1+1/h1, 1-1/h1, h1); grid_lr_x / grid_lr_y: linspace(-1+4/w1, 1-4/w1, w1/4),
+ * linspace(-1+4/h1, 1-4/h1, h1/4) (not the centres of the sub-sampled pixels; reproduced as the reference has them).  h1 % 4 == w1 % 4 == 0. */
+typedef struct {
+    const float* f0; const float* f1; float* state;
+    int32_t batch, h0, w0, h1, w1, c; float scale; int32_t exact;
+    const float* grid_x; const float* grid_y; const float* grid_lr_x; const float* grid_lr_y;
+} rb_tiny_pos_embed_args;
+int romab200_tiny_pos_embed(const rb_tiny_pos_embed_args* args, void* stream);
+
+/* Warp-and-concat prologue of the matcher heads (tiny.py:205-214): out[b,p,:] = [f0[b,p,0:c] | grid_sample(f1[b], flow) | flow],
+ * flow = state[b,p,0:2]; bilinear, zero padding, align_corners=False.  f0 [B,h0,w0,ldf0], f1 [B,h1,w1,ldf1], state [B,h0,w0,lds],
+ * out [B,h0,w0,ldo] (columns 2c+2 .. ldo-1 untouched). */
+typedef struct {
+    const float* f0; const float* f1; const float* state; float* out;
+    int64_t ldf0, ldf1, lds, ldo; int32_t batch, h0, w0, h1, w1, c;
+} rb_tiny_warp_concat_args;
+int romab200_tiny_warp_concat(const rb_tiny_warp_concat_args* args, void* stream);
+
+/* match() epilogue of TinyRoMa (tiny.py:216-232): state [B,H,W,3] (already resized to the input size) ->
+ * warp [B,H,W,4] = (grid_x[x], grid_y[y], state.x, state.y), cert [B,H,W] = sigmoid(state.z).  No clamp, no mask. */
+typedef struct { const float* state; float* warp; float* cert; int32_t batch, h, w; const float* grid_x; const float* grid_y; } rb_tiny_epilogue_args;
+int romab200_tiny_match_epilogue(const rb_tiny_epilogue_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -135,6 +135,13 @@ _FIELD_DTYPES = {
     "rb_preprocess_args": {"in": torch.uint8, "tmp": torch.uint8, "out_u8": torch.uint8, "out": _F32, "bounds_x": torch.int32, "kk_x": torch.int32,
                            "bounds_y": torch.int32, "kk_y": torch.int32},
     "rb_sample_args": {"values": _F32, "out_idx": torch.int32, "out_weights": _F32, "keys": _F32, "scratch": torch.int32, "seed_dev": torch.int64},
+    "rb_tiny_conv_args": {"in": _F32, "out": _F32, "weight": _F32, "bias": _F32, "col_scale": _F32, "R": _F32},
+    "rb_tiny_gray_args": {"in": _F32, "out": _F32},
+    "rb_tiny_avgpool_args": {"in": _F32, "out": _F32},
+    "rb_tiny_add3_args": {"a": _F32, "b": _F32, "c": _F32, "out": _F32},
+    "rb_tiny_pos_embed_args": {"f0": _F32, "f1": _F32, "state": _F32, "grid_x": _F32, "grid_y": _F32, "grid_lr_x": _F32, "grid_lr_y": _F32},
+    "rb_tiny_warp_concat_args": {"f0": _F32, "f1": _F32, "state": _F32, "out": _F32},
+    "rb_tiny_epilogue_args": {"state": _F32, "warp": _F32, "cert": _F32, "grid_x": _F32, "grid_y": _F32},
 }
 
 

@@ -31,7 +31,7 @@ from typing import Dict, Optional, Tuple
 import torch
 import torch.nn.functional as F
 
-from . import arch, cabi
+from . import arch, cabi, sampling
 from .cabi import call
 from .packing import PackedWeights, Split, pad8
 
@@ -667,13 +667,4 @@ class Engine:
         return warp, cert
 
     def kde(self, x: torch.Tensor, std: float = 0.1, half: bool = True):
-        x = x.contiguous().float()
-        n = x.shape[0]
-        out = torch.empty(n, dtype=torch.float32, device=x.device)
-        splits = 16 if n >= 8192 else 1
-        sym = bool(half) and splits > 1 and self.kde_symmetric      # every pair once: (splits + blocks of 256) * n floats of workspace
-        nws = (splits + (n + 255) // 256) * n if sym else splits * n
-        ws = torch.empty(nws, dtype=torch.float32, device=x.device) if splits > 1 else None
-        call("romab200_kde_density", "rb_kde_args", x=x, density=out, n=n, std=std, half=int(half), workspace=ws, splits=splits,
-             symmetric=int(sym), workspace_floats=nws if ws is not None else 0)
-        return out
+        return sampling.kde(x, std, half, self.kde_symmetric)

@@ -20,6 +20,7 @@ from PIL import Image
 from . import cabi
 from .engine import Engine
 from .preprocess import DevicePreprocessor, check_input
+from .sampling import sample_device
 
 
 class RegressionMatcher:
@@ -238,56 +239,8 @@ class RegressionMatcher:
         return good_matches[balanced_samples], good_certainty[balanced_samples]
 
     def _sample_device(self, matches, certainty, num):
-        """Device sampler; from the second call with the same sizes on, the whole chain (two draws, sort, gathers, KDE) is one
-        CUDA-graph replay fed through static buffers, with the two seeds of a call written to a device word."""
-        balanced = "balanced" in self.sample_mode
-        thresholded = "threshold" in self.sample_mode
-        dev = matches.device
-        with torch.cuda.device(dev):
-            n = certainty.numel()
-            key = (n, num, self.sample_mode, float(self.sample_thresh), dev.index)
-            st = self._sample_state.get(key)
-            if st is None:
-                k1 = min((4 if balanced else 1) * num, n)
-                st = dict(m=torch.empty(n, 4, device=dev), c=torch.empty(n, device=dev), seeds=torch.zeros(2, dtype=torch.int64, device=dev),
-                          seeds_host=torch.zeros(2, dtype=torch.int64).pin_memory(), idx1=torch.empty(k1, dtype=torch.int32, device=dev),
-                          idx2=torch.empty(min(num, k1), dtype=torch.int32, device=dev), keys=torch.empty(n, device=dev),
-                          scratch=torch.empty(2056, dtype=torch.int32, device=dev), k1=k1, graph=None, calls=0, out=None)
-                self._sample_state[key] = st
-            st["m"].copy_(matches.reshape(-1, 4), non_blocking=True)
-            st["c"].copy_(certainty.reshape(-1), non_blocking=True)
-            st["seeds_host"].copy_(torch.randint(0, 2 ** 62, (2,), dtype=torch.int64))       # CPU generator: follows torch.manual_seed
-            st["seeds"].copy_(st["seeds_host"], non_blocking=True)
-
-            def chain():
-                m, c, k1 = st["m"], st["c"], st["k1"]
-                cabi.call("romab200_weighted_sample", "rb_sample_args", values=c, n=n, k=k1, batch=1, stride=n, seed=0, seed_dev=st["seeds"],
-                          transform=cabi.SAMPLE_THRESHOLD if thresholded else cabi.SAMPLE_IDENTITY, param=float(self.sample_thresh),
-                          out_idx=st["idx1"], out_weights=None, keys=st["keys"], scratch=st["scratch"])
-                sel1 = st["idx1"].long().sort().values           # the compaction order is not deterministic; the drawn SET is
-                good_matches = m[sel1]
-                w1 = torch.where(c[sel1] > self.sample_thresh, torch.ones((), device=dev), c[sel1]) if thresholded else c[sel1]
-                if not balanced:
-                    return good_matches, w1
-                density = self.engine.kde(good_matches, std=0.1, half=True).to(torch.float16).float().contiguous()     # kde.py: x.half()
-                cabi.call("romab200_weighted_sample", "rb_sample_args", values=density, n=k1, k=st["idx2"].numel(), batch=1, stride=k1, seed=0,
-                          seed_dev=st["seeds"][1:], transform=cabi.SAMPLE_BALANCE, param=0.0, out_idx=st["idx2"], out_weights=None, keys=st["keys"],
-                          scratch=st["scratch"])
-                sel = st["idx2"].long().sort().values
-                return good_matches[sel], w1[sel]
-
-            st["calls"] += 1
-            if st["graph"] is not None:
-                st["graph"].replay()
-                return st["out"][0].clone(), st["out"][1].clone()
-            out = chain()
-            if self.use_cuda_graph and st["calls"] >= 2:
-                torch.cuda.synchronize(dev)
-                graph = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(graph):
-                    st["out"] = chain()
-                st["graph"] = graph
-            return out
+        return sample_device(self._sample_state, self.engine.kde, matches, certainty, num, self.sample_mode, self.sample_thresh,
+                             self.use_cuda_graph)
 
     # ---- small geometry helpers (matcher.py:672-773) ---------------------------------------------------
     def _to_pixel_coordinates(self, coords, H, W):

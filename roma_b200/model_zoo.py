@@ -89,7 +89,14 @@ def roma_indoor(device, weights=None, dinov2_weights=None, coarse_res: Union[int
 
 
 def tiny_roma_v1_outdoor(device, weights=None, xfeat=None):
-    """TinyRoMa needs the XFeat backbone, which the reference pulls from an un-vendored, unpinned torch.hub
-    repository (`model_zoo/__init__.py:23-26`); it is a "next" row of the scope table (SURVEY §8f), not built."""
-    raise NotImplementedError("tiny_roma_v1_outdoor is outside the match() hot path built here (XFeat backbone "
-                              "source is not part of the reference tree); see DESIGN.md")
+    """TinyRoMa (`model_zoo/__init__.py:18-28`, `roma_models.py:21-29`).  Like the reference, `weights=None` downloads the
+    checkpoint and `xfeat=None` loads XFeat through torch.hub ("verlab/accelerated_features"); the engine reads the backbone's
+    layer structure from that module and its weights from the checkpoint's `xfeat.0.*` entries."""
+    if torch.device(device).type != "cuda":
+        raise RuntimeError(f"roma_b200 runs on a CUDA device only (there is no CPU fallback); got device={device!r}")
+    if weights is None:
+        weights = torch.hub.load_state_dict_from_url(weight_urls["tiny_roma_v1"]["outdoor"], map_location="cpu")
+    if xfeat is None:
+        xfeat = torch.hub.load("verlab/accelerated_features", "XFeat", pretrained=True, top_k=4096).net
+    from .tiny import TinyRoMa
+    return TinyRoMa(xfeat, weights, device)

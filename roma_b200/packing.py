@@ -25,11 +25,14 @@ def pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
-def fold_bn(w: torch.Tensor, b: torch.Tensor, sd: Dict[str, torch.Tensor], bn: str):
-    """Fold eval-mode BatchNorm `bn` into the conv (w [cout, ...], b [cout])."""
-    scale = sd[f"{bn}.weight"].double() / torch.sqrt(sd[f"{bn}.running_var"].double() + arch.BN_EPS)
+def fold_bn(w: torch.Tensor, b: torch.Tensor, sd: Dict[str, torch.Tensor], bn: str, eps: float = arch.BN_EPS):
+    """Fold eval-mode BatchNorm `bn` into the conv (w [cout, ...], b [cout]).  A BatchNorm2d(affine=False) has no
+    `weight` / `bias` entries: gamma = 1, beta = 0."""
+    gamma = sd[f"{bn}.weight"].double() if f"{bn}.weight" in sd else 1.0
+    beta = sd[f"{bn}.bias"].double() if f"{bn}.bias" in sd else 0.0
+    scale = gamma / torch.sqrt(sd[f"{bn}.running_var"].double() + eps)
     w2 = w.double() * scale.view(-1, *([1] * (w.dim() - 1)))
-    b2 = (b.double() - sd[f"{bn}.running_mean"].double()) * scale + sd[f"{bn}.bias"].double()
+    b2 = (b.double() - sd[f"{bn}.running_mean"].double()) * scale + beta
     return w2.float(), b2.float()
 
 

@@ -88,16 +88,21 @@ def wire_bytes(n_pairs: int, world: int, in_bytes_per_pair: int, out_bytes_per_p
 
 
 def match_sharded(model, im_A, im_B, im_A_high_res=None, im_B_high_res=None, n_pairs: Optional[int] = None, src: int = 0,
-                  group=None, max_batch: Optional[int] = None, on_batch=None):
+                  group=None, max_batch: Optional[int] = None, on_batch=None, pair_shapes=None):
     """`model.match` over a pair batch sharded across the process group.  Rank `src` passes the full tensors (other ranks
-    pass None and `n_pairs` + shapes via the model's configured resolutions); returns (warp, certainty) on `src`, None
-    elsewhere.  `on_batch(warp, certainty)` is called on every rank after each local sub-batch (e.g. to run `sample`)."""
+    pass None and `n_pairs`); returns (warp, certainty) on `src`, None elsewhere.  The per-pair input shapes the other ranks
+    allocate for are the model's configured resolutions, or `pair_shapes` = ((C, H, W) of im_A, (C, H, W) of im_B) when given —
+    needed for models without a configured resolution (TinyRoMa matches at the input size).  `on_batch(warp, certainty)` is
+    called on every rank after each local sub-batch (e.g. to run `sample`)."""
     rank = dist.get_rank(group)
-    device = model._get_device()
-    h, w = model.h_resized, model.w_resized
-    tails = [(3, h, w), (3, h, w)]
+    device = model._get_device() if hasattr(model, "_get_device") else model.device
+    if pair_shapes is not None:
+        tails = [tuple(pair_shapes[0]), tuple(pair_shapes[1])]
+    else:
+        h, w = model.h_resized, model.w_resized
+        tails = [(3, h, w), (3, h, w)]
     tensors = [im_A, im_B]
-    if model.upsample_preds:
+    if getattr(model, "upsample_preds", False):
         hu, wu = model.upsample_res
         tails += [(3, hu, wu), (3, hu, wu)]
         tensors += [im_A_high_res, im_B_high_res]
@@ -110,12 +115,15 @@ def match_sharded(model, im_A, im_B, im_A_high_res=None, im_B_high_res=None, n_p
         mb = max_batch or shards[0].shape[0]
         outs = []
         for a in range(0, shards[0].shape[0], mb):
-            kw = dict(im_A_high_res=shards[2][a:a + mb], im_B_high_res=shards[3][a:a + mb]) if model.upsample_preds else {}
+            kw = dict(im_A_high_res=shards[2][a:a + mb], im_B_high_res=shards[3][a:a + mb]) if len(shards) == 4 else {}
             outs.append(model.match(shards[0][a:a + mb], shards[1][a:a + mb], **kw))
             if on_batch is not None:
                 on_batch(*outs[-1])
         warp = outs[0][0] if len(outs) == 1 else torch.cat([o[0] for o in outs])
         cert = outs[0][1] if len(outs) == 1 else torch.cat([o[1] for o in outs])
+    elif not hasattr(model, "get_output_resolution"):        # TinyRoMa: one warp per pixel of im_A
+        warp = torch.empty((0,) + tuple(tails[0][1:]) + (4,), device=device)
+        cert = torch.empty((0,) + tuple(tails[0][1:]), device=device)
     else:
         ho, wo = model.get_output_resolution()
         wout = 2 * wo if model.symmetric else wo

@@ -118,3 +118,74 @@ def make_pil_pair(seed: int = 3, size_a=(200, 150), size_b=(180, 220)):
         arr = (img[0].clamp(0, 1) * 255).round().to(torch.uint8).permute(1, 2, 0).numpy()
         out.append(Image.fromarray(np.ascontiguousarray(arr), "RGB"))
     return out[0], out[1]
+
+
+# ---- TinyRoMa ----------------------------------------------------------------------------------------
+class _ConvBN(torch.nn.Module):
+    """Conv2d (no bias) -> BatchNorm2d(affine=False) -> ReLU, wrapped as `self.layer` (XFeat's basic layer as publicly described)."""
+
+    def __init__(self, cin, cout, k=3, stride=1, relu=True):
+        super().__init__()
+        nn = torch.nn
+        self.layer = nn.Sequential(nn.Conv2d(cin, cout, k, stride=stride, padding=k // 2, bias=False), nn.BatchNorm2d(cout, affine=False),
+                                   nn.ReLU(inplace=True) if relu else nn.Identity())
+
+    def forward(self, x):
+        return self.layer(x)
+
+
+class XFeatStandIn(torch.nn.Module):
+    """A module with the XFeat backbone layout as publicly described (SURVEY §8f): InstanceNorm -> block1 (x4, two stride-2
+    layers) + skip1 (AvgPool 4 + 1x1) -> block2 -> block3 (s2) -> block4 (s2) -> block5 (s2) -> fusion of x3 + up(x4) + up(x5).
+    It is NOT verified against the real XFeat network (that source is not available offline); TinyRoMa reads the structure of
+    whatever module it is given, so nothing depends on this one.  `heatmap_head` / `keypoint_head` / `fine_matcher` are dummies
+    that TinyRoMa's constructor deletes."""
+
+    def __init__(self, widths=(4, 8, 24, 64, 128), fusion_extra=True):
+        super().__init__()
+        nn = torch.nn
+        w1, w2, w3, w4, w5 = widths
+        self.norm = nn.InstanceNorm2d(1)
+        self.skip1 = nn.Sequential(nn.AvgPool2d(4, stride=4), nn.Conv2d(1, w3, 1, stride=1, padding=0))
+        self.block1 = nn.Sequential(_ConvBN(1, w1), _ConvBN(w1, w2, stride=2), _ConvBN(w2, w2), _ConvBN(w2, w3, stride=2))
+        self.block2 = nn.Sequential(_ConvBN(w3, w3), _ConvBN(w3, w3))
+        self.block3 = nn.Sequential(_ConvBN(w3, w4, stride=2), _ConvBN(w4, w4), _ConvBN(w4, w4, k=1))
+        self.block4 = nn.Sequential(_ConvBN(w4, w4, stride=2), _ConvBN(w4, w4), _ConvBN(w4, w4))
+        self.block5 = nn.Sequential(_ConvBN(w4, w5, stride=2), _ConvBN(w5, w5), _ConvBN(w5, w5), _ConvBN(w5, w4, k=1))
+        fusion = [_ConvBN(w4, w4), _ConvBN(w4, w4)] if fusion_extra else [_ConvBN(w4, w4)]
+        self.block_fusion = nn.Sequential(*fusion, nn.Conv2d(w4, w4, 1, padding=0))
+        self.heatmap_head = nn.Conv2d(w4, 1, 1)
+        self.keypoint_head = nn.Conv2d(w4, 65, 1)
+        self.fine_matcher = nn.Linear(2 * w4, 64)
+
+
+def xfeat_standin(**kw) -> torch.nn.Module:
+    """The stand-in XFeat backbone used by the tests, goldens and benchmark (see XFeatStandIn), in eval mode."""
+    return XFeatStandIn(**kw).eval()
+
+
+def make_tiny_weights(seed: int, xfeat: torch.nn.Module) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded TinyRoMa checkpoint in the reference key layout for this `xfeat` (`xfeat.0.*`, `coarse_matcher.*`, `fine_matcher.*`):
+    the keys and shapes `tiny_roma_v1_model(weights, xfeat=xfeat)` loads strictly.  BN statistics are randomised so that folding is
+    exercised; the last 1x1 convs of the heads are kept small so that the flow updates stay moderate."""
+    from .tiny import expected_state_dict_shapes
+    g = torch.Generator(device="cpu")
+    g.manual_seed(4099 * (seed + 1) + 11)
+    sd = OrderedDict()
+    for k, shape in expected_state_dict_shapes(xfeat).items():
+        leaf = k.rsplit(".", 1)[1]
+        if leaf == "num_batches_tracked":
+            sd[k] = torch.zeros((), dtype=torch.int64)
+        elif leaf == "running_var":
+            sd[k] = _fill("bn_var", shape, g)
+        elif leaf == "running_mean":
+            sd[k] = _fill("bn_mean", shape, g)
+        elif leaf == "bias":
+            sd[k] = _fill("bias", shape, g)
+        elif len(shape) == 4 and shape[0] == 3 and ("coarse_matcher" in k or "fine_matcher" in k):
+            sd[k] = _fill("out_conv", shape, g)
+        elif len(shape) == 4:
+            sd[k] = _fill("conv_relu", shape, g)
+        else:
+            sd[k] = _fill("bn_w", shape, g)
+    return sd
