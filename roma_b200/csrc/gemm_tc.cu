@@ -2,11 +2,12 @@
 //
 // Persistent kernel; one CTA computes one 128 x BN output tile at a time (BN in {32, 64, 128, 144, 192, 256}).  Warp roles:
 //   warps 0-7   two consumer warpgroups, 64 rows of the tile each: wgmma.mma_async (m64 x BN x k16, 4 per k-block) from the
-//               STAGES-deep 128B-swizzled shared-memory ring into fp32 register accumulators, then the fused epilogue
-//               straight from the accumulator fragments;
+//               STAGES-deep 128B-swizzled shared-memory ring into fp32 register accumulators, then the fused epilogue: 32
+//               columns at a time, the accumulators go through the warpgroup's shared-memory staging buffer, and a rolled loop
+//               in which each thread owns 8 consecutive columns of a row applies the epilogue and stores 16-byte vectors;
 //   warps 8-11  TMA producer: one lane issues cp.async.bulk.tensor loads of the A (128 x 64) and B (BN x 64, or 64 x BN when B
 //               is [K,N]) tiles; it runs ahead into the next tile while the consumers are in their epilogue.  The producer
-//               warpgroup hands its registers to the consumers (setmaxnreg), whose accumulators take up to 128 per thread.
+//               warpgroup hands its registers to the consumers (setmaxnreg), whose accumulators take up to 144 per thread.
 // A-operand "taps" (the 9 shifted row blocks of a 3x3 convolution on a zero-padded channels-last map) are just a per-k-block row
 // offset on the TMA coordinate; out-of-range rows/columns are zero-filled by TMA, which also handles M/N/K tails, so no operand is
 // ever padded or copied.  Batched GEMMs (attention heads) use the 3rd/4th tensor-map dimension.
@@ -68,53 +69,143 @@ struct TcParams {
 
 constexpr int TC_BM = 128, TC_BK = 64;
 constexpr int TC_THREADS = 384;                    // two consumer warpgroups + one producer warpgroup
+// epilogue staging: each consumer warpgroup owns a 64 x TC_CW fp32 buffer; rows are TC_SP floats apart (40: the accumulator
+// fragments' float2 writes and the row readers' float4 reads are both free of bank conflicts)
+constexpr int TC_CW = 32, TC_SP = 40;
+constexpr int TC_STAGING = 2 * 64 * TC_SP * 4;
 
 template <int BN, bool SPLIT> struct TcCfg {
     static constexpr int NOPS = SPLIT ? 2 : 1;                           // operand planes per matrix
     static constexpr int A_BYTES = TC_BM * TC_BK * 2;
     static constexpr int B_BYTES = BN * TC_BK * 2;                       // a multiple of 1024: every plane stays swizzle-atom aligned
     static constexpr int STAGE_BYTES = NOPS * (A_BYTES + B_BYTES);
-    static constexpr int STAGES = (200 * 1024) / STAGE_BYTES > 8 ? 8 : (200 * 1024) / STAGE_BYTES;
-    static constexpr int SMEM = STAGES * STAGE_BYTES + 1024 /*align*/ + 256 /*barriers*/;
-    static_assert(STAGES >= 2 && SMEM <= 232448, "shared memory budget");
+    static constexpr int RING_MAX = 232448 - TC_STAGING - 1024 /*align*/ - 256 /*barriers*/;
+    static constexpr int STAGES = RING_MAX / STAGE_BYTES > 8 ? 8 : RING_MAX / STAGE_BYTES;
+    static constexpr int SMEM = STAGES * STAGE_BYTES + TC_STAGING + 1024 + 256;
+    static_assert(STAGES >= 3 && SMEM <= 232448, "shared memory budget");
 };
 
-// two adjacent output columns (n, n + 1) of row m: fused epilogue, then one vector store where the layout allows it; columns in
-// [N, nz) receive zeros
-__device__ __forceinline__ void tc_store_pair(const Epilogue& e, int nz, int m, int n, float v0, float v1) {
-    if (m >= e.M || n >= nz) return;
-    const int64_t orow = e.map_row(m);
-    if (orow < 0) return;
-    const int64_t i = orow * e.ldc + n;
-    v0 = n < e.N ? e.apply(v0, m, n, orow) : 0.f;
-    if (n + 1 >= nz) { store_split_any(e.C, e.C_lo, i, e.dtype_c, v0); return; }
-    v1 = n + 1 < e.N ? e.apply(v1, m, n + 1, orow) : 0.f;
-    if (e.dtype_c == RB_F32) {
-        float* c = (float*)e.C + i;
-        if ((reinterpret_cast<uintptr_t>(c) & 7) == 0) *reinterpret_cast<float2*>(c) = make_float2(v0, v1);
-        else { c[0] = v0; c[1] = v1; }
+__device__ __forceinline__ void bar_named(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
+
+// cnt (<= 8) consecutive elements of a 16-bit or fp32 matrix as floats: two 16-byte loads (fp32) or one (16-bit) when all 8 are
+// wanted and the address allows it
+__device__ __forceinline__ void load8(const void* p, int64_t i, int dtype, int cnt, float (&v)[8]) {
+    if (dtype == RB_F32) {
+        const float* s = (const float*)p + i;
+        if (cnt == 8 && (reinterpret_cast<uintptr_t>(s) & 15) == 0) {
+            const float4 a = reinterpret_cast<const float4*>(s)[0], b = reinterpret_cast<const float4*>(s)[1];
+            v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = k < cnt ? s[k] : 0.f;
+        }
         return;
     }
-    uint32_t w, wl = 0;
-    if (e.dtype_c == RB_BF16) {
-        __nv_bfloat162 h = __floats2bfloat162_rn(v0, v1); w = *reinterpret_cast<uint32_t*>(&h);
+    const uint16_t* s = (const uint16_t*)p + i;
+    uint16_t h[8];
+    if (cnt == 8 && (reinterpret_cast<uintptr_t>(s) & 15) == 0) {
+        const uint4 q = *reinterpret_cast<const uint4*>(s);
+        const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { h[2 * k] = (uint16_t)w[k]; h[2 * k + 1] = (uint16_t)(w[k] >> 16); }
     } else {
-        const __half2 h = __floats2half2_rn(v0, v1); w = *reinterpret_cast<const uint32_t*>(&h);
-        if (e.dtype_c == RB_F16S) {
-            const float2 hf = __half22float2(h);
-            const __half2 l = __floats2half2_rn((v0 - hf.x) * RB_SPLIT_SCALE, (v1 - hf.y) * RB_SPLIT_SCALE);
-            wl = *reinterpret_cast<const uint32_t*>(&l);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) h[k] = k < cnt ? s[k] : 0;
+    }
+    if (dtype == RB_F16) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = __half2float(__ushort_as_half(h[k]));
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = __bfloat162float(__ushort_as_bfloat16(h[k]));
+    }
+}
+
+// cnt (<= 8) consecutive output elements starting at element i of C (and C_lo): 16-byte stores when all 8 go out and the address
+// allows it, scalar stores otherwise.  Rounding is that of store_split_any.
+__device__ __forceinline__ void store8(const Epilogue& e, int64_t i, int cnt, const float (&v)[8]) {
+    if (e.dtype_c == RB_F32) {
+        float* c = (float*)e.C + i;
+        if (cnt == 8 && (reinterpret_cast<uintptr_t>(c) & 15) == 0) {
+            reinterpret_cast<float4*>(c)[0] = make_float4(v[0], v[1], v[2], v[3]);
+            reinterpret_cast<float4*>(c)[1] = make_float4(v[4], v[5], v[6], v[7]);
+        } else {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) if (k < cnt) c[k] = v[k];
+        }
+        return;
+    }
+    uint16_t h[8], l[8];
+    const bool two = e.dtype_c == RB_F16S;
+    if (e.dtype_c == RB_BF16) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) h[k] = __bfloat16_as_ushort(__float2bfloat16_rn(v[k]));
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            __half hi, lo;
+            split_f16s(v[k], hi, lo);
+            h[k] = __half_as_ushort(hi); l[k] = __half_as_ushort(lo);
         }
     }
     uint16_t* c = (uint16_t*)e.C + i;
-    uint16_t* cl = e.dtype_c == RB_F16S ? (uint16_t*)e.C_lo + i : nullptr;
-    if ((reinterpret_cast<uintptr_t>(c) & 3) == 0 && (!cl || (reinterpret_cast<uintptr_t>(cl) & 3) == 0)) {
-        *reinterpret_cast<uint32_t*>(c) = w;
-        if (cl) *reinterpret_cast<uint32_t*>(cl) = wl;
+    uint16_t* cl = two ? (uint16_t*)e.C_lo + i : nullptr;
+    if (cnt == 8 && (reinterpret_cast<uintptr_t>(c) & 15) == 0 && (!two || (reinterpret_cast<uintptr_t>(cl) & 15) == 0)) {
+        *reinterpret_cast<uint4*>(c) = make_uint4(h[0] | (uint32_t)h[1] << 16, h[2] | (uint32_t)h[3] << 16, h[4] | (uint32_t)h[5] << 16,
+                                                  h[6] | (uint32_t)h[7] << 16);
+        if (two) *reinterpret_cast<uint4*>(cl) = make_uint4(l[0] | (uint32_t)l[1] << 16, l[2] | (uint32_t)l[3] << 16,
+                                                            l[4] | (uint32_t)l[5] << 16, l[6] | (uint32_t)l[7] << 16);
     } else {
-        c[0] = (uint16_t)w; c[1] = (uint16_t)(w >> 16);
-        if (cl) { cl[0] = (uint16_t)wl; cl[1] = (uint16_t)(wl >> 16); }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) if (k < cnt) { c[k] = h[k]; if (two) cl[k] = l[k]; }
     }
+}
+
+// Epilogue of 8 consecutive columns n .. n + 7 of one stored row (logical row m, stored row orow): the same operations in the same
+// order as Epilogue::apply (the _rn intrinsics keep the multiplies and adds from being contracted into FMAs), with every per-launch
+// option tested once for the 8 values.  cb / cs hold bias (COSKERNEL: norm_b) and col_scale of the 8 columns, na norm_a[m].
+// Columns in [N, nz) become zeros; cnt = the number of columns below nz.
+__device__ __forceinline__ void epilogue8(const Epilogue& e, int m, int n, int64_t orow, int cnt, const float (&cb)[8],
+                                          const float (&cs)[8], float na, float (&v)[8]) {
+    const int nv = min(8, e.N - n);                  // columns holding results
+    if (e.epi == RB_EPI_COSKERNEL) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const float p = na * cb[k];
+            const float s = e.cos_normalized ? p / (p + e.eps) : 1.0f / (p + e.eps);
+            v[k] = expf((v[k] * s - 1.0f) * e.inv_t);
+            if (m == n + k) v[k] += e.diag_add;
+        }
+    } else {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) v[k] = __fmul_rn(e.alpha, v[k]);
+        if (e.bias) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = __fadd_rn(v[k], cb[k]);
+        }
+        if (e.act == RB_ACT_RELU) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = fmaxf(v[k], 0.0f);
+        } else if (e.act == RB_ACT_GELU) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = gelu_erf(v[k]);
+        }
+        if (e.col_scale) {
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = __fmul_rn(v[k], cs[k]);
+        }
+        if (e.R) {
+            float r[8];
+            load8(e.R, orow * e.ldr + n, e.dtype_r, nv, r);
+#pragma unroll
+            for (int k = 0; k < 8; ++k) v[k] = __fadd_rn(v[k], r[k]);
+        }
+    }
+    if (nv < 8) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) if (k >= nv) v[k] = 0.f;
+    }
+    store8(e, orow * e.ldc + n, cnt, v);
 }
 
 // Persistent kernel: every CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (m fastest, so CTAs that run together share
@@ -129,7 +220,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     constexpr int OFF_A_LO = A_BYTES, OFF_B = Cfg::NOPS * A_BYTES, OFF_B_LO = Cfg::NOPS * A_BYTES + B_BYTES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);   // offset on the array: keeps ld/st.shared
-    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    float* staging = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + TC_STAGING);
     uint64_t* empty_bar = full_bar + STAGES;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -228,26 +320,72 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
         if constexpr (SPLIT) wgmma_fence_regs(acc2);
         if (t == 0) mbar_arrive(&empty_bar[prev]);
 
-        // ===== epilogue from the accumulator fragments: thread t holds rows r0, r0 + 8 and column pairs 8 j + 2 (t % 4) =====
+        // ===== epilogue, TC_CW columns at a time: the warpgroup copies its accumulator fragments (thread t: rows fr, fr + 8, column
+        // pairs 8 j + 2 (t % 4)) into its staging buffer, then every thread takes 8 consecutive columns of rows rr and rr + 32 of the
+        // chunk and runs the fused epilogue on them with 16-byte stores.  Named barriers: the other warpgroup and the producer run on.
         Epilogue e = p.epi;
         e.C = (char*)e.C + (z0 * p.sc0 + z1 * p.sc1) * dtype_size(e.dtype_c);
         if (e.C_lo) e.C_lo = (char*)e.C_lo + (z0 * p.sc0 + z1 * p.sc1) * 2;
         if (e.R) e.R = (const char*)e.R + (z0 * p.sr0 + z1 * p.sr1) * dtype_size(e.dtype_r);
         if (e.norm_a) e.norm_a += z0 * p.sna0;
         if (e.norm_b) e.norm_b += z0 * p.snb0;
-        const int r0 = m0 + wg * 64 + (t >> 5) * 16 + ((t & 31) >> 2);
-        const int c0 = n0 + 2 * (t & 3);
+        float* stg = staging + wg * (64 * TC_SP);
+        const int fr = (t >> 5) * 16 + ((t & 31) >> 2), fc = 2 * (t & 3);
+        const int g = t & 3, rr = t >> 2;
+        // the two rows this thread stores: logical row, stored row (-1: not stored) and norm_a
+        int mrow[2]; int64_t orow[2]; float na[2] = {0.f, 0.f};
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-            if (c0 + 8 * j >= p.n_zero_to) break;
+        for (int h = 0; h < 2; ++h) {
+            mrow[h] = m0 + wg * 64 + rr + 32 * h;
+            orow[h] = mrow[h] < e.M ? e.map_row(mrow[h]) : -1;
+            if (orow[h] >= 0 && e.epi == RB_EPI_COSKERNEL) na[h] = e.norm_a[mrow[h]];
+        }
+        constexpr int NCH = (BN + TC_CW - 1) / TC_CW;
+#pragma unroll 1
+        for (int ch = 0; ch < NCH; ++ch) {
+            if (n0 + ch * TC_CW >= p.n_zero_to) break;
+            bar_named(1 + wg, 128);                 // the previous chunk's readers are done with the buffer
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+                if (c != ch) continue;
+#pragma unroll
+                for (int jj = 0; jj < TC_CW / 8; ++jj) {
+                    const int j = c * (TC_CW / 8) + jj;
+                    if (j >= BN / 8) break;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+                        if constexpr (SPLIT) {
+                            v0 = fmaf(acc2[4 * j + 2 * h], 1.0f / RB_SPLIT_SCALE, v0);
+                            v1 = fmaf(acc2[4 * j + 2 * h + 1], 1.0f / RB_SPLIT_SCALE, v1);
+                        }
+                        *reinterpret_cast<float2*>(stg + (fr + 8 * h) * TC_SP + 8 * jj + fc) = make_float2(v0, v1);
+                    }
+                }
+            }
+            bar_named(1 + wg, 128);
+            const int n = n0 + ch * TC_CW + 8 * g;
+            if (ch * TC_CW + 8 * g >= BN || n >= p.n_zero_to) continue;
+            const int cnt = min(8, p.n_zero_to - n);
+            float cb[8], cs[8];
+            const float* colb = e.epi == RB_EPI_COSKERNEL ? e.norm_b : e.bias;
+#pragma unroll
+            for (int k = 0; k < 8; ++k) {
+                const bool in = n + k < e.N;
+                cb[k] = colb && in ? colb[n + k] : 0.f;
+                cs[k] = e.col_scale && in ? e.col_scale[n + k] : 0.f;
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
-                if constexpr (SPLIT) {
-                    v0 = fmaf(acc2[4 * j + 2 * h], 1.0f / RB_SPLIT_SCALE, v0);
-                    v1 = fmaf(acc2[4 * j + 2 * h + 1], 1.0f / RB_SPLIT_SCALE, v1);
-                }
-                tc_store_pair(e, p.n_zero_to, r0 + 8 * h, c0 + 8 * j, v0, v1);
+                if (orow[h] < 0) continue;
+                // odd rows read their two halves in the other order: the 8 lanes of a 16-byte load phase then hit 32 distinct banks
+                const float* src = stg + (rr + 32 * h) * TC_SP + 8 * g;
+                const int q = (rr & 1) * 4;
+                const float4 a = *reinterpret_cast<const float4*>(src + q), b = *reinterpret_cast<const float4*>(src + (4 - q));
+                float v[8];
+                if (q == 0) { v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w; }
+                else        { v[0] = b.x; v[1] = b.y; v[2] = b.z; v[3] = b.w; v[4] = a.x; v[5] = a.y; v[6] = a.z; v[7] = a.w; }
+                epilogue8(e, mrow[h], n, orow[h], cnt, cb, cs, na[h], v);
             }
         }
     }
@@ -334,11 +472,11 @@ static int dispatch_tc(int BN, int trans_b, const TcMaps& maps, TcParams& p, int
         case 32: return launch_tc<32, SPLIT, BF16, 0>(maps, p, zdim, max_ctas, st);
         case 64: return launch_tc<64, SPLIT, BF16, 0>(maps, p, zdim, max_ctas, st);
         case 128: return launch_tc<128, SPLIT, BF16, 0>(maps, p, zdim, max_ctas, st);
+        case 144: return launch_tc<144, SPLIT, BF16, 0>(maps, p, zdim, max_ctas, st);
         default:
-            if constexpr (SPLIT) { set_error("gemm_tc: split-fp16 tiles are at most 128 columns wide (got %d)", BN); return 1; }
+            if constexpr (SPLIT) { set_error("gemm_tc: split-fp16 tiles are at most 144 columns wide (got %d)", BN); return 1; }
             else {
                 switch (BN) {
-                    case 144: return launch_tc<144, false, BF16, 0>(maps, p, zdim, max_ctas, st);
                     case 192: return launch_tc<192, false, BF16, 0>(maps, p, zdim, max_ctas, st);
                     default: return launch_tc<256, false, BF16, 0>(maps, p, zdim, max_ctas, st);
                 }
@@ -371,10 +509,11 @@ int gemm_tc(const rb_gemm_args* a, cudaStream_t stream) {
     const int64_t a_rows = a->a_rows > 0 ? a->a_rows : a->M;
     // tile width: the narrowest that covers N up to 128; [N,K] weights wider than that take the width that wastes the fewest
     // columns (C = 144 / 569 / 1137 ...).  [K,N] operands load boxes of 64 columns (64 or 128 wide); split operands hold two
-    // accumulators in registers, which caps them at 128.
+    // accumulators in registers, which caps them at 144: of 128 and 144 they take the one that pads fewer columns (ties: 128).
     int BN = a->N <= 32 && !a->trans_b ? 32 : (a->N <= 64 ? 64 : 128);
-    if (!a->trans_b && !split && a->N > 128) {
-        if (a->N <= 144) BN = 144;
+    if (!a->trans_b && a->N > 128) {
+        if (split) BN = (a->N + 143) / 144 * 144 < (a->N + 127) / 128 * 128 ? 144 : 128;
+        else if (a->N <= 144) BN = 144;
         else if (a->N <= 192) BN = 192;
         else {
             const int w192 = (a->N + 191) / 192 * 192 - a->N, w256 = (a->N + 255) / 256 * 256 - a->N;
