@@ -13,40 +13,9 @@
 //   * 4 compute warps each own two output rows of the tile: 120 LDS.32 + 800 FFMA2 per 64 outputs.
 // ncu on the previous version (software loads in the compute warps): 2690 instructions per warp and tile of which 800
 // FFMA2, FMA pipe 50 % busy, 115 us for the 216x216x569 map; see DESIGN.md for the numbers of this one.
-#include "common.cuh"
-#include <cuda.h>
+#include "tma.cuh"
 
 namespace rb {
-namespace dwt {
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-}  // namespace dwt
 
 constexpr int DT_TW = 16, DT_CH = 64, DT_IW = DT_TW + 4;
 
@@ -73,7 +42,6 @@ struct DwTmaParams {
 // TIN = __half / __nv_bfloat16: output in the same type.  TIN = float: output as an RB_F16S pair (out = hi plane, out_lo).
 template <typename TIN>
 __global__ void __launch_bounds__(DwCfg<TIN>::THREADS) dwconv5x5_relu_tma_kernel(const __grid_constant__ CUtensorMap map_in, const DwTmaParams p) {
-    using namespace dwt;
     using Cfg = DwCfg<TIN>;
     constexpr int STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES, TH = Cfg::TH, NW = Cfg::NWARPS;
     constexpr bool F32IN = sizeof(TIN) == 4;
@@ -189,10 +157,6 @@ __global__ void __launch_bounds__(DwCfg<TIN>::THREADS) dwconv5x5_relu_tma_kernel
     }
 }
 
-typedef CUresult (*EncodeTiledFnDw)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 #ifdef RB_FZ_CLK
 extern "C" int romab200_debug_dwclk(long long* out, int reset) {
     if (reset) { long long z[16] = {0}; return (int)cudaMemcpyToSymbol(g_dw_clk, z, sizeof(z)); }
@@ -203,12 +167,7 @@ extern "C" int romab200_debug_dwclk(long long* out, int reset) {
 template <typename TIN>
 static int launch_dw(const CUtensorMap& map, const DwTmaParams& p, dim3 grid, cudaStream_t st) {
     using Cfg = DwCfg<TIN>;
-    static bool cfg[64] = {};            // function attributes are per device
-    const int dev = current_device() & 63;
-    if (!cfg[dev]) {
-        RB_REQUIRE(cudaFuncSetAttribute(dwconv5x5_relu_tma_kernel<TIN>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM) == cudaSuccess, "dwconv: smem attribute");
-        cfg[dev] = true;
-    }
+    if (ensure_smem<dwconv5x5_relu_tma_kernel<TIN>>(Cfg::SMEM, "dwconv")) return 1;
     rb::launch_pdl(dwconv5x5_relu_tma_kernel<TIN>, grid, dim3(Cfg::THREADS), Cfg::SMEM, st, map, p);
     return check_launch("dwconv5x5_relu_tma");
 }
@@ -216,14 +175,6 @@ static int launch_dw(const CUtensorMap& map, const DwTmaParams& p, dim3 grid, cu
 // 16-bit maps (same type out), or fp32 maps with an RB_F16S result (a->out_lo != NULL); the caller has checked the pitches
 // (ldi * element size % 16 == 0, ldo % 2 == 0) and the 16-byte alignment of the input.
 int dwconv_tma(const rb_dwconv_args* a, cudaStream_t st) {
-    static EncodeTiledFnDw enc = nullptr;
-    if (!enc) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        RB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && ptr,
-                   "dwconv: cuTensorMapEncodeTiled not available");
-        enc = (EncodeTiledFnDw)ptr;
-    }
     const bool f32 = a->dtype == RB_F32;
     RB_REQUIRE(!f32 || a->out_lo, "dwconv_tma: fp32 maps need the RB_F16S output planes");
     const uint64_t es = f32 ? 4 : 2;
@@ -232,11 +183,8 @@ int dwconv_tma(const rb_dwconv_args* a, cudaStream_t st) {
     cuuint64_t d4[4] = {(cuuint64_t)a->c, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
     cuuint64_t s4[3] = {(cuuint64_t)a->ldi * es, (cuuint64_t)a->w * a->ldi * es, (cuuint64_t)a->h * a->w * a->ldi * es};
     cuuint32_t b4[4] = {(cuuint32_t)DT_CH, (cuuint32_t)DT_IW, (cuuint32_t)(TH + 4), 1};
-    cuuint32_t e4[4] = {1, 1, 1, 1};
     const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
-    CUresult r4 = enc(&map, dt, 4, const_cast<void*>(a->in), d4, s4, b4, e4, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    RB_REQUIRE(r4 == CUDA_SUCCESS, "dwconv: cuTensorMapEncodeTiled failed with %d (c=%d w=%d h=%d ldi=%lld)", (int)r4, a->c, a->w, a->h, (long long)a->ldi);
+    if (encode_tiled(&map, "dwconv", dt, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
     DwTmaParams p;
     p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ldo; p.wgt = a->weight; p.ldw = a->ldw; p.bias = a->bias;
     p.H = a->h; p.W = a->w; p.C = a->c;
@@ -247,9 +195,7 @@ int dwconv_tma(const rb_dwconv_args* a, cudaStream_t st) {
     p.total_tiles = (int)total;
     const int groups = (a->c + DT_CH - 1) / DT_CH;
     RB_REQUIRE(groups <= 65535, "dwconv: too many channel groups");
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, current_device());
-    int per_group = (f32 ? 1 : 2) * sms / groups;              // resident CTAs per SM (one for the fp32 ring), never more CTAs than fit at once
+    int per_group = (f32 ? 1 : 2) * sm_count() / groups;             // resident CTAs per SM (one for the fp32 ring), never more CTAs than fit at once
     if (per_group < 1) per_group = 1;
     if (per_group > p.total_tiles) per_group = p.total_tiles;
     dim3 grid(per_group, groups);

@@ -23,43 +23,14 @@
 //         Pt <= 2048 never overflows; the unscaled low part Pt_lo only underflows for p < 6e-5, where its absolute error
 //         (1.5e-11 in units of p) is irrelevant.
 //   out  = O' / (2048 l) written as an RB_F16S pair for the projection GEMM.
-#include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
-#include <cuda.h>
 #include <type_traits>
 
 namespace rb {
 
-// ---- PTX helpers (same conventions as gemm_tc.cu) --------------------------------------------------------------
+// ---- softmax and fragment helpers ------------------------------------------------------------------------------
 namespace fa {
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
 __device__ __forceinline__ float ex2(float x) {
     float y;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -284,21 +255,11 @@ __global__ void __launch_bounds__(384, 1) flash_attn_kernel(const __grid_constan
     }
 }
 
-typedef CUresult (*EncodeTiledFnFa)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
 template <int D, typename T, bool SPLIT>
 static int launch_fa(const CUtensorMap& map_hi, const CUtensorMap& map_lo, const FaParams& p, int batch, cudaStream_t st) {
     using Cfg = FaCfg<D, SPLIT>;
     auto kernel = flash_attn_kernel<D, T, SPLIT>;
-    static bool configured[64] = {};      // function attributes are per device
-    const int dev = current_device() & 63;
-    if (!configured[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-        RB_REQUIRE(e == cudaSuccess, "flash_attn: cannot set %d bytes of dynamic shared memory: %s", Cfg::SMEM, cudaGetErrorString(e));
-        configured[dev] = true;
-    }
+    if (ensure_smem<flash_attn_kernel<D, T, SPLIT>>(Cfg::SMEM, "flash_attn")) return 1;
     dim3 grid((p.N + Cfg::BQ - 1) / Cfg::BQ, p.heads, batch);
     rb::launch_pdl(kernel, dim3(grid), dim3(384), Cfg::SMEM, st, map_hi, map_lo, p);
     return check_launch(SPLIT ? "flash_attn_split" : "flash_attn");
@@ -318,30 +279,17 @@ extern "C" int romab200_flash_attn(const rb_flash_attn_args* a, void* stream) {
     RB_REQUIRE(a->ld_qkv >= 3 * dim && (a->ld_qkv * 2) % 16 == 0 && ((uintptr_t)a->qkv) % 16 == 0, "flash_attn: qkv pitch/alignment");
     RB_REQUIRE(a->ld_out >= dim && (a->ld_out * 2) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0, "flash_attn: out pitch/alignment");
     RB_REQUIRE(a->batch > 0 && a->batch <= 65535 && a->n_tokens > 0, "flash_attn: bad batch / token count");
-    static EncodeTiledFnFa enc = nullptr;
-    if (!enc) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        RB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && ptr,
-                   "flash_attn: cuTensorMapEncodeTiled not available");
-        enc = (EncodeTiledFnFa)ptr;
-    }
     // [batch, tokens, 3 * dim] with boxes of 64 tokens x 64 columns, 128B-swizzled: one plane (hi) or two (hi, lo)
     cuuint64_t dims[3] = {(cuuint64_t)(3 * dim), (cuuint64_t)a->n_tokens, (cuuint64_t)a->batch};
     cuuint64_t strides[2] = {(cuuint64_t)a->ld_qkv * 2, (cuuint64_t)a->ld_qkv * 2 * (cuuint64_t)a->n_tokens};
     cuuint32_t box[3] = {64, 64, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
     CUtensorMap map_hi, map_lo;
-    CUresult r = enc(&map_hi, a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv),
-                     dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    RB_REQUIRE(r == CUDA_SUCCESS, "flash_attn: cuTensorMapEncodeTiled failed with %d", (int)r);
+    if (encode_tiled(&map_hi, "flash_attn", a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->qkv,
+                     dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
     map_lo = map_hi;
-    if (a->dtype == RB_F16S) {
-        r = enc(&map_lo, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(a->qkv_lo), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RB_REQUIRE(r == CUDA_SUCCESS, "flash_attn: cuTensorMapEncodeTiled (lo plane) failed with %d", (int)r);
-    }
+    if (a->dtype == RB_F16S &&
+        encode_tiled(&map_lo, "flash_attn (lo plane)", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->qkv_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+        return 1;
     FaParams p;
     p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ld_out; p.N = a->n_tokens; p.heads = a->heads; p.dim = dim;
     p.scale_log2 = 1.4426950408889634f / sqrtf((float)a->head_dim);

@@ -17,44 +17,10 @@
 // the low part.  Per k-step each warpgroup issues three MMAs into two accumulators, acc0 += A_hi.B_hi and acc1 += A_hi.B_lo +
 // A_lo.B_hi; the epilogue forms acc0 + acc1 * 2^-11 (the dropped A_lo.B_lo term is 2^-22 relative).  Products of fp16 values are
 // exact in the fp32 accumulator, so the only error left is the 2^-22 operand representation and the fp32 accumulation itself.
-#include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
-#include <cuda.h>
 
 namespace rb {
-
-// ------------------------------------------------------------------------------------------------
-// PTX wrappers
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
 
 // ------------------------------------------------------------------------------------------------
 struct TcParams {
@@ -84,8 +50,6 @@ template <int BN, bool SPLIT> struct TcCfg {
     static constexpr int SMEM = STAGES * STAGE_BYTES + TC_STAGING + 1024 + 256;
     static_assert(STAGES >= 3 && SMEM <= 232448, "shared memory budget");
 };
-
-__device__ __forceinline__ void bar_named(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
 // cnt (<= 8) consecutive elements of a 16-bit or fp32 matrix as floats: two 16-byte loads (fp32) or one (16-bit) when all 8 are
 // wanted and the address allows it
@@ -394,64 +358,25 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    if (!fn) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) != cudaSuccess || !ptr) return nullptr;
-        fn = (EncodeTiledFn)ptr;
-    }
-    return fn;
-}
-
 // 4-D map over (inner, rows, batch1, batch0) of a 16-bit matrix
 static int make_map(CUtensorMap* map, const void* base, int is_bf16, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint64_t b1,
                     uint64_t s1_elems, uint64_t b0, uint64_t s0_elems, uint32_t box_inner, uint32_t box_rows) {
-    EncodeTiledFn enc = get_encode();
-    RB_REQUIRE(enc, "gemm_tc: cuTensorMapEncodeTiled not available (driver too old?)");
     RB_REQUIRE(((uintptr_t)base) % 16 == 0 && (pitch_elems * 2) % 16 == 0, "gemm_tc: operand base/pitch must be 16-byte aligned (pitch %llu elems)", (unsigned long long)pitch_elems);
     RB_REQUIRE((b1 <= 1 || (s1_elems * 2) % 16 == 0) && (b0 <= 1 || (s0_elems * 2) % 16 == 0), "gemm_tc: batch strides must be 16-byte aligned");
     cuuint64_t dims[4] = {inner, rows, b1 > 0 ? b1 : 1, b0 > 0 ? b0 : 1};
     cuuint64_t strides[3] = {pitch_elems * 2, (b1 > 1 ? s1_elems : pitch_elems * rows) * 2, (b0 > 1 ? s0_elems : pitch_elems * rows) * 2};
     cuuint32_t box[4] = {box_inner, box_rows, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(map, is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(base), dims,
-                     strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    RB_REQUIRE(r == CUDA_SUCCESS, "gemm_tc: cuTensorMapEncodeTiled failed with %d (inner=%llu rows=%llu pitch=%llu)", (int)r,
-               (unsigned long long)inner, (unsigned long long)rows, (unsigned long long)pitch_elems);
-    return 0;
+    return encode_tiled(map, "gemm_tc", is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
+                        CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
 struct TcMaps { CUtensorMap a, b, a_lo, b_lo; };
-
-static int sm_count() {
-    static int n[64] = {};
-    const int dev = current_device() & 63;
-    if (!n[dev]) {
-        cudaDeviceGetAttribute(&n[dev], cudaDevAttrMultiProcessorCount, dev);
-        if (n[dev] <= 0) n[dev] = 132;
-    }
-    return n[dev];
-}
 
 template <int BN, bool SPLIT, bool BF16, int TB>
 static int launch_tc(const TcMaps& maps, TcParams& p, int zdim, int max_ctas, cudaStream_t st) {
     using Cfg = TcCfg<BN, SPLIT>;
     auto kernel = gemm_tc_kernel<BN, SPLIT, BF16, TB>;
-    // function attributes are per device: one flag per device ordinal (several engines on different GPUs in one process)
-    static bool configured[64] = {};
-    const int dev = current_device();
-    if (!configured[dev & 63]) {
-        cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM);
-        RB_REQUIRE(e == cudaSuccess, "gemm_tc: cannot set %d bytes of dynamic shared memory: %s", Cfg::SMEM, cudaGetErrorString(e));
-        configured[dev & 63] = true;
-    }
+    if (ensure_smem<gemm_tc_kernel<BN, SPLIT, BF16, TB>>(Cfg::SMEM, "gemm_tc")) return 1;
     p.tiles_m = (p.M + TC_BM - 1) / TC_BM;
     p.tiles_n = (p.N + BN - 1) / BN;
     const long long total = (long long)p.tiles_m * p.tiles_n * zdim;

@@ -14,7 +14,7 @@
 //   0                         32-wide panels as a chain of small kernels (chol_diag / chol_panel / trsm_back + GEMMs)
 //   1                         one cooperative persistent kernel with device-wide barriers
 // All O(n^3) work is in the trailing updates, which are romab200 fp32 GEMMs (lower triangle only).
-#include "common.cuh"
+#include "tma.cuh"
 
 namespace rb {
 
@@ -376,9 +376,6 @@ __device__ long long g_cb_clk[32];
 #define CBCLK(i)
 #endif
 
-__device__ __forceinline__ void bar_named(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-__device__ __forceinline__ void bar_arrive(int id, int nthreads) { asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
-
 // 1/sqrt(p) of a pivot.  This sits on the serial chain of the whole factorisation, hence MUFU.RSQ and one Newton step
 // (full fp32 accuracy; pivots of K + sigma*I are far from the denormal range) instead of a division and a square root.
 __device__ __forceinline__ float rsqrt_newton(float p) {
@@ -619,14 +616,8 @@ static int gp_solve_block128(const rb_gp_solve_args* a, cudaStream_t st) {
     const int64_t ws_stride = (int64_t)nblk * BB * BB;
     float* W = a->W;
     float* ws = (float*)a->workspace;
-    static bool configured[64] = {};           // function attributes are per device
-    const int dev = current_device() & 63;
     const size_t smem = (size_t)CB_SMEM_FLOATS * sizeof(float);
-    if (!configured[dev]) {
-        RB_REQUIRE(cudaFuncSetAttribute(chol_block128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess,
-                   "gp_solve: cannot reserve %zu bytes of shared memory", smem);
-        configured[dev] = true;
-    }
+    if (ensure_smem<chol_block128_kernel>((int)smem, "gp_solve")) return 1;
     for (int kb = 0; kb < nblk; ++kb) {
         const int k = kb * BB, bs = n - k < BB ? n - k : BB;
         rb::launch_pdl(chol_block128_kernel, dim3(a->batch), dim3(CB_THREADS), smem, st, W, ws, a->ldw, a->stride, ws_stride, k, kb, bs);
@@ -687,14 +678,8 @@ static int gp_solve_tc(const rb_gp_solve_args* a, cudaStream_t st) {
     const int64_t sh = gp_tc_scratch_halves(n, a->nrhs, a->ldw);          // plane stride between problems
     __half* s_hi = reinterpret_cast<__half*>(ws + (int64_t)a->batch * ws_stride);
     __half* s_lo = s_hi + (int64_t)a->batch * sh;
-    static bool configured[64] = {};
-    const int dev = current_device() & 63;
     const size_t smem = (size_t)CB_SMEM_FLOATS * sizeof(float);
-    if (!configured[dev]) {
-        RB_REQUIRE(cudaFuncSetAttribute(chol_block128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) == cudaSuccess,
-                   "gp_solve: cannot reserve %zu bytes of shared memory", smem);
-        configured[dev] = true;
-    }
+    if (ensure_smem<chol_block128_kernel>((int)smem, "gp_solve")) return 1;
     for (int kb = 0; kb < nblk; ++kb) {
         const int k = kb * BB, bs = n - k < BB ? n - k : BB;
         rb::launch_pdl(chol_block128_kernel, dim3(a->batch), dim3(CB_THREADS), smem, st, W, ws, a->ldw, a->stride, ws_stride, k, kb, bs);
@@ -768,13 +753,11 @@ extern "C" int romab200_gp_solve(const rb_gp_solve_args* a, void* stream) {
         p.W = a->W; p.diag = (float*)a->workspace; p.counter = (unsigned int*)((float*)a->workspace + diag_floats);
         p.n = a->n; p.nrhs = a->nrhs; p.batch = a->batch; p.ldw = a->ldw; p.stride = a->stride;
         RB_REQUIRE(cudaMemsetAsync(p.counter, 0, 4, st) == cudaSuccess, "gp_solve: memset failed");
-        int dev = 0, sms = 0, per_sm = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+        int per_sm = 0;
         cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, gp_solve_persistent_kernel, GP_THREADS, 0);
-        RB_REQUIRE(sms > 0 && per_sm > 0, "gp_solve: cannot size the cooperative grid");
+        RB_REQUIRE(per_sm > 0, "gp_solve: cannot size the cooperative grid");
         void* kargs[] = {(void*)&p};
-        cudaError_t err = cudaLaunchCooperativeKernel((void*)gp_solve_persistent_kernel, dim3(sms), dim3(GP_THREADS), kargs, 0, st);
+        cudaError_t err = cudaLaunchCooperativeKernel((void*)gp_solve_persistent_kernel, dim3(sm_count()), dim3(GP_THREADS), kargs, 0, st);
         RB_REQUIRE(err == cudaSuccess, "gp_solve: cooperative launch failed: %s", cudaGetErrorString(err));
         return check_launch("gp_solve_persistent");
     }

@@ -13,6 +13,7 @@
 // e.g. the seeded synthetic weights) writes tile_done = 0 and leaves its pixels to refiner_prologue_kernel
 // (refiner.cu), which skips the pixels of finished tiles.
 #include "refiner_common.cuh"
+#include "tma.cuh"
 
 namespace rb {
 
@@ -211,13 +212,7 @@ refiner_prologue_tile_kernel(const PrologueParams p, unsigned char* __restrict__
 template <int R>
 static int launch_tile(const PrologueParams& p, unsigned char* tile_done, cudaStream_t st) {
     using SM = LcTileSmem<R>;
-    static bool cfg[64] = {};                                       // function attributes are per device
-    const int dev = current_device() & 63;
-    if (!cfg[dev]) {
-        RB_REQUIRE(cudaFuncSetAttribute(refiner_prologue_tile_kernel<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, SM::BYTES) == cudaSuccess,
-                   "refiner_prologue (tile): smem attribute");
-        cfg[dev] = true;
-    }
+    if (ensure_smem<refiner_prologue_tile_kernel<R>>(SM::BYTES, "refiner_prologue (tile)")) return 1;
     const int tiles = p.D * ((p.h + LcTile<R>::TQY - 1) / LcTile<R>::TQY) * ((p.w + LcTile<R>::TQX - 1) / LcTile<R>::TQX);
     rb::launch_pdl(refiner_prologue_tile_kernel<R>, dim3((unsigned)tiles), dim3(SM::THREADS), (size_t)SM::BYTES, st, p, tile_done);
     return check_launch("refiner_prologue_tile");

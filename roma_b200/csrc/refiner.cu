@@ -6,6 +6,7 @@
 // All kernels here are gather / streaming kernels (HBM- or L2-bound); one warp per pixel with lanes over
 // channels, so every global access is a contiguous run of the channel vector.
 #include "refiner_common.cuh"
+#include "tma.cuh"
 
 namespace rb {
 
@@ -921,13 +922,7 @@ extern "C" int romab200_refiner_block_small(const rb_refiner_block_small_args* a
         pw.b[co] = a->pw_bias_host[co];
     }
     if (a->dtype == RB_F32) {
-        static bool cfg[64] = {};            // function attributes are per device
-        const int dev = current_device() & 63;
-        if (!cfg[dev]) {
-            RB_REQUIRE(cudaFuncSetAttribute(refiner_block_small_f32_kernel<24>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmallF32Cfg<24>::SMEM) == cudaSuccess,
-                       "refiner_block_small: smem attribute");
-            cfg[dev] = true;
-        }
+        if (ensure_smem<refiner_block_small_f32_kernel<24>>(SmallF32Cfg<24>::SMEM, "refiner_block_small")) return 1;
         rb::launch_pdl(refiner_block_small_f32_kernel<24>, dim3(grid), dim3(256), SmallF32Cfg<24>::SMEM, st, (const float*)a->in, (float*)a->out, a->ld, a->dw_weight, a->ldw,
                        a->dw_bias, pw, a->h, a->w, tiles_x);
     } else if (a->dtype == RB_F16)

@@ -8,48 +8,11 @@
 //     straight into the 128B-swizzled K-major layout of a wgmma A operand;
 //   * 1 warpgroup multiplies it with the pointwise weights (TMA-loaded into shared memory once, resident for the whole
 //     persistent kernel): per 64-pixel half 9 wgmma (M=64, N=144, K=16) into registers, then + bias -> 16-bit rows.
-#include "common.cuh"
+#include "tma.cuh"
 #include "wgmma.cuh"
-#include <cuda.h>
 #include <type_traits>
 
 namespace rb {
-namespace fz {
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n"
-            ".reg .pred p;\n"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n"
-            "selp.u32 %0, 1, 0, p;\n"
-            "}\n" : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(map)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-}  // namespace fz
 
 #ifdef RB_FZ_CLK
 __device__ long long g_fz_clk[64];
@@ -77,7 +40,6 @@ constexpr int FZ_SMEM = FZ_A_BYTES + FZ_B_BYTES + FZ_IN_BYTES + FZ_W_BYTES + 102
 template <typename T>
 __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_in, const FusedParams p) {
     rb::pdl_wait();
-    using namespace fz;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);   // offset on the array: keeps ld/st.shared
     uint8_t* sA = smem;
@@ -225,10 +187,6 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const
         }
     }
 }
-
-typedef CUresult (*EncodeTiledFnFz)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                    const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                    CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
 }  // namespace rb
 
 using namespace rb;
@@ -247,33 +205,18 @@ extern "C" int romab200_refiner_block_c144(const rb_refiner_block_c144_args* a, 
     RB_REQUIRE(a->ld % 8 == 0 && a->ld >= FZ_C && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0 && a->in != a->out,
                "refiner_block_c144: bad activation layout");
     RB_REQUIRE(a->ld_pw % 8 == 0 && a->ld_pw >= FZ_C && ((uintptr_t)a->pw_weight) % 16 == 0, "refiner_block_c144: bad weight layout");
-    static EncodeTiledFnFz enc = nullptr;
-    if (!enc) {
-        void* ptr = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        RB_REQUIRE(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &q) == cudaSuccess && ptr,
-                   "refiner_block_c144: cuTensorMapEncodeTiled not available");
-        enc = (EncodeTiledFnFz)ptr;
-    }
+    const CUtensorMapDataType dt = a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
     CUtensorMap map;
     cuuint64_t dims[2] = {(cuuint64_t)FZ_C, (cuuint64_t)FZ_C};
     cuuint64_t strides[1] = {(cuuint64_t)a->ld_pw * 2};
     cuuint32_t box[2] = {64, (cuuint32_t)FZ_C};
-    cuuint32_t estr[2] = {1, 1};
-    CUresult r = enc(&map, a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(a->pw_weight),
-                     dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    RB_REQUIRE(r == CUDA_SUCCESS, "refiner_block_c144: cuTensorMapEncodeTiled failed with %d", (int)r);
+    if (encode_tiled(&map, "refiner_block_c144", dt, 2, a->pw_weight, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
     CUtensorMap map_in;          // activation [B, H, W, C] with pitch ld: box = 12 x 20 pixels x 144 channels, borders zero-filled
     {
         cuuint64_t d4[4] = {(cuuint64_t)FZ_C, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
         cuuint64_t s4[3] = {(cuuint64_t)a->ld * 2, (cuuint64_t)a->w * a->ld * 2, (cuuint64_t)a->h * a->w * a->ld * 2};
         cuuint32_t b4[4] = {(cuuint32_t)FZ_C, (cuuint32_t)FZ_IW, (cuuint32_t)FZ_IH, 1};
-        cuuint32_t e4[4] = {1, 1, 1, 1};
-        CUresult r4 = enc(&map_in, a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(a->in),
-                          d4, s4, b4, e4, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        RB_REQUIRE(r4 == CUDA_SUCCESS, "refiner_block_c144: cuTensorMapEncodeTiled (input) failed with %d", (int)r4);
+        if (encode_tiled(&map_in, "refiner_block_c144 (input)", dt, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
     }
     FusedParams p;
     p.in = a->in; p.out = a->out; p.ld = a->ld; p.dw_w = a->dw_weight; p.ldw = a->ldw; p.dw_b = a->dw_bias; p.pw_b = a->pw_bias;
@@ -281,17 +224,13 @@ extern "C" int romab200_refiner_block_c144(const rb_refiner_block_c144_args* a, 
     const long long total = (long long)p.tiles_x * p.tiles_y * a->batch;
     RB_REQUIRE(total > 0 && total < (1ll << 31), "refiner_block_c144: bad tile count");
     p.total_tiles = (int)total; p.is_bf16 = a->dtype == RB_BF16;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    const int sms = sm_count();
     const int grid = p.total_tiles < sms ? p.total_tiles : sms;
     if (a->dtype == RB_F16) {
-        static bool cfg[64] = {};            // function attributes are per device
-        if (!cfg[dev & 63]) { RB_REQUIRE(cudaFuncSetAttribute(refiner_block_c144_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM) == cudaSuccess, "refiner_block_c144: smem attribute"); cfg[dev & 63] = true; }
+        if (ensure_smem<refiner_block_c144_kernel<__half>>(FZ_SMEM, "refiner_block_c144")) return 1;
         rb::launch_pdl(refiner_block_c144_kernel<__half>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
     } else {
-        static bool cfg[64] = {};
-        if (!cfg[dev & 63]) { RB_REQUIRE(cudaFuncSetAttribute(refiner_block_c144_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, FZ_SMEM) == cudaSuccess, "refiner_block_c144: smem attribute"); cfg[dev & 63] = true; }
+        if (ensure_smem<refiner_block_c144_kernel<__nv_bfloat16>>(FZ_SMEM, "refiner_block_c144")) return 1;
         rb::launch_pdl(refiner_block_c144_kernel<__nv_bfloat16>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
     }
     return check_launch("refiner_block_c144");
