@@ -352,6 +352,41 @@ typedef struct {
 } rb_transpose_args;
 int romab200_transpose(const rb_transpose_args* args, void* stream);
 
+/* ---- match_keypoints (matcher.py:743-762): grid samples at the keypoints + mutual nearest neighbours in O(N_A + N_B) memory ----
+ * romab200_keypoints_sample replaces the two F.grid_sample calls (matcher.py:743-754):
+ *   x_to_B[i] = grid_sample(warp[..., 0:2], x[i]), cert_out[i] = grid_sample(cert, x[i]); bilinear, zero padding, align_corners=False,
+ *   ATen's unnormalisation ((x + 1) * size - 1) / 2; a NaN position gives NaN.  x [n, 2] fp32 contiguous (normalised (x, y));
+ *   warp: element (y, x, c) of the two sampled channels at warp[y * warp_ld_row + x * warp_ld_px + c * warp_ld_ch] (strides in floats,
+ *   so views such as the A half of a symmetric warp are read in place); cert: element (y, x) at cert[y * cert_ld_row + x * cert_ld_px];
+ *   x_to_B [n, 2], cert_out [n]. */
+typedef struct {
+    const float* x; int32_t n;
+    const float* warp; int32_t warp_h, warp_w; int64_t warp_ld_row, warp_ld_px, warp_ld_ch;
+    const float* cert; int32_t cert_h, cert_w; int64_t cert_ld_row, cert_ld_px;
+    float* x_to_B; float* cert_out;
+} rb_keypoints_sample_args;
+int romab200_keypoints_sample(const rb_keypoints_sample_args* args, void* stream);
+
+/* romab200_keypoints_mnn_count + romab200_keypoints_mnn_emit replace torch.cdist and the mutual-nearest-neighbour nonzero
+ * (matcher.py:755-762) without an N_A x N_B buffer.  With D[i, j] = sqrt_rn(dx*dx + dy*dy), dx = x_A_to_B[i].x - x_B[j].x (every
+ * operation rounded to fp32, no FMA contraction: the exact-difference distance), the pair (i, j) is a match iff
+ *   D[i,j] == min_j' D[i,j'] && D[i,j] == min_i' D[i',j] && cert_A[i] > cert_th && D[i,j] < max_dist,
+ * minima with torch.min's NaN propagation (a NaN anywhere in a row or column leaves it without matches); ties are all kept.
+ * x_A_to_B [n_a, 2], cert_A [n_a], x_B [n_b, 2] fp32 contiguous; n_a, n_b > 0.
+ * workspace: >= (16 + 1) * (n_a + n_b) floats; it holds the row and column minima between the two calls (pass it unchanged).
+ * count: offsets [n_a + 1] int64 receives the exclusive prefix sums of the per-row match counts, offsets[n_a] = number of matches.
+ * emit (after the caller has read offsets[n_a] and sized the outputs): inds_A, inds_B [offsets[n_a]] int64 receive the matches in
+ * row-major order (i ascending, then j), the order of torch.nonzero.  Deterministic. */
+typedef struct {
+    const float* x_A_to_B; const float* cert_A; const float* x_B; int32_t n_a, n_b;
+    float cert_th, max_dist;
+    float* workspace; int64_t workspace_floats;
+    int64_t* offsets;
+    int64_t* inds_A; int64_t* inds_B;   /* emit only */
+} rb_keypoints_mnn_args;
+int romab200_keypoints_mnn_count(const rb_keypoints_mnn_args* args, void* stream);
+int romab200_keypoints_mnn_emit(const rb_keypoints_mnn_args* args, void* stream);
+
 /* ---- TinyRoMa (romatch/models/tiny.py), fp32 throughout like the reference ------------------------ */
 /* Direct convolution on channels-last fp32 maps, CUDA-core FFMA (the XFeat backbone convs, tiny.py:87-97, and the
  * BasicLayer / 1x1 heads of the coarse and fine matchers, tiny.py:47-61,208-215):

@@ -142,7 +142,12 @@ _FIELD_DTYPES = {
     "rb_tiny_pos_embed_args": {"f0": _F32, "f1": _F32, "state": _F32, "grid_x": _F32, "grid_y": _F32, "grid_lr_x": _F32, "grid_lr_y": _F32},
     "rb_tiny_warp_concat_args": {"f0": _F32, "f1": _F32, "state": _F32, "out": _F32},
     "rb_tiny_epilogue_args": {"state": _F32, "warp": _F32, "cert": _F32, "grid_x": _F32, "grid_y": _F32},
+    "rb_keypoints_sample_args": {"x": _F32, "warp": _F32, "cert": _F32, "x_to_B": _F32, "cert_out": _F32},
+    "rb_keypoints_mnn_args": {"x_A_to_B": _F32, "cert_A": _F32, "x_B": _F32, "workspace": _F32, "offsets": torch.int64, "inds_A": torch.int64,
+                              "inds_B": torch.int64},
 }
+# tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
+_STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}}
 
 
 def _gemm_min_elems(kw):
@@ -167,12 +172,13 @@ def _validate(fn_name, struct_name, kw):
     table = _FIELD_DTYPES.get(struct_name, {})
     cur = torch.cuda.current_device() if torch.cuda.is_available() else None
     mins = _gemm_min_elems(kw) if struct_name == "rb_gemm_args" else {}
+    strided = _STRIDED_FIELDS.get(struct_name, ())
     for k, v in kw.items():
         if not isinstance(v, torch.Tensor):
             continue
         if not v.is_cuda or (cur is not None and v.device.index != cur):
             raise RuntimeError(f"{fn_name}: argument `{k}` lives on {v.device}, expected the current CUDA device cuda:{cur}")
-        if not v.is_contiguous():
+        if k not in strided and not v.is_contiguous():
             raise RuntimeError(f"{fn_name}: argument `{k}` is not contiguous (shape {tuple(v.shape)}, strides {v.stride()})")
         want = table.get(k)
         if isinstance(want, str):

@@ -279,13 +279,20 @@ class RegressionMatcher:
         return in_th if has_batch else in_th[0]
 
     def match_keypoints(self, x_A, x_B, warp, certainty, return_tuple=True, return_inds=False, max_dist=0.005, cert_th=0):
-        x_A_to_B = F.grid_sample(warp[..., -2:].permute(2, 0, 1)[None], x_A[None, None], align_corners=False,
-                                 mode="bilinear")[0, :, 0].mT
-        cert_A_to_B = F.grid_sample(certainty[None, None, ...], x_A[None, None], align_corners=False,
-                                    mode="bilinear")[0, 0, 0]
-        D = torch.cdist(x_A_to_B, x_B)
-        mutual = (D == D.min(dim=-1, keepdim=True).values) * (D == D.min(dim=-2, keepdim=True).values)
-        inds_A, inds_B = torch.nonzero(mutual * (cert_A_to_B[:, None] > cert_th) * (D < max_dist), as_tuple=True)
+        """Mutual nearest neighbours of the keypoints x_A carried through the warp and the keypoints x_B (matcher.py:732-773).
+        fp32 CUDA inputs of the expected shapes run on the device (`romab200_keypoints_*`) in O(N_A + N_B) memory, with the
+        exact-difference distance sqrt(dx² + dy²) where `torch.cdist` expands ‖a‖² + ‖b‖² − 2a·b; everything else runs the
+        reference's torch statement."""
+        if _keypoints_on_device(x_A, x_B, warp, certainty):
+            inds_A, inds_B = _match_keypoints_device(x_A, x_B, warp, certainty, max_dist, cert_th)
+        else:
+            x_A_to_B = F.grid_sample(warp[..., -2:].permute(2, 0, 1)[None], x_A[None, None], align_corners=False,
+                                     mode="bilinear")[0, :, 0].mT
+            cert_A_to_B = F.grid_sample(certainty[None, None, ...], x_A[None, None], align_corners=False,
+                                        mode="bilinear")[0, 0, 0]
+            D = torch.cdist(x_A_to_B, x_B)
+            mutual = (D == D.min(dim=-1, keepdim=True).values) * (D == D.min(dim=-2, keepdim=True).values)
+            inds_A, inds_B = torch.nonzero(mutual * (cert_A_to_B[:, None] > cert_th) * (D < max_dist), as_tuple=True)
         if return_tuple:
             return (inds_A, inds_B) if return_inds else (x_A[inds_A], x_B[inds_B])
         if return_inds:
@@ -322,3 +329,56 @@ class RegressionMatcher:
             arr = (arr.clamp(0, 1) * 255).byte().permute(1, 2, 0).cpu().numpy()
             Image.fromarray(arr).save(save_path)
         return vis_im
+
+
+def _keypoints_on_device(x_A, x_B, warp, certainty) -> bool:
+    """The inputs `match_keypoints` runs on the device: fp32 CUDA tensors on one device, points [N, 2], warp [H, W, >= 2],
+    certainty [H', W'] (non-empty maps)."""
+    ts = (x_A, x_B, warp, certainty)
+    if not all(isinstance(t, torch.Tensor) and t.is_cuda and t.dtype == torch.float32 for t in ts):
+        return False
+    if len({t.device for t in ts}) != 1:
+        return False
+    return (x_A.dim() == 2 and x_A.shape[1] == 2 and x_B.dim() == 2 and x_B.shape[1] == 2 and warp.dim() == 3 and warp.shape[-1] >= 2
+            and warp.numel() > 0 and certainty.dim() == 2 and certainty.numel() > 0)
+
+
+def _match_keypoints_device(x_A, x_B, warp, certainty, max_dist, cert_th):
+    """(inds_A, inds_B) int64 of the mutual nearest neighbours, row-major like torch.nonzero.  One host read: the match count."""
+    if x_A.shape[0] == 0 or x_B.shape[0] == 0:
+        raise IndexError("min(): Expected reduction dim to have non-zero size.")      # what the torch statement's D.min raises
+    x_A_to_B, cert_A = _keypoints_sample_device(x_A, warp, certainty)
+    return _mutual_nn_device(x_A_to_B, cert_A, x_B, max_dist, cert_th)
+
+
+def _keypoints_sample_device(x_A, warp, certainty):
+    """(x_A_to_B [N, 2], cert_A [N]): the two grid samples of match_keypoints (matcher.py:743-754) in one kernel; warp and
+    certainty are read in place through their strides."""
+    n_a, dev = x_A.shape[0], x_A.device
+    with torch.cuda.device(dev):
+        x_A = x_A.contiguous()
+        w2 = warp[..., -2:]
+        x_A_to_B = torch.empty(n_a, 2, dtype=torch.float32, device=dev)
+        cert_A = torch.empty(n_a, dtype=torch.float32, device=dev)
+        cabi.call("romab200_keypoints_sample", "rb_keypoints_sample_args", x=x_A, n=n_a,
+                  warp=w2, warp_h=w2.shape[0], warp_w=w2.shape[1], warp_ld_row=w2.stride(0), warp_ld_px=w2.stride(1), warp_ld_ch=w2.stride(2),
+                  cert=certainty, cert_h=certainty.shape[0], cert_w=certainty.shape[1], cert_ld_row=certainty.stride(0),
+                  cert_ld_px=certainty.stride(1), x_to_B=x_A_to_B, cert_out=cert_A)
+    return x_A_to_B, cert_A
+
+
+def _mutual_nn_device(x_A_to_B, cert_A, x_B, max_dist, cert_th):
+    """(inds_A, inds_B) of the mutual nearest neighbours under the exact-difference distance (include/romab200.h)."""
+    n_a, n_b, dev = x_A_to_B.shape[0], x_B.shape[0], x_B.device
+    with torch.cuda.device(dev):
+        x_B = x_B.contiguous()
+        workspace = torch.empty(17 * (n_a + n_b), dtype=torch.float32, device=dev)
+        offsets = torch.empty(n_a + 1, dtype=torch.int64, device=dev)
+        kw = dict(x_A_to_B=x_A_to_B, cert_A=cert_A, x_B=x_B, n_a=n_a, n_b=n_b, cert_th=float(cert_th), max_dist=float(max_dist),
+                  workspace=workspace, workspace_floats=workspace.numel(), offsets=offsets)
+        cabi.call("romab200_keypoints_mnn_count", "rb_keypoints_mnn_args", **kw)
+        total = int(offsets[n_a].item())
+        inds = torch.empty(2, total, dtype=torch.int64, device=dev)
+        if total:
+            cabi.call("romab200_keypoints_mnn_emit", "rb_keypoints_mnn_args", inds_A=inds[0], inds_B=inds[1], **kw)
+    return inds[0], inds[1]
