@@ -445,6 +445,37 @@ int romab200_tiny_warp_concat(const rb_tiny_warp_concat_args* args, void* stream
 typedef struct { const float* state; float* warp; float* cert; int32_t batch, h, w; const float* grid_x; const float* grid_y; } rb_tiny_epilogue_args;
 int romab200_tiny_match_epilogue(const rb_tiny_epilogue_args* args, void* stream);
 
+/* ---- JPEG decoding (roma_b200/jpeg.py), byte-identical to libjpeg-turbo's default decompression (Pillow's Image.open) ----
+ * One launch set decodes a batch of baseline / extended sequential Huffman JPEGs that roma_b200.jpeg.parse accepted:
+ * romab200_jpeg_entropy (unstuff + restart markers, self-synchronising parallel Huffman decode, coefficient emit, DC
+ * prediction), then romab200_jpeg_pixels (dequantise + ISLOW IDCT into planes, fancy upsampling + YCbCr -> RGB).
+ * The host fills `desc` (int64 [batch, 64], layout D_* in jpeg.py) and `tables` (int32 [batch, 6 * 804 + 192]: per scan
+ * component a DC and an AC Huffman lookup, then 3 quantisation tables in natural order) and sizes every buffer from the
+ * headers alone.  A stream the decoder rejects (corrupt entropy data, restart markers out of sequence, no EOI after the scan)
+ * sets state[b * 8 + 1] (a status word per image, 0 = ok) instead of faulting; every read is bounded by the stream length
+ * and every write by the header's block count, for any byte string.  Deterministic: no output depends on timing. */
+typedef struct {
+    int32_t batch;
+    const uint8_t* stream;    /* entropy-coded data of every image (from the byte after SOS to the end of the file), each zero-padded by >= 16 bytes */
+    const int64_t* desc;      /* [batch, 64] */
+    const int32_t* tables;    /* [batch, 6 * 804 + 192] */
+    uint8_t* comp;            /* compacted (unstuffed) bitstreams, stream_len + 16 bytes per image */
+    int32_t* chunks;          /* [2 * chunks]: kept bytes / RST markers per 4096-byte chunk, scanned in place */
+    int32_t* istart;          /* [sum (n_intervals + 1)]: first byte of every restart interval in the compacted stream, then its length */
+    int64_t* exits;           /* [2 * total_slots]: decoder exit states of the sync passes (double-buffered) */
+    int32_t* counts;          /* [2 * total_slots]: blocks started per subsequence | first block of each subsequence in its interval */
+    int16_t* coef;            /* [total_blocks, 64] natural order, zero-filled by the caller; DC resolved after the entropy stage */
+    int32_t* state;           /* [batch, 8]: scan end, status, compacted length, RST count, completed blocks */
+    int32_t* flags;           /* [8] zero-filled: change flags of the sync passes, pass count (flags[3]), barrier counter, no-convergence */
+    int32_t max_chunks, max_intervals;
+    int64_t total_slots, total_blocks;
+    uint8_t* planes;          /* pixels: per-component IDCT output planes (desc D_PLANE_*) */
+    uint8_t* out;             /* pixels: uint8 [H, W, C] per image at desc D_OUT_OFF */
+    int64_t max_pixels;       /* pixels: max H * W over the batch */
+} rb_jpeg_args;
+int romab200_jpeg_entropy(const rb_jpeg_args* args, void* stream);
+int romab200_jpeg_pixels(const rb_jpeg_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -19,4 +19,7 @@ def __getattr__(name):
     if name in ("roma_outdoor", "roma_indoor", "tiny_roma_v1_outdoor", "roma_model"):
         from . import model_zoo
         return getattr(model_zoo, name)
+    if name == "decode_jpeg":
+        from .jpeg import decode_jpeg
+        return decode_jpeg
     raise AttributeError(name)

@@ -145,6 +145,9 @@ _FIELD_DTYPES = {
     "rb_keypoints_sample_args": {"x": _F32, "warp": _F32, "cert": _F32, "x_to_B": _F32, "cert_out": _F32},
     "rb_keypoints_mnn_args": {"x_A_to_B": _F32, "cert_A": _F32, "x_B": _F32, "workspace": _F32, "offsets": torch.int64, "inds_A": torch.int64,
                               "inds_B": torch.int64},
+    "rb_jpeg_args": {"stream": torch.uint8, "desc": torch.int64, "tables": torch.int32, "comp": torch.uint8, "chunks": torch.int32,
+                     "istart": torch.int32, "exits": torch.int64, "counts": torch.int32, "coef": torch.int16, "state": torch.int32,
+                     "flags": torch.int32, "planes": torch.uint8, "out": torch.uint8},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}}

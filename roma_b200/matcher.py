@@ -19,7 +19,7 @@ from PIL import Image
 
 from . import cabi
 from .engine import Engine
-from .preprocess import DevicePreprocessor, check_input
+from .preprocess import DeviceImage, DevicePreprocessor, open_inputs
 from .sampling import sample_device
 
 
@@ -114,17 +114,18 @@ class RegressionMatcher:
             device = eng.device
         if torch.device(device).type != "cuda":
             raise RuntimeError("roma_b200 computes on CUDA only; device=%r" % (device,))
-        im_A = check_input(im_A_input)
-        im_B = check_input(im_B_input)
+        # JPEG paths are decoded on the device (both in one launch set); other paths, PIL images and tensors as before
+        im_A, im_B = open_inputs([im_A_input, im_B_input], eng.device)
         symmetric = self.symmetric
         ws, hs = self.w_resized, self.h_resized
         scale_factor = math.sqrt(hs * ws / (560 ** 2))
-        pil_route = isinstance(im_A, Image.Image) and isinstance(im_B, Image.Image)
+        pil_route = isinstance(im_A, (Image.Image, DeviceImage)) and isinstance(im_B, (Image.Image, DeviceImage))
         if pil_route:
-            # raw RGB bytes go up once per image; Pillow's bicubic resize + normalisation run on the device (csrc/preprocess.cu)
+            # raw RGB bytes go up once per image (or were decoded there); Pillow's bicubic resize + normalisation run on the
+            # device (csrc/preprocess.cu)
             b = 1
             pre = self._preprocessor()
-            raw_a, raw_b = pre.upload(im_A), pre.upload(im_B)
+            raw_a, raw_b = (im.raw if isinstance(im, DeviceImage) else pre.upload(im) for im in (im_A, im_B))
             a_t = pre.resize_normalize(raw_a, (hs, ws))[None]
             b_t = pre.resize_normalize(raw_b, (hs, ws))[None]
         elif isinstance(im_A, torch.Tensor) and isinstance(im_B, torch.Tensor):

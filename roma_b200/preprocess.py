@@ -18,7 +18,7 @@ import numpy as np
 import torch
 from PIL import Image
 
-from . import cabi
+from . import cabi, jpeg
 
 IMAGENET_MEAN = (0.485, 0.456, 0.406)
 IMAGENET_STD = (0.229, 0.224, 0.225)
@@ -41,6 +41,44 @@ def check_input(im_input):
     assert H % 14 == 0, "im_input must be a multiple of 14"
     assert W % 14 == 0, "im_input must be a multiple of 14"
     return im_input
+
+
+class DeviceImage:
+    """An input file decoded on the device: `raw` is uint8 [H, W, C], the bytes Pillow would give."""
+
+    def __init__(self, raw: torch.Tensor):
+        self.raw = raw
+
+
+def open_inputs(inputs, device, rgb: bool = True):
+    """Inputs of one `match` call.  Paths are opened with `Image.open` (lazy: the I;16 and decompression-bomb checks and the
+    format detection stay Pillow's); the JPEG files among them that `jpeg.parse` accepts are decoded on the device in one
+    launch set and come back as `DeviceImage`.  Every other path, and a JPEG the device decoder rejects, takes the host route
+    unchanged: `Image.open(p).convert("RGB")` when `rgb`, else the opened image.  Non-path inputs go through `check_input`
+    when `rgb`, else are returned as they are."""
+    out, pending = [], []
+    for x in inputs:
+        if isinstance(x, (str, os.PathLike)):
+            im = Image.open(x)
+            if rgb and im.mode == "I;16":
+                raise NotImplementedError("Can't handle 16 bit images")
+            found = jpeg.probe(x) if im.format == "JPEG" else None
+            if found is not None:
+                pending.append((len(out), found, im))
+                out.append(None)
+                continue
+            out.append(im.convert("RGB") if rgb else im)
+        else:
+            out.append(check_input(x) if rgb else x)
+    if pending:
+        res, _ = jpeg.decode_device([f[0] for _, f, _ in pending], [f[1] for _, f, _ in pending], device, [rgb] * len(pending))
+        for (k, _, im), r in zip(pending, res):
+            if isinstance(r, str):
+                out[k] = im.convert("RGB") if rgb else im
+            else:
+                im.close()              # decoded on the device: release the file Image.open keeps open
+                out[k] = DeviceImage(r)
+    return out
 
 
 def pil_to_normalized(im: Image.Image, size_hw) -> torch.Tensor:

@@ -189,3 +189,122 @@ def make_tiny_weights(seed: int, xfeat: torch.nn.Module) -> "OrderedDict[str, to
         else:
             sd[k] = _fill("bn_w", shape, g)
     return sd
+
+
+def _jpeg_image(rng, w: int, h: int, gray: bool):
+    """Smooth gradients + sharp-edged rectangles + noise, so that long Huffman codes and large AC categories occur."""
+    import numpy as np
+    y, x = np.mgrid[0:h, 0:w].astype(np.float64)
+    c = 1 if gray else 3
+    img = np.empty((h, w, c))
+    for k in range(c):
+        img[..., k] = 128 + 100 * np.sin(x / (7 + 13 * rng.rand()) + k) * np.cos(y / (5 + 11 * rng.rand()))
+    for _ in range(6):
+        x0, y0 = rng.randint(0, w), rng.randint(0, h)
+        img[y0:y0 + rng.randint(1, h + 1), x0:x0 + rng.randint(1, w + 1)] = rng.randint(0, 256, size=c)
+    img += rng.randn(h, w, c) * rng.choice([2.0, 20.0, 60.0])
+    img = np.clip(img, 0, 255).astype(np.uint8)
+    return img[..., 0] if gray else img
+
+
+def jpeg_corpus(seed: int = 0, max_pixels: int = None):
+    """Seeded JPEG test/benchmark corpus encoded with the installed Pillow: [(name, bytes, decline)], `decline` None for
+    files the device decoder handles, else a substring of the reason it declines them.  Covers quality 50 / 90 / 100,
+    subsampling 0 / 1 / 2, optimised Huffman tables, restart intervals (1 and 3 blocks, one row), "L" images, sizes from
+    1 x 1 to 6000 x 4000 (entries above `max_pixels` are left out), and progressive, CMYK and 4:4:0 files to decline."""
+    import io
+
+    import numpy as np
+    from PIL import Image
+
+    rng = np.random.RandomState(seed)
+    out = []
+
+    def add(name, w, h, gray=False, decline=None, edit=None, **kw):
+        if max_pixels is not None and w * h > max_pixels:
+            return
+        arr = _jpeg_image(rng, w, h, gray)
+        im = Image.fromarray(arr, "L" if gray else "RGB")
+        if kw.pop("cmyk", False):
+            im = im.convert("CMYK")
+        buf = io.BytesIO()
+        im.save(buf, "JPEG", **kw)
+        data = buf.getvalue()
+        if edit is not None:
+            data = edit(data)
+        out.append((name, data, decline))
+
+    for w, h in ((1, 1), (1, 17), (7, 9), (17, 33), (64, 48)):
+        for q in (50, 90, 100):
+            for ss in (0, 1, 2):
+                add(f"rgb_{w}x{h}_q{q}_s{ss}", w, h, quality=q, subsampling=ss)
+        add(f"gray_{w}x{h}_q90", w, h, gray=True, quality=90)
+    add("rgb_17x33_opt", 17, 33, quality=90, subsampling=2, optimize=True)
+    add("rgb_17x33_rst1", 17, 33, quality=90, subsampling=2, restart_marker_blocks=1)
+    add("gray_64x48_rst3", 64, 48, gray=True, quality=90, restart_marker_blocks=3)
+    add("rgb_640x480_q90_s2", 640, 480, quality=90, subsampling=2)
+    add("rgb_640x480_q50_s0", 640, 480, quality=50, subsampling=0)
+    add("rgb_640x480_q100_s1", 640, 480, quality=100, subsampling=1)
+    add("rgb_640x480_opt", 640, 480, quality=90, subsampling=2, optimize=True)
+    add("rgb_640x480_rst1", 640, 480, quality=90, subsampling=2, restart_marker_blocks=1)
+    add("rgb_640x480_rst3", 640, 480, quality=75, subsampling=2, restart_marker_blocks=3)
+    add("rgb_640x480_rstrow", 640, 480, quality=90, subsampling=1, restart_marker_rows=1)
+    add("gray_640x480_q90", 640, 480, gray=True, quality=90)
+    add("rgb_2040x1530_q90_s2", 2040, 1530, quality=90, subsampling=2)
+    add("rgb_6000x4000_q90_s2", 6000, 4000, quality=90, subsampling=2)
+    add("progressive_64x48", 64, 48, quality=90, progressive=True, decline="progressive")
+    add("cmyk_64x48", 64, 48, quality=90, cmyk=True, decline="4 components")
+
+    def to_440(data):
+        i = data.index(b"\xff\xc0")             # SOF0 of a 4:4:4 file: luma sampling byte 0x11 -> 0x12 (h 1, v 2)
+        b = bytearray(data)
+        assert b[i + 11] == 0x11
+        b[i + 11] = 0x12
+        return bytes(b)
+
+    add("rgb_64x48_440", 64, 48, quality=90, subsampling=0, edit=to_440, decline="sampling layout")
+    return out
+
+
+def jpeg_edits(seed: int = 0):
+    """Deterministic edits of small corpus files for the tests of the JPEG decoders: [(name, bytes)].
+      - 16 x 16 grayscale and 4:2:0 q100 files whose quantisation tables are all set to 1, 2, 8 or 32: from 8 up, the
+        dequantised coefficients leave the range of the 16-bit IDCT Pillow runs;
+      - single-bit flips at evenly spaced offsets of the entropy-coded data of every accepted 64 x 48 corpus file.
+    Each edit either decodes to exactly Pillow's bytes or is declined."""
+    import io
+
+    import numpy as np
+    from PIL import Image
+
+    from .jpeg import parse
+
+    out = []
+    rng = np.random.RandomState(seed + 7)
+    for gray in (True, False):
+        im = Image.fromarray(_jpeg_image(rng, 16, 16, gray), "L" if gray else "RGB")
+        buf = io.BytesIO()
+        im.save(buf, "JPEG", quality=100, subsampling=2)
+        base = buf.getvalue()
+        for qv in (1, 2, 8, 32):
+            b = bytearray(base)
+            i = 0
+            while True:                                 # every DQT segment: 8-bit tables, entries -> qv
+                i = b.find(b"\xff\xdb", i)
+                if i < 0:
+                    break
+                n = (b[i + 2] << 8 | b[i + 3]) - 2
+                for t in range(n // 65):
+                    b[i + 5 + 65 * t:i + 5 + 65 * t + 64] = bytes([qv]) * 64
+                i += 2 + n
+            out.append((f"dqt{qv}_{'gray' if gray else 'rgb'}_16x16", bytes(b)))
+    for name, data, decline in jpeg_corpus(seed, max_pixels=64 * 48):
+        if decline is not None or "64x48" not in name:
+            continue
+        s0 = parse(data).scan_data
+        for off in range(s0, len(data) - 2, max(1, (len(data) - 2 - s0) // 12)):
+            for bit in (0, 2, 5):
+                b = bytearray(data)
+                b[off] ^= 1 << bit
+                out.append((f"{name}_flip{off}.{bit}", bytes(b)))
+    return out

@@ -29,6 +29,7 @@ from PIL import Image
 
 from . import cabi
 from .cabi import call
+from .preprocess import DeviceImage, open_inputs
 from .matcher import RegressionMatcher
 from .packing import fold_bn
 from .sampling import kde, sample_device
@@ -354,7 +355,10 @@ class TinyRoMa:
 
     # ---- inputs ---------------------------------------------------------------------------------------
     def _to_tensor(self, im):
-        """torchvision ToTensor of an "RGB" or "L" PIL image: [1, C, H, W] fp32 in [0, 1] on the device."""
+        """torchvision ToTensor of an "RGB" or "L" PIL image (or of the same bytes decoded on the device): [1, C, H, W] fp32 in
+        [0, 1] on the device."""
+        if isinstance(im, DeviceImage):
+            return im.raw.permute(2, 0, 1)[None].float().div(255)
         if im.mode not in ("RGB", "L"):
             raise NotImplementedError(f"TinyRoMa: PIL images of mode {im.mode!r} are not supported (RGB or L)")
         arr = torch.from_numpy(np.array(im, copy=True))
@@ -371,7 +375,9 @@ class TinyRoMa:
     # ---- public API -----------------------------------------------------------------------------------
     @torch.inference_mode()
     def match_from_path(self, im0_path, im1_path):
-        return self.match(Image.open(im0_path), Image.open(im1_path))
+        # JPEG files are decoded on the device ("RGB" or "L", as Image.open gives them); other files take Image.open
+        im0, im1 = open_inputs([im0_path, im1_path], self._device, rgb=False)
+        return self.match(im0, im1)
 
     @torch.inference_mode()
     def match(self, im0, im1, *args, batched=True):
@@ -379,7 +385,7 @@ class TinyRoMa:
         return [H0,W0,4] / [H0,W0]."""
         if isinstance(im0, (str, Path, os.PathLike)):
             return self.match_from_path(im0, im1)
-        if isinstance(im0, Image.Image):
+        if isinstance(im0, (Image.Image, DeviceImage)):
             batched = False
             im0, im1 = self._to_tensor(im0), self._to_tensor(im1)
         im0, im1 = self._check(im0), self._check(im1)
