@@ -476,6 +476,55 @@ typedef struct {
 int romab200_jpeg_entropy(const rb_jpeg_args* args, void* stream);
 int romab200_jpeg_pixels(const rb_jpeg_args* args, void* stream);
 
+/* ---- relative pose: `estimate_pose` (romatch/utils/utils.py:30-51) = cv2.findEssentialMat (five-point RANSAC) + cv2.recoverPose ----
+ * B pairs with ragged point counts, packed: pair b owns points [offsets[b], offsets[b+1]).  All arithmetic is float64.
+ *   romab200_pose_hypotheses  normalises every point, xn = inv(K[:2,:2]) (x - K[:2,2]) with the closed-form 2x2 inverse
+ *                             (utils.py:33-37), then draws and solves the RB_POSE_ROUND hypotheses of round `round`:
+ *                             hypothesis h of pair b takes 5 distinct indices from Philox4x32-10 with key (seed lo, seed hi) and
+ *                             counter (h, b, s, 0), s = 0, 1, ...; the four words of each block are used in order, word w
+ *                             gives index (w * n) >> 32, a repeated index is skipped.  Nister's five-point solver gives up
+ *                             to RB_POSE_MAX_SOL essential matrices, unit Frobenius norm, largest-magnitude entry positive.
+ *                             A pair with n == 5 solves its 5 points once (hypothesis 0).
+ *   romab200_pose_score       inlier counts of every solution: OpenCV's E error (Sampson) in float64 without contraction,
+ *                             rounded to float, <= (float)(thresh^2); point slices over grid.y, partial counts, no atomics.
+ *   romab200_pose_select      one thread per pair replays OpenCV's sequential RANSAC loop over the round (best model changes
+ *                             iff count > max(best, 4), niters = RANSACUpdateNumIters(conf, (n - count) / n, 5, niters), stop
+ *                             at iter >= niters), keeps the best E and sets running[0] when a pair needs another round.
+ *   romab200_pose_recover     recoverPose(E, xn0, xn1, I, 1e9, mask) on the best E (n == 5: on every solution in turn, the
+ *                             mask carried from one call to the next, as the reference's loop does): SVD decomposition,
+ *                             DLT triangulation of the four (R, +-t), chirality and distance tests, OpenCV's candidate order.
+ * The caller zero-fills `state` before round 0 and calls hypotheses / score / select for rounds 0, 1, ... while
+ * running[0] != 0 and round * RB_POSE_ROUND < max_iters, then recover once. */
+#define RB_POSE_ROUND 1024
+#define RB_POSE_MAX_SOL 10
+#define RB_POSE_MAX_SPLITS 16
+#define RB_POSE_STATE 8       /* state[b, :]: iter, niters, best count, best hypothesis, best solution, E to recover, running, n */
+typedef struct {
+    int32_t batch;
+    const double* x0; const double* x1;   /* [total, 2] pixel coordinates in image 0 / image 1 */
+    const int64_t* offsets;               /* [batch + 1] */
+    const double* K;                      /* [batch, 2, 3, 3]: K0, K1 of each pair */
+    int64_t max_n;                        /* largest pair (sizes the point slices of the score) */
+    double thresh, conf;
+    int32_t max_iters, round;
+    uint64_t seed;
+    double* xn;                           /* [total, 4] normalised (x0, y0, x1, y1) */
+    int32_t* sample;                      /* [batch, RB_POSE_ROUND, 5] drawn indices of the round */
+    double* E;                            /* [batch, RB_POSE_ROUND, RB_POSE_MAX_SOL, 9] solutions of the round, row-major */
+    int32_t* nsol;                        /* [batch, RB_POSE_ROUND] */
+    int32_t* counts;                      /* [batch, RB_POSE_MAX_SPLITS, RB_POSE_MAX_SOL, RB_POSE_ROUND] partial inlier counts */
+    int32_t* state;                       /* [batch, RB_POSE_STATE] */
+    double* best_E;                       /* [batch, RB_POSE_MAX_SOL, 9] */
+    int32_t* running;                     /* [1] */
+    double* R; double* t;                 /* [batch, 3, 3], [batch, 3] */
+    uint8_t* ok;                          /* [batch] */
+    uint8_t* mask;                        /* [total] */
+} rb_pose_args;
+int romab200_pose_hypotheses(const rb_pose_args* args, void* stream);
+int romab200_pose_score(const rb_pose_args* args, void* stream);
+int romab200_pose_select(const rb_pose_args* args, void* stream);
+int romab200_pose_recover(const rb_pose_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -28,7 +28,7 @@ SAMPLE_IDENTITY, SAMPLE_THRESHOLD, SAMPLE_BALANCE = 0, 1, 2
 DTYPE_CODE = {torch.float32: RB_F32, torch.float16: RB_F16, torch.bfloat16: RB_BF16}
 
 _CTYPES = {
-    "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "float": ctypes.c_float,
+    "int32_t": ctypes.c_int32, "int64_t": ctypes.c_int64, "uint64_t": ctypes.c_uint64, "float": ctypes.c_float, "double": ctypes.c_double,
 }
 
 
@@ -106,6 +106,7 @@ launch_count = 0      # number of C-ABI calls made (bench.py reports kernel laun
 # For every struct: tensor field -> the field that carries its dtype code (or a fixed torch dtype).
 _CODE_DTYPE = {RB_F32: torch.float32, RB_F16: torch.float16, RB_BF16: torch.bfloat16, RB_F16S: torch.float16}
 _F32 = torch.float32
+_F64 = torch.float64
 _FIELD_DTYPES = {
     "rb_gemm_args": {"A": "dtype_ab", "B": "dtype_ab", "A_lo": torch.float16, "B_lo": torch.float16, "C": "dtype_c", "C_lo": torch.float16,
                      "R": "dtype_r", "bias": _F32, "col_scale": _F32, "norm_a": _F32, "norm_b": _F32},
@@ -148,6 +149,9 @@ _FIELD_DTYPES = {
     "rb_jpeg_args": {"stream": torch.uint8, "desc": torch.int64, "tables": torch.int32, "comp": torch.uint8, "chunks": torch.int32,
                      "istart": torch.int32, "exits": torch.int64, "counts": torch.int32, "coef": torch.int16, "state": torch.int32,
                      "flags": torch.int32, "planes": torch.uint8, "out": torch.uint8},
+    "rb_pose_args": {"x0": _F64, "x1": _F64, "offsets": torch.int64, "K": _F64, "xn": _F64, "sample": torch.int32, "E": _F64, "nsol": torch.int32,
+                     "counts": torch.int32, "state": torch.int32, "best_E": _F64, "running": torch.int32, "R": _F64, "t": _F64, "ok": torch.uint8,
+                     "mask": torch.uint8},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}}

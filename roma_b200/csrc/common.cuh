@@ -47,6 +47,17 @@ __device__ __forceinline__ void store_any(void* p, int64_t i, int dtype, float v
     else ((__nv_bfloat16*)p)[i] = __float2bfloat16_rn(v);
 }
 
+// Philox4x32-10 (Salmon et al. 2011, Random123): the four output words of counter c under key (k0, k1)
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint64_t p0 = (uint64_t)0xD2511F53u * c.x, p1 = (uint64_t)0xCD9E8D57u * c.z;
+        c = make_uint4((uint32_t)(p1 >> 32) ^ c.y ^ k0, (uint32_t)p1, (uint32_t)(p0 >> 32) ^ c.w ^ k1, (uint32_t)p0);
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    return c;
+}
+
 // bytes per element of one plane (RB_F16S = two fp16 planes of the same pitch)
 __host__ __device__ __forceinline__ int dtype_size(int dtype) { return dtype == RB_F32 ? 4 : 2; }
 

@@ -18,25 +18,9 @@
 
 namespace rb {
 
-__device__ __forceinline__ uint32_t mulhilo32(uint32_t a, uint32_t b, uint32_t* hi) {
-    const uint64_t p = (uint64_t)a * b;
-    *hi = (uint32_t)(p >> 32);
-    return (uint32_t)p;
-}
-
-// Philox4x32-10 (Salmon et al. 2011): counter (c0, c1, 0, 0), key (k0, k1); returns the first output word
+// Philox4x32-10: counter (c0, c1, 0, 0), key (k0, k1); returns the first output word
 __device__ __forceinline__ uint32_t philox_u32(uint32_t c0, uint32_t c1, uint32_t k0, uint32_t k1) {
-    uint32_t c[4] = {c0, c1, 0u, 0u};
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        uint32_t hi0, hi1;
-        const uint32_t lo0 = mulhilo32(0xD2511F53u, c[0], &hi0);
-        const uint32_t lo1 = mulhilo32(0xCD9E8D57u, c[2], &hi1);
-        const uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
-        c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    return c[0];
+    return philox4x32_10(make_uint4(c0, c1, 0u, 0u), k0, k1).x;
 }
 
 // weight transforms (matcher.py:604-607, 622-625)

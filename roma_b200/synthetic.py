@@ -308,3 +308,35 @@ def jpeg_edits(seed: int = 0):
                 b[off] ^= 1 << bit
                 out.append((f"{name}_flip{off}.{bit}", bytes(b)))
     return out
+
+
+def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, width: int = 1600, height: int = 1200):
+    """A seeded calibrated two-view scene for the pose estimator: focal lengths near 1200 px, a 5-20 degree rotation about a
+    random axis, a unit baseline in a random direction, `n` points seen by camera 0 at depths 6-14, Gaussian pixel noise of
+    `noise` px in both images, and a fraction `outlier_frac` of correspondences whose second point is uniform in image 1.
+    Returns float64 numpy arrays: kpts0, kpts1 [n, 2], K0, K1 [3, 3], R [3, 3], t [3] (x1 ~ K1 (R X + t))."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+
+    def intrinsics():
+        f = rng.uniform(1100.0, 1300.0)
+        return np.array([[f, 0.0, width / 2 + rng.uniform(-20, 20)], [0.0, f * rng.uniform(0.98, 1.02), height / 2 + rng.uniform(-20, 20)],
+                         [0.0, 0.0, 1.0]])
+
+    K0, K1 = intrinsics(), intrinsics()
+    axis = rng.normal(size=3)
+    axis /= np.linalg.norm(axis)
+    ang = np.deg2rad(rng.uniform(5.0, 20.0))
+    S = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+    R = np.eye(3) + np.sin(ang) * S + (1 - np.cos(ang)) * S @ S
+    t = rng.normal(size=3)
+    t /= np.linalg.norm(t)
+    px = np.c_[rng.uniform(0, width, n), rng.uniform(0, height, n), np.ones(n)]
+    X = (np.linalg.inv(K0) @ px.T).T * rng.uniform(6.0, 14.0, n)[:, None]
+    x1 = (K1 @ (X @ R.T + t).T).T
+    kpts0 = px[:, :2] + rng.normal(scale=noise, size=(n, 2))
+    kpts1 = x1[:, :2] / x1[:, 2:] + rng.normal(scale=noise, size=(n, 2))
+    out = rng.random(n) < outlier_frac
+    kpts1[out] = np.c_[rng.uniform(0, width, out.sum()), rng.uniform(0, height, out.sum())]
+    return {"kpts0": kpts0, "kpts1": kpts1, "K0": K0, "K1": K1, "R": R, "t": t}
