@@ -525,6 +525,65 @@ int romab200_pose_score(const rb_pose_args* args, void* stream);
 int romab200_pose_select(const rb_pose_args* args, void* stream);
 int romab200_pose_recover(const rb_pose_args* args, void* stream);
 
+/* ---- homography: cv2.findHomography(pos_a, pos_b, cv2.RANSAC, ...) of the HPatches harness
+ *      (romatch/benchmarks/hpatches_sequences_homog_benchmark.py:80-86), OpenCV 4.13's estimator with the sample stream replaced ----
+ * B pairs with ragged point counts, packed: pair b owns points [offsets[b], offsets[b+1]).  The points are float32, as cv2 converts them.
+ *   romab200_homography_hypotheses  one thread per hypothesis of round `round`.  Hypothesis h of pair b, attempt a (a = 0, 1, ...)
+ *                             draws 4 distinct indices from Philox4x32-10 with key (seed lo, seed hi) and counter (h, b, a, s),
+ *                             s = 0, 1, ...; the four words of each block are used in order, word w gives index (w * n) >> 32, a
+ *                             repeated index is skipped.  The attempt is rejected, and attempt a + 1 drawn, when OpenCV's checkSubset
+ *                             fails: haveCollinearPoints on either image (the last point against every pair of earlier ones,
+ *                             |dx2 dy1 - dy2 dx1| <= FLT_EPSILON (|dx1| + |dy1| + |dx2| + |dy2|), differences taken in float, the test
+ *                             in double), or the signs of det(A) det(B) over the triples 012, 123, 023, 130 are not all equal.  After
+ *                             RB_HOMOG_MAX_ATTEMPTS rejections the hypothesis is "not found" (status -1).  Otherwise the 4 points are
+ *                             solved with OpenCV's normalisation (centroid, scale = count / sum |x - c| per axis, no model when a sum is
+ *                             below DBL_EPSILON) and the null vector of the normalised 8x9 system by Gauss-Jordan with partial pivoting
+ *                             (no model on a pivot that is not finite or below 1e-12 of the first), de-normalised and multiplied by
+ *                             1 / H[2][2] (status 1; 0 = no model).  A pair with n == 4 solves its 4 points once (hypothesis 0, no check).
+ *   romab200_homography_score  inlier counts: OpenCV's computeError in float32 with every operation rounded separately, H cast to
+ *                             float, ww = 1 / (h6 x + h7 y + 1), dx = (h0 x + h1 y + h2) ww - x', err = dx^2 + dy^2 <= (float)(thresh^2);
+ *                             point slices over grid.y, integer partial counts, no atomics.
+ *   romab200_homography_select one warp per pair replays OpenCV's sequential loop over the round, 32 hypotheses per step: the best
+ *                             model changes iff count > max(best, 3), then niters = RANSACUpdateNumIters(conf, (n - count) / n, 4, niters);
+ *                             a "not found" hypothesis ends the loop (at iteration 0: no model); the loop stops at iter >= niters.
+ *                             Sets running[0] when a pair needs another round.
+ *   romab200_homography_refine one CTA per pair: the mask of the best model (the score's test), then (n > 4) the normalised DLT on
+ *                             all inliers (the smallest eigenvector of the 9x9 L^T L, cyclic Jacobi) and at most 10 Levenberg-Marquardt
+ *                             steps on the 8 parameters with H[2][2] = 1 (OpenCV's HomographyRefineCallback residual, in double).  Every
+ *                             sum over the inliers runs in a fixed order.  method == 0: the same on all points, without RANSAC.
+ *                             For n > 4 the returned mask is the inlier set of the refined model by the score's test, which is what
+ *                             cv2 4.13 returns (n == 4: all ones).
+ * The caller zero-fills `state` before round 0 and calls hypotheses / score / select for rounds 0, 1, ... while running[0] != 0 and
+ * round * RB_HOMOG_ROUND < max_iters, then refine once (method 0: refine only). */
+#define RB_HOMOG_ROUND 2048
+#define RB_HOMOG_MAX_SPLITS 32
+#define RB_HOMOG_MAX_ATTEMPTS 10000
+#define RB_HOMOG_STATE 8      /* state[b, :]: iter, niters, best count, best hypothesis, running, n, failed, unused */
+typedef struct {
+    int32_t batch;
+    const float* src; const float* dst;   /* [total, 2] points in image A / image B */
+    const int64_t* offsets;               /* [batch + 1] */
+    int64_t max_n;                        /* largest pair (sizes the point slices of the score) */
+    double thresh, conf;
+    int32_t max_iters, round, method;     /* method: 0 (least squares on all points) or 8 (RANSAC) */
+    uint64_t seed;
+    int32_t* sample;                      /* [batch, RB_HOMOG_ROUND, 4] drawn indices of the round */
+    int32_t* attempts;                    /* [batch, RB_HOMOG_ROUND] rejected attempts before the drawn subset */
+    int32_t* status;                      /* [batch, RB_HOMOG_ROUND]: 1 model, 0 no model, -1 not found */
+    double* H;                            /* [batch, RB_HOMOG_ROUND, 9] models of the round, row-major */
+    int32_t* counts;                      /* [batch, RB_HOMOG_MAX_SPLITS, RB_HOMOG_ROUND] partial inlier counts */
+    int32_t* state;                       /* [batch, RB_HOMOG_STATE] */
+    double* best_H;                       /* [batch, 9] the best RANSAC model */
+    int32_t* running;                     /* [1] */
+    double* out_H;                        /* [batch, 9] the refined model */
+    uint8_t* ok;                          /* [batch] */
+    uint8_t* mask;                        /* [total] */
+} rb_homography_args;
+int romab200_homography_hypotheses(const rb_homography_args* args, void* stream);
+int romab200_homography_score(const rb_homography_args* args, void* stream);
+int romab200_homography_select(const rb_homography_args* args, void* stream);
+int romab200_homography_refine(const rb_homography_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,7 +22,7 @@ def __getattr__(name):
     if name == "decode_jpeg":
         from .jpeg import decode_jpeg
         return decode_jpeg
-    if name in ("estimate_pose", "estimate_pose_batched"):
+    if name in ("estimate_pose", "estimate_pose_batched", "find_homography", "find_homography_batched", "RANSAC"):
         from . import geometry
         return getattr(geometry, name)
     raise AttributeError(name)

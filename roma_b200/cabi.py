@@ -152,6 +152,9 @@ _FIELD_DTYPES = {
     "rb_pose_args": {"x0": _F64, "x1": _F64, "offsets": torch.int64, "K": _F64, "xn": _F64, "sample": torch.int32, "E": _F64, "nsol": torch.int32,
                      "counts": torch.int32, "state": torch.int32, "best_E": _F64, "running": torch.int32, "R": _F64, "t": _F64, "ok": torch.uint8,
                      "mask": torch.uint8},
+    "rb_homography_args": {"src": _F32, "dst": _F32, "offsets": torch.int64, "sample": torch.int32, "attempts": torch.int32, "status": torch.int32,
+                           "H": _F64, "counts": torch.int32, "state": torch.int32, "best_H": _F64, "running": torch.int32, "out_H": _F64,
+                           "ok": torch.uint8, "mask": torch.uint8},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}}

@@ -13,7 +13,7 @@
 //   recover    one CTA per pair: 3x3 SVD of E (Jacobi on E^T E), linear (DLT) triangulation of every point for the four
 //              (R, +-t) with the smallest eigenvector of A^T A (4x4 Jacobi), OpenCV's chirality / distance tests.
 // Everything is deterministic: no atomics, no order-dependent sums.
-#include "common.cuh"
+#include "geometry.cuh"
 
 namespace rb {
 
@@ -532,19 +532,6 @@ __global__ void __launch_bounds__(PS_THREADS) pose_score_kernel(rb_pose_args a, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------- select
-// cv::RANSACUpdateNumIters(p, ep, 5, maxIters), with (1 - ep)^5 as four products
-__device__ __forceinline__ int ransac_update_num_iters(double p, double ep, int max_iters) {
-    p = fmin(fmax(p, 0.0), 1.0);
-    ep = fmin(fmax(ep, 0.0), 1.0);
-    double num = fmax(1.0 - p, 2.2250738585072014e-308);
-    const double q = 1.0 - ep;
-    double denom = 1.0 - q * q * q * q * q;
-    if (denom < 2.2250738585072014e-308) return 0;
-    num = log(num);
-    denom = log(denom);
-    return denom >= 0.0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
-}
-
 __global__ void __launch_bounds__(128) pose_select_kernel(rb_pose_args a, int splits) {
     rb::pdl_wait();
     const int b = blockIdx.x * 128 + threadIdx.x;
@@ -576,7 +563,7 @@ __global__ void __launch_bounds__(128) pose_select_kernel(rb_pose_args a, int sp
                 best = cnt;
                 st[ST_HYP] = iter; st[ST_SOL] = s;
                 for (int i = 0; i < 9; ++i) a.best_E[(int64_t)b * PS_SOL * 9 + i] = a.E[((slot0 + hl) * PS_SOL + s) * 9 + i];
-                niters = ransac_update_num_iters(a.conf, (double)(n - cnt) / (double)n, niters);
+                niters = ransac_update_num_iters<5>(a.conf, (double)(n - cnt) / (double)n, niters);
             }
         }
     }
@@ -586,43 +573,6 @@ __global__ void __launch_bounds__(128) pose_select_kernel(rb_pose_args a, int sp
 }
 
 // ---------------------------------------------------------------------------------------------------------------- recover
-// cyclic Jacobi on a symmetric N x N matrix: on return the columns of V are eigenvectors, diag(A) the eigenvalues
-template <int N>
-__device__ __forceinline__ void jacobi_eig(double (&A)[N][N], double (&V)[N][N], int sweeps) {
-#pragma unroll
-    for (int i = 0; i < N; ++i)
-#pragma unroll
-        for (int j = 0; j < N; ++j) V[i][j] = i == j ? 1.0 : 0.0;
-#pragma unroll 1
-    for (int sw = 0; sw < sweeps; ++sw) {
-#pragma unroll
-        for (int p = 0; p < N - 1; ++p)
-#pragma unroll
-            for (int q = p + 1; q < N; ++q) {
-                const double apq = A[p][q];
-                if (apq == 0.0) continue;
-                const double theta = (A[q][q] - A[p][p]) / (2.0 * apq);
-                const double tt = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-                const double c = 1.0 / sqrt(tt * tt + 1.0), s = tt * c;
-#pragma unroll
-                for (int k = 0; k < N; ++k) {
-                    const double akp = A[k][p], akq = A[k][q];
-                    A[k][p] = c * akp - s * akq; A[k][q] = s * akp + c * akq;
-                }
-#pragma unroll
-                for (int k = 0; k < N; ++k) {
-                    const double apk = A[p][k], aqk = A[q][k];
-                    A[p][k] = c * apk - s * aqk; A[q][k] = s * apk + c * aqk;
-                }
-#pragma unroll
-                for (int k = 0; k < N; ++k) {
-                    const double vkp = V[k][p], vkq = V[k][q];
-                    V[k][p] = c * vkp - s * vkq; V[k][q] = s * vkp + c * vkq;
-                }
-            }
-    }
-}
-
 // cv::decomposeEssentialMat: E = U diag V^T with det U = det V = 1, R1 = U W V^T, R2 = U W^T V^T, t = U[:, 2]
 __device__ void decompose_essential(const double* E, double (&R1)[9], double (&R2)[9], double (&tv)[3]) {
     double A[3][3], V[3][3];

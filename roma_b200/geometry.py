@@ -1,4 +1,5 @@
-"""Relative pose on the device: a drop-in for `romatch.utils.estimate_pose` (romatch/utils/utils.py:30-51).
+"""Two-view geometry on the device: relative pose, a drop-in for `romatch.utils.estimate_pose` (romatch/utils/utils.py:30-51),
+and homographies, a drop-in for the `cv2.findHomography` call of the HPatches harness.
 
 The reference normalises the keypoints with the intrinsics, runs `cv2.findEssentialMat` (plain RANSAC over the five-point
 solver) and `cv2.recoverPose` on one host core.  Here the same estimator runs in `csrc/pose.cu`: the same E error, threshold
@@ -8,6 +9,13 @@ is deterministic for a given seed.  There is no CPU fallback and cv2 is never ca
 
     from roma_b200 import estimate_pose
     R, t, mask = estimate_pose(kpts0, kpts1, K0, K1, norm_thresh)
+
+`find_homography` runs OpenCV 4.13's `findHomography(..., RANSAC)` in `csrc/homography.cu`: the same subset checks, normalised
+four-point solver, float32 reprojection error, sequential best-model replay and stopping rule, and least-squares refinement of
+the final model.  Again only the stream of minimal samples differs (Philox4x32-10 keyed by `seed`; include/romab200.h).
+
+    from roma_b200 import find_homography, RANSAC
+    H, mask = find_homography(pos_a, pos_b, RANSAC, 3.0, confidence=0.99999)
 """
 from __future__ import annotations
 
@@ -22,9 +30,9 @@ from . import cabi
 ROUND, MAX_SOL, MAX_SPLITS, STATE = 1024, 10, 16, 8
 
 
-def _device():
+def _device(what="estimate_pose"):
     if not torch.cuda.is_available():
-        raise RuntimeError("estimate_pose runs on the GPU only (there is no CPU fallback): no CUDA device is available")
+        raise RuntimeError(f"{what} runs on the GPU only (there is no CPU fallback): no CUDA device is available")
     return torch.device("cuda", torch.cuda.current_device())
 
 
@@ -124,3 +132,121 @@ def estimate_pose(kpts0, kpts1, K0, K1, norm_thresh, conf=0.99999, *, max_iters=
     if not bool(ok[0]):
         return None
     return R[0], t[0], masks[0]
+
+
+# ---- homographies --------------------------------------------------------------------------------------------------------
+RANSAC = 8                      # cv2.RANSAC
+# include/romab200.h: RB_HOMOG_ROUND, RB_HOMOG_MAX_SPLITS, RB_HOMOG_STATE
+HOMOG_ROUND, HOMOG_MAX_SPLITS, HOMOG_STATE = 2048, 32, 8
+# cv2's other findHomography methods, which are not restated here
+_HOMOG_UNSUPPORTED = {4: "LMEDS", 16: "RHO", 32: "USAC_DEFAULT", 33: "USAC_PARALLEL", 34: "USAC_FM_8PTS", 35: "USAC_FAST",
+                      36: "USAC_ACCURATE", 37: "USAC_PROSAC", 38: "USAC_MAGSAC"}
+
+
+def _homog_points(p, dev):
+    """[N, 2] or [N, 1, 2] points -> float32 [N, 2] on `dev`, rounded to float32 first as cv2 does."""
+    t = p if isinstance(p, torch.Tensor) else torch.as_tensor(np.asarray(p))
+    if t.dim() == 3 and t.shape[1] == 1:
+        t = t[:, 0]
+    if t.dim() != 2 or t.shape[1] != 2:
+        raise ValueError(f"points must be [N, 2] or [N, 1, 2], got {tuple(t.shape)}")
+    if t.dtype.is_complex or t.dtype == torch.bool:
+        raise TypeError(f"points must be real numbers, got {t.dtype}")
+    return t.to(torch.float32).to(dev).contiguous()
+
+
+def _homog_args(method, thr, conf, max_iters):
+    """Mirrors cv2.findHomography's argument handling; returns (method, threshold, confidence, maxIters) as the estimator uses them."""
+    method = int(method)
+    if method in _HOMOG_UNSUPPORTED:
+        raise NotImplementedError(f"find_homography implements method 0 and RANSAC only, not {_HOMOG_UNSUPPORTED[method]}")
+    if method not in (0, RANSAC):
+        raise ValueError(f"unknown estimation method {method}")
+    thr = float(thr)
+    if thr <= 0:                # OpenCV substitutes its default threshold
+        thr = 3.0
+    conf = float(conf)
+    if method == RANSAC and not 0 < conf < 1:
+        raise ValueError(f"confidence must lie in (0, 1), got {conf}")
+    return method, thr, conf, max(int(max_iters), 1)
+
+
+def _homog_launch(src, dst, offsets, max_n, method, thr, conf, max_iters, seed):
+    """Enqueues the whole estimate on the current stream.  src, dst: float32 [total, 2] device tensors, offsets: int64 [B + 1].
+    With max_iters <= HOMOG_ROUND this is one round and reads nothing back, so it can be captured in a CUDA graph; each further
+    round costs one 4-byte read of the `running` flag.  Returns the buffers (out_H, ok, mask, state, best_H, sample, attempts,
+    status, H, counts)."""
+    dev = src.device
+    B = offsets.numel() - 1
+    total = src.shape[0]
+    f64, i32 = dict(device=dev, dtype=torch.float64), dict(device=dev, dtype=torch.int32)
+    ransac = method == RANSAC
+    R = HOMOG_ROUND if ransac else 1
+    buf = dict(
+        sample=torch.empty(B, R, 4, **i32), attempts=torch.empty(B, R, **i32), status=torch.empty(B, R, **i32),
+        H=torch.empty(B, R, 9, **f64), counts=torch.empty(B, HOMOG_MAX_SPLITS if ransac else 1, R, **i32),
+        state=torch.zeros(B, HOMOG_STATE, **i32), best_H=torch.zeros(B, 9, **f64), running=torch.zeros(1, **i32),
+        out_H=torch.empty(B, 9, **f64), ok=torch.empty(B, device=dev, dtype=torch.uint8),
+        mask=torch.empty(max(total, 1), device=dev, dtype=torch.uint8))
+    kw = dict(batch=B, src=src, dst=dst, offsets=offsets, max_n=int(max_n), thresh=float(thr), conf=float(conf), max_iters=int(max_iters),
+              method=int(method), seed=int(seed) & (2 ** 64 - 1), round=0, **buf)
+    if ransac:
+        rounds = (int(max_iters) + HOMOG_ROUND - 1) // HOMOG_ROUND
+        for r in range(rounds):
+            kw["round"] = r
+            cabi.call("romab200_homography_hypotheses", "rb_homography_args", **kw)
+            cabi.call("romab200_homography_score", "rb_homography_args", **kw)
+            cabi.call("romab200_homography_select", "rb_homography_args", **kw)
+            if r + 1 < rounds and int(buf["running"].item()) == 0:
+                break
+        kw["round"] = 0
+    cabi.call("romab200_homography_refine", "rb_homography_args", **kw)
+    return buf
+
+
+def find_homography_batched(src_list, dst_list, method=RANSAC, ransacReprojThreshold=3, maxIters=2000, confidence=0.995, *, seed=0):
+    """`find_homography` for B pairs in one launch set.  src_list, dst_list: B arrays / tensors [N_b, 2] or [N_b, 1, 2] (ragged N).
+    Pair b draws its samples from the stream keyed by (seed, b), so pair 0 is bit-identical to `find_homography` of that pair alone.
+    Returns (H [B, 3, 3] float64, ok [B] bool, masks: list of uint8 [N_b, 1]); numpy inputs give numpy outputs, tensors give
+    device tensors.  ok[b] is False where `find_homography` returns None, and for pairs of fewer than 4 points (mask all zero);
+    H[b] is zero there."""
+    if len(src_list) != len(dst_list) or len(src_list) == 0:
+        raise ValueError("src_list and dst_list must be non-empty and of the same length")
+    method, thr, conf, max_iters = _homog_args(method, ransacReprojThreshold, confidence, maxIters)
+    dev = _device("find_homography")
+    as_numpy = not isinstance(src_list[0], torch.Tensor)
+    ps = [_homog_points(p, dev) for p in src_list]
+    pd = [_homog_points(p, dev) for p in dst_list]
+    for a, b in zip(ps, pd):
+        if a.shape != b.shape:
+            raise ValueError(f"srcPoints and dstPoints differ in shape: {tuple(a.shape)} vs {tuple(b.shape)}")
+    B = len(ps)
+    ns = [a.shape[0] for a in ps]
+    offsets = torch.tensor(np.concatenate([[0], np.cumsum(ns)]), dtype=torch.int64, device=dev)
+    src = torch.cat(ps) if sum(ns) else torch.zeros(1, 2, dtype=torch.float32, device=dev)
+    dst = torch.cat(pd) if sum(ns) else torch.zeros(1, 2, dtype=torch.float32, device=dev)
+    buf = _homog_launch(src, dst, offsets, max(ns), method, thr, conf, max_iters, seed)
+    ok = buf["ok"].bool()
+    masks = [m.view(-1, 1) for m in buf["mask"][:sum(ns)].split(ns)]
+    H = buf["out_H"].view(B, 3, 3)
+    if as_numpy:
+        return H.cpu().numpy(), ok.cpu().numpy(), [m.cpu().numpy() for m in masks]
+    return H, ok, masks
+
+
+def find_homography(srcPoints, dstPoints, method=0, ransacReprojThreshold=3, mask=None, maxIters=2000, confidence=0.995, *, seed=0):
+    """Drop-in for `cv2.findHomography` with method 0 (least squares over all points) or RANSAC: the same signature, defaults and
+    return form.  Returns (H float64 [3, 3], mask uint8 [N, 1]): H is refined (normalised DLT, then Levenberg-Marquardt) on the
+    inliers of the best RANSAC hypothesis, and mask holds the inliers of the refined H, as cv2 4.13 returns them (all ones for 4
+    points); (None, zeros) when no model is found.  `mask` is accepted and
+    ignored, as in cv2's Python binding.  numpy in gives numpy out; tensors give device tensors.  Raises ValueError for fewer
+    than 4 points and NotImplementedError for LMEDS, RHO and the USAC methods."""
+    del mask
+    method, thr, conf, max_iters = _homog_args(method, ransacReprojThreshold, confidence, maxIters)
+    n = len(srcPoints)
+    if n < 4 or len(dstPoints) != n:
+        raise ValueError(f"find_homography needs the same number (>= 4) of source and destination points, got {n} and {len(dstPoints)}")
+    H, ok, masks = find_homography_batched([srcPoints], [dstPoints], method, thr, max_iters, conf, seed=seed)
+    if not bool(ok[0]):
+        return None, masks[0]
+    return H[0], masks[0]

@@ -340,3 +340,56 @@ def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, w
     out = rng.random(n) < outlier_frac
     kpts1[out] = np.c_[rng.uniform(0, width, out.sum()), rng.uniform(0, height, out.sum())]
     return {"kpts0": kpts0, "kpts1": kpts1, "K0": K0, "K1": K1, "R": R, "t": t}
+
+
+def planar_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, width: int = 640, height: int = 480):
+    """A seeded HPatches-like homography pair: H is a random perspective warp of the image that moves each corner by up to a
+    fifth of the image size, `n` points uniform in image A, their images under H with Gaussian noise of `noise` px, and a
+    fraction `outlier_frac` of correspondences whose second point is uniform in image B.  Returns float64 numpy arrays: src,
+    dst [n, 2], H [3, 3] (dst ~ H src), inlier [n] bool, and the image size (w, h)."""
+    import numpy as np
+
+    rng = np.random.default_rng(seed)
+    c = np.array([[0.0, 0.0], [0.0, height - 1.0], [width - 1.0, 0.0], [width - 1.0, height - 1.0]])
+    moved = c + rng.uniform(-0.2, 0.2, size=(4, 2)) * np.array([width, height])
+    A = []
+    for (x, y), (u, v) in zip(c, moved):
+        A.append([x, y, 1, 0, 0, 0, -u * x, -u * y, -u])
+        A.append([0, 0, 0, x, y, 1, -v * x, -v * y, -v])
+    H = np.linalg.svd(np.array(A))[2][-1].reshape(3, 3)
+    H = H / H[2, 2]
+    src = np.c_[rng.uniform(0, width, n), rng.uniform(0, height, n)]
+    p = np.c_[src, np.ones(n)] @ H.T
+    dst = p[:, :2] / p[:, 2:] + rng.normal(scale=noise, size=(n, 2))
+    out = rng.random(n) < outlier_frac
+    dst[out] = np.c_[rng.uniform(0, width, out.sum()), rng.uniform(0, height, out.sum())]
+    return {"src": src, "dst": dst, "H": H, "inlier": ~out, "size": (width, height)}
+
+
+def homography_corner_error(H_pred, H_gt, width: int, height: int):
+    """The HPatches harness's error (hpatches_sequences_homog_benchmark.py): the mean distance of the four image corners mapped by
+    the predicted and the true homography, divided by min(w, h) / 480.  A missing prediction (None) counts as infinite."""
+    import numpy as np
+
+    if H_pred is None:
+        return float("inf")
+    c = np.array([[0, 0, 1], [0, height - 1, 1], [width - 1, 0, 1], [width - 1, height - 1, 1]], dtype=np.float64)
+    a = c @ np.asarray(H_pred, dtype=np.float64).T
+    b = c @ np.asarray(H_gt, dtype=np.float64).T
+    d = np.linalg.norm(a[:, :2] / a[:, 2:] - b[:, :2] / b[:, 2:], axis=1).mean()
+    return float(d / (min(width, height) / 480.0))
+
+
+def homography_auc(errors, thresholds=(3, 5, 10)):
+    """Area under the recall-error curve up to each threshold (px), normalised to [0, 1], as the harness reports AUC@3/5/10."""
+    import numpy as np
+
+    errors = np.sort(np.r_[0.0, np.asarray(errors, dtype=np.float64)])
+    recall = np.r_[0.0, (np.arange(len(errors) - 1) + 1) / (len(errors) - 1)]
+    out = []
+    for th in thresholds:
+        last = np.searchsorted(errors, th)
+        r = np.r_[recall[:last], recall[last - 1]]
+        e = np.r_[errors[:last], th]
+        out.append(float(np.trapezoid(r, x=e) / th))
+    return out
