@@ -28,6 +28,7 @@ struct TcParams {
     int batch1;
     int ntaps, k_per_tap; int tap_rows[9];
     int tiles_m, tiles_n, total_tiles;
+    int band_m;                   // M-tiles per band of the tile order (tile_coords); tiles_m: plain m-fastest order
     int n_zero_to;                // columns [N, n_zero_to) of every stored row are written with zeros (pad up to a 16-byte granule)
     int64_t sc0, sc1, sr0, sr1, sna0, snb0;
     Epilogue epi;
@@ -172,8 +173,24 @@ __device__ __forceinline__ void epilogue8(const Epilogue& e, int m, int n, int64
     store8(e, orow * e.ldc + n, cnt, v);
 }
 
-// Persistent kernel: every CTA walks tiles t = blockIdx.x, blockIdx.x + gridDim.x, ... (m fastest, so CTAs that run together share
-// the same weight tile in L2).
+// Output tile of work index w: z outermost; inside one z, bands of p.band_m consecutive M-tiles (the last band may be shorter), each
+// band walked m-fastest over all tiles_n N-tiles.  band_m == tiles_m is the plain m-fastest order.
+__device__ __forceinline__ void tile_coords(const TcParams& p, int w, int& z, int& mt, int& nt) {
+    const int per_z = p.tiles_m * p.tiles_n;
+    z = w / per_z;
+    const int r = w - z * per_z;
+    const int m_lo = r / (p.band_m * p.tiles_n) * p.band_m;
+    const int rows = min(p.band_m, p.tiles_m - m_lo);
+    const int rb = r - m_lo * p.tiles_n;
+    nt = rb / rows;
+    mt = m_lo + (rb - nt * rows);
+}
+
+// Persistent kernel: every CTA walks work indices w = blockIdx.x, blockIdx.x + gridDim.x, ... in the order of tile_coords.  The
+// host picks the band height (launch_tc): m-fastest (one band), so that CTAs that run together share the weight tile in L2, unless
+// the activation A is too big to stay in L2 while the N-tiles sweep over it; then bands of about one wave of the grid read each
+// A row from HBM once while the weights stay resident.  Only the assignment of tiles to CTAs changes: every tile's result is
+// computed by the same instructions on the same data, so the results are bit-identical in either order.
 template <int BN, bool SPLIT, bool BF16, int TB>
 __global__ void __launch_bounds__(TC_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant__ CUtensorMap map_b,
@@ -190,7 +207,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int kblocks = (p.K + TC_BK - 1) / TC_BK;
-    const int tiles_per_z = p.tiles_m * p.tiles_n;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 2); }
@@ -208,8 +224,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
             const int kb_per_tap = p.ntaps > 1 ? p.k_per_tap / TC_BK : kblocks;
             uint32_t it = 0;
             for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-                const int z = tile / tiles_per_z, r = tile - z * tiles_per_z;
-                const int nt = r / p.tiles_m, mt = r - nt * p.tiles_m;
+                int z, mt, nt;
+                tile_coords(p, tile, z, mt, nt);
                 const int m0 = mt * TC_BM, n0 = nt * BN, z0 = z / p.batch1, z1 = z - z0 * p.batch1;
                 for (int kb = 0; kb < kblocks; ++kb, ++it) {
                     const int s = it % STAGES;
@@ -245,8 +261,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
     float acc2[SPLIT ? BN / 2 : 1];
     uint32_t it = 0;
     for (int tile = blockIdx.x; tile < p.total_tiles; tile += gridDim.x) {
-        const int z = tile / tiles_per_z, r = tile - z * tiles_per_z;
-        const int nt = r / p.tiles_m, mt = r - nt * p.tiles_m;
+        int z, mt, nt;
+        tile_coords(p, tile, z, mt, nt);
         const int m0 = mt * TC_BM, n0 = nt * BN, z0 = z / p.batch1, z1 = z - z0 * p.batch1;
         int prev = -1;
         for (int kb = 0; kb < kblocks; ++kb, ++it) {
@@ -385,6 +401,17 @@ static int launch_tc(const TcMaps& maps, TcParams& p, int zdim, int max_ctas, cu
     int resident = sm_count();
     if (max_ctas > 0 && max_ctas < resident) resident = max_ctas;
     const int grid = p.total_tiles < resident ? p.total_tiles : resident;
+    // Tile order.  m-fastest comes back to an A row once per N-tile, after a sweep over all of A (per z) and the C it writes: when
+    // A is more than half the L2, the row has been evicted and is read from HBM tiles_n times.  Bands of grid / tiles_n M-tiles
+    // (one wave: every CTA that reads a band's A rows runs at once) read A from HBM once; every band reads all of B, so B must
+    // stay resident beside the band (at most half the L2).  Measured with scripts/bench_gemm.py on the parity-mode step (H100,
+    // 50 MB L2): the refiner pointwise GEMMs at C = 569 / 1137 (A 45-212 MB) run 6-14% faster in bands, and launches with A
+    // between a half and one L2 (41-50 MB) from 3% slower to 27% faster, most of them faster; the ViT qkv / fc1 and decoder GEMMs (A <= 18 MB) keep m-fastest.
+    const int64_t a_bytes = (int64_t)p.M * (p.ntaps > 1 ? p.k_per_tap : p.K) * Cfg::NOPS * 2;
+    const int64_t b_bytes = (int64_t)p.N * p.K * Cfg::NOPS * 2;
+    const bool bands = p.tiles_n > 1 && 2 * a_bytes > l2_bytes() && 2 * b_bytes <= l2_bytes();
+    const int band_m = grid / p.tiles_n > 1 ? grid / p.tiles_n : 1;
+    p.band_m = bands && band_m < p.tiles_m ? band_m : p.tiles_m;
     cudaError_t err = rb::launch_pdl(kernel, dim3(grid), dim3(TC_THREADS), Cfg::SMEM, st, maps.a, maps.b, maps.a_lo, maps.b_lo, (const TcParams)p);
     if (err != cudaSuccess) { set_error("gemm_tc: launch failed: %s", cudaGetErrorString(err)); return 1; }
     return check_launch("gemm_tc");

@@ -111,4 +111,15 @@ inline int sm_count() {
     return n[dev];
 }
 
+// L2 cache bytes of the current device, queried once per device
+inline int64_t l2_bytes() {
+    static int n[64] = {};
+    const int dev = current_device() & 63;
+    if (!n[dev]) {
+        cudaDeviceGetAttribute(&n[dev], cudaDevAttrL2CacheSize, dev);
+        if (n[dev] <= 0) n[dev] = 50 << 20;
+    }
+    return n[dev];
+}
+
 }  // namespace rb

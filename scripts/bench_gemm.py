@@ -6,7 +6,9 @@
    `romab200_gemm` call the engine makes (by wrapping `roma_b200.engine.call`).  Each distinct launch is replayed `--reps` times from
    one CUDA graph, so the table holds device time only: shape, tile width, epilogue, output dtype, row map, ms per launch, TFLOP/s
    counted as 3 * 2MNK (three MMAs per k-step) and the share of the summed GEMM time.  GEMMs issued from inside the GP solve's C++
-   chain do not pass through Python and are not in the table.
+   chain do not pass through Python and are not in the table.  Per launch also the tile order (m-fastest or bands of M-tiles),
+   the compulsory HBM bytes (A once, B once, C, R), the bytes under the order used, achieved GB/s, and the least time at the
+   data-sheet HBM bandwidth and fp16 tensor rate: the larger of the two says whether the launch is HBM- or tensor-bound.
 2. K-sweep: for the step's dominant GEMM groups, times the same launch (same M, N, epilogue, output dtype and row map) on fresh
    operands at several K and fits t = a + b K.  The intercept `a` (per tile wave) is the fixed cost per tile, epilogue and set-up;
    the slope `b` gives the main-loop rate.
@@ -29,6 +31,8 @@ EPI = {0: "linear", 1: "coskernel"}
 ACT = {0: "none", 1: "relu", 2: "gelu"}
 DT = {0: "f32", 1: "f16", 2: "bf16", 3: "f16s"}
 ROWMAP = {0: "none", 1: "pad_keep", 2: "pad_to_compact", 3: "segment"}
+# NVIDIA H100 SXM data sheet (a card allowed 700 W): HBM3 bandwidth and dense fp16 tensor rate
+DATASHEET_HBM_GBS, DATASHEET_F16_TFLOPS = 3350.0, 989.0
 
 
 def tile_width(N, M, z, trans_b, split, sms, max_split_bn):
@@ -49,6 +53,45 @@ def tile_width(N, M, z, trans_b, split, sms, max_split_bn):
     if math.ceil(M / 128) * math.ceil(N / bn) * z < sms * 2 // 3:
         bn = 128
     return bn
+
+
+def operand_bytes(kw):
+    """HBM bytes of one pass over A (per z: rows x K-extent, the map of a 9-tap launch once), B (per z), C and R (all z)."""
+    M, N, K = kw["M"], kw["N"], kw["K"]
+    z = (kw.get("batch0") or 1) * (kw.get("batch1") or 1)
+    ntaps = kw.get("ntaps", 1) or 1
+    planes = 2 if kw.get("dtype_ab") == 3 else 1
+    es = {0: 4, 1: 2, 2: 2, 3: 4}                        # RB_F16S: two fp16 planes
+    a = M * (K // ntaps if ntaps > 1 else K) * planes * 2
+    b = N * K * planes * 2
+    c = M * N * z * es[kw.get("dtype_c", 0)]
+    r = M * N * z * es[kw.get("dtype_r", 0)] if kw.get("R") is not None else 0
+    return a, b, c, r
+
+
+def tile_order(kw, tiles_m, tiles_n, sms, l2, bands_enabled):
+    """(order, M-tiles per band) gemm_tc() picks (launch_tc in gemm_tc.cu); bands_enabled = False reproduces builds that always walk
+    the tiles m-fastest."""
+    z = (kw.get("batch0") or 1) * (kw.get("batch1") or 1)
+    a, b, _, _ = operand_bytes(kw)
+    resident = min(sms, kw["max_ctas"]) if kw.get("max_ctas") else sms
+    grid = min(tiles_m * tiles_n * z, resident)
+    band_m = max(1, grid // tiles_n)
+    if bands_enabled and tiles_n > 1 and 2 * a > l2 and 2 * b <= l2 and band_m < tiles_m:
+        return "bands", band_m
+    return "m_fastest", tiles_m
+
+
+def hbm_bytes(kw, order, tiles_n, n_bands, l2):
+    """(compulsory, scheduled) HBM bytes of one launch.  Compulsory: A once + B once + C + R (R is read even when it is C).
+    Scheduled, by the model the order rule rests on: m-fastest reads A once per N-tile when A exceeds half the L2 (the sweep over
+    all of A evicts a row before its next N-tile comes back to it); bands read A once and B once per band when B exceeds half the L2."""
+    a, b, c, r = operand_bytes(kw)
+    z = (kw.get("batch0") or 1) * (kw.get("batch1") or 1)
+    compulsory = (a + b) * z + c + r
+    a_reads = tiles_n if order == "m_fastest" and 2 * a > l2 else 1
+    b_reads = n_bands if order == "bands" and 2 * b > l2 else 1
+    return compulsory, (a * a_reads + b * b_reads) * z + c + r
 
 
 def gpu_info():
@@ -134,16 +177,22 @@ def time_launch(kw, reps, trials=5):
     return best
 
 
-def describe(kw, sms, max_split_bn):
+def describe(kw, sms, max_split_bn, l2, bands_enabled):
     M, N, K = kw["M"], kw["N"], kw["K"]
     z = (kw.get("batch0") or 1) * (kw.get("batch1") or 1)
     split = kw.get("dtype_ab") == 3
     bn = tile_width(N, M, z, kw.get("trans_b", 0), split, sms, max_split_bn)
-    tiles = math.ceil(M / 128) * math.ceil(N / bn) * z
+    tiles_m, tiles_n = math.ceil(M / 128), math.ceil(N / bn)
+    tiles = tiles_m * tiles_n * z
+    order, band_m = tile_order(kw, tiles_m, tiles_n, sms, l2, bands_enabled)
+    compulsory, scheduled = hbm_bytes(kw, order, tiles_n, math.ceil(tiles_m / band_m), l2)
     return dict(M=M, N=N, K=K, batch=z, ntaps=kw.get("ntaps", 1) or 1, trans_b=kw.get("trans_b", 0), operands=DT[kw.get("dtype_ab", 0)],
-                bn=bn, tiles=tiles, waves=math.ceil(tiles / sms), epi=EPI[kw.get("epi", 0)], act=ACT[kw.get("act", 0)],
+                bn=bn, tiles=tiles, tiles_n=tiles_n, waves=math.ceil(tiles / sms), order=order, band_m=band_m,
+                epi=EPI[kw.get("epi", 0)], act=ACT[kw.get("act", 0)],
                 out=DT[kw.get("dtype_c", 0)], rowmap=ROWMAP[kw.get("rowmap", 0)], residual=kw.get("R") is not None,
-                bias=kw.get("bias") is not None, col_scale=kw.get("col_scale") is not None)
+                residual_is_c=kw.get("R") is not None and _same(kw.get("R"), kw.get("C")),
+                bias=kw.get("bias") is not None, col_scale=kw.get("col_scale") is not None,
+                a_mb=operand_bytes(kw)[0] / 1e6, hbm_mb_compulsory=compulsory / 1e6, hbm_mb_scheduled=scheduled / 1e6)
 
 
 def sweep_case(kw, Ks):
@@ -177,13 +226,17 @@ def main():
     ap.add_argument("--reps", type=int, default=20, help="launches per CUDA graph in the per-launch table")
     ap.add_argument("--max-split-bn", type=int, default=144, choices=[128, 144],
                     help="widest split-fp16 tile of the build being measured (labels the table only)")
+    ap.add_argument("--no-bands", action="store_true",
+                    help="the build being measured always walks its tiles m-fastest (labels the table only)")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     import torch
     assert torch.cuda.is_available(), "bench_gemm.py needs a GPU"
     torch.cuda.set_device(0)
-    sms = torch.cuda.get_device_properties(0).multi_processor_count
-    doc = {"gpu": gpu_info(), "workload": f"parity-mode match() at {COARSE} -> {UPSAMPLE}, one symmetric pair"}
+    props = torch.cuda.get_device_properties(0)
+    sms, l2 = props.multi_processor_count, props.L2_cache_size
+    doc = {"gpu": dict(gpu_info(), l2_bytes=l2, datasheet_hbm_gbs=DATASHEET_HBM_GBS, datasheet_f16_tflops=DATASHEET_F16_TFLOPS),
+           "workload": f"parity-mode match() at {COARSE} -> {UPSAMPLE}, one symmetric pair"}
     model, calls = record_step()
 
     groups = {}
@@ -197,9 +250,15 @@ def main():
     for g in groups.values():
         kw = g["kw"]
         ms = time_launch(kw, args.reps)
-        d = describe(kw, sms, args.max_split_bn)
+        d = describe(kw, sms, args.max_split_bn, l2, not args.no_bands)
         flop = (3 if kw.get("dtype_ab") == 3 else 1) * 2.0 * d["M"] * d["N"] * d["K"] * d["batch"]
-        d.update(count=g["count"], ms=ms, ms_total=ms * g["count"], tflops=flop / (ms * 1e-3) / 1e12)
+        # least time at the data-sheet rates: which of the two bounds the launch (labelled as data-sheet figures)
+        ms_hbm = d["hbm_mb_scheduled"] * 1e6 / (DATASHEET_HBM_GBS * 1e9) * 1e3
+        ms_tc = flop / (DATASHEET_F16_TFLOPS * 1e12) * 1e3
+        d.update(count=g["count"], ms=ms, ms_total=ms * g["count"], tflops=flop / (ms * 1e-3) / 1e12,
+                 gbs_scheduled=d["hbm_mb_scheduled"] / ms, gbs_compulsory=d["hbm_mb_compulsory"] / ms,
+                 hbm_share_scheduled=d["hbm_mb_scheduled"] / ms / DATASHEET_HBM_GBS,
+                 datasheet_min_ms_hbm=ms_hbm, datasheet_min_ms_tc=ms_tc, bound="hbm" if ms_hbm > ms_tc else "tensor")
         rows.append(d)
     total = sum(r["ms_total"] for r in rows)
     for r in rows:
@@ -235,7 +294,7 @@ def main():
         Ks = [ntaps * k for k in ((64, 128, 256) if ntaps > 1 else (64, 128, 256, 512, 1024))]
         pts = sweep_case(kw, Ks)
         a, b = fit(pts)
-        d = describe(kw, sms, args.max_split_bn)
+        d = describe(kw, sms, args.max_split_bn, l2, not args.no_bands)
         t_at_k = a + b * kw["K"]
         sweep[name] = {"M": d["M"], "N": d["N"], "K_in_step": kw["K"], "bn": d["bn"], "tiles": d["tiles"], "waves": d["waves"],
                        "epi": d["epi"], "act": d["act"], "out": d["out"], "rowmap": d["rowmap"], "residual": d["residual"],
