@@ -272,6 +272,17 @@ typedef struct {
 } rb_refiner_block_c144_args;
 int romab200_refiner_block_c144(const rb_refiner_block_c144_args* args, void* stream);
 
+/* The same block in the parity mode: fp32 maps, split-fp16 pointwise GEMM.  Bit-identical to romab200_dwconv5x5_relu (fp32 in,
+ * RB_F16S out) followed by romab200_gemm (RB_F16S operands, fp32 out, bias), with the RB_F16S intermediate kept on chip.
+ * in/out [batch, h, w, ld] fp32 (in != out; ld % 8 == 0, ld >= 144); dw_weight [25][ldw] fp32 (BN folded);
+ * pw_weight / pw_weight_lo: the hi / lo fp16 planes of the RB_F16S weights [144][ld_pw] (ld_pw % 8 == 0, ld_pw >= 144);
+ * all pointers 16-byte aligned. */
+typedef struct {
+    const float* in; float* out; int64_t ld; const float* dw_weight; int64_t ldw; const float* dw_bias;
+    const void* pw_weight; const void* pw_weight_lo; int64_t ld_pw; const float* pw_bias; int32_t batch, h, w, c;
+} rb_refiner_block_c144_split_args;
+int romab200_refiner_block_c144_split(const rb_refiner_block_c144_split_args* args, void* stream);
+
 /* out_conv (fp32 1x1, C -> 3) + flow/certainty update (matcher.py:177-179, 496-506):
  * state[...,0] += scale_x * o0 ; state[...,1] += scale_y * o1 ; state[...,2] += o2 */
 typedef struct {

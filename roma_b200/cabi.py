@@ -129,6 +129,8 @@ _FIELD_DTYPES = {
     "rb_dwconv_args": {"in": "dtype", "weight": _F32, "bias": _F32, "out_lo": torch.float16},
     "rb_refiner_block_small_args": {"in": "dtype", "out": "dtype", "dw_weight": _F32, "dw_bias": _F32},
     "rb_refiner_block_c144_args": {"in": "dtype", "out": "dtype", "dw_weight": _F32, "dw_bias": _F32, "pw_weight": "dtype", "pw_bias": _F32},
+    "rb_refiner_block_c144_split_args": {"in": _F32, "out": _F32, "dw_weight": _F32, "dw_bias": _F32, "pw_weight": torch.float16,
+                                         "pw_weight_lo": torch.float16, "pw_bias": _F32},
     "rb_refiner_tail_args": {"d": "dtype", "weight": _F32, "bias": _F32, "state": _F32, "delta_out": _F32},
     "rb_resize_args": {"in": _F32, "out": _F32},
     "rb_match_epilogue_args": {"state": _F32, "coarse_state": _F32, "warp": _F32, "cert": _F32, "grid_x": _F32, "grid_y": _F32},

@@ -8,6 +8,7 @@
 //     straight into the 128B-swizzled K-major layout of a wgmma A operand;
 //   * 1 warpgroup multiplies it with the pointwise weights (TMA-loaded into shared memory once, resident for the whole
 //     persistent kernel): per 64-pixel half 9 wgmma (M=64, N=144, K=16) into registers, then + bias -> 16-bit rows.
+// The parity mode (fp32 maps, split-fp16 pointwise operands) has its own kernel below, refiner_block_c144_split_kernel.
 #include "tma.cuh"
 #include "wgmma.cuh"
 #include <type_traits>
@@ -187,6 +188,205 @@ __global__ void __launch_bounds__(FZ_THREADS, 1) refiner_block_c144_kernel(const
         }
     }
 }
+
+// ===== parity mode: the same block on fp32 maps with split-fp16 pointwise operands =====
+// Bit-identical to the two launches it replaces, dwconv5x5_relu_tma_kernel<float> (fp32 map -> RB_F16S pair) followed by
+// gemm_tc_kernel<144, true> (RB_F16S pair x RB_F16S weights -> fp32 map + bias): every result goes through the same operations
+// in the same order, only the intermediate pair stays in shared memory.  The block moves 8 B per map element (read 4, write 4)
+// instead of 16.  The fp32 input window and the two planes of both operands are twice the size of the fast-mode kernel's, so
+//   * the tile is 4 x 16 = 64 pixels (one m64 wgmma row block; the warpgroup's accumulators acc / acc2 take 144 registers);
+//   * the input window (8 x 20 pixels) arrives in chunks of 16 channels through a TMA ring of 7 slots, one per depthwise warp;
+//   * the 7 depthwise warps take the chunks in turn (chunk g: warp and slot g % 7; lane = channel x row pair, 2 rows x 16
+//     pixels each) and write the ReLU'd, split result as one k-step (16 channels, 32-byte swizzle) of a double-buffered A
+//     operand, so the next tile's depthwise stage overlaps this tile's MMAs and stores.  A slot has one consumer, which waits
+//     for its phases in order: with more consumers than slots a warp could wait on a phase two ahead and pass early;
+//   * the pointwise weights stay resident as 9 k-steps of 16 channels per plane (32-byte swizzle: no zero-padded k-block).
+struct FusedSplitParams {
+    float* out; int64_t ld;
+    const float* dw_w; int64_t ldw; const float* dw_b; const float* pw_b;
+    int H, W, tiles_x, tiles_per_img, total_tiles;
+};
+
+constexpr int FS_TH = 4, FS_TW = 16, FS_IH = FS_TH + 4, FS_IW = FS_TW + 4, FS_CH = 16, FS_KSTEPS = FZ_C / FS_CH;   // 9 chunks
+constexpr int FS_DW_WARPS = 7, FS_STAGES = FS_DW_WARPS;           // one ring slot per depthwise warp
+constexpr int FS_THREADS = 128 + 32 + 32 * FS_DW_WARPS;               // warps 0-3: MMA + epilogue, warp 4: input TMA, 5-11: depthwise
+constexpr int FS_STAGE_BYTES = FS_IH * FS_IW * FS_CH * 4;             // 10240: one fp32 chunk of the window
+constexpr int FS_A_KS = 64 * 32, FS_A_PLANE = FS_KSTEPS * FS_A_KS, FS_A_BYTES = 2 * FS_A_PLANE;            // 36864 per A buffer
+constexpr int FS_B_KS = FZ_C * 32, FS_B_PLANE = FS_KSTEPS * FS_B_KS, FS_B_BYTES = 2 * FS_B_PLANE;          // 82944
+constexpr int FS_OFF_A = FS_B_BYTES, FS_OFF_RING = FS_OFF_A + 2 * FS_A_BYTES, FS_OFF_BIAS = FS_OFF_RING + FS_STAGES * FS_STAGE_BYTES;
+constexpr int FS_OFF_BARS = FS_OFF_BIAS + FZ_C * 4;
+constexpr int FS_SMEM = FS_OFF_BARS + 256 + 1024;
+static_assert(FS_OFF_A % 1024 == 0 && FS_OFF_RING % 1024 == 0 && FS_SMEM <= 232448, "shared memory layout");
+
+__global__ void __launch_bounds__(FS_THREADS, 1) refiner_block_c144_split_kernel(const __grid_constant__ CUtensorMap map_w, const __grid_constant__ CUtensorMap map_w_lo,
+                                                                               const __grid_constant__ CUtensorMap map_in, const FusedSplitParams p) {
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - ((uint32_t)__cvta_generic_to_shared(smem_raw) & 1023u)) & 1023u);   // offset on the array: keeps ld/st.shared
+    uint8_t* sB = smem;
+    uint8_t* sA = smem + FS_OFF_A;
+    uint8_t* ring = smem + FS_OFF_RING;
+    float* s_pwb = reinterpret_cast<float*>(smem + FS_OFF_BIAS);          // [144] pointwise bias
+    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + FS_OFF_BARS);
+    uint64_t* full = bars;                          // input chunk landed (TMA transaction bytes)
+    uint64_t* empty = bars + FS_STAGES;             // its depthwise warp has read it
+    uint64_t* a_full = bars + 2 * FS_STAGES;        // [2] all 9 k-steps of the A buffer written (one arrival per chunk)
+    uint64_t* a_empty = a_full + 2;                 // [2] the MMAs that read the A buffer retired
+    uint64_t* w_full = a_empty + 2;                 // pointwise weights landed
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    if (threadIdx.x == 0) {
+        for (int s = 0; s < FS_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
+        for (int b = 0; b < 2; ++b) { mbar_init(&a_full[b], FS_KSTEPS); mbar_init(&a_empty[b], 1); }
+        mbar_init(w_full, 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    rb::pdl_wait();                                    // everything above overlapped the previous kernel's tail
+    for (int i = threadIdx.x; i < FZ_C; i += FS_THREADS) s_pwb[i] = p.pw_b[i];
+    __syncthreads();
+    const int my_tiles = p.total_tiles > (int)blockIdx.x ? (p.total_tiles - 1 - (int)blockIdx.x) / (int)gridDim.x + 1 : 0;
+
+    if (warp < 4) {
+        // ===== pointwise GEMM + epilogue, as gemm_tc_kernel<144, true> issues it for one 64-row half of its tile =====
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");     // acc + acc2: 144 registers a thread
+        const int t = threadIdx.x;
+        if (t == 0) {
+            mbar_expect_tx(w_full, FS_B_BYTES);
+            for (int j = 0; j < FS_KSTEPS; ++j) {
+                tma_load_2d(sB + j * FS_B_KS, &map_w, w_full, j * FS_CH, 0);
+                tma_load_2d(sB + FS_B_PLANE + j * FS_B_KS, &map_w_lo, w_full, j * FS_CH, 0);
+            }
+        }
+        mbar_wait(w_full, 0);
+        const uint32_t b_addr = smem_u32(sB);
+        float acc[FZ_C / 2], acc2[FZ_C / 2];
+        for (int it = 0; it < my_tiles; ++it) {
+            const int tile = blockIdx.x + it * gridDim.x;
+            const int img = tile / p.tiles_per_img, r = tile - img * p.tiles_per_img;
+            const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
+            const int ab = it & 1;
+            const uint32_t a_addr = smem_u32(sA + ab * FS_A_BYTES);
+            mbar_wait(&a_full[ab], (it >> 1) & 1);
+            // K = 144 in 9 k-steps of 16 channels, ascending.  gemm_tc_kernel also issues the three k-steps of channels 144-191
+            // of its last k-block; their operands are TMA zero fill, and adding zero products leaves an accumulator unchanged
+            // (up to the sign of a zero), so they are not issued here.
+            wgmma_fence();
+#pragma unroll
+            for (int j = 0; j < FS_KSTEPS; ++j) {
+                const uint64_t a_hi = gmma_desc(a_addr + j * FS_A_KS, 16, 256, GMMA_SW32);
+                const uint64_t a_lo = gmma_desc(a_addr + FS_A_PLANE + j * FS_A_KS, 16, 256, GMMA_SW32);
+                const uint64_t b_hi = gmma_desc(b_addr + j * FS_B_KS, 16, 256, GMMA_SW32);
+                const uint64_t b_lo = gmma_desc(b_addr + FS_B_PLANE + j * FS_B_KS, 16, 256, GMMA_SW32);
+                Wgmma<FZ_C, false>::ss<0>(acc, a_hi, b_hi, j != 0);
+                Wgmma<FZ_C, false>::ss<0>(acc2, a_hi, b_lo, j != 0);
+                Wgmma<FZ_C, false>::ss<0>(acc2, a_lo, b_hi, 1);
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            wgmma_fence_regs(acc);
+            wgmma_fence_regs(acc2);
+            if (t == 0) mbar_arrive(&a_empty[ab]);          // the depthwise warps may overwrite this A buffer
+            // epilogue (Epilogue::apply with alpha = 1, bias, fp32 out): acc + acc2 * 2^-11, then + bias.  Accumulator fragment:
+            // pixels m and m + 8, channel pairs 8 i + 2 (t % 4).
+            const int m0 = (t >> 5) * 16 + ((t & 31) >> 2), cn = 2 * (t & 3);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = m0 + 8 * h;
+                const int yy = ty * FS_TH + m / FS_TW, xx = tx * FS_TW + m % FS_TW;
+                if (yy >= p.H || xx >= p.W) continue;
+                float* orow = p.out + (((int64_t)img * p.H + yy) * p.W + xx) * p.ld + cn;
+#pragma unroll
+                for (int i = 0; i < FZ_C / 8; ++i) {
+                    const float v0 = fmaf(acc2[4 * i + 2 * h], 1.0f / RB_SPLIT_SCALE, acc[4 * i + 2 * h]);
+                    const float v1 = fmaf(acc2[4 * i + 2 * h + 1], 1.0f / RB_SPLIT_SCALE, acc[4 * i + 2 * h + 1]);
+                    *reinterpret_cast<float2*>(orow + 8 * i) = make_float2(__fadd_rn(v0, s_pwb[8 * i + cn]), __fadd_rn(v1, s_pwb[8 * i + cn + 1]));
+                }
+            }
+        }
+    } else {
+        // 12 warps leave 3 on some SM sub-partition, whose register file then caps a thread at 168 registers: warpgroups 1-2
+        // (loader, depthwise) hand theirs to the MMA warpgroup
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 104;");
+        if (warp == 4) {
+            // ===== input loader: chunk j of tile it is ring slot (9 it + j) % FS_STAGES =====
+            if (lane == 0) {
+                uint32_t g = 0;
+                for (int it = 0; it < my_tiles; ++it) {
+                    const int tile = blockIdx.x + it * gridDim.x;
+                    const int img = tile / p.tiles_per_img, r = tile - img * p.tiles_per_img;
+                    const int ty = r / p.tiles_x, tx = r - ty * p.tiles_x;
+                    for (int j = 0; j < FS_KSTEPS; ++j, ++g) {
+                        const uint32_t s = g % FS_STAGES, round = g / FS_STAGES;
+                        if (round > 0) mbar_wait(&empty[s], (round - 1) & 1);
+                        mbar_expect_tx(&full[s], FS_STAGE_BYTES);
+                        tma_load_4d(ring + s * FS_STAGE_BYTES, &map_in, &full[s], j * FS_CH, tx * FS_TW - 2, ty * FS_TH - 2, img);
+                    }
+                }
+            }
+        } else {
+            // ===== depthwise warps: warp w takes chunks g = w, w + 7, ... (tile g / 9, channels 16 (g % 9) ..), all from slot w =====
+            // lane = (channel c of the chunk, row pair rp): output rows 2 rp, 2 rp + 1 x 16 pixels.  The arithmetic is that of
+            // dwconv5x5_relu_tma_kernel<float>: bias, then fmaf over the taps ky-major, kx-minor, ReLU, split_f16s.
+            const int c = lane & 15, rp = lane >> 4;
+            const uint32_t n_chunks = (uint32_t)my_tiles * FS_KSTEPS;
+            for (uint32_t g = warp - 5; g < n_chunks; g += FS_DW_WARPS) {
+                const int it = g / FS_KSTEPS, j = g - it * FS_KSTEPS;
+                const uint32_t s = g % FS_STAGES;
+                const int ch = j * FS_CH + c;
+                float wv[25];
+    #pragma unroll
+                for (int k = 0; k < 25; ++k) wv[k] = __ldg(&p.dw_w[(int64_t)k * p.ldw + ch]);    // 14 KB for all chunks: L1 hits
+                const float bv = __ldg(&p.dw_b[ch]);
+                float acc[2][FS_TW];
+    #pragma unroll
+                for (int rr = 0; rr < 2; ++rr)
+    #pragma unroll
+                    for (int i = 0; i < FS_TW; ++i) acc[rr][i] = bv;
+                mbar_wait(&full[s], (g / FS_STAGES) & 1);
+                const float* win = reinterpret_cast<const float*>(ring + s * FS_STAGE_BYTES) + c;
+    #pragma unroll
+                for (int iy = 0; iy < 6; ++iy) {                   // window rows 2 rp + iy feed output rows 2 rp + {0, 1}
+    #pragma unroll
+                    for (int ix = 0; ix < FS_IW; ++ix) {
+                        const float v = win[((2 * rp + iy) * FS_IW + ix) * FS_CH];
+    #pragma unroll
+                        for (int rr = 0; rr < 2; ++rr) {
+                            const int ky = iy - rr;
+                            if (ky >= 0 && ky < 5) {
+    #pragma unroll
+                                for (int kx = 0; kx < 5; ++kx) {
+                                    const int ox = ix - kx;
+                                    if (ox >= 0 && ox < FS_TW) acc[rr][ox] = fmaf(wv[ky * 5 + kx], v, acc[rr][ox]);
+                                }
+                            }
+                        }
+                    }
+                }
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty[s]);             // this warp no longer reads the slot
+                const int ab = it & 1;
+                mbar_wait(&a_empty[ab], ((it >> 1) & 1) ^ 1);     // the MMAs of tile it - 2 no longer read the buffer
+                // k-step j of both planes: row m (pixel) is 32 B, channel c at 16-byte chunk (c / 8) ^ ((m / 4) % 2), element c % 8
+                uint8_t* a_hi = sA + ab * FS_A_BYTES + j * FS_A_KS;
+    #pragma unroll
+                for (int rr = 0; rr < 2; ++rr) {
+    #pragma unroll
+                    for (int i = 0; i < FS_TW; ++i) {
+                        const int m = (2 * rp + rr) * FS_TW + i;
+                        __half hi, lo;
+                        split_f16s(fmaxf(acc[rr][i], 0.f), hi, lo);
+                        const int off = m * 32 + ((((c >> 3) ^ (m >> 2)) & 1) << 4) + (c & 7) * 2;
+                        *reinterpret_cast<__half*>(a_hi + off) = hi;
+                        *reinterpret_cast<__half*>(a_hi + FS_A_PLANE + off) = lo;
+                    }
+                }
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&a_full[ab]);
+            }
+        }
+    }
+}
 }  // namespace rb
 
 using namespace rb;
@@ -234,4 +434,41 @@ extern "C" int romab200_refiner_block_c144(const rb_refiner_block_c144_args* a, 
         rb::launch_pdl(refiner_block_c144_kernel<__nv_bfloat16>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
     }
     return check_launch("refiner_block_c144");
+}
+
+extern "C" int romab200_refiner_block_c144_split(const rb_refiner_block_c144_split_args* a, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    RB_REQUIRE(a->c == FZ_C, "refiner_block_c144_split: C must be 144 (got %d)", a->c);
+    RB_REQUIRE(a->in != a->out, "refiner_block_c144_split: in and out must differ (the block reads a 5x5 halo)");
+    RB_REQUIRE(a->ld % 8 == 0 && a->ld >= FZ_C && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0,
+               "refiner_block_c144_split: bad activation layout (ld %lld)", (long long)a->ld);
+    RB_REQUIRE(a->ld_pw % 8 == 0 && a->ld_pw >= FZ_C && ((uintptr_t)a->pw_weight) % 16 == 0 && ((uintptr_t)a->pw_weight_lo) % 16 == 0,
+               "refiner_block_c144_split: bad weight layout (ld_pw %lld)", (long long)a->ld_pw);
+    RB_REQUIRE(a->ldw >= FZ_C, "refiner_block_c144_split: ldw %lld < 144", (long long)a->ldw);
+    CUtensorMap map_w, map_w_lo;       // pointwise weights [144 x 144] per plane: boxes of 16 channels x 144 rows, 32-byte swizzle
+    {
+        cuuint64_t dims[2] = {(cuuint64_t)FZ_C, (cuuint64_t)FZ_C};
+        cuuint64_t strides[1] = {(cuuint64_t)a->ld_pw * 2};
+        cuuint32_t box[2] = {FS_CH, (cuuint32_t)FZ_C};
+        if (encode_tiled(&map_w, "refiner_block_c144_split", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, a->pw_weight, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_32B)) return 1;
+        if (encode_tiled(&map_w_lo, "refiner_block_c144_split", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, a->pw_weight_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_32B)) return 1;
+    }
+    CUtensorMap map_in;          // fp32 activation [B, H, W, C] with pitch ld: box = 8 x 20 pixels x 16 channels, borders zero-filled
+    {
+        cuuint64_t d4[4] = {(cuuint64_t)FZ_C, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
+        cuuint64_t s4[3] = {(cuuint64_t)a->ld * 4, (cuuint64_t)a->w * a->ld * 4, (cuuint64_t)a->h * a->w * a->ld * 4};
+        cuuint32_t b4[4] = {FS_CH, FS_IW, FS_IH, 1};
+        if (encode_tiled(&map_in, "refiner_block_c144_split (input)", CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
+    }
+    FusedSplitParams p;
+    p.out = a->out; p.ld = a->ld; p.dw_w = a->dw_weight; p.ldw = a->ldw; p.dw_b = a->dw_bias; p.pw_b = a->pw_bias;
+    p.H = a->h; p.W = a->w; p.tiles_x = (a->w + FS_TW - 1) / FS_TW; p.tiles_per_img = p.tiles_x * ((a->h + FS_TH - 1) / FS_TH);
+    const long long total = (long long)p.tiles_per_img * a->batch;
+    RB_REQUIRE(a->h > 0 && a->w > 0 && total > 0 && total < (1ll << 31) / FS_KSTEPS, "refiner_block_c144_split: bad tile count");
+    p.total_tiles = (int)total;
+    const int sms = sm_count();
+    const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+    if (ensure_smem<refiner_block_c144_split_kernel>(FS_SMEM, "refiner_block_c144_split")) return 1;
+    rb::launch_pdl(refiner_block_c144_split_kernel, dim3(grid), dim3(FS_THREADS), FS_SMEM, st, map_w, map_w_lo, map_in, p);
+    return check_launch("refiner_block_c144_split");
 }

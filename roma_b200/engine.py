@@ -529,6 +529,15 @@ class Engine:
                 call("romab200_refiner_block_c144", "rb_refiner_block_c144_args", **{"in": d}, out=t, ld=cp, dw_weight=blk["dw_w"], ldw=cp,
                      dw_bias=blk["dw_b"], pw_weight=blk["pw_w"], ld_pw=cp, pw_bias=blk["pw_b"], batch=D, h=h, w=w, c=c, dtype=self.dt)
                 d, t = t, d
+        elif c == 144 and self.split and self.fused_c144:
+            # parity mode, stride-2 maps: the same fusion on fp32 maps with the split-fp16 pointwise GEMM (bit-identical to the
+            # two launches below); the fp32 ping-pong buffer takes the place of their RB_F16S intermediate
+            t = self.buf(f"ref.t.{tag}", (D * h * w, cp), zero=True)
+            for blk in R["blocks"]:
+                call("romab200_refiner_block_c144_split", "rb_refiner_block_c144_split_args", **{"in": d}, out=t, ld=cp, dw_weight=blk["dw_w"],
+                     ldw=cp, dw_bias=blk["dw_b"], pw_weight=blk["pw_w"].hi, pw_weight_lo=blk["pw_w"].lo, ld_pw=cp, pw_bias=blk["pw_b"],
+                     batch=D, h=h, w=w, c=c)
+                d, t = t, d
         elif self.split:
             # parity mode: fp32 maps; the depthwise kernel writes its result as the RB_F16S A operand of the pointwise GEMM
             ts = self.sbuf(f"ref.ts.{tag}", (D * h * w, cp), zero=True)
