@@ -26,7 +26,7 @@ import math
 
 import numpy as np
 
-from oracle.pose_ransac import philox4x32_10
+from oracle.ransac import draw_distinct, ransac_update_num_iters
 
 FLT_EPS = float(np.finfo(np.float32).eps)
 DBL_EPS = float(np.finfo(np.float64).eps)
@@ -63,15 +63,8 @@ def check_subset(s4, d4):
 
 def draw_subset(h, b, n, seed, src, dst):
     """Hypothesis h of pair b (n > 4): returns (indices, rejected attempts, found)."""
-    key = (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
     for att in range(MAX_ATTEMPTS):
-        idx, sub = [], 0
-        while len(idx) < 4:
-            for w in philox4x32_10(np.array([h, b, att, sub], dtype=np.uint64), key):
-                v = (int(w) * n) >> 32
-                if v not in idx and len(idx) < 4:
-                    idx.append(v)
-            sub += 1
+        idx = draw_distinct(4, n, seed, lambda sub: (h, b, att, sub))
         if check_subset(src[idx], dst[idx]):
             return idx, att, True
     return idx, MAX_ATTEMPTS, False
@@ -209,21 +202,6 @@ def inlier_mask(H, src, dst, thresh):
     return err <= np.float32(thresh * thresh)
 
 
-def ransac_update_num_iters(p, ep, max_iters, model_points=4):
-    p = min(max(p, 0.0), 1.0)
-    ep = min(max(ep, 0.0), 1.0)
-    num = max(1.0 - p, 2.2250738585072014e-308)
-    q = 1.0 - ep
-    pw = q
-    for _ in range(model_points - 1):
-        pw = pw * q
-    denom = 1.0 - pw
-    if denom < 2.2250738585072014e-308:
-        return 0
-    num, denom = math.log(num), math.log(denom)
-    return max_iters if denom >= 0 or -num >= max_iters * (-denom) else int(np.rint(num / denom))
-
-
 def select(hypothesis, n, conf, max_iters):
     """OpenCV's loop: hypothesis(h) -> (status, count) with status 1 (model), 0 (no model) or -1 (not found).
     Returns (best hypothesis, best count, final niters, iterations run, ended on a not-found hypothesis)."""
@@ -235,7 +213,7 @@ def select(hypothesis, n, conf, max_iters):
             break
         if status == 1 and c > max(best, 3):
             best, hyp = c, it
-            niters = ransac_update_num_iters(conf, (n - c) / n, niters)
+            niters = ransac_update_num_iters(conf, (n - c) / n, niters, 4)
         it += 1
     return hyp, best, niters, it, nf
 

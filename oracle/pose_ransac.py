@@ -16,33 +16,12 @@ import math
 
 import numpy as np
 
-M32 = np.uint64(0xFFFFFFFF)
-
-
-def philox4x32_10(ctr, key):
-    """Philox4x32-10 (Salmon et al. 2011) of counters ctr [..., 4] (uint32) under key (k0, k1); returns [..., 4] uint32."""
-    c = [np.asarray(ctr, dtype=np.uint64)[..., i] for i in range(4)]
-    k0, k1 = np.uint64(key[0]), np.uint64(key[1])
-    for _ in range(10):
-        p0 = np.uint64(0xD2511F53) * c[0]
-        p1 = np.uint64(0xCD9E8D57) * c[2]
-        c = [(p1 >> np.uint64(32)) ^ c[1] ^ k0, p1 & M32, (p0 >> np.uint64(32)) ^ c[3] ^ k1, p0 & M32]
-        k0 = (k0 + np.uint64(0x9E3779B9)) & M32
-        k1 = (k1 + np.uint64(0xBB67AE85)) & M32
-    return np.stack(c, axis=-1).astype(np.uint32)
+from oracle.ransac import draw_distinct, philox4x32_10, ransac_update_num_iters  # noqa: F401  (philox4x32_10 stays importable here)
 
 
 def draw_sample(h, b, n, seed):
     """The 5 distinct indices of hypothesis h of pair b (n > 5 points)."""
-    key = (seed & 0xFFFFFFFF, (seed >> 32) & 0xFFFFFFFF)
-    out, sub = [], 0
-    while len(out) < 5:
-        for w in philox4x32_10(np.array([h, b, sub, 0], dtype=np.uint64), key):
-            v = (int(w) * n) >> 32
-            if v not in out and len(out) < 5:
-                out.append(v)
-        sub += 1
-    return out
+    return draw_distinct(5, n, seed, lambda sub: (h, b, sub, 0))
 
 
 def normalise(x, K):
@@ -207,18 +186,6 @@ def inlier_mask(E, xn, thresh):
     return err <= np.float32(thresh * thresh)
 
 
-def ransac_update_num_iters(p, ep, max_iters):
-    p = min(max(p, 0.0), 1.0)
-    ep = min(max(ep, 0.0), 1.0)
-    num = max(1.0 - p, 2.2250738585072014e-308)
-    q = 1.0 - ep
-    denom = 1.0 - q * q * q * q * q
-    if denom < 2.2250738585072014e-308:
-        return 0
-    num, denom = math.log(num), math.log(denom)
-    return max_iters if denom >= 0 or -num >= max_iters * (-denom) else int(np.rint(num / denom))
-
-
 def select(counts_of, n, conf, max_iters):
     """OpenCV's loop over hypotheses: counts_of(h) -> list of inlier counts of hypothesis h's solutions.
     Returns (best hypothesis, best solution, best count, final niters, iterations run)."""
@@ -227,7 +194,7 @@ def select(counts_of, n, conf, max_iters):
         for s, c in enumerate(counts_of(it)):
             if c > max(best, 4):
                 best, hyp, sol = c, it, s
-                niters = ransac_update_num_iters(conf, (n - c) / n, niters)
+                niters = ransac_update_num_iters(conf, (n - c) / n, niters, 5)
         it += 1
     return hyp, sol, best, niters, it
 

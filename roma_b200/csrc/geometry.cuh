@@ -11,6 +11,75 @@ __device__ __forceinline__ double pow_left(double q) {
     else return pow_left<M - 1>(q) * q;
 }
 
+// Whether OpenCV's loop draws hypothesis h for a pair of n points: it needs M points, draws once when there are exactly M,
+// and stops at max_iters.  After the first round a caller also skips the pairs whose state row no longer says running.
+template <int M>
+__device__ __forceinline__ bool ransac_drawn(int64_t n, int64_t h, int max_iters) {
+    return n >= M && h < max_iters && (n > M || h == 0);
+}
+
+// M distinct indices in [0, n): the four words of philox4x32_10(ctr(sub), seed) for sub = 0, 1, ... in order, index
+// (w * n) >> 32, repeats skipped.  Only the counter differs between the estimators' streams (include/romab200.h).
+template <int M, typename CtrOf>
+__device__ __forceinline__ void ransac_draw(int (&id)[M], int64_t n, uint64_t seed, CtrOf ctr) {
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
+    int got = 0;
+    for (uint32_t sub = 0; got < M; ++sub) {
+        const uint4 r = philox4x32_10(ctr(sub), k0, k1);
+        const uint32_t words[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+            const int v = (int)(((uint64_t)words[q] * (uint64_t)n) >> 32);
+            bool dup = false;
+#pragma unroll
+            for (int k = 0; k < M; ++k) dup |= (k < got && id[k] == v);
+            if (!dup && got < M) {
+#pragma unroll
+                for (int k = 0; k < M; ++k)
+                    if (k == got) id[k] = v;
+                ++got;
+            }
+        }
+    }
+}
+
+// Inliers of this thread's model among the points of score slice blockIdx.y (per_split points each, n in all).  The CTA of
+// THREADS threads stages the points through `tile`, load(j) giving point j; inlier(p) tests one.  Every thread must call
+// it; the count is meaningful for the threads with act set.  Integer counts: the slices add up in any order.
+template <int THREADS, typename T, int TILE, typename Load, typename Inlier>
+__device__ __forceinline__ int ransac_count(T (&tile)[TILE], int64_t n, int per_split, bool act, Load load, Inlier inlier) {
+    const int64_t j0 = (int64_t)blockIdx.y * per_split, j1 = min(n, j0 + per_split);
+    int cnt = 0;
+    for (int64_t t0 = j0; t0 < j1; t0 += TILE) {
+        const int m = (int)min((int64_t)TILE, j1 - t0);
+        __syncthreads();
+        for (int j = threadIdx.x; j < m; j += THREADS) tile[j] = load(t0 + j);
+        __syncthreads();
+        if (act) {
+#pragma unroll 4
+            for (int j = 0; j < m; ++j) cnt += inlier(tile[j]);
+        }
+    }
+    return cnt;
+}
+
+// Score slices of one pair: one per points_per_split points, at least 1 and at most max_splits
+static inline int ransac_splits(int64_t max_n, int points_per_split, int max_splits) {
+    const int64_t s = (max_n + points_per_split - 1) / points_per_split;
+    return s < 1 ? 1 : (s > max_splits ? max_splits : (int)s);
+}
+
+// The checks every RANSAC stage shares: pair layout, state rows, batch size and the round within max_iters
+template <typename Args>
+static int ransac_check(const Args* a, const char* what, int max_batch, int round_size) {
+    RB_REQUIRE(a && a->offsets && a->state, "%s: null argument", what);
+    RB_REQUIRE(a->batch > 0 && a->batch <= max_batch, "%s: batch %d outside [1, %d]", what, a->batch, max_batch);
+    RB_REQUIRE(a->max_n >= 0 && a->max_n < (1ll << 31), "%s: bad max_n %lld", what, (long long)a->max_n);
+    RB_REQUIRE(a->max_iters > 0 && a->round >= 0 && (int64_t)a->round * round_size < a->max_iters, "%s: round %d outside max_iters %d",
+               what, a->round, a->max_iters);
+    return 0;
+}
+
 // cv::RANSACUpdateNumIters(p, ep, model_points, maxIters), with (1 - ep)^model_points as products from the left
 template <int MODEL_POINTS>
 __device__ __forceinline__ int ransac_update_num_iters(double p, double ep, int max_iters) {

@@ -166,8 +166,7 @@ __global__ void __launch_bounds__(HG_THREADS) homog_hypotheses_kernel(rb_homogra
     const int64_t h = (int64_t)a.round * HG_ROUND + hl;
     const int64_t slot = (int64_t)b * HG_ROUND + hl;
     const int64_t off = a.offsets[b], n = a.offsets[b + 1] - off;
-    const bool active = n >= 4 && h < a.max_iters && (n > 4 || h == 0) && (a.round == 0 || a.state[b * RB_HOMOG_STATE + HS_RUN] != 0);
-    if (!active) {
+    if (!(ransac_drawn<4>(n, h, a.max_iters) && (a.round == 0 || a.state[b * RB_HOMOG_STATE + HS_RUN] != 0))) {
         a.status[slot] = 0;
         return;
     }
@@ -181,26 +180,8 @@ __global__ void __launch_bounds__(HG_THREADS) homog_hypotheses_kernel(rb_homogra
 #pragma unroll
         for (int k = 0; k < 4; ++k) { sx[k] = S[2 * k]; sy[k] = S[2 * k + 1]; dx[k] = D[2 * k]; dy[k] = D[2 * k + 1]; }
     } else {
-        const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
         for (; att < RB_HOMOG_MAX_ATTEMPTS; ++att) {
-            int got = 0;
-            for (uint32_t sub = 0; got < 4; ++sub) {
-                const uint4 r = philox4x32_10(make_uint4((uint32_t)h, (uint32_t)b, (uint32_t)att, sub), k0, k1);
-                const uint32_t words[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const int v = (int)(((uint64_t)words[q] * (uint64_t)n) >> 32);
-                    bool dup = false;
-#pragma unroll
-                    for (int k = 0; k < 4; ++k) dup |= (k < got && id[k] == v);
-                    if (!dup && got < 4) {
-#pragma unroll
-                        for (int k = 0; k < 4; ++k)
-                            if (k == got) id[k] = v;
-                        ++got;
-                    }
-                }
-            }
+            ransac_draw(id, n, a.seed, [&](uint32_t sub) { return make_uint4((uint32_t)h, (uint32_t)b, (uint32_t)att, sub); });
 #pragma unroll
             for (int k = 0; k < 4; ++k) {
                 const float2 s = reinterpret_cast<const float2*>(S)[id[k]], d = reinterpret_cast<const float2*>(D)[id[k]];
@@ -249,26 +230,13 @@ __global__ void __launch_bounds__(HG_THREADS) homog_score_kernel(rb_homography_a
     for (int i = 0; i < 8; ++i) f[i] = act ? __double2float_rn(a.H[slot * 9 + i]) : 0.0f;
     const float t = homog_thresh(a.thresh);
     const int64_t off = a.offsets[b], n = a.offsets[b + 1] - off;
-    const int64_t j0 = (int64_t)blockIdx.y * per_split, j1 = min(n, j0 + per_split);
     const float2* S = reinterpret_cast<const float2*>(a.src) + off;
     const float2* D = reinterpret_cast<const float2*>(a.dst) + off;
-    int cnt = 0;
-    for (int64_t t0 = j0; t0 < j1; t0 += HG_TILE) {
-        const int m = (int)min((int64_t)HG_TILE, j1 - t0);
-        __syncthreads();
-        for (int j = threadIdx.x; j < m; j += HG_THREADS) {
-            const float2 s = S[t0 + j], d = D[t0 + j];
-            tile[j] = make_float4(s.x, s.y, d.x, d.y);
-        }
-        __syncthreads();
-        if (act) {
-#pragma unroll 4
-            for (int j = 0; j < m; ++j) {
-                const float4 p = tile[j];
-                cnt += homog_inlier(f, p.x, p.y, p.z, p.w, t);
-            }
-        }
-    }
+    auto load = [&](int64_t j) {
+        const float2 s = S[j], d = D[j];
+        return make_float4(s.x, s.y, d.x, d.y);
+    };
+    const int cnt = ransac_count<HG_THREADS>(tile, n, per_split, act, load, [&](const float4& p) { return homog_inlier(f, p.x, p.y, p.z, p.w, t); });
     if (act) a.counts[((int64_t)b * RB_HOMOG_MAX_SPLITS + blockIdx.y) * HG_ROUND + hl] = cnt;
 }
 
@@ -696,19 +664,13 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
 }
 
 static int homog_check(const rb_homography_args* a, const char* what) {
-    RB_REQUIRE(a && a->src && a->dst && a->offsets && a->state, "%s: null argument", what);
-    RB_REQUIRE(a->batch > 0 && a->batch <= 65535, "%s: batch %d outside [1, 65535]", what, a->batch);
-    RB_REQUIRE(a->max_n >= 0 && a->max_n < (1ll << 31), "%s: bad max_n %lld", what, (long long)a->max_n);
+    if (ransac_check(a, what, 65535, HG_ROUND)) return 1;
+    RB_REQUIRE(a->src && a->dst, "%s: null argument", what);
     RB_REQUIRE(a->method == 0 || a->method == 8, "%s: method %d is neither 0 nor RANSAC (8)", what, a->method);
-    RB_REQUIRE(a->max_iters > 0 && a->round >= 0 && (int64_t)a->round * HG_ROUND < a->max_iters, "%s: round %d outside max_iters %d", what,
-               a->round, a->max_iters);
     return 0;
 }
 
-static int homog_splits(int64_t max_n) {
-    const int64_t s = (max_n + 511) / 512;
-    return s < 1 ? 1 : (s > RB_HOMOG_MAX_SPLITS ? RB_HOMOG_MAX_SPLITS : (int)s);
-}
+static int homog_splits(int64_t max_n) { return ransac_splits(max_n, 512, RB_HOMOG_MAX_SPLITS); }
 
 }  // namespace rb
 

@@ -171,34 +171,13 @@ __global__ void __launch_bounds__(PS_WARPS * 32) pose_solve_kernel(rb_pose_args 
     const int64_t h = (int64_t)a.round * PS_ROUND + hl;
     const int64_t slot = (int64_t)b * PS_ROUND + hl;
     const int64_t off = a.offsets[b], n = a.offsets[b + 1] - off;
-    const bool active = n >= 5 && h < a.max_iters && (n > 5 || h == 0) && (a.round == 0 || a.state[b * RB_POSE_STATE + ST_RUN] != 0);
-    if (!active) {
+    if (!(ransac_drawn<5>(n, h, a.max_iters) && (a.round == 0 || a.state[b * RB_POSE_STATE + ST_RUN] != 0))) {
         if (lane == 0) a.nsol[slot] = 0;
         return;
     }
     // ---- draw 5 distinct indices (lane 0), broadcast
     int id[5] = {0, 1, 2, 3, 4};
-    if (n > 5 && lane == 0) {
-        const uint32_t k0 = (uint32_t)a.seed, k1 = (uint32_t)(a.seed >> 32);
-        int got = 0;
-        for (uint32_t sub = 0; got < 5; ++sub) {
-            const uint4 r = philox4x32_10(make_uint4((uint32_t)h, (uint32_t)b, sub, 0u), k0, k1);
-            const uint32_t words[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                const int v = (int)(((uint64_t)words[q] * (uint64_t)n) >> 32);
-                bool dup = false;
-#pragma unroll
-                for (int k = 0; k < 5; ++k) dup |= (k < got && id[k] == v);
-                if (!dup && got < 5) {
-#pragma unroll
-                    for (int k = 0; k < 5; ++k)
-                        if (k == got) id[k] = v;
-                    ++got;
-                }
-            }
-        }
-    }
+    if (n > 5 && lane == 0) ransac_draw(id, n, a.seed, [&](uint32_t sub) { return make_uint4((uint32_t)h, (uint32_t)b, sub, 0u); });
 #pragma unroll
     for (int k = 0; k < 5; ++k) {
         id[k] = __shfl_sync(FULL, id[k], 0);
@@ -512,22 +491,9 @@ __global__ void __launch_bounds__(PS_THREADS) pose_score_kernel(rb_pose_args a, 
     for (int i = 0; i < 9; ++i) e[i] = act ? a.E[(slot * PS_SOL + s) * 9 + i] : 0.0;
     const float t = pose_thresh(a.thresh);
     const int64_t off = a.offsets[b], n = a.offsets[b + 1] - off;
-    const int64_t j0 = (int64_t)blockIdx.y * per_split, j1 = min(n, j0 + per_split);
-    int cnt = 0;
     const double4* pts = reinterpret_cast<const double4*>(a.xn) + off;
-    for (int64_t t0 = j0; t0 < j1; t0 += PS_TILE) {
-        const int m = (int)min((int64_t)PS_TILE, j1 - t0);
-        __syncthreads();
-        for (int j = threadIdx.x; j < m; j += PS_THREADS) tile[j] = pts[t0 + j];
-        __syncthreads();
-        if (act) {
-#pragma unroll 4
-            for (int j = 0; j < m; ++j) {
-                const double4 p = tile[j];
-                cnt += pose_inlier(e, p.x, p.y, p.z, p.w, t);
-            }
-        }
-    }
+    const int cnt = ransac_count<PS_THREADS>(tile, n, per_split, act, [&](int64_t j) { return pts[j]; },
+                                             [&](const double4& p) { return pose_inlier(e, p.x, p.y, p.z, p.w, t); });
     if (act) a.counts[(((int64_t)b * RB_POSE_MAX_SPLITS + blockIdx.y) * PS_SOL + s) * PS_ROUND + hl] = cnt;
 }
 
@@ -726,18 +692,12 @@ __global__ void __launch_bounds__(PS_RECOVER_THREADS, 1) pose_recover_kernel(rb_
 }
 
 static int pose_check(const rb_pose_args* a, const char* what) {
-    RB_REQUIRE(a && a->x0 && a->x1 && a->offsets && a->K && a->xn && a->state, "%s: null argument", what);
-    RB_REQUIRE(a->batch > 0 && a->batch <= 4096, "%s: batch %d outside [1, 4096]", what, a->batch);
-    RB_REQUIRE(a->max_n >= 0 && a->max_n < (1ll << 31), "%s: bad max_n %lld", what, (long long)a->max_n);
-    RB_REQUIRE(a->max_iters > 0 && a->round >= 0 && (int64_t)a->round * PS_ROUND < a->max_iters, "%s: round %d outside max_iters %d", what, a->round,
-               a->max_iters);
+    if (ransac_check(a, what, 4096, PS_ROUND)) return 1;
+    RB_REQUIRE(a->x0 && a->x1 && a->K && a->xn, "%s: null argument", what);
     return 0;
 }
 
-static int pose_splits(int64_t max_n) {
-    const int64_t s = (max_n + 1023) / 1024;
-    return s < 1 ? 1 : (s > RB_POSE_MAX_SPLITS ? RB_POSE_MAX_SPLITS : (int)s);
-}
+static int pose_splits(int64_t max_n) { return ransac_splits(max_n, 1024, RB_POSE_MAX_SPLITS); }
 
 }  // namespace rb
 

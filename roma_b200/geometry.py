@@ -70,17 +70,46 @@ def _launch(x0, x1, offsets, K, max_n, norm_thresh, conf, max_iters, seed):
         best_E=torch.zeros(B, MAX_SOL, 9, **f64), running=torch.zeros(1, **i32), R=torch.empty(B, 3, 3, **f64), t=torch.empty(B, 3, **f64),
         ok=torch.empty(B, device=dev, dtype=torch.uint8), mask=torch.empty(max(total, 1), device=dev, dtype=torch.uint8))
     kw = dict(batch=B, x0=x0, x1=x1, offsets=offsets, K=K, max_n=int(max_n), thresh=float(norm_thresh), conf=float(conf),
-              max_iters=int(max_iters), seed=int(seed) & (2 ** 64 - 1), **buf)
-    rounds = (int(max_iters) + ROUND - 1) // ROUND
-    for r in range(rounds):
-        kw["round"] = r
-        cabi.call("romab200_pose_hypotheses", "rb_pose_args", **kw)
-        cabi.call("romab200_pose_score", "rb_pose_args", **kw)
-        cabi.call("romab200_pose_select", "rb_pose_args", **kw)
-        if r + 1 < rounds and int(buf["running"].item()) == 0:
-            break
+              max_iters=int(max_iters), seed=int(seed) & (2 ** 64 - 1), round=0, **buf)
+    _ransac_rounds("pose", "rb_pose_args", kw, ROUND)
     cabi.call("romab200_pose_recover", "rb_pose_args", **kw)
     return buf
+
+
+def _ransac_rounds(prefix, struct, kw, round_size):
+    """Enqueues the hypotheses -> score -> select rounds of `romab200_<prefix>_*`.  A round after the first runs only when the
+    previous select left the `running` flag set, which costs one 4-byte read."""
+    rounds = (kw["max_iters"] + round_size - 1) // round_size
+    for r in range(rounds):
+        for stage in ("hypotheses", "score", "select"):
+            cabi.call(f"romab200_{prefix}_{stage}", struct, **{**kw, "round": r})
+        if r + 1 < rounds and int(kw["running"].item()) == 0:
+            break
+
+
+def _pack_pairs(a_list, b_list, to_points, what, list_names, point_names):
+    """Validates two lists of per-pair point sets and packs them for the device: returns (a, b, offsets int64 [B + 1], ns) with
+    a and b the concatenated points of every pair (one zero row when there are none, so the buffers are never empty)."""
+    if len(a_list) != len(b_list) or len(a_list) == 0:
+        raise ValueError(f"{list_names[0]} and {list_names[1]} must be non-empty and of the same length")
+    dev = _device(what)
+    pa = [to_points(p, dev) for p in a_list]
+    pb = [to_points(p, dev) for p in b_list]
+    for a, b in zip(pa, pb):
+        if a.shape != b.shape:
+            raise ValueError(f"{point_names[0]} and {point_names[1]} differ in shape: {tuple(a.shape)} vs {tuple(b.shape)}")
+    ns = [a.shape[0] for a in pa]
+    offsets = torch.tensor(np.concatenate([[0], np.cumsum(ns)]), dtype=torch.int64, device=dev)
+    if not sum(ns):
+        pa = pb = [torch.zeros(1, 2, dtype=pa[0].dtype, device=dev)]
+    return torch.cat(pa), torch.cat(pb), offsets, ns
+
+
+def _outputs(as_numpy, *outs):
+    """The estimators' return: device tensors as they are, or (for numpy inputs) host arrays; a list is converted item by item."""
+    if not as_numpy:
+        return outs
+    return tuple([m.cpu().numpy() for m in o] if isinstance(o, list) else o.cpu().numpy() for o in outs)
 
 
 def _check_args(norm_thresh, conf, max_iters):
@@ -96,29 +125,13 @@ def estimate_pose_batched(kpts0_list, kpts1_list, K0, K1, norm_thresh, conf=0.99
     bit-identical to `estimate_pose` of that pair alone when b == 0, and to the pair-b stream otherwise.
     Returns (R [B, 3, 3] float64, t [B, 3, 1] float64, ok [B] bool, masks: list of bool [N_b]); numpy keypoints give numpy
     outputs, CUDA tensors give device tensors.  ok[b] is False where `estimate_pose` returns None."""
-    if len(kpts0_list) != len(kpts1_list) or len(kpts0_list) == 0:
-        raise ValueError("kpts0_list and kpts1_list must be non-empty and of the same length")
     _check_args(norm_thresh, conf, max_iters)
-    dev = _device()
-    as_numpy = not isinstance(kpts0_list[0], torch.Tensor)
-    p0 = [_points(k, dev) for k in kpts0_list]
-    p1 = [_points(k, dev) for k in kpts1_list]
-    for a, b in zip(p0, p1):
-        if a.shape != b.shape:
-            raise ValueError(f"kpts0 and kpts1 differ in shape: {tuple(a.shape)} vs {tuple(b.shape)}")
-    B = len(p0)
-    ns = [a.shape[0] for a in p0]
-    offsets = torch.tensor(np.concatenate([[0], np.cumsum(ns)]), dtype=torch.int64, device=dev)
+    x0, x1, offsets, ns = _pack_pairs(kpts0_list, kpts1_list, _points, "estimate_pose", ("kpts0_list", "kpts1_list"), ("kpts0", "kpts1"))
+    B, dev = len(ns), offsets.device
     K = torch.stack([_intrinsics(K0, B, dev), _intrinsics(K1, B, dev)], dim=1).contiguous()
-    x0 = torch.cat(p0) if sum(ns) else torch.zeros(1, 2, dtype=torch.float64, device=dev)
-    x1 = torch.cat(p1) if sum(ns) else torch.zeros(1, 2, dtype=torch.float64, device=dev)
     buf = _launch(x0, x1, offsets, K, max(ns), norm_thresh, conf, max_iters, seed)
-    ok = buf["ok"].bool()
     masks = list(buf["mask"][:sum(ns)].bool().split(ns))
-    R, t = buf["R"], buf["t"].view(B, 3, 1)
-    if as_numpy:
-        return R.cpu().numpy(), t.cpu().numpy(), ok.cpu().numpy(), [m.cpu().numpy() for m in masks]
-    return R, t, ok, masks
+    return _outputs(not isinstance(kpts0_list[0], torch.Tensor), buf["R"], buf["t"].view(B, 3, 1), buf["ok"].bool(), masks)
 
 
 def estimate_pose(kpts0, kpts1, K0, K1, norm_thresh, conf=0.99999, *, max_iters=1000, seed=0):
@@ -191,15 +204,7 @@ def _homog_launch(src, dst, offsets, max_n, method, thr, conf, max_iters, seed):
     kw = dict(batch=B, src=src, dst=dst, offsets=offsets, max_n=int(max_n), thresh=float(thr), conf=float(conf), max_iters=int(max_iters),
               method=int(method), seed=int(seed) & (2 ** 64 - 1), round=0, **buf)
     if ransac:
-        rounds = (int(max_iters) + HOMOG_ROUND - 1) // HOMOG_ROUND
-        for r in range(rounds):
-            kw["round"] = r
-            cabi.call("romab200_homography_hypotheses", "rb_homography_args", **kw)
-            cabi.call("romab200_homography_score", "rb_homography_args", **kw)
-            cabi.call("romab200_homography_select", "rb_homography_args", **kw)
-            if r + 1 < rounds and int(buf["running"].item()) == 0:
-                break
-        kw["round"] = 0
+        _ransac_rounds("homography", "rb_homography_args", kw, HOMOG_ROUND)
     cabi.call("romab200_homography_refine", "rb_homography_args", **kw)
     return buf
 
@@ -210,28 +215,12 @@ def find_homography_batched(src_list, dst_list, method=RANSAC, ransacReprojThres
     Returns (H [B, 3, 3] float64, ok [B] bool, masks: list of uint8 [N_b, 1]); numpy inputs give numpy outputs, tensors give
     device tensors.  ok[b] is False where `find_homography` returns None, and for pairs of fewer than 4 points (mask all zero);
     H[b] is zero there."""
-    if len(src_list) != len(dst_list) or len(src_list) == 0:
-        raise ValueError("src_list and dst_list must be non-empty and of the same length")
     method, thr, conf, max_iters = _homog_args(method, ransacReprojThreshold, confidence, maxIters)
-    dev = _device("find_homography")
-    as_numpy = not isinstance(src_list[0], torch.Tensor)
-    ps = [_homog_points(p, dev) for p in src_list]
-    pd = [_homog_points(p, dev) for p in dst_list]
-    for a, b in zip(ps, pd):
-        if a.shape != b.shape:
-            raise ValueError(f"srcPoints and dstPoints differ in shape: {tuple(a.shape)} vs {tuple(b.shape)}")
-    B = len(ps)
-    ns = [a.shape[0] for a in ps]
-    offsets = torch.tensor(np.concatenate([[0], np.cumsum(ns)]), dtype=torch.int64, device=dev)
-    src = torch.cat(ps) if sum(ns) else torch.zeros(1, 2, dtype=torch.float32, device=dev)
-    dst = torch.cat(pd) if sum(ns) else torch.zeros(1, 2, dtype=torch.float32, device=dev)
+    src, dst, offsets, ns = _pack_pairs(src_list, dst_list, _homog_points, "find_homography", ("src_list", "dst_list"),
+                                        ("srcPoints", "dstPoints"))
     buf = _homog_launch(src, dst, offsets, max(ns), method, thr, conf, max_iters, seed)
-    ok = buf["ok"].bool()
     masks = [m.view(-1, 1) for m in buf["mask"][:sum(ns)].split(ns)]
-    H = buf["out_H"].view(B, 3, 3)
-    if as_numpy:
-        return H.cpu().numpy(), ok.cpu().numpy(), [m.cpu().numpy() for m in masks]
-    return H, ok, masks
+    return _outputs(not isinstance(src_list[0], torch.Tensor), buf["out_H"].view(len(ns), 3, 3), buf["ok"].bool(), masks)
 
 
 def find_homography(srcPoints, dstPoints, method=0, ransacReprojThreshold=3, mask=None, maxIters=2000, confidence=0.995, *, seed=0):
