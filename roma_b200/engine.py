@@ -26,24 +26,25 @@ from __future__ import annotations
 import math
 import os
 from contextlib import contextmanager
-from typing import Dict, Optional, Tuple
+from typing import Optional, Tuple
 
 import torch
 import torch.nn.functional as F
 
 from . import arch, cabi, sampling
 from .cabi import call
+from .cache import BufferArena
 from .packing import PackedWeights, Split, pad8
 
 PRECISIONS = {"fp32": torch.float32, "fp32_simt": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
 F16S = cabi.RB_F16S
 
 
-class Engine:
+class Engine(BufferArena):
     def __init__(self, matcher_sd, dino_sd, device, precision: str = "fp32"):
         if precision not in PRECISIONS:
             raise ValueError(f"precision must be one of {list(PRECISIONS)}")
-        self.device = torch.device(device)
+        super().__init__(device)                 # activation buffers and per-resolution constants
         if self.device.type != "cuda":
             raise RuntimeError("roma_b200 runs on a CUDA device only (there is no CPU fallback); "
                                f"got device={device!r}")
@@ -55,9 +56,6 @@ class Engine:
         self._lane = "main"                      # scratch buffers are per stream ("main" / "side")
         with torch.cuda.device(self.device):
             self.w = PackedWeights(matcher_sd, dino_sd, self.device, self.dtype, split=self.split)
-        self._buf: Dict[tuple, torch.Tensor] = {}
-        self.generation = 0
-        self._const: Dict[tuple, torch.Tensor] = {}
         self.debug: Optional[dict] = None        # set to {} to keep stage tensors (tests)
         self.use_flash_attn = True               # fused tensor-core attention in the 16-bit modes (else QK^T / softmax / PV GEMMs)
         self.gp_algo = 2 if precision == "fp32_simt" else 3   # 3: 128-wide blocks factored in shared memory + explicit block inverses, the
@@ -90,28 +88,13 @@ class Engine:
 
     # ------------------------------------------------------------------ buffers and constants
     def buf(self, name, shape, dtype=None, zero=False):
-        dtype = dtype or self.dtype
-        key = (name, tuple(shape), dtype)
-        t = self._buf.get(key)
-        if t is None:
-            t = (torch.zeros if zero else torch.empty)(tuple(shape), dtype=dtype, device=self.device)
-            self._buf[key] = t
-        return t
+        return super().buf(name, shape, dtype or self.dtype, zero)
 
     def sbuf(self, name, shape, zero=False) -> Split:
         """A cached RB_F16S buffer: two fp16 planes of `shape`."""
         return Split(self.buf(name + ".hi", shape, torch.float16, zero), self.buf(name + ".lo", shape, torch.float16, zero))
 
-    def free_buffers(self):
-        self._buf.clear()
-        self.generation += 1       # captured CUDA graphs hold raw pointers into these buffers: the matcher drops them
-
-    def const(self, key, make):
-        t = self._const.get(key)
-        if t is None:
-            t = make().to(self.device)
-            self._const[key] = t
-        return t
+    free_buffers = BufferArena.free
 
     def grid_axis(self, n):
         """linspace(-1+1/n, 1-1/n, n): pixel-centre coordinates (matcher.py:365-377)."""

@@ -18,6 +18,7 @@ import torch.nn.functional as F
 from PIL import Image
 
 from . import cabi
+from .cache import GraphCache
 from .engine import Engine
 from .preprocess import DeviceImage, DevicePreprocessor, open_inputs
 from .sampling import sample_device
@@ -39,10 +40,9 @@ class RegressionMatcher:
         self.training = False
         self.device_sampler = True      # sample(): weighted sampling without replacement in one kernel per draw (False: torch.multinomial)
         self.use_cuda_graph = True      # replay the whole device side of match() as one CUDA graph per input shape
-        self._graphs = {}
+        self._graphs = GraphCache()
         self._pre = None
-        self._sample_state = {}         # static buffers + CUDA graph of the device sampler, per (n, num, mode)
-        self.graph_launches = 0         # kernels launched through graph replays (cabi.kernel_launches counts eager ones)
+        self._sample_graphs = GraphCache()      # static buffers + CUDA graph of the device sampler, per (n, num, mode)
 
     # ---- nn.Module-ish conveniences callers rely on ------------------------------------------------
     def train(self, mode: bool = True):
@@ -58,10 +58,15 @@ class RegressionMatcher:
     def _get_device(self):
         return self.engine.device
 
+    @property
+    def graph_launches(self):
+        """Kernels launched through replays of the match() graphs (cabi.kernel_launches() counts eager ones)."""
+        return self._graphs.launches
+
     def free_buffers(self):
         """Release every cached activation buffer and the CUDA graphs recorded over them."""
         self._graphs.clear()
-        self._sample_state.clear()
+        self._sample_graphs.clear()
         self.engine.free_buffers()
 
     def get_output_resolution(self):
@@ -157,11 +162,6 @@ class RegressionMatcher:
         with torch.cuda.device(eng.device):
             return self._match_device(a_t, b_t, a_h, b_h, b, symmetric, scale_factor)
 
-    def _run_device(self, images, images_hi, b, symmetric, scale_factor, attenuate, warp, cert):
-        """Both passes + epilogue on the current stream; no allocation, no host sync (CUDA-graph capturable)."""
-        sf_hi = math.sqrt(self.upsample_res[0] * self.upsample_res[1] / (560 ** 2))
-        self.engine.run_match(images, images_hi, b, symmetric, scale_factor, sf_hi, attenuate, warp, cert)
-
     def _match_device(self, a_t, b_t, a_h, b_h, b, symmetric, scale_factor):
         eng = self.engine
         dev = eng.device
@@ -172,43 +172,23 @@ class RegressionMatcher:
         use_graph = self.use_cuda_graph and eng.debug is None and eng.profile is None and eng.gemm_profile is None
         key = (b, hs, ws, ho if a_h is not None else 0, wo if a_h is not None else 0, symmetric, attenuate, float(scale_factor),
                tuple(self.upsample_res))
-        entry = self._graphs.get(key) if use_graph else None
-        if entry is not None and entry["generation"] != eng.generation:
-            # Engine.free_buffers() released the activation buffers this graph's kernels point into: re-record
-            del self._graphs[key]
-            entry = None
-        if entry is None:
-            images = torch.empty(2 * b, 3, hs, ws, dtype=torch.float32, device=dev)
-            images_hi = torch.empty(2 * b, 3, ho, wo, dtype=torch.float32, device=dev) if a_h is not None else None
-            warp = torch.empty(b, ho, wout, 4, dtype=torch.float32, device=dev)
-            cert = torch.empty(b, ho, wout, dtype=torch.float32, device=dev)
-            entry = dict(images=images, images_hi=images_hi, warp=warp, cert=cert, graph=None, calls=0, generation=eng.generation)
-            if use_graph:
-                self._graphs[key] = entry
-        entry["images"][:b].copy_(a_t, non_blocking=True)
-        entry["images"][b:].copy_(b_t, non_blocking=True)
+        entry = self._graphs.entry(key, lambda: dict(
+            images=torch.empty(2 * b, 3, hs, ws, dtype=torch.float32, device=dev),
+            images_hi=torch.empty(2 * b, 3, ho, wo, dtype=torch.float32, device=dev) if a_h is not None else None,
+            warp=torch.empty(b, ho, wout, 4, dtype=torch.float32, device=dev), cert=torch.empty(b, ho, wout, dtype=torch.float32, device=dev)),
+            use_graph, eng.generation)
+        bufs = entry["bufs"]
+        bufs["images"][:b].copy_(a_t, non_blocking=True)
+        bufs["images"][b:].copy_(b_t, non_blocking=True)
         if a_h is not None:
-            entry["images_hi"][:b].copy_(a_h, non_blocking=True)
-            entry["images_hi"][b:].copy_(b_h, non_blocking=True)
-        args = (entry["images"], entry["images_hi"], b, symmetric, scale_factor, attenuate, entry["warp"], entry["cert"])
+            bufs["images_hi"][:b].copy_(a_h, non_blocking=True)
+            bufs["images_hi"][b:].copy_(b_h, non_blocking=True)
+        sf_hi = math.sqrt(self.upsample_res[0] * self.upsample_res[1] / (560 ** 2))
+        self._graphs.run(entry, lambda: eng.run_match(bufs["images"], bufs["images_hi"], b, symmetric, scale_factor, sf_hi, attenuate,
+                                                      bufs["warp"], bufs["cert"]))
         if not use_graph:
-            self._run_device(*args)
-            return entry["warp"], entry["cert"]
-        entry["calls"] += 1
-        if entry["graph"] is None:
-            self._run_device(*args)                 # eager: also allocates every activation buffer
-            if entry["calls"] >= 2:                 # second call with this shape: capture for all later calls
-                torch.cuda.synchronize(dev)
-                graph = torch.cuda.CUDAGraph()
-                launches0 = cabi.kernel_launches()
-                with torch.cuda.graph(graph):
-                    self._run_device(*args)
-                entry["graph"] = graph
-                entry["launches"] = cabi.kernel_launches() - launches0
-        else:
-            entry["graph"].replay()
-            self.graph_launches += entry["launches"]
-        return entry["warp"].clone(), entry["cert"].clone()
+            return bufs["warp"], bufs["cert"]
+        return bufs["warp"].clone(), bufs["cert"].clone()
 
     # ---- sampling (matcher.py:598-629) ----------------------------------------------------------------
     def sample(self, matches, certainty, num=10000):
@@ -240,7 +220,7 @@ class RegressionMatcher:
         return good_matches[balanced_samples], good_certainty[balanced_samples]
 
     def _sample_device(self, matches, certainty, num):
-        return sample_device(self._sample_state, self.engine.kde, matches, certainty, num, self.sample_mode, self.sample_thresh,
+        return sample_device(self._sample_graphs, self.engine.kde, matches, certainty, num, self.sample_mode, self.sample_thresh,
                              self.use_cuda_graph)
 
     # ---- small geometry helpers (matcher.py:672-773) ---------------------------------------------------

@@ -5,10 +5,11 @@ from __future__ import annotations
 import torch
 
 from . import cabi
+from .cache import GraphCache
 
 
-def sample_device(cache: dict, kde, matches, certainty, num, sample_mode, sample_thresh, use_cuda_graph=True):
-    """Device sampler; from the second call with the same sizes on, the whole chain (two draws, sort, gathers, KDE) is one
+def sample_device(cache: GraphCache, kde, matches, certainty, num, sample_mode, sample_thresh, use_cuda_graph=True):
+    """Device sampler; from the third call with the same sizes on, the whole chain (two draws, sort, gathers, KDE) is one
     CUDA-graph replay fed through static buffers, with the two seeds of a call written to a device word.  `cache` holds those
     buffers and graphs per (n, num, mode) for the owning matcher; `kde(x, std, half)` is the density kernel's wrapper."""
     balanced = "balanced" in sample_mode
@@ -17,21 +18,20 @@ def sample_device(cache: dict, kde, matches, certainty, num, sample_mode, sample
     with torch.cuda.device(dev):
         n = certainty.numel()
         key = (n, num, sample_mode, float(sample_thresh), dev.index)
-        st = cache.get(key)
-        if st is None:
-            k1 = min((4 if balanced else 1) * num, n)
-            st = dict(m=torch.empty(n, 4, device=dev), c=torch.empty(n, device=dev), seeds=torch.zeros(2, dtype=torch.int64, device=dev),
-                      seeds_host=torch.zeros(2, dtype=torch.int64).pin_memory(), idx1=torch.empty(k1, dtype=torch.int32, device=dev),
-                      idx2=torch.empty(min(num, k1), dtype=torch.int32, device=dev), keys=torch.empty(n, device=dev),
-                      scratch=torch.empty(2056, dtype=torch.int32, device=dev), k1=k1, graph=None, calls=0, out=None)
-            cache[key] = st
+        k1 = min((4 if balanced else 1) * num, n)
+        entry = cache.entry(key, lambda: dict(
+            m=torch.empty(n, 4, device=dev), c=torch.empty(n, device=dev), seeds=torch.zeros(2, dtype=torch.int64, device=dev),
+            seeds_host=torch.zeros(2, dtype=torch.int64).pin_memory(), idx1=torch.empty(k1, dtype=torch.int32, device=dev),
+            idx2=torch.empty(min(num, k1), dtype=torch.int32, device=dev), keys=torch.empty(n, device=dev),
+            scratch=torch.empty(2056, dtype=torch.int32, device=dev)), use_cuda_graph)
+        st = entry["bufs"]
         st["m"].copy_(matches.reshape(-1, 4), non_blocking=True)
         st["c"].copy_(certainty.reshape(-1), non_blocking=True)
         st["seeds_host"].copy_(torch.randint(0, 2 ** 62, (2,), dtype=torch.int64))       # CPU generator: follows torch.manual_seed
         st["seeds"].copy_(st["seeds_host"], non_blocking=True)
 
         def chain():
-            m, c, k1 = st["m"], st["c"], st["k1"]
+            m, c = st["m"], st["c"]
             cabi.call("romab200_weighted_sample", "rb_sample_args", values=c, n=n, k=k1, batch=1, stride=n, seed=0, seed_dev=st["seeds"],
                       transform=cabi.SAMPLE_THRESHOLD if thresholded else cabi.SAMPLE_IDENTITY, param=float(sample_thresh),
                       out_idx=st["idx1"], out_weights=None, keys=st["keys"], scratch=st["scratch"])
@@ -47,18 +47,8 @@ def sample_device(cache: dict, kde, matches, certainty, num, sample_mode, sample
             sel = st["idx2"].long().sort().values
             return good_matches[sel], w1[sel]
 
-        st["calls"] += 1
-        if st["graph"] is not None:
-            st["graph"].replay()
-            return st["out"][0].clone(), st["out"][1].clone()
-        out = chain()
-        if use_cuda_graph and st["calls"] >= 2:
-            torch.cuda.synchronize(dev)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph):
-                st["out"] = chain()
-            st["graph"] = graph
-        return out
+        out, replayed = cache.run(entry, chain)
+        return (out[0].clone(), out[1].clone()) if replayed else out
 
 
 def kde(x: torch.Tensor, std: float = 0.1, half: bool = True, symmetric: bool = True):

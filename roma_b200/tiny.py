@@ -29,6 +29,7 @@ from PIL import Image
 
 from . import cabi
 from .cabi import call
+from .cache import BufferArena, GraphCache
 from .preprocess import DeviceImage, open_inputs
 from .matcher import RegressionMatcher
 from .packing import fold_bn
@@ -177,8 +178,8 @@ class TinyRoMa:
         self.exact_softmax = exact_softmax
         self.training = False
         self.use_cuda_graph = True
-        self._buf, self._const, self._graphs, self._sample_state = {}, {}, {}, {}
-        self.generation = 0
+        self.arena = BufferArena(self._device)
+        self._graphs, self._sample_graphs = GraphCache(), GraphCache()
         with torch.cuda.device(self._device):
             xsd = {k[len("xfeat.0."):]: v for k, v in sd.items() if k.startswith("xfeat.0.")}
             self.norm = self.plan["norm"][0] if self.plan["norm"] else None
@@ -217,29 +218,16 @@ class TinyRoMa:
     def free_buffers(self):
         """Release every cached activation buffer and the CUDA graphs recorded over them."""
         self._graphs.clear()
-        self._sample_state.clear()
-        self._buf.clear()
-        self.generation += 1
+        self._sample_graphs.clear()
+        self.arena.free()
 
     # ---- buffers and constants --------------------------------------------------------------------------
     def _b(self, name, shape):
-        key = (name, tuple(shape))
-        t = self._buf.get(key)
-        if t is None:
-            t = torch.zeros(tuple(shape), dtype=torch.float32, device=self._device)     # zero: pad channels must read as 0
-            self._buf[key] = t
-        return t
-
-    def _c(self, key, make):
-        t = self._const.get(key)
-        if t is None:
-            t = make().to(self._device)
-            self._const[key] = t
-        return t
+        return self.arena.buf(name, shape, torch.float32, zero=True)     # zero: pad channels must read as 0
 
     def _linspace(self, lo, n):
         """torch.linspace(-1 + lo, 1 - lo, n) evaluated on the host like the reference, then uploaded."""
-        return self._c(("lin", lo, n), lambda: torch.linspace(-1 + lo, 1 - lo, n))
+        return self.arena.const(("lin", lo, n), lambda: torch.linspace(-1 + lo, 1 - lo, n))
 
     # ---- device pipeline ------------------------------------------------------------------------------
     def _conv(self, L, x, n, h, w, c, out_name, R=None, col_scale=None):
@@ -321,7 +309,7 @@ class TinyRoMa:
         H1, W1 = p1.shape[-2:]
         if min(p0.shape[-2:]) < 32 or min(H1, W1) < 32:
             raise ValueError("TinyRoMa needs images of at least 32 x 32 pixels")
-        self._to_normalized = self._c(("to_normalized", H1, W1), lambda: torch.tensor((2 / W1, 2 / H1, 1)))
+        self._to_normalized = self.arena.const(("to_normalized", H1, W1), lambda: torch.tensor((2 / W1, 2 / H1, 1)))
         if p0.shape[1:] == p1.shape[1:]:
             both = self._b("pre01", (2 * B,) + tuple(p0.shape[1:]))
             both[:B].copy_(p0)
@@ -393,33 +381,17 @@ class TinyRoMa:
             raise ValueError(f"TinyRoMa.match: batch sizes differ ({im0.shape[0]} vs {im1.shape[0]})")
         B, _, H0, W0 = im0.shape
         exact = bool(self.exact_softmax)
-        use_graph = self.use_cuda_graph
         key = (tuple(im0.shape), tuple(im1.shape), exact)
-        with torch.cuda.device(self._device):
-            entry = self._graphs.get(key) if use_graph else None
-            if entry is not None and entry["generation"] != self.generation:
-                entry = None
-            if entry is None:
-                entry = dict(im0=torch.empty(im0.shape, device=self._device), im1=torch.empty(im1.shape, device=self._device),
-                             warp=torch.empty(B, H0, W0, 4, device=self._device), cert=torch.empty(B, H0, W0, device=self._device),
-                             graph=None, calls=0, generation=self.generation)
-                if use_graph:
-                    self._graphs[key] = entry
-            entry["im0"].copy_(im0, non_blocking=True)
-            entry["im1"].copy_(im1, non_blocking=True)
-            args = (entry["im0"], entry["im1"], exact, entry["warp"], entry["cert"])
-            entry["calls"] += 1
-            if entry["graph"] is not None:
-                entry["graph"].replay()
-            else:
-                self._match_device(*args)           # eager: also allocates every activation buffer
-                if use_graph and entry["calls"] >= 2:      # second call with this shape: capture for all later calls
-                    torch.cuda.synchronize(self._device)
-                    graph = torch.cuda.CUDAGraph()
-                    with torch.cuda.graph(graph):
-                        self._match_device(*args)
-                    entry["graph"] = graph
-            warp, cert = entry["warp"].clone(), entry["cert"].clone()
+        dev = self._device
+        with torch.cuda.device(dev):
+            entry = self._graphs.entry(key, lambda: dict(
+                im0=torch.empty(im0.shape, device=dev), im1=torch.empty(im1.shape, device=dev),
+                warp=torch.empty(B, H0, W0, 4, device=dev), cert=torch.empty(B, H0, W0, device=dev)), self.use_cuda_graph, self.arena.generation)
+            bufs = entry["bufs"]
+            bufs["im0"].copy_(im0, non_blocking=True)
+            bufs["im1"].copy_(im1, non_blocking=True)
+            self._graphs.run(entry, lambda: self._match_device(bufs["im0"], bufs["im1"], exact, bufs["warp"], bufs["cert"]))
+            warp, cert = bufs["warp"].clone(), bufs["cert"].clone()
         return (warp, cert) if batched else (warp[0], cert[0])
 
     @torch.inference_mode()
@@ -439,7 +411,7 @@ class TinyRoMa:
         H, W, _ = matches.shape
         if not matches.is_cuda:
             raise RuntimeError("roma_b200.sample needs CUDA tensors (no CPU fallback)")
-        return sample_device(self._sample_state, kde, matches, certainty, num, self.sample_mode, self.sample_thresh, self.use_cuda_graph)
+        return sample_device(self._sample_graphs, kde, matches, certainty, num, self.sample_mode, self.sample_thresh, self.use_cuda_graph)
 
     # ---- geometry helpers (identical to RoMa's, tiny.py:102-113) ----------------------------------------
     _to_pixel_coordinates = RegressionMatcher._to_pixel_coordinates

@@ -242,3 +242,43 @@ def test_prologue_tiles_matches_kernel_geometry():
     for r, (tx, ty) in shapes.items():
         for h, w in ((40, 40), (70, 70), (108, 108), (13, 9), (1, 1)):
             assert cabi.prologue_tiles(r, h, w) == -(-h // ty) * -(-w // tx), (r, h, w)
+
+
+def test_graph_cache_policy(monkeypatch):
+    """GraphCache: eager on call 1, eager then capture on call 2, replay from call 3 (counting the captured launches); an entry
+    of an older arena generation is made again; a disabled entry is neither kept nor captured.  CUDA graphs are a host stand-in."""
+    from contextlib import contextmanager
+    from roma_b200 import cache
+    events, launches = [], [0]
+
+    class FakeGraph:
+        def replay(self):
+            events.append("replay")
+
+    @contextmanager
+    def capture(graph):
+        events.append("capture")
+        yield
+    monkeypatch.setattr(torch.cuda, "CUDAGraph", FakeGraph)
+    monkeypatch.setattr(torch.cuda, "graph", capture)
+    monkeypatch.setattr(torch.cuda, "synchronize", lambda *a: None)
+    monkeypatch.setattr(cache.cabi, "kernel_launches", lambda: launches[0])
+
+    def work(i):
+        events.append("run")
+        launches[0] += 3
+        return i
+    gc, outs = cache.GraphCache(), []
+    for i in range(4):
+        e = gc.entry("k", lambda: {"i": i}, True, 0)
+        outs.append(gc.run(e, lambda: work(i)))
+    assert events == ["run", "run", "capture", "run", "replay", "replay"]
+    assert outs == [(0, False), (1, False), (1, True), (1, True)] and e["bufs"] == {"i": 0} and gc.launches == 6
+    e2 = gc.entry("k", lambda: {"i": 9}, True, 1)
+    assert e2 is not e and e2["bufs"] == {"i": 9} and gc.run(e2, lambda: work(9)) == (9, False) and gc["k"] is e2
+    events.clear()
+    for _ in range(3):
+        assert gc.run(gc.entry("off", lambda: {}, False), lambda: work(5)) == (5, False)
+    assert events == ["run"] * 3 and "off" not in gc
+    gc.clear()
+    assert not gc and gc.launches == 6

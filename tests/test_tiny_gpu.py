@@ -172,6 +172,12 @@ def test_match_graph_replay_bit_equal(tiny):
     outs = [model.match(a, b) for _ in range(4)]          # eager, eager + capture, replay, replay
     key = next(k for k in model._graphs if k[0] == (1, 3, 96, 128))
     assert model._graphs[key]["graph"] is not None
+    model.free_buffers()                                  # drops the graphs with the buffers they point into
+    outs += [model.match(a, b) for _ in range(3)]
+    graph = model._graphs[key]["graph"]
+    model.arena.free()                                    # the buffers alone: the graph recorded over them must not be replayed
+    outs += [model.match(a, b) for _ in range(3)]
+    assert model._graphs[key]["graph"] not in (None, graph)
     for w, c in outs[1:]:
         assert torch.equal(w, outs[0][0]) and torch.equal(c, outs[0][1])
 
