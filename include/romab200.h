@@ -12,7 +12,8 @@
  *     immediately: 0 = ok, non-zero = error, message via romab200_last_error() (thread-local);
  *   - activations are channels-last ("NHWC"): a [B,H,W,C] map is a row-major [B*H*W, C] matrix with an
  *     explicit row pitch, so 1x1 convolutions and Linear layers are the same GEMM;
- *   - dtypes: RB_F32 / RB_F16 / RB_BF16; accumulation is always fp32.
+ *   - dtypes: RB_F32 / RB_F16 / RB_BF16; accumulation is always fp32.  An entry point refuses a dtype code it has no kernel
+ *     for, before any CUDA call: non-zero return, message "<op>: unsupported dtype <code>".
  *   - RB_F16S ("split fp16 pair") is the storage format of the tensor-core parity mode: a matrix is held as TWO fp16
  *     planes of the same pitch, hi = fp16(x) and lo = fp16((x - hi) * 2^11), value = hi + lo * 2^-11: 22 significand bits
  *     with the exponent range of fp16 (the reference's own CUDA autocast range).  romab200_gemm contracts such operands

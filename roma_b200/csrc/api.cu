@@ -45,6 +45,9 @@ extern "C" int romab200_gemm(const rb_gemm_args* a, void* stream) {
     using namespace rb;
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a && a->A && a->B && a->C, "gemm: null operand");
+    // the epilogues of both back-ends convert the output and the residual at run time
+    if (a->dtype_c != RB_F16S && check_dtype<float, __half, __nv_bfloat16>(a->dtype_c, "gemm")) return 1;
+    if (a->R && check_dtype<float, __half, __nv_bfloat16>(a->dtype_r, "gemm")) return 1;
     int backend = a->backend;
     if (backend == RB_BACKEND_AUTO) backend = a->dtype_ab == RB_F32 ? RB_BACKEND_SIMT : RB_BACKEND_TCGEN05;
     if (backend == RB_BACKEND_SIMT) return gemm_simt(a, st);

@@ -7,6 +7,7 @@
 #include <stdint.h>
 #include <stdio.h>
 #include <stdarg.h>
+#include <type_traits>
 #include "../../include/romab200.h"
 
 namespace rb {
@@ -26,6 +27,40 @@ template <typename T> struct DT;
 template <> struct DT<float> { static constexpr int id = RB_F32; };
 template <> struct DT<__half> { static constexpr int id = RB_F16; };
 template <> struct DT<__nv_bfloat16> { static constexpr int id = RB_BF16; };
+
+// Dtype dispatch of the entry points: returns f(type_tag<T>{}) for the T among Ts whose code is `code`; any other code is refused
+// with "<what>: unsupported dtype <code>" and 1.  List exactly the types the caller has kernels for: a generic lambda instantiates
+// its body (and the kernels it launches) once per listed type.
+template <typename T> struct type_tag { using type = T; };
+template <typename... Ts, typename F>
+inline int with_dtype(int code, const char* what, F&& f) {
+    int rc = 0;
+    if (((code == DT<Ts>::id ? (rc = f(type_tag<Ts>{}), true) : false) || ...)) return rc;
+    set_error("%s: unsupported dtype %d", what, code);
+    return 1;
+}
+// the same refusal for kernels that take the code itself and convert at run time
+template <typename... Ts>
+inline int check_dtype(int code, const char* what) { return with_dtype<Ts...>(code, what, [](auto) { return 0; }); }
+
+// The same for an integer template parameter (window radius, lanes per pixel): f(std::integral_constant<int, V>{}) for the V among
+// Vs equal to v; any other value: "<what> <v> unsupported (<Vs>)", 1.
+template <int... Vs, typename F>
+inline int with_value(int v, const char* what, F&& f) {
+    int rc = 0;
+    if (((v == Vs ? (rc = f(std::integral_constant<int, Vs>{}), true) : false) || ...)) return rc;
+    const int vs[] = {Vs...};
+    char list[64] = "";
+    for (int i = 0, n = 0; i < (int)sizeof...(Vs); ++i) n += snprintf(list + n, sizeof(list) - n, i ? ", %d" : "%d", vs[i]);
+    set_error("%s %d unsupported (%s)", what, v, list);
+    return 1;
+}
+
+// 1-D grid of `block`-thread CTAs over `total` elements: at least one CTA and at most `cap` (the kernels loop over the rest)
+inline unsigned grid1d(int64_t total, int block, int64_t cap) {
+    const int64_t g = (total + block - 1) / block;
+    return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
+}
 
 __device__ __forceinline__ float to_f(float v) { return v; }
 __device__ __forceinline__ float to_f(__half v) { return __half2float(v); }

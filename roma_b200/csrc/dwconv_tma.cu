@@ -164,44 +164,37 @@ extern "C" int romab200_debug_dwclk(long long* out, int reset) {
 }
 #endif
 
-template <typename TIN>
-static int launch_dw(const CUtensorMap& map, const DwTmaParams& p, dim3 grid, cudaStream_t st) {
-    using Cfg = DwCfg<TIN>;
-    if (ensure_smem<dwconv5x5_relu_tma_kernel<TIN>>(Cfg::SMEM, "dwconv")) return 1;
-    rb::launch_pdl(dwconv5x5_relu_tma_kernel<TIN>, grid, dim3(Cfg::THREADS), Cfg::SMEM, st, map, p);
-    return check_launch("dwconv5x5_relu_tma");
-}
-
 // 16-bit maps (same type out), or fp32 maps with an RB_F16S result (a->out_lo != NULL); the caller has checked the pitches
 // (ldi * element size % 16 == 0, ldo % 2 == 0) and the 16-byte alignment of the input.
 int dwconv_tma(const rb_dwconv_args* a, cudaStream_t st) {
-    const bool f32 = a->dtype == RB_F32;
-    RB_REQUIRE(!f32 || a->out_lo, "dwconv_tma: fp32 maps need the RB_F16S output planes");
-    const uint64_t es = f32 ? 4 : 2;
-    const int TH = f32 ? DwCfg<float>::TH : DwCfg<__half>::TH;
-    CUtensorMap map;             // activation [B, H, W, C] with pitch ldi: box = (TH+4) x 20 pixels x 64 channels, borders zero-filled
-    cuuint64_t d4[4] = {(cuuint64_t)a->c, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
-    cuuint64_t s4[3] = {(cuuint64_t)a->ldi * es, (cuuint64_t)a->w * a->ldi * es, (cuuint64_t)a->h * a->w * a->ldi * es};
-    cuuint32_t b4[4] = {(cuuint32_t)DT_CH, (cuuint32_t)DT_IW, (cuuint32_t)(TH + 4), 1};
-    const CUtensorMapDataType dt = f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
-    if (encode_tiled(&map, "dwconv", dt, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
-    DwTmaParams p;
-    p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ldo; p.wgt = a->weight; p.ldw = a->ldw; p.bias = a->bias;
-    p.H = a->h; p.W = a->w; p.C = a->c;
-    p.tiles_x = (a->w + DT_TW - 1) / DT_TW;
-    p.tiles_per_img = p.tiles_x * ((a->h + TH - 1) / TH);
-    const long long total = (long long)p.tiles_per_img * a->batch;
-    RB_REQUIRE(total > 0 && total < (1ll << 31), "dwconv: bad tile count");
-    p.total_tiles = (int)total;
-    const int groups = (a->c + DT_CH - 1) / DT_CH;
-    RB_REQUIRE(groups <= 65535, "dwconv: too many channel groups");
-    int per_group = (f32 ? 1 : 2) * sm_count() / groups;             // resident CTAs per SM (one for the fp32 ring), never more CTAs than fit at once
-    if (per_group < 1) per_group = 1;
-    if (per_group > p.total_tiles) per_group = p.total_tiles;
-    dim3 grid(per_group, groups);
-    if (f32) return launch_dw<float>(map, p, grid, st);
-    if (a->dtype == RB_F16) return launch_dw<__half>(map, p, grid, st);
-    return launch_dw<__nv_bfloat16>(map, p, grid, st);
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "dwconv", [&](auto t) {
+        using TIN = typename decltype(t)::type;
+        using Cfg = DwCfg<TIN>;
+        constexpr bool f32 = std::is_same_v<TIN, float>;
+        RB_REQUIRE(!f32 || a->out_lo, "dwconv_tma: fp32 maps need the RB_F16S output planes");
+        const uint64_t es = sizeof(TIN);
+        CUtensorMap map;             // activation [B, H, W, C] with pitch ldi: box = (TH+4) x 20 pixels x 64 channels, borders zero-filled
+        cuuint64_t d4[4] = {(cuuint64_t)a->c, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
+        cuuint64_t s4[3] = {(cuuint64_t)a->ldi * es, (cuuint64_t)a->w * a->ldi * es, (cuuint64_t)a->h * a->w * a->ldi * es};
+        cuuint32_t b4[4] = {(cuuint32_t)DT_CH, (cuuint32_t)DT_IW, (cuuint32_t)(Cfg::TH + 4), 1};
+        if (encode_tiled(&map, "dwconv", tma_dtype(a->dtype), 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
+        DwTmaParams p;
+        p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ldo; p.wgt = a->weight; p.ldw = a->ldw; p.bias = a->bias;
+        p.H = a->h; p.W = a->w; p.C = a->c;
+        p.tiles_x = (a->w + DT_TW - 1) / DT_TW;
+        p.tiles_per_img = p.tiles_x * ((a->h + Cfg::TH - 1) / Cfg::TH);
+        const long long total = (long long)p.tiles_per_img * a->batch;
+        RB_REQUIRE(total > 0 && total < (1ll << 31), "dwconv: bad tile count");
+        p.total_tiles = (int)total;
+        const int groups = (a->c + DT_CH - 1) / DT_CH;
+        RB_REQUIRE(groups <= 65535, "dwconv: too many channel groups");
+        int per_group = (f32 ? 1 : 2) * sm_count() / groups;             // resident CTAs per SM (one for the fp32 ring), never more CTAs than fit at once
+        if (per_group < 1) per_group = 1;
+        if (per_group > p.total_tiles) per_group = p.total_tiles;
+        if (ensure_smem<dwconv5x5_relu_tma_kernel<TIN>>(Cfg::SMEM, "dwconv")) return 1;
+        rb::launch_pdl(dwconv5x5_relu_tma_kernel<TIN>, dim3(per_group, groups), dim3(Cfg::THREADS), Cfg::SMEM, st, map, p);
+        return check_launch("dwconv5x5_relu_tma");
+    });
 }
 
 }  // namespace rb

@@ -358,18 +358,13 @@ __global__ void transpose_kernel(const T* __restrict__ src, T* __restrict__ dst,
     }
 }
 
-static inline int grid_for(int64_t total, int block, int cap = 132 * 32) {
-    int64_t g = (total + block - 1) / block;
-    return (int)(g < cap ? (g > 0 ? g : 1) : cap);
-}
-
 // fp32 [batch][rows, cols] (pitch ldx, matrix stride sx) -> RB_F16S planes [batch][rows, ldd] (matrix stride sd); cols % 4 == 0,
 // 16-byte aligned rows
 int split_f16s_batched(const float* x, void* hi, void* lo, int64_t rows, int cols, int64_t ldx, int64_t ldd, int batch, int64_t sx, int64_t sd, cudaStream_t st) {
     RB_REQUIRE(cols % 4 == 0 && ldx % 4 == 0 && ldd % 4 == 0 && sx % 4 == 0 && sd % 4 == 0 && ((uintptr_t)x) % 16 == 0 && ((uintptr_t)hi) % 8 == 0 && ((uintptr_t)lo) % 8 == 0,
                "split_f16s_batched: alignment");
     RB_REQUIRE(batch > 0 && batch <= 65535 && rows > 0, "split_f16s_batched: bad shape");
-    dim3 grid(grid_for(rows * (cols / 4), 256, 132 * 8), batch);
+    dim3 grid(grid1d(rows * (cols / 4), 256, 132 * 8), batch);
     rb::launch_pdl(split_f16s_batched_kernel, grid, dim3(256), 0, st, x, (__half*)hi, (__half*)lo, rows, cols / 4, ldx, ldd, sx, sd);
     return check_launch("split_f16s_batched");
 }
@@ -381,7 +376,6 @@ using namespace rb;
 extern "C" int romab200_layernorm(const rb_layernorm_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0, "layernorm: empty input");
-    const int esy = a->dtype_y == RB_F32 ? 4 : 2;
     RB_REQUIRE(a->dtype_y != RB_F16S || (a->y_lo && a->dtype_x == RB_F32), "layernorm: RB_F16S output needs y_lo and fp32 input");
     if (a->dtype_y == RB_F16S && !(a->cols == 1024 && a->ldx % 4 == 0 && a->ldy % 4 == 0 && ((uintptr_t)a->x) % 16 == 0 &&
                                    ((uintptr_t)a->y) % 8 == 0 && ((uintptr_t)a->y_lo) % 8 == 0 && ((uintptr_t)a->gamma) % 16 == 0 && ((uintptr_t)a->beta) % 16 == 0)) {
@@ -394,30 +388,23 @@ extern "C" int romab200_layernorm(const rb_layernorm_args* a, void* stream) {
         rb::launch_pdl(layernorm_vec_kernel<__half, 8, true>, gridv, dim3(128), 0, st, (const float*)a->x, (__half*)a->y, a->gamma, a->beta, a->rows, a->ldx, a->ldy, a->eps, (__half*)a->y_lo);
         return check_launch("layernorm");
     }
-    if (a->dtype_x == RB_F32 && a->cols == 1024 && a->ldx % 4 == 0 && (a->ldy * esy) % 16 == 0 && ((uintptr_t)a->x) % 16 == 0 &&
-        ((uintptr_t)a->y) % 16 == 0 && ((uintptr_t)a->gamma) % 16 == 0 && ((uintptr_t)a->beta) % 16 == 0) {
-        dim3 gridv((unsigned)((a->rows + 3) / 4));
-#define LNV(TO) rb::launch_pdl(layernorm_vec_kernel<TO, 8, false>, gridv, dim3(128), 0, st, (const float*)a->x, (TO*)a->y, a->gamma, a->beta, a->rows, a->ldx, a->ldy, a->eps, (TO*)nullptr)
-        if (a->dtype_y == RB_F32) LNV(float); else if (a->dtype_y == RB_F16) LNV(__half); else LNV(__nv_bfloat16);
-#undef LNV
+    if (check_dtype<float>(a->dtype_x, "layernorm")) return 1;
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype_y, "layernorm", [&](auto t) {
+        using TO = typename decltype(t)::type;
+        if (a->cols == 1024 && a->ldx % 4 == 0 && (a->ldy * (int)sizeof(TO)) % 16 == 0 && ((uintptr_t)a->x) % 16 == 0 &&
+            ((uintptr_t)a->y) % 16 == 0 && ((uintptr_t)a->gamma) % 16 == 0 && ((uintptr_t)a->beta) % 16 == 0)
+            rb::launch_pdl(layernorm_vec_kernel<TO, 8, false>, dim3((unsigned)((a->rows + 3) / 4)), dim3(128), 0, st, (const float*)a->x, (TO*)a->y, a->gamma, a->beta,
+                           a->rows, a->ldx, a->ldy, a->eps, (TO*)nullptr);
+        else
+            rb::launch_pdl(layernorm_kernel<float, TO>, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, (const float*)a->x, (TO*)a->y, a->gamma, a->beta,
+                           a->rows, a->cols, a->ldx, a->ldy, a->eps);
         return check_launch("layernorm");
-    }
-    int wpb = 8;
-    dim3 grid((unsigned)((a->rows + wpb - 1) / wpb));
-#define LN(TI, TO) rb::launch_pdl(layernorm_kernel<TI, TO>, dim3(grid), dim3(wpb * 32), 0, st, (const TI*)a->x, (TO*)a->y, a->gamma, a->beta, a->rows, a->cols, a->ldx, a->ldy, a->eps)
-    if (a->dtype_x == RB_F32 && a->dtype_y == RB_F32) LN(float, float);
-    else if (a->dtype_x == RB_F32 && a->dtype_y == RB_F16) LN(float, __half);
-    else if (a->dtype_x == RB_F32 && a->dtype_y == RB_BF16) LN(float, __nv_bfloat16);
-    else RB_REQUIRE(false, "layernorm: unsupported dtypes %d -> %d", a->dtype_x, a->dtype_y);
-#undef LN
-    return check_launch("layernorm");
+    });
 }
 
 extern "C" int romab200_softmax_rows(const rb_softmax_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0 && a->rows < (1ll << 31), "softmax: bad shape");
-    const int es = a->dtype == RB_F32 ? 4 : 2;
-    const int vn = 16 / es;
     if (a->out_hi) {
         RB_REQUIRE(a->dtype == RB_F32 && a->out_lo && a->cols <= 2048 && a->lds % 4 == 0 && a->ldo % 4 == 0 && (a->cols + 3) / 4 * 4 <= a->ldo &&
                    (a->cols + 3) / 4 * 4 <= a->lds && ((uintptr_t)a->s) % 16 == 0 && ((uintptr_t)a->out_hi) % 8 == 0 && ((uintptr_t)a->out_lo) % 8 == 0,
@@ -426,34 +413,32 @@ extern "C" int romab200_softmax_rows(const rb_softmax_args* a, void* stream) {
                        a->rows, a->cols, a->lds, a->ldo, a->scale);
         return check_launch("softmax_rows");
     }
-    // rows must be padded to whole 16-byte vectors (the pad columns are rewritten with zeros)
-    if (a->cols <= 2048 && (a->lds * es) % 16 == 0 && ((uintptr_t)a->s) % 16 == 0 && (a->cols + vn - 1) / vn * vn <= a->lds) {
-        unsigned grid = (unsigned)((a->rows + 7) / 8);
-        if (a->dtype == RB_F32) rb::launch_pdl(softmax_rows_warp_kernel<float>, dim3(grid), dim3(256), 0, st, (float*)a->s, a->rows, a->cols, a->lds, a->scale);
-        else if (a->dtype == RB_F16) rb::launch_pdl(softmax_rows_warp_kernel<__half>, dim3(grid), dim3(256), 0, st, (__half*)a->s, a->rows, a->cols, a->lds, a->scale);
-        else rb::launch_pdl(softmax_rows_warp_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (__nv_bfloat16*)a->s, a->rows, a->cols, a->lds, a->scale);
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "softmax_rows", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int vn = 16 / sizeof(T);
+        // warp per row when the rows are padded to whole 16-byte vectors (the pad columns are rewritten with zeros), else block per row
+        const bool warp = a->cols <= 2048 && (a->lds * (int)sizeof(T)) % 16 == 0 && ((uintptr_t)a->s) % 16 == 0 && (a->cols + vn - 1) / vn * vn <= a->lds;
+        rb::launch_pdl(warp ? softmax_rows_warp_kernel<T> : softmax_rows_kernel<T>, dim3((unsigned)(warp ? (a->rows + 7) / 8 : a->rows)), dim3(256), 0, st,
+                       (T*)a->s, a->rows, a->cols, a->lds, a->scale);
         return check_launch("softmax_rows");
-    }
-    if (a->dtype == RB_F32) rb::launch_pdl(softmax_rows_kernel<float>, dim3((unsigned)a->rows), dim3(256), 0, st, (float*)a->s, a->rows, a->cols, a->lds, a->scale);
-    else if (a->dtype == RB_F16) rb::launch_pdl(softmax_rows_kernel<__half>, dim3((unsigned)a->rows), dim3(256), 0, st, (__half*)a->s, a->rows, a->cols, a->lds, a->scale);
-    else rb::launch_pdl(softmax_rows_kernel<__nv_bfloat16>, dim3((unsigned)a->rows), dim3(256), 0, st, (__nv_bfloat16*)a->s, a->rows, a->cols, a->lds, a->scale);
-    return check_launch("softmax_rows");
+    });
 }
 
 extern "C" int romab200_row_norms(const rb_rownorm_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0, "row_norms: empty input");
-    dim3 grid((unsigned)((a->rows + 7) / 8));
-    if (a->dtype == RB_F32) rb::launch_pdl(row_norms_kernel<float>, dim3(grid), dim3(256), 0, st, (const float*)a->x, a->out, a->rows, a->cols, a->ldx);
-    else if (a->dtype == RB_F16) rb::launch_pdl(row_norms_kernel<__half>, dim3(grid), dim3(256), 0, st, (const __half*)a->x, a->out, a->rows, a->cols, a->ldx);
-    else rb::launch_pdl(row_norms_kernel<__nv_bfloat16>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)a->x, a->out, a->rows, a->cols, a->ldx);
-    return check_launch("row_norms");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "row_norms", [&](auto t) {
+        using T = typename decltype(t)::type;
+        rb::launch_pdl(row_norms_kernel<T>, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, (const T*)a->x, a->out, a->rows, a->cols, a->ldx);
+        return check_launch("row_norms");
+    });
 }
 
 extern "C" int romab200_copy2d(const rb_copy2d_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0, "copy2d: empty input");
-    rb::launch_pdl(copy2d_kernel, dim3(grid_for(a->rows * a->cols, 256)), dim3(256), 0, st, a->src, a->dst, a->rows, a->cols, a->lds, a->ldd,
+    if (check_dtype<float, __half, __nv_bfloat16>(a->dtype_src, "copy2d") || check_dtype<float, __half, __nv_bfloat16>(a->dtype_dst, "copy2d")) return 1;
+    rb::launch_pdl(copy2d_kernel, dim3(grid1d(a->rows * a->cols, 256, 132 * 32)), dim3(256), 0, st, a->src, a->dst, a->rows, a->cols, a->lds, a->ldd,
                                                                    a->dtype_src, a->dtype_dst, a->row_scale, a->row_scale_reciprocal);
     return check_launch("copy2d");
 }
@@ -461,7 +446,7 @@ extern "C" int romab200_copy2d(const rb_copy2d_args* a, void* stream) {
 extern "C" int romab200_split_f16x3(const rb_split_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0 && a->ldd >= 3 * a->cols, "split_f16x3: bad shape");
-    rb::launch_pdl(split_f16x3_kernel, dim3(grid_for(a->rows * a->cols, 256)), dim3(256), 0, st, a->x, (__half*)a->dst, a->rows, a->cols, a->ldx, a->ldd,
+    rb::launch_pdl(split_f16x3_kernel, dim3(grid1d(a->rows * a->cols, 256, 132 * 32)), dim3(256), 0, st, a->x, (__half*)a->dst, a->rows, a->cols, a->ldx, a->ldd,
                                                                         a->row_norm, a->layout_b);
     return check_launch("split_f16x3");
 }
@@ -472,10 +457,10 @@ extern "C" int romab200_split_f16s(const rb_split_pair_args* a, void* stream) {
     const int cols4 = (a->cols + 3) / 4;
     if (a->ldx % 4 == 0 && a->ldd % 4 == 0 && (int64_t)cols4 * 4 <= a->ldx && (int64_t)cols4 * 4 <= a->ldd && ((uintptr_t)a->x) % 16 == 0 &&
         ((uintptr_t)a->hi) % 8 == 0 && ((uintptr_t)a->lo) % 8 == 0) {
-        rb::launch_pdl(split_f16s_vec_kernel, dim3(grid_for(a->rows * cols4, 256)), dim3(256), 0, st, a->x, (__half*)a->hi, (__half*)a->lo, a->rows, cols4,
+        rb::launch_pdl(split_f16s_vec_kernel, dim3(grid1d(a->rows * cols4, 256, 132 * 32)), dim3(256), 0, st, a->x, (__half*)a->hi, (__half*)a->lo, a->rows, cols4,
                        a->cols, a->ldx, a->ldd, a->row_norm);
     } else {
-        rb::launch_pdl(split_f16s_kernel, dim3(grid_for(a->rows * a->cols, 256)), dim3(256), 0, st, a->x, (__half*)a->hi, (__half*)a->lo, a->rows, a->cols,
+        rb::launch_pdl(split_f16s_kernel, dim3(grid1d(a->rows * a->cols, 256, 132 * 32)), dim3(256), 0, st, a->x, (__half*)a->hi, (__half*)a->lo, a->rows, a->cols,
                        a->ldx, a->ldd, a->row_norm);
     }
     return check_launch("split_f16s");
@@ -485,17 +470,17 @@ extern "C" int romab200_im2col_patch(const rb_im2col_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->height % a->patch == 0 && a->width % a->patch == 0, "im2col: %dx%d not a multiple of patch %d", a->height, a->width, a->patch);
     int64_t total = (int64_t)a->batch * (a->height / a->patch) * (a->width / a->patch) * 3 * a->patch * a->patch;
-    int g = grid_for(total, 256);
-    if (a->dtype_out == RB_F32) rb::launch_pdl(im2col_patch_kernel<float>, dim3(g), dim3(256), 0, st, a->image, (float*)a->out, a->batch, a->height, a->width, a->patch, a->ldo);
-    else if (a->dtype_out == RB_F16) rb::launch_pdl(im2col_patch_kernel<__half>, dim3(g), dim3(256), 0, st, a->image, (__half*)a->out, a->batch, a->height, a->width, a->patch, a->ldo);
-    else rb::launch_pdl(im2col_patch_kernel<__nv_bfloat16>, dim3(g), dim3(256), 0, st, a->image, (__nv_bfloat16*)a->out, a->batch, a->height, a->width, a->patch, a->ldo);
-    return check_launch("im2col_patch");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype_out, "im2col_patch", [&](auto t) {
+        using TO = typename decltype(t)::type;
+        rb::launch_pdl(im2col_patch_kernel<TO>, dim3(grid1d(total, 256, 132 * 32)), dim3(256), 0, st, a->image, (TO*)a->out, a->batch, a->height, a->width, a->patch, a->ldo);
+        return check_launch("im2col_patch");
+    });
 }
 
 extern "C" int romab200_assemble_tokens(const rb_tokens_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     int64_t total = (int64_t)a->batch * (a->npatch + 1) * a->dim;
-    rb::launch_pdl(assemble_tokens_kernel, dim3(grid_for(total, 256)), dim3(256), 0, st, a->patch, a->cls, a->pos, a->tokens, a->batch, a->npatch, a->dim);
+    rb::launch_pdl(assemble_tokens_kernel, dim3(grid1d(total, 256, 132 * 32)), dim3(256), 0, st, a->patch, a->cls, a->pos, a->tokens, a->batch, a->npatch, a->dim);
     return check_launch("assemble_tokens");
 }
 
@@ -504,9 +489,10 @@ extern "C" int romab200_transpose(const rb_transpose_args* a, void* stream) {
     int b0 = a->batch0 > 0 ? a->batch0 : 1, b1 = a->batch1 > 0 ? a->batch1 : 1;
     dim3 grid((a->cols + 31) / 32, (a->rows + 31) / 32, b0 * b1), block(32, 8);
     RB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "transpose: grid too large");
-    if (a->dtype == RB_F32)
-        rb::launch_pdl(transpose_kernel<float>, dim3(grid), dim3(block), 0, st, (const float*)a->src, (float*)a->dst, a->rows, a->cols, a->lds, a->ldd, b1, a->ss0, a->ss1, a->sd0, a->sd1);
-    else
-        rb::launch_pdl(transpose_kernel<uint16_t>, dim3(grid), dim3(block), 0, st, (const uint16_t*)a->src, (uint16_t*)a->dst, a->rows, a->cols, a->lds, a->ldd, b1, a->ss0, a->ss1, a->sd0, a->sd1);
-    return check_launch("transpose");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "transpose", [&](auto t) {
+        // a transpose only moves bits: the 16-bit types share one kernel
+        using T = std::conditional_t<sizeof(typename decltype(t)::type) == 4, float, uint16_t>;
+        rb::launch_pdl(transpose_kernel<T>, grid, block, 0, st, (const T*)a->src, (T*)a->dst, a->rows, a->cols, a->lds, a->ldd, b1, a->ss0, a->ss1, a->sd0, a->sd1);
+        return check_launch("transpose");
+    });
 }

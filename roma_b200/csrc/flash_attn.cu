@@ -271,30 +271,31 @@ using namespace rb;
 
 extern "C" int romab200_flash_attn(const rb_flash_attn_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    RB_REQUIRE(a->dtype == RB_F16 || a->dtype == RB_BF16 || a->dtype == RB_F16S, "flash_attn: 16-bit or split-fp16 inputs only");
-    RB_REQUIRE(a->head_dim == 64 || (a->head_dim == 128 && a->dtype != RB_F16S), "flash_attn: head_dim %d unsupported (64, 128; split-fp16: 64)", a->head_dim);
-    RB_REQUIRE(a->dtype != RB_F16S || (a->qkv_lo && a->out_lo && ((uintptr_t)a->qkv_lo) % 16 == 0 && ((uintptr_t)a->out_lo) % 16 == 0),
-               "flash_attn: split-fp16 needs 16-byte aligned qkv_lo and out_lo planes");
-    const int dim = a->heads * a->head_dim;
-    RB_REQUIRE(a->ld_qkv >= 3 * dim && (a->ld_qkv * 2) % 16 == 0 && ((uintptr_t)a->qkv) % 16 == 0, "flash_attn: qkv pitch/alignment");
-    RB_REQUIRE(a->ld_out >= dim && (a->ld_out * 2) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0, "flash_attn: out pitch/alignment");
-    RB_REQUIRE(a->batch > 0 && a->batch <= 65535 && a->n_tokens > 0, "flash_attn: bad batch / token count");
-    // [batch, tokens, 3 * dim] with boxes of 64 tokens x 64 columns, 128B-swizzled: one plane (hi) or two (hi, lo)
-    cuuint64_t dims[3] = {(cuuint64_t)(3 * dim), (cuuint64_t)a->n_tokens, (cuuint64_t)a->batch};
-    cuuint64_t strides[2] = {(cuuint64_t)a->ld_qkv * 2, (cuuint64_t)a->ld_qkv * 2 * (cuuint64_t)a->n_tokens};
-    cuuint32_t box[3] = {64, 64, 1};
-    CUtensorMap map_hi, map_lo;
-    if (encode_tiled(&map_hi, "flash_attn", a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->qkv,
-                     dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
-    map_lo = map_hi;
-    if (a->dtype == RB_F16S &&
-        encode_tiled(&map_lo, "flash_attn (lo plane)", CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, a->qkv_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
-        return 1;
-    FaParams p;
-    p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ld_out; p.N = a->n_tokens; p.heads = a->heads; p.dim = dim;
-    p.scale_log2 = 1.4426950408889634f / sqrtf((float)a->head_dim);
-    if (a->dtype == RB_F16S) return launch_fa<64, __half, true>(map_hi, map_lo, p, a->batch, st);
-    if (a->head_dim == 64)
-        return a->dtype == RB_F16 ? launch_fa<64, __half, false>(map_hi, map_lo, p, a->batch, st) : launch_fa<64, __nv_bfloat16, false>(map_hi, map_lo, p, a->batch, st);
-    return a->dtype == RB_F16 ? launch_fa<128, __half, false>(map_hi, map_lo, p, a->batch, st) : launch_fa<128, __nv_bfloat16, false>(map_hi, map_lo, p, a->batch, st);
+    const bool split = a->dtype == RB_F16S;
+    // RB_F16S is a pair of fp16 planes
+    return with_dtype<__half, __nv_bfloat16>(split ? RB_F16 : a->dtype, "flash_attn", [&](auto t) {
+        using T = typename decltype(t)::type;
+        RB_REQUIRE(a->head_dim == 64 || (a->head_dim == 128 && !split), "flash_attn: head_dim %d unsupported (64, 128; split-fp16: 64)", a->head_dim);
+        RB_REQUIRE(!split || (a->qkv_lo && a->out_lo && ((uintptr_t)a->qkv_lo) % 16 == 0 && ((uintptr_t)a->out_lo) % 16 == 0),
+                   "flash_attn: split-fp16 needs 16-byte aligned qkv_lo and out_lo planes");
+        const int dim = a->heads * a->head_dim;
+        RB_REQUIRE(a->ld_qkv >= 3 * dim && (a->ld_qkv * 2) % 16 == 0 && ((uintptr_t)a->qkv) % 16 == 0, "flash_attn: qkv pitch/alignment");
+        RB_REQUIRE(a->ld_out >= dim && (a->ld_out * 2) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0, "flash_attn: out pitch/alignment");
+        RB_REQUIRE(a->batch > 0 && a->batch <= 65535 && a->n_tokens > 0, "flash_attn: bad batch / token count");
+        // [batch, tokens, 3 * dim] with boxes of 64 tokens x 64 columns, 128B-swizzled: one plane (hi) or two (hi, lo)
+        cuuint64_t dims[3] = {(cuuint64_t)(3 * dim), (cuuint64_t)a->n_tokens, (cuuint64_t)a->batch};
+        cuuint64_t strides[2] = {(cuuint64_t)a->ld_qkv * 2, (cuuint64_t)a->ld_qkv * 2 * (cuuint64_t)a->n_tokens};
+        cuuint32_t box[3] = {64, 64, 1};
+        CUtensorMap map_hi, map_lo;
+        if (encode_tiled(&map_hi, "flash_attn", tma_dtype(a->dtype), 3, a->qkv, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+        map_lo = map_hi;
+        if (split && encode_tiled(&map_lo, "flash_attn (lo plane)", tma_dtype(a->dtype), 3, a->qkv_lo, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))
+            return 1;
+        FaParams p;
+        p.out = a->out; p.out_lo = a->out_lo; p.ldo = a->ld_out; p.N = a->n_tokens; p.heads = a->heads; p.dim = dim;
+        p.scale_log2 = 1.4426950408889634f / sqrtf((float)a->head_dim);
+        if constexpr (std::is_same_v<T, __half>)
+            if (split) return launch_fa<64, __half, true>(map_hi, map_lo, p, a->batch, st);
+        return a->head_dim == 64 ? launch_fa<64, T, false>(map_hi, map_lo, p, a->batch, st) : launch_fa<128, T, false>(map_hi, map_lo, p, a->batch, st);
+    });
 }

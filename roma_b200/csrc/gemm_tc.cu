@@ -374,15 +374,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap map_a, const __grid_constant_
 // ------------------------------------------------------------------------------------------------
 // host side
 // ------------------------------------------------------------------------------------------------
-// 4-D map over (inner, rows, batch1, batch0) of a 16-bit matrix
-static int make_map(CUtensorMap* map, const void* base, int is_bf16, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint64_t b1,
+// 4-D map over (inner, rows, batch1, batch0) of a 16-bit matrix of dtype code `dtype` (RB_F16S: either plane)
+static int make_map(CUtensorMap* map, const void* base, int dtype, uint64_t inner, uint64_t rows, uint64_t pitch_elems, uint64_t b1,
                     uint64_t s1_elems, uint64_t b0, uint64_t s0_elems, uint32_t box_inner, uint32_t box_rows) {
     RB_REQUIRE(((uintptr_t)base) % 16 == 0 && (pitch_elems * 2) % 16 == 0, "gemm_tc: operand base/pitch must be 16-byte aligned (pitch %llu elems)", (unsigned long long)pitch_elems);
     RB_REQUIRE((b1 <= 1 || (s1_elems * 2) % 16 == 0) && (b0 <= 1 || (s0_elems * 2) % 16 == 0), "gemm_tc: batch strides must be 16-byte aligned");
     cuuint64_t dims[4] = {inner, rows, b1 > 0 ? b1 : 1, b0 > 0 ? b0 : 1};
     cuuint64_t strides[3] = {pitch_elems * 2, (b1 > 1 ? s1_elems : pitch_elems * rows) * 2, (b0 > 1 ? s0_elems : pitch_elems * rows) * 2};
     cuuint32_t box[4] = {box_inner, box_rows, 1, 1};
-    return encode_tiled(map, "gemm_tc", is_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, base, dims, strides, box,
+    return encode_tiled(map, "gemm_tc", tma_dtype(dtype), 4, base, dims, strides, box,
                         CU_TENSOR_MAP_SWIZZLE_128B);
 }
 
@@ -476,20 +476,20 @@ int gemm_tc(const rb_gemm_args* a, cudaStream_t stream) {
     }
     TcMaps maps;
     const uint64_t a_inner = p.ntaps > 1 ? p.k_per_tap : a->K;
-    if (make_map(&maps.a, a->A, bf16, a_inner, a_rows, a->lda, p.batch1, a->sa1, batch0, a->sa0, TC_BK, TC_BM)) return 1;
-    if (split && make_map(&maps.a_lo, a->A_lo, 0, a_inner, a_rows, a->lda, p.batch1, a->sa1, batch0, a->sa0, TC_BK, TC_BM)) return 1;
+    if (make_map(&maps.a, a->A, a->dtype_ab, a_inner, a_rows, a->lda, p.batch1, a->sa1, batch0, a->sa0, TC_BK, TC_BM)) return 1;
+    if (split && make_map(&maps.a_lo, a->A_lo, a->dtype_ab, a_inner, a_rows, a->lda, p.batch1, a->sa1, batch0, a->sa0, TC_BK, TC_BM)) return 1;
     if (!a->trans_b) {
-        if (make_map(&maps.b, a->B, bf16, a->K, a->N, a->ldb, p.batch1, a->sb1, batch0, a->sb0, TC_BK, BN)) return 1;
-        if (split && make_map(&maps.b_lo, a->B_lo, 0, a->K, a->N, a->ldb, p.batch1, a->sb1, batch0, a->sb0, TC_BK, BN)) return 1;
+        if (make_map(&maps.b, a->B, a->dtype_ab, a->K, a->N, a->ldb, p.batch1, a->sb1, batch0, a->sb0, TC_BK, BN)) return 1;
+        if (split && make_map(&maps.b_lo, a->B_lo, a->dtype_ab, a->K, a->N, a->ldb, p.batch1, a->sb1, batch0, a->sb0, TC_BK, BN)) return 1;
     } else {
-        if (make_map(&maps.b, a->B, bf16, a->N, a->K, a->ldb, p.batch1, a->sb1, batch0, a->sb0, 64, TC_BK)) return 1;
-        if (split && make_map(&maps.b_lo, a->B_lo, 0, a->N, a->K, a->ldb, p.batch1, a->sb1, batch0, a->sb0, 64, TC_BK)) return 1;
+        if (make_map(&maps.b, a->B, a->dtype_ab, a->N, a->K, a->ldb, p.batch1, a->sb1, batch0, a->sb0, 64, TC_BK)) return 1;
+        if (split && make_map(&maps.b_lo, a->B_lo, a->dtype_ab, a->N, a->K, a->ldb, p.batch1, a->sb1, batch0, a->sb0, 64, TC_BK)) return 1;
     }
     if (!split) { maps.a_lo = maps.a; maps.b_lo = maps.b; }
     {
         // a plain (or zero-bordered) output with 16-byte aligned pitches and no residual operand gets the pad columns of its last
         // 16-byte granule zeroed, so that a later consumer reading whole granules never meets stale values
-        const int es_c = a->dtype_c == RB_F32 ? 4 : 2;
+        const int es_c = dtype_size(a->dtype_c);
         const bool align_ok = ((uintptr_t)a->C) % 16 == 0 && (a->ldc * es_c) % 16 == 0 && (p.batch1 <= 1 || (a->sc1 * es_c) % 16 == 0) &&
                               (batch0 <= 1 || (a->sc0 * es_c) % 16 == 0) && (a->dtype_c != RB_F16S || ((uintptr_t)a->C_lo) % 16 == 0);
         const bool rowmap_ok = a->rowmap == RB_ROWMAP_NONE || a->rowmap == RB_ROWMAP_PAD_KEEP;

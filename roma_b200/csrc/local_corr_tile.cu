@@ -209,25 +209,17 @@ refiner_prologue_tile_kernel(const PrologueParams p, unsigned char* __restrict__
     }
 }
 
-template <int R>
-static int launch_tile(const PrologueParams& p, unsigned char* tile_done, cudaStream_t st) {
-    using SM = LcTileSmem<R>;
-    if (ensure_smem<refiner_prologue_tile_kernel<R>>(SM::BYTES, "refiner_prologue (tile)")) return 1;
-    const int tiles = p.D * ((p.h + LcTile<R>::TQY - 1) / LcTile<R>::TQY) * ((p.w + LcTile<R>::TQX - 1) / LcTile<R>::TQX);
-    rb::launch_pdl(refiner_prologue_tile_kernel<R>, dim3((unsigned)tiles), dim3(SM::THREADS), (size_t)SM::BYTES, st, p, tile_done);
-    return check_launch("refiner_prologue_tile");
-}
-
 // fp32 maps with 16-byte aligned rows and cf a multiple of the staged chunk; the caller has checked the rest
 int refiner_prologue_tile(const PrologueParams& p, int radius, unsigned char* tile_done, cudaStream_t st) {
     RB_REQUIRE((int64_t)p.D * p.h * p.w < (1ll << 31) && (int64_t)p.h * p.w * p.ldf < (1ll << 31), "refiner_prologue (tile): map too large for 32-bit offsets");
-    switch (radius) {
-        case 2: return launch_tile<2>(p, tile_done, st);
-        case 3: return launch_tile<3>(p, tile_done, st);
-        case 7: return launch_tile<7>(p, tile_done, st);
-        default: RB_REQUIRE(false, "refiner_prologue (tile): radius %d unsupported", radius);
-    }
-    return 0;
+    return with_value<2, 3, 7>(radius, "refiner_prologue (tile): radius", [&](auto r) {
+        constexpr int R = decltype(r)::value;
+        using SM = LcTileSmem<R>;
+        if (ensure_smem<refiner_prologue_tile_kernel<R>>(SM::BYTES, "refiner_prologue (tile)")) return 1;
+        const int tiles = p.D * ((p.h + LcTile<R>::TQY - 1) / LcTile<R>::TQY) * ((p.w + LcTile<R>::TQX - 1) / LcTile<R>::TQX);
+        rb::launch_pdl(refiner_prologue_tile_kernel<R>, dim3((unsigned)tiles), dim3(SM::THREADS), (size_t)SM::BYTES, st, p, tile_done);
+        return check_launch("refiner_prologue_tile");
+    });
 }
 
 }  // namespace rb

@@ -789,12 +789,6 @@ __global__ void match_epilogue_kernel(const float* __restrict__ state, const flo
 
 using namespace rb;
 
-static inline unsigned grid1d(int64_t total, int block) {
-    int64_t g = (total + block - 1) / block;
-    int64_t cap = 132 * 64;
-    return (unsigned)(g < 1 ? 1 : (g > cap ? cap : g));
-}
-
 // ROMAB200_LC_TILE=0 keeps every pixel on the per-pixel kernel (A/B measurements)
 static inline bool lc_tile_enabled() { static const bool on = [] { const char* e = getenv("ROMAB200_LC_TILE"); return !e || atoi(e) != 0; }(); return on; }
 
@@ -802,75 +796,62 @@ extern "C" int romab200_refiner_prologue(const rb_refiner_prologue_args* a, void
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->cf > 0 && a->cf <= 512, "refiner_prologue: cf=%d", a->cf);
     RB_REQUIRE(a->ldd >= 2 * a->cf + a->emb + (2 * a->radius + 1) * (2 * a->radius + 1) * (a->radius > 0), "refiner_prologue: ldd too small");
-    if (a->radius > 0) {
-        int vn = a->dtype == RB_F32 ? 4 : 8;
-        RB_REQUIRE(a->cf % vn == 0 && a->ldf % vn == 0 && ((uintptr_t)a->feat) % 16 == 0,
-                   "refiner_prologue: local correlation needs 16-byte aligned channel vectors (cf=%d ldf=%lld)", a->cf, (long long)a->ldf);
-        RB_REQUIRE(a->win_x && a->win_y, "refiner_prologue: window offsets missing");
-    }
-    PrologueParams p;
-    p.feat = a->feat; p.ldf = a->ldf; p.n_img = a->n_img; p.y_shift = a->y_shift; p.state = a->state; p.d = a->d; p.ldd = a->ldd;
-    p.D = a->D; p.h = a->h; p.w = a->w; p.cf = a->cf; p.emb = a->emb; p.emb_w = a->emb_weight; p.emb_b = a->emb_bias;
-    p.disp_scale = a->disp_scale; p.gx = a->grid_x; p.gy = a->grid_y; p.winx = a->win_x; p.winy = a->win_y;
-    const int es = a->dtype == RB_F32 ? 4 : 2;
-    p.vec_ok = (a->ldf * es) % 16 == 0 && (a->ldd * es) % 16 == 0 && ((uintptr_t)a->feat) % 16 == 0 && ((uintptr_t)a->d) % 16 == 0;
-    p.tile_done = nullptr;
-    p.corr_table = a->corr_table; p.ld_table = a->ld_corr_table;
-    RB_REQUIRE(!a->corr_table || (a->radius > 0 && a->ld_corr_table >= (int64_t)a->h * a->w), "refiner_prologue: corr_table needs a local correlation and ld >= h*w");
-    int64_t pixels = (int64_t)a->D * a->h * a->w;
-    if (a->radius > 0 && a->dtype == RB_F32 && a->tile_done && !a->corr_table && p.vec_ok && a->cf % 16 == 0 && lc_tile_enabled()) {
-        const int tqy = a->radius == 7 ? LcTile<7>::TQY : LcTile<3>::TQY, tqx = LcTile<3>::TQX;
-        const int64_t tiles = (int64_t)a->D * ((a->h + tqy - 1) / tqy) * ((a->w + tqx - 1) / tqx);
-        RB_REQUIRE(a->radius == 2 || a->radius == 3 || a->radius == 7, "refiner_prologue: radius %d unsupported", a->radius);
-        RB_REQUIRE(a->tile_done_len >= tiles, "refiner_prologue: tile_done holds %d bytes, %lld tiles", a->tile_done_len, (long long)tiles);
-        if (int rc = refiner_prologue_tile(p, a->radius, (unsigned char*)a->tile_done, st)) return rc;
-        p.tile_done = (const unsigned char*)a->tile_done;
-    }
-    if (a->radius == 0 && 2 * a->cf + a->emb <= 32 && a->ldd <= 32 && p.vec_ok) {
-        unsigned g = (unsigned)((pixels + 255) / 256);      // thin stride-1 maps: one thread per pixel
-        if (a->dtype == RB_F32) rb::launch_pdl(refiner_prologue_small_kernel<float>, dim3(g), dim3(256), 0, st, p);
-        else if (a->dtype == RB_F16) rb::launch_pdl(refiner_prologue_small_kernel<__half>, dim3(g), dim3(256), 0, st, p);
-        else rb::launch_pdl(refiner_prologue_small_kernel<__nv_bfloat16>, dim3(g), dim3(256), 0, st, p);
-        return check_launch("refiner_prologue_small");
-    }
-    unsigned grid = (unsigned)((pixels + 3) / 4);
-#define LAUNCH(T, R) rb::launch_pdl(refiner_prologue_kernel<T, R>, dim3(grid), dim3(128), 0, st, p)
-#define BYR(T)                                                                                        \
-    switch (a->radius) {                                                                              \
-        case 0: LAUNCH(T, 0); break; case 2: LAUNCH(T, 2); break; case 3: LAUNCH(T, 3); break;        \
-        case 7: LAUNCH(T, 7); break; default: RB_REQUIRE(false, "refiner_prologue: radius %d unsupported", a->radius); \
-    }
-    if (a->dtype == RB_F32) { BYR(float) } else if (a->dtype == RB_F16) { BYR(__half) } else { BYR(__nv_bfloat16) }
-#undef BYR
-#undef LAUNCH
-    return check_launch("refiner_prologue");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "refiner_prologue", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int es = sizeof(T);
+        if (a->radius > 0) {
+            RB_REQUIRE(a->cf % (16 / es) == 0 && a->ldf % (16 / es) == 0 && ((uintptr_t)a->feat) % 16 == 0,
+                       "refiner_prologue: local correlation needs 16-byte aligned channel vectors (cf=%d ldf=%lld)", a->cf, (long long)a->ldf);
+            RB_REQUIRE(a->win_x && a->win_y, "refiner_prologue: window offsets missing");
+        }
+        PrologueParams p;
+        p.feat = a->feat; p.ldf = a->ldf; p.n_img = a->n_img; p.y_shift = a->y_shift; p.state = a->state; p.d = a->d; p.ldd = a->ldd;
+        p.D = a->D; p.h = a->h; p.w = a->w; p.cf = a->cf; p.emb = a->emb; p.emb_w = a->emb_weight; p.emb_b = a->emb_bias;
+        p.disp_scale = a->disp_scale; p.gx = a->grid_x; p.gy = a->grid_y; p.winx = a->win_x; p.winy = a->win_y;
+        p.vec_ok = (a->ldf * es) % 16 == 0 && (a->ldd * es) % 16 == 0 && ((uintptr_t)a->feat) % 16 == 0 && ((uintptr_t)a->d) % 16 == 0;
+        p.tile_done = nullptr;
+        p.corr_table = a->corr_table; p.ld_table = a->ld_corr_table;
+        RB_REQUIRE(!a->corr_table || (a->radius > 0 && a->ld_corr_table >= (int64_t)a->h * a->w), "refiner_prologue: corr_table needs a local correlation and ld >= h*w");
+        int64_t pixels = (int64_t)a->D * a->h * a->w;
+        if (a->radius > 0 && std::is_same_v<T, float> && a->tile_done && !a->corr_table && p.vec_ok && a->cf % 16 == 0 && lc_tile_enabled()) {
+            const int tqy = a->radius == 7 ? LcTile<7>::TQY : LcTile<3>::TQY, tqx = LcTile<3>::TQX;
+            const int64_t tiles = (int64_t)a->D * ((a->h + tqy - 1) / tqy) * ((a->w + tqx - 1) / tqx);
+            RB_REQUIRE(a->radius == 2 || a->radius == 3 || a->radius == 7, "refiner_prologue: radius %d unsupported", a->radius);
+            RB_REQUIRE(a->tile_done_len >= tiles, "refiner_prologue: tile_done holds %d bytes, %lld tiles", a->tile_done_len, (long long)tiles);
+            if (int rc = refiner_prologue_tile(p, a->radius, (unsigned char*)a->tile_done, st)) return rc;
+            p.tile_done = (const unsigned char*)a->tile_done;
+        }
+        if (a->radius == 0 && 2 * a->cf + a->emb <= 32 && a->ldd <= 32 && p.vec_ok) {
+            rb::launch_pdl(refiner_prologue_small_kernel<T>, dim3((unsigned)((pixels + 255) / 256)), dim3(256), 0, st, p);      // thin stride-1 maps: one thread per pixel
+            return check_launch("refiner_prologue_small");
+        }
+        return with_value<0, 2, 3, 7>(a->radius, "refiner_prologue: radius", [&](auto r) {
+            rb::launch_pdl(refiner_prologue_kernel<T, decltype(r)::value>, dim3((unsigned)((pixels + 3) / 4)), dim3(128), 0, st, p);
+            return check_launch("refiner_prologue");
+        });
+    });
 }
 
 extern "C" int romab200_local_corr(const rb_local_corr_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->c > 0 && a->c <= 512, "local_corr: c=%d (max 512)", a->c);
-    int vn = a->dtype_f == RB_F32 ? 4 : 8;
-    RB_REQUIRE(a->c % vn == 0 && a->ldf0 % vn == 0 && a->ldf1 % vn == 0 && a->f0_img_stride % vn == 0 && a->f1_img_stride % vn == 0 &&
-               ((uintptr_t)a->f0) % 16 == 0 && ((uintptr_t)a->f1) % 16 == 0, "local_corr: channel vectors must be 16-byte aligned");
-    RB_REQUIRE(a->dtype_out == RB_F32 || a->dtype_out == a->dtype_f, "local_corr: output dtype must be fp32 or the feature dtype");
-    LocalCorrParams p;
-    p.f0 = a->f0; p.f1 = a->f1; p.ldf0 = a->ldf0; p.ldf1 = a->ldf1; p.f0_img_stride = a->f0_img_stride; p.f1_img_stride = a->f1_img_stride;
-    p.flow = a->flow; p.ldflow = a->ldflow; p.out = a->out; p.ldo = a->ldo; p.batch = a->batch; p.h = a->h; p.w = a->w; p.c = a->c;
-    p.scale = a->scale; p.n_img = a->n_img > 0 ? a->n_img : a->batch; p.y_shift = a->y_shift; p.winx = a->win_x; p.winy = a->win_y;
-    int64_t pixels = (int64_t)a->batch * a->h * a->w;
-    unsigned grid = (unsigned)((pixels + 3) / 4);
-#define LAUNCH(T, R, TO) rb::launch_pdl(local_corr_kernel<T, R, TO>, dim3(grid), dim3(128), 0, st, p)
-#define BYR(T, TO)                                                                                    \
-    switch (a->radius) {                                                                              \
-        case 2: LAUNCH(T, 2, TO); break; case 3: LAUNCH(T, 3, TO); break; case 7: LAUNCH(T, 7, TO); break; \
-        default: RB_REQUIRE(false, "local_corr: radius %d unsupported (2, 3, 7)", a->radius);         \
-    }
-    if (a->dtype_f == RB_F32) { BYR(float, float) }
-    else if (a->dtype_f == RB_F16) { if (a->dtype_out == RB_F32) { BYR(__half, float) } else { BYR(__half, __half) } }
-    else { if (a->dtype_out == RB_F32) { BYR(__nv_bfloat16, float) } else { BYR(__nv_bfloat16, __nv_bfloat16) } }
-#undef BYR
-#undef LAUNCH
-    return check_launch("local_corr");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype_f, "local_corr", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int vn = 16 / sizeof(T);
+        RB_REQUIRE(a->c % vn == 0 && a->ldf0 % vn == 0 && a->ldf1 % vn == 0 && a->f0_img_stride % vn == 0 && a->f1_img_stride % vn == 0 &&
+                   ((uintptr_t)a->f0) % 16 == 0 && ((uintptr_t)a->f1) % 16 == 0, "local_corr: channel vectors must be 16-byte aligned");
+        RB_REQUIRE(a->dtype_out == RB_F32 || a->dtype_out == a->dtype_f, "local_corr: output dtype must be fp32 or the feature dtype");
+        LocalCorrParams p;
+        p.f0 = a->f0; p.f1 = a->f1; p.ldf0 = a->ldf0; p.ldf1 = a->ldf1; p.f0_img_stride = a->f0_img_stride; p.f1_img_stride = a->f1_img_stride;
+        p.flow = a->flow; p.ldflow = a->ldflow; p.out = a->out; p.ldo = a->ldo; p.batch = a->batch; p.h = a->h; p.w = a->w; p.c = a->c;
+        p.scale = a->scale; p.n_img = a->n_img > 0 ? a->n_img : a->batch; p.y_shift = a->y_shift; p.winx = a->win_x; p.winy = a->win_y;
+        const int64_t pixels = (int64_t)a->batch * a->h * a->w;
+        return with_value<2, 3, 7>(a->radius, "local_corr: radius", [&](auto r) {
+            constexpr int R = decltype(r)::value;
+            rb::launch_pdl(a->dtype_out == RB_F32 ? local_corr_kernel<T, R, float> : local_corr_kernel<T, R, T>, dim3((unsigned)((pixels + 3) / 4)), dim3(128), 0, st, p);
+            return check_launch("local_corr");
+        });
+    });
 }
 
 extern "C" int romab200_local_corr_warp(const rb_local_corr_warp_args* a, void* stream) {
@@ -891,81 +872,80 @@ extern "C" int romab200_dwconv5x5_relu(const rb_dwconv_args* a, void* stream) {
     dim3 grid(tiles_x * tiles_y, (a->c + 31) / 32, a->batch);
     RB_REQUIRE(grid.y <= 65535 && grid.z <= 65535, "dwconv: grid too large");
     const int cpad = (a->c + 7) & ~7;
-    if (a->dtype != RB_F32 && a->ldi % 8 == 0 && a->ldo % 2 == 0 && a->ldi >= cpad && a->ldo >= cpad &&
-        ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 4 == 0) {
-        return dwconv_tma(a, st);
-    }
-    if (a->dtype == RB_F32 && a->out_lo && a->ldi % 4 == 0 && a->ldo % 2 == 0 && a->ldi >= cpad && a->ldo >= cpad &&
-        ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 4 == 0 && ((uintptr_t)a->out_lo) % 4 == 0) {
-        return dwconv_tma(a, st);           // parity mode: fp32 map -> RB_F16S pair, TMA-fed persistent kernel
-    }
-    RB_REQUIRE(!a->out_lo || a->dtype == RB_F32, "dwconv: the RB_F16S output (out_lo) is for fp32 maps");
-    if (a->dtype == RB_F32 && a->out_lo) rb::launch_pdl(dwconv5x5_relu_kernel<float, true>, dim3(grid), dim3(256), 0, st, (const float*)a->in, (float*)a->out, a->ldi, a->ldo, a->weight, a->ldw, a->bias, a->h, a->w, a->c, tiles_x, (__half*)a->out_lo);
-    else if (a->dtype == RB_F32) rb::launch_pdl(dwconv5x5_relu_kernel<float, false>, dim3(grid), dim3(256), 0, st, (const float*)a->in, (float*)a->out, a->ldi, a->ldo, a->weight, a->ldw, a->bias, a->h, a->w, a->c, tiles_x, (__half*)nullptr);
-    else if (a->dtype == RB_F16) rb::launch_pdl(dwconv5x5_relu_kernel<__half, false>, dim3(grid), dim3(256), 0, st, (const __half*)a->in, (__half*)a->out, a->ldi, a->ldo, a->weight, a->ldw, a->bias, a->h, a->w, a->c, tiles_x, (__half*)nullptr);
-    else rb::launch_pdl(dwconv5x5_relu_kernel<__nv_bfloat16, false>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)a->in, (__nv_bfloat16*)a->out, a->ldi, a->ldo, a->weight, a->ldw, a->bias, a->h, a->w, a->c, tiles_x, (__half*)nullptr);
-    return check_launch("dwconv5x5_relu");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "dwconv5x5_relu", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr bool f32 = std::is_same_v<T, float>;
+        if (!f32 && a->ldi % 8 == 0 && a->ldo % 2 == 0 && a->ldi >= cpad && a->ldo >= cpad && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 4 == 0)
+            return dwconv_tma(a, st);
+        if (f32 && a->out_lo && a->ldi % 4 == 0 && a->ldo % 2 == 0 && a->ldi >= cpad && a->ldo >= cpad &&
+            ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 4 == 0 && ((uintptr_t)a->out_lo) % 4 == 0)
+            return dwconv_tma(a, st);           // parity mode: fp32 map -> RB_F16S pair, TMA-fed persistent kernel
+        RB_REQUIRE(!a->out_lo || f32, "dwconv: the RB_F16S output (out_lo) is for fp32 maps");
+        auto kernel = dwconv5x5_relu_kernel<T, false>;
+        if constexpr (f32) if (a->out_lo) kernel = dwconv5x5_relu_kernel<float, true>;
+        rb::launch_pdl(kernel, grid, dim3(256), 0, st, (const T*)a->in, (T*)a->out, a->ldi, a->ldo, a->weight, a->ldw, a->bias, a->h, a->w, a->c, tiles_x, (__half*)a->out_lo);
+        return check_launch("dwconv5x5_relu");
+    });
 }
 
 extern "C" int romab200_refiner_block_small(const rb_refiner_block_small_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->c == 24, "refiner_block_small: only C = 24 is instantiated (got %d)", a->c);
-    RB_REQUIRE(a->dtype == RB_F16 || a->dtype == RB_BF16 || a->dtype == RB_F32, "refiner_block_small: fp16 / bf16 / fp32 activations");
-    RB_REQUIRE(a->ld % (a->dtype == RB_F32 ? 4 : 8) == 0 && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0 && a->in != a->out, "refiner_block_small: bad layout");
-    int tiles_x = (a->w + 15) / 16, tiles_y = (a->h + 15) / 16;
-    dim3 grid(tiles_x * tiles_y, a->batch);
-    RB_REQUIRE(grid.y <= 65535, "refiner_block_small: batch too large");
-    RB_REQUIRE(a->pw_weight_host && a->pw_bias_host, "refiner_block_small: the pointwise weights must be given as HOST arrays (they are passed as kernel parameters)");
-    SmallPw<24> pw;
-    for (int co = 0; co < 24; ++co) {
-        for (int ci = 0; ci < 24; ++ci) pw.w[co][ci] = a->pw_weight_host[co * 24 + ci];
-        pw.b[co] = a->pw_bias_host[co];
-    }
-    if (a->dtype == RB_F32) {
-        if (ensure_smem<refiner_block_small_f32_kernel<24>>(SmallF32Cfg<24>::SMEM, "refiner_block_small")) return 1;
-        rb::launch_pdl(refiner_block_small_f32_kernel<24>, dim3(grid), dim3(256), SmallF32Cfg<24>::SMEM, st, (const float*)a->in, (float*)a->out, a->ld, a->dw_weight, a->ldw,
-                       a->dw_bias, pw, a->h, a->w, tiles_x);
-    } else if (a->dtype == RB_F16)
-        rb::launch_pdl(refiner_block_small_kernel<__half, 24>, dim3(grid), dim3(256), 0, st, (const __half*)a->in, (__half*)a->out, a->ld, a->dw_weight, a->ldw, a->dw_bias,
-                       pw, a->h, a->w, tiles_x);
-    else
-        rb::launch_pdl(refiner_block_small_kernel<__nv_bfloat16, 24>, dim3(grid), dim3(256), 0, st, (const __nv_bfloat16*)a->in, (__nv_bfloat16*)a->out, a->ld, a->dw_weight,
-                       a->ldw, a->dw_bias, pw, a->h, a->w, tiles_x);
-    return check_launch("refiner_block_small");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "refiner_block_small", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr bool f32 = std::is_same_v<T, float>;
+        RB_REQUIRE(a->ld % (16 / sizeof(T)) == 0 && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0 && a->in != a->out, "refiner_block_small: bad layout");
+        int tiles_x = (a->w + 15) / 16, tiles_y = (a->h + 15) / 16;
+        dim3 grid(tiles_x * tiles_y, a->batch);
+        RB_REQUIRE(grid.y <= 65535, "refiner_block_small: batch too large");
+        RB_REQUIRE(a->pw_weight_host && a->pw_bias_host, "refiner_block_small: the pointwise weights must be given as HOST arrays (they are passed as kernel parameters)");
+        SmallPw<24> pw;
+        for (int co = 0; co < 24; ++co) {
+            for (int ci = 0; ci < 24; ++ci) pw.w[co][ci] = a->pw_weight_host[co * 24 + ci];
+            pw.b[co] = a->pw_bias_host[co];
+        }
+        auto kernel = [] { if constexpr (f32) return refiner_block_small_f32_kernel<24>; else return refiner_block_small_kernel<T, 24>; }();
+        constexpr int smem = f32 ? SmallF32Cfg<24>::SMEM : 0;      // the fp32 kernel stages its tile in dynamic shared memory
+        if constexpr (f32) if (ensure_smem<refiner_block_small_f32_kernel<24>>(smem, "refiner_block_small")) return 1;
+        rb::launch_pdl(kernel, grid, dim3(256), smem, st, (const T*)a->in, (T*)a->out, a->ld, a->dw_weight, a->ldw, a->dw_bias, pw, a->h, a->w, tiles_x);
+        return check_launch("refiner_block_small");
+    });
 }
 
 extern "C" int romab200_refiner_tail(const rb_refiner_tail_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
-    const int vn = a->dtype == RB_F32 ? 4 : 8;
-    const int cpad = (a->c + vn - 1) / vn * vn;
-    RB_REQUIRE(a->ldd >= cpad && a->ldw >= cpad && a->ldd % vn == 0 && a->ldw % 4 == 0 && ((uintptr_t)a->d) % 16 == 0 &&
-               ((uintptr_t)a->weight) % 16 == 0, "refiner_tail: rows must be zero-padded to whole 16-byte vectors (c=%d ldd=%lld ldw=%lld)",
-               a->c, (long long)a->ldd, (long long)a->ldw);
-    const int lpp = a->c <= 32 ? 4 : (a->c <= 256 ? 8 : 32);
-    unsigned grid = (unsigned)((a->rows * lpp + 255) / 256);
-#define TAIL(T, L) rb::launch_pdl(refiner_tail_kernel<T, L>, dim3(grid), dim3(256), 0, st, (const T*)a->d, a->ldd, a->weight, a->ldw, a->bias, a->state, a->rows, a->c, a->scale_x, a->scale_y, a->delta_out)
-#define BYL(T) if (lpp == 4) TAIL(T, 4); else if (lpp == 8) TAIL(T, 8); else TAIL(T, 32);
-    if (a->dtype == RB_F32) { BYL(float) } else if (a->dtype == RB_F16) { BYL(__half) } else { BYL(__nv_bfloat16) }
-#undef BYL
-#undef TAIL
-    return check_launch("refiner_tail");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "refiner_tail", [&](auto t) {
+        using T = typename decltype(t)::type;
+        constexpr int vn = 16 / sizeof(T);
+        const int cpad = (a->c + vn - 1) / vn * vn;
+        RB_REQUIRE(a->ldd >= cpad && a->ldw >= cpad && a->ldd % vn == 0 && a->ldw % 4 == 0 && ((uintptr_t)a->d) % 16 == 0 &&
+                   ((uintptr_t)a->weight) % 16 == 0, "refiner_tail: rows must be zero-padded to whole 16-byte vectors (c=%d ldd=%lld ldw=%lld)",
+                   a->c, (long long)a->ldd, (long long)a->ldw);
+        const int lpp = a->c <= 32 ? 4 : (a->c <= 256 ? 8 : 32);
+        return with_value<4, 8, 32>(lpp, "refiner_tail: lanes per pixel", [&](auto l) {
+            rb::launch_pdl(refiner_tail_kernel<T, decltype(l)::value>, dim3((unsigned)((a->rows * lpp + 255) / 256)), dim3(256), 0, st, (const T*)a->d, a->ldd, a->weight,
+                           a->ldw, a->bias, a->state, a->rows, a->c, a->scale_x, a->scale_y, a->delta_out);
+            return check_launch("refiner_tail");
+        });
+    });
 }
 
 extern "C" int romab200_bilinear_resize(const rb_resize_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     int64_t total = (int64_t)a->batch * a->ho * a->wo * a->c;
     RB_REQUIRE(total > 0, "bilinear_resize: empty");
-    rb::launch_pdl(bilinear_resize_kernel, dim3(grid1d(total, 256)), dim3(256), 0, st, a->in, a->out, a->batch, a->hi, a->wi, a->ho, a->wo, a->c);
+    rb::launch_pdl(bilinear_resize_kernel, dim3(grid1d(total, 256, 132 * 64)), dim3(256), 0, st, a->in, a->out, a->batch, a->hi, a->wi, a->ho, a->wo, a->c);
     return check_launch("bilinear_resize");
 }
 
 extern "C" int romab200_cls_to_flow_refine(const rb_cls_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->rows < (1ll << 31) && a->ldl > (int64_t)a->res * a->res, "cls_to_flow_refine: bad shape");
-    if (a->dtype == RB_F32) rb::launch_pdl(cls_to_flow_kernel<float>, dim3((unsigned)a->rows), dim3(256), 0, st, (const float*)a->logits, a->state, a->ldl, a->res);
-    else if (a->dtype == RB_F16) rb::launch_pdl(cls_to_flow_kernel<__half>, dim3((unsigned)a->rows), dim3(256), 0, st, (const __half*)a->logits, a->state, a->ldl, a->res);
-    else rb::launch_pdl(cls_to_flow_kernel<__nv_bfloat16>, dim3((unsigned)a->rows), dim3(256), 0, st, (const __nv_bfloat16*)a->logits, a->state, a->ldl, a->res);
-    return check_launch("cls_to_flow_refine");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "cls_to_flow_refine", [&](auto t) {
+        using T = typename decltype(t)::type;
+        rb::launch_pdl(cls_to_flow_kernel<T>, dim3((unsigned)a->rows), dim3(256), 0, st, (const T*)a->logits, a->state, a->ldl, a->res);
+        return check_launch("cls_to_flow_refine");
+    });
 }
 
 extern "C" int romab200_match_epilogue(const rb_match_epilogue_args* a, void* stream) {
@@ -973,7 +953,7 @@ extern "C" int romab200_match_epilogue(const rb_match_epilogue_args* a, void* st
     int D = a->symmetric ? 2 * a->b : a->b;
     int64_t total = (int64_t)D * a->H * a->W;
     RB_REQUIRE(total > 0 && a->grid_x && a->grid_y, "match_epilogue: bad arguments");
-    rb::launch_pdl(match_epilogue_kernel, dim3(grid1d(total, 256)), dim3(256), 0, st, a->state, a->coarse_state, a->hc, a->wc, a->warp, a->cert, a->b, a->H, a->W,
+    rb::launch_pdl(match_epilogue_kernel, dim3(grid1d(total, 256, 132 * 64)), dim3(256), 0, st, a->state, a->coarse_state, a->hc, a->wc, a->warp, a->cert, a->b, a->H, a->W,
                                                               a->symmetric, a->grid_x, a->grid_y);
     return check_launch("match_epilogue");
 }

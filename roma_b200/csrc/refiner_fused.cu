@@ -401,39 +401,36 @@ extern "C" int romab200_debug_fzclk(long long* out, int reset) {
 extern "C" int romab200_refiner_block_c144(const rb_refiner_block_c144_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->c == FZ_C, "refiner_block_c144: C must be 144 (got %d)", a->c);
-    RB_REQUIRE(a->dtype == RB_F16 || a->dtype == RB_BF16, "refiner_block_c144: 16-bit activations only");
-    RB_REQUIRE(a->ld % 8 == 0 && a->ld >= FZ_C && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0 && a->in != a->out,
-               "refiner_block_c144: bad activation layout");
-    RB_REQUIRE(a->ld_pw % 8 == 0 && a->ld_pw >= FZ_C && ((uintptr_t)a->pw_weight) % 16 == 0, "refiner_block_c144: bad weight layout");
-    const CUtensorMapDataType dt = a->dtype == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-    CUtensorMap map;
-    cuuint64_t dims[2] = {(cuuint64_t)FZ_C, (cuuint64_t)FZ_C};
-    cuuint64_t strides[1] = {(cuuint64_t)a->ld_pw * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)FZ_C};
-    if (encode_tiled(&map, "refiner_block_c144", dt, 2, a->pw_weight, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
-    CUtensorMap map_in;          // activation [B, H, W, C] with pitch ld: box = 12 x 20 pixels x 144 channels, borders zero-filled
-    {
-        cuuint64_t d4[4] = {(cuuint64_t)FZ_C, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
-        cuuint64_t s4[3] = {(cuuint64_t)a->ld * 2, (cuuint64_t)a->w * a->ld * 2, (cuuint64_t)a->h * a->w * a->ld * 2};
-        cuuint32_t b4[4] = {(cuuint32_t)FZ_C, (cuuint32_t)FZ_IW, (cuuint32_t)FZ_IH, 1};
-        if (encode_tiled(&map_in, "refiner_block_c144 (input)", dt, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
-    }
-    FusedParams p;
-    p.in = a->in; p.out = a->out; p.ld = a->ld; p.dw_w = a->dw_weight; p.ldw = a->ldw; p.dw_b = a->dw_bias; p.pw_b = a->pw_bias;
-    p.batch = a->batch; p.H = a->h; p.W = a->w; p.tiles_x = (a->w + FZ_TW - 1) / FZ_TW; p.tiles_y = (a->h + FZ_TH - 1) / FZ_TH;
-    const long long total = (long long)p.tiles_x * p.tiles_y * a->batch;
-    RB_REQUIRE(total > 0 && total < (1ll << 31), "refiner_block_c144: bad tile count");
-    p.total_tiles = (int)total; p.is_bf16 = a->dtype == RB_BF16;
-    const int sms = sm_count();
-    const int grid = p.total_tiles < sms ? p.total_tiles : sms;
-    if (a->dtype == RB_F16) {
-        if (ensure_smem<refiner_block_c144_kernel<__half>>(FZ_SMEM, "refiner_block_c144")) return 1;
-        rb::launch_pdl(refiner_block_c144_kernel<__half>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
-    } else {
-        if (ensure_smem<refiner_block_c144_kernel<__nv_bfloat16>>(FZ_SMEM, "refiner_block_c144")) return 1;
-        rb::launch_pdl(refiner_block_c144_kernel<__nv_bfloat16>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
-    }
-    return check_launch("refiner_block_c144");
+    return with_dtype<__half, __nv_bfloat16>(a->dtype, "refiner_block_c144", [&](auto t) {
+        using T = typename decltype(t)::type;
+        RB_REQUIRE(a->ld % 8 == 0 && a->ld >= FZ_C && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0 && a->in != a->out,
+                   "refiner_block_c144: bad activation layout");
+        RB_REQUIRE(a->ld_pw % 8 == 0 && a->ld_pw >= FZ_C && ((uintptr_t)a->pw_weight) % 16 == 0, "refiner_block_c144: bad weight layout");
+        const CUtensorMapDataType dt = tma_dtype(a->dtype);
+        CUtensorMap map;
+        cuuint64_t dims[2] = {(cuuint64_t)FZ_C, (cuuint64_t)FZ_C};
+        cuuint64_t strides[1] = {(cuuint64_t)a->ld_pw * 2};
+        cuuint32_t box[2] = {64, (cuuint32_t)FZ_C};
+        if (encode_tiled(&map, "refiner_block_c144", dt, 2, a->pw_weight, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return 1;
+        CUtensorMap map_in;          // activation [B, H, W, C] with pitch ld: box = 12 x 20 pixels x 144 channels, borders zero-filled
+        {
+            cuuint64_t d4[4] = {(cuuint64_t)FZ_C, (cuuint64_t)a->w, (cuuint64_t)a->h, (cuuint64_t)a->batch};
+            cuuint64_t s4[3] = {(cuuint64_t)a->ld * 2, (cuuint64_t)a->w * a->ld * 2, (cuuint64_t)a->h * a->w * a->ld * 2};
+            cuuint32_t b4[4] = {(cuuint32_t)FZ_C, (cuuint32_t)FZ_IW, (cuuint32_t)FZ_IH, 1};
+            if (encode_tiled(&map_in, "refiner_block_c144 (input)", dt, 4, a->in, d4, s4, b4, CU_TENSOR_MAP_SWIZZLE_NONE)) return 1;
+        }
+        FusedParams p;
+        p.in = a->in; p.out = a->out; p.ld = a->ld; p.dw_w = a->dw_weight; p.ldw = a->ldw; p.dw_b = a->dw_bias; p.pw_b = a->pw_bias;
+        p.batch = a->batch; p.H = a->h; p.W = a->w; p.tiles_x = (a->w + FZ_TW - 1) / FZ_TW; p.tiles_y = (a->h + FZ_TH - 1) / FZ_TH;
+        const long long total = (long long)p.tiles_x * p.tiles_y * a->batch;
+        RB_REQUIRE(total > 0 && total < (1ll << 31), "refiner_block_c144: bad tile count");
+        p.total_tiles = (int)total; p.is_bf16 = a->dtype == RB_BF16;
+        const int sms = sm_count();
+        const int grid = p.total_tiles < sms ? p.total_tiles : sms;
+        if (ensure_smem<refiner_block_c144_kernel<T>>(FZ_SMEM, "refiner_block_c144")) return 1;
+        rb::launch_pdl(refiner_block_c144_kernel<T>, dim3(grid), dim3(FZ_THREADS), FZ_SMEM, st, map, map_in, p);
+        return check_launch("refiner_block_c144");
+    });
 }
 
 extern "C" int romab200_refiner_block_c144_split(const rb_refiner_block_c144_split_args* a, void* stream) {

@@ -71,6 +71,11 @@ inline PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
     return fn;
 }
 
+// tensor-map element type of a dtype code (RB_F16S: each of its two planes is fp16)
+inline CUtensorMapDataType tma_dtype(int code) {
+    return code == RB_F32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : (code == RB_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16);
+}
+
 // Tiled tensor map of `rank` dimensions over `base`: dims[rank], byte strides[rank - 1] of dimensions 1.., box[rank]; dense
 // element strides, 256-byte L2 promotion, zero fill out of bounds.  Errors are reported as "<what>: ...".
 inline int encode_tiled(CUtensorMap* map, const char* what, CUtensorMapDataType dtype, int rank, const void* base, const cuuint64_t* dims,

@@ -91,6 +91,9 @@ __device__ __forceinline__ uint4 max4(const uint4 a, const uint4 b) {
     for (int i = 0; i < 4; ++i) pr[i] = __hmax2(pa[i], pb[i]);
     return r;
 }
+template <typename T> struct Pair2;     // the packed pair type of a 16-bit element type
+template <> struct Pair2<__half> { using type = __half2; };
+template <> struct Pair2<__nv_bfloat16> { using type = __nv_bfloat162; };
 template <typename T2>
 __global__ void __launch_bounds__(256) maxpool2x2_padded_vec_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, int B, int H, int W, int C8) {
     rb::pdl_wait();
@@ -150,10 +153,11 @@ extern "C" int romab200_conv3x3_first(const rb_conv_first_args* a, void* stream)
         rb::launch_pdl(conv3x3_first_kernel<__half, true>, dim3(grid), dim3(128), smem, st, a->image, (__half*)a->out, a->weight, a->bias, a->batch, a->height, a->width, a->cout, (__half*)a->out_lo);
         return check_launch("conv3x3_first");
     }
-    if (a->dtype_out == RB_F32) rb::launch_pdl(conv3x3_first_kernel<float, false>, dim3(grid), dim3(128), smem, st, a->image, (float*)a->out, a->weight, a->bias, a->batch, a->height, a->width, a->cout, (float*)nullptr);
-    else if (a->dtype_out == RB_F16) rb::launch_pdl(conv3x3_first_kernel<__half, false>, dim3(grid), dim3(128), smem, st, a->image, (__half*)a->out, a->weight, a->bias, a->batch, a->height, a->width, a->cout, (__half*)nullptr);
-    else rb::launch_pdl(conv3x3_first_kernel<__nv_bfloat16, false>, dim3(grid), dim3(128), smem, st, a->image, (__nv_bfloat16*)a->out, a->weight, a->bias, a->batch, a->height, a->width, a->cout, (__nv_bfloat16*)nullptr);
-    return check_launch("conv3x3_first");
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype_out, "conv3x3_first", [&](auto t) {
+        using TO = typename decltype(t)::type;
+        rb::launch_pdl(conv3x3_first_kernel<TO, false>, grid, dim3(128), smem, st, a->image, (TO*)a->out, a->weight, a->bias, a->batch, a->height, a->width, a->cout, (TO*)nullptr);
+        return check_launch("conv3x3_first");
+    });
 }
 
 extern "C" int romab200_maxpool2x2_padded(const rb_maxpool_args* a, void* stream) {
@@ -169,16 +173,18 @@ extern "C" int romab200_maxpool2x2_padded(const rb_maxpool_args* a, void* stream
                        a->batch, a->height, a->width, a->channels / 8);
         return check_launch("maxpool2x2_padded");
     }
-    if (a->dtype != RB_F32 && a->channels % 8 == 0 && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0) {
-        const int64_t tv = total / 8, gv = (tv + 255) / 256;
-        RB_REQUIRE(gv < (1ll << 31), "maxpool: grid too large");
-        if (a->dtype == RB_F16) rb::launch_pdl(maxpool2x2_padded_vec_kernel<__half2>, dim3((unsigned)gv), dim3(256), 0, st, (const uint4*)a->in, (uint4*)a->out, a->batch, a->height, a->width, a->channels / 8);
-        else rb::launch_pdl(maxpool2x2_padded_vec_kernel<__nv_bfloat162>, dim3((unsigned)gv), dim3(256), 0, st, (const uint4*)a->in, (uint4*)a->out, a->batch, a->height, a->width, a->channels / 8);
+    return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "maxpool2x2_padded", [&](auto t) {
+        using T = typename decltype(t)::type;
+        if constexpr (sizeof(T) == 2) {
+            if (a->channels % 8 == 0 && ((uintptr_t)a->in) % 16 == 0 && ((uintptr_t)a->out) % 16 == 0) {
+                const int64_t tv = total / 8, gv = (tv + 255) / 256;
+                RB_REQUIRE(gv < (1ll << 31), "maxpool: grid too large");
+                rb::launch_pdl(maxpool2x2_padded_vec_kernel<typename Pair2<T>::type>, dim3((unsigned)gv), dim3(256), 0, st, (const uint4*)a->in, (uint4*)a->out,
+                               a->batch, a->height, a->width, a->channels / 8);
+                return check_launch("maxpool2x2_padded");
+            }
+        }
+        rb::launch_pdl(maxpool2x2_padded_kernel<T>, dim3(grid1d(total, 256, 132 * 64)), dim3(256), 0, st, (const T*)a->in, (T*)a->out, a->batch, a->height, a->width, a->channels);
         return check_launch("maxpool2x2_padded");
-    }
-    int64_t g = (total + 255) / 256; if (g > 132 * 64) g = 132 * 64;
-    if (a->dtype == RB_F32) rb::launch_pdl(maxpool2x2_padded_kernel<float>, dim3((unsigned)g), dim3(256), 0, st, (const float*)a->in, (float*)a->out, a->batch, a->height, a->width, a->channels);
-    else if (a->dtype == RB_F16) rb::launch_pdl(maxpool2x2_padded_kernel<__half>, dim3((unsigned)g), dim3(256), 0, st, (const __half*)a->in, (__half*)a->out, a->batch, a->height, a->width, a->channels);
-    else rb::launch_pdl(maxpool2x2_padded_kernel<__nv_bfloat16>, dim3((unsigned)g), dim3(256), 0, st, (const __nv_bfloat16*)a->in, (__nv_bfloat16*)a->out, a->batch, a->height, a->width, a->channels);
-    return check_launch("maxpool2x2_padded");
+    });
 }
