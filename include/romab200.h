@@ -14,6 +14,8 @@
  *     explicit row pitch, so 1x1 convolutions and Linear layers are the same GEMM;
  *   - dtypes: RB_F32 / RB_F16 / RB_BF16; accumulation is always fp32.  An entry point refuses a dtype code it has no kernel
  *     for, before any CUDA call: non-zero return, message "<op>: unsupported dtype <code>".
+ *   - RB_F64 exists for the float64 evaluation geometry only (romab200_warp_kpts and its two siblings, which take float32 or
+ *     float64 depth maps and points and compute in float64); every other entry point refuses it like any code it has no kernel for.
  *   - RB_F16S ("split fp16 pair") is the storage format of the tensor-core parity mode: a matrix is held as TWO fp16
  *     planes of the same pitch, hi = fp16(x) and lo = fp16((x - hi) * 2^11), value = hi + lo * 2^-11: 22 significand bits
  *     with the exponent range of fp16 (the reference's own CUDA autocast range).  romab200_gemm contracts such operands
@@ -31,7 +33,7 @@ extern "C" {
 
 #define ROMAB200_ABI_VERSION 4
 
-enum rb_dtype { RB_F32 = 0, RB_F16 = 1, RB_BF16 = 2, RB_F16S = 3 };
+enum rb_dtype { RB_F32 = 0, RB_F16 = 1, RB_BF16 = 2, RB_F16S = 3, RB_F64 = 4 };
 enum rb_act { RB_ACT_NONE = 0, RB_ACT_RELU = 1, RB_ACT_GELU = 2 };
 enum rb_rowmap { RB_ROWMAP_NONE = 0, RB_ROWMAP_PAD_KEEP = 1, RB_ROWMAP_PAD_TO_COMPACT = 2, RB_ROWMAP_SEGMENT = 3 };
 enum rb_epi { RB_EPI_LINEAR = 0, RB_EPI_COSKERNEL = 1 };
@@ -595,6 +597,70 @@ int romab200_homography_hypotheses(const rb_homography_args* args, void* stream)
 int romab200_homography_score(const rb_homography_args* args, void* stream);
 int romab200_homography_select(const rb_homography_args* args, void* stream);
 int romab200_homography_refine(const rb_homography_args* args, void* stream);
+
+/* ---- depth-based ground-truth warps and the MegaDepth dense metric: `warp_kpts`, `get_gt_warp` (romatch/utils/utils.py:325-454)
+ *      and `MegadepthDenseBenchmark.geometric_dist` (romatch/benchmarks/megadepth_dense_benchmark.py:17-42) ----
+ * One float64 statement of the geometry, shared by the three entry points.  For a normalised point (x, y) of view 0 of pair b:
+ *   d0 = grid_sample(depth0[b], (x, y))            zero padding, align_corners=False, ATen's unnormalisation ((x + 1) * w0 - 1) / 2;
+ *                                                  mode 0 bilinear (corners accumulated nw, ne, sw, se), mode 1 nearest (nearbyint)
+ *   X  = inv(K0[b]) ((w0 (x + 1) / 2, h0 (y + 1) / 2, 1) d0),  Y = R X + t with [R | t] = T[b, :3, :4],  z = Y[2]
+ *   p  = K1[b] Y,  u = p[0] / (p[2] + 1e-4),  v = p[1] / (p[2] + 1e-4)
+ *   warped = (2 u / w1 - 1, 2 v / h1 - 1),  d1 = grid_sample(depth1[b], warped)
+ *   valid = d0 != 0  &&  0 < u < w1 - 1  &&  0 < v < h1 - 1  &&  |(d1 - z) / d1| < rel_threshold   (a NaN compares false)
+ * Every operation is a separately rounded float64 operation (no FMA contraction), so the three entry points give the same bits
+ * for the same point.  inv(K0) is the adjugate over the determinant, computed once per CTA; nothing is inverted on the host.
+ * depth0 [batch, h0, w0] and depth1 [batch, h1, w1] are contiguous maps of dtype `depth_dtype` (RB_F32 or RB_F64, converted in
+ * registers; the two views may differ in size); T [batch, T_rows, 4] (T_rows 3 or 4), K0, K1 [batch, 3, 3] contiguous float64.
+ * warped is written for every point, valid or not.  Deterministic.
+ *
+ * romab200_warp_kpts: arbitrary points kpts [batch, L, 2] of dtype `kpts_dtype` (RB_F32 or RB_F64) -> warped [batch, L, 2] float64,
+ * valid [batch, L] uint8 (utils.py:399-454 with smooth_mask = False, return_relative_depth_error = False). */
+typedef struct {
+    const void* depth0; const void* depth1; int32_t depth_dtype; int32_t h0, w0, h1, w1;
+    const double* T; int32_t T_rows; const double* K0; const double* K1;
+    int32_t batch; int32_t mode; double rel_threshold;
+    const void* kpts; int32_t kpts_dtype; int64_t L;
+    double* warped; uint8_t* valid;
+} rb_warp_kpts_args;
+int romab200_warp_kpts(const rb_warp_kpts_args* args, void* stream);
+
+/* get_gt_warp (utils.py:325-354): the points are the pixel centres of an H x W image, point (i, j) = (grid_x[j], grid_y[i]).
+ * grid_x [W], grid_y [H] are the float32 linspace(-1 + 1/n, 1 - 1/n, n) vectors the reference builds (it widens them to float64
+ * afterwards; the closed form -1 + (2 i + 1) / n in float64 differs from them in the 8th digit for most n, so they are taken
+ * as data).  x2 [batch, H, W, 2] float64 = warped, prob [batch, H, W] float32 = valid as 0 / 1.  Apart from the two depth maps
+ * nothing of size batch * H * W is read. */
+typedef struct {
+    const void* depth0; const void* depth1; int32_t depth_dtype; int32_t h0, w0, h1, w1;
+    const double* T; int32_t T_rows; const double* K0; const double* K1;
+    int32_t batch; int32_t mode; double rel_threshold;
+    const float* grid_x; const float* grid_y; int32_t H, W;
+    double* x2; float* prob;
+} rb_gt_warp_args;
+int romab200_gt_warp(const rb_gt_warp_args* args, void* stream);
+
+/* MegadepthDenseBenchmark.geometric_dist (megadepth_dense_benchmark.py:17-42), bilinear, rel_threshold as given (the harness: 0.05).
+ * dense_matches [batch, H, W, 4] float32 is read in place: element (b, i, j, c) at dense_matches[b * dm_sb + i * dm_sy + j * dm_sx +
+ * c * dm_sc] (strides in floats, so the left half of a symmetric warp [batch, H, 2W, 4] needs no copy).  Per pixel: warp
+ * dense_matches[..., 0:2]; ground truth in pixels (W (wx + 1) / 2, H (wy + 1) / 2) in float64; prediction in pixels from
+ * dense_matches[..., 2:4] by the same expression in float32, as the harness computes it; gd = sqrt(dx^2 + dy^2) in float64.
+ * gd [batch, H, W] float64 receives the distance, NaN where the pixel is not valid; prob [batch, H, W] float32 = valid as 0 / 1.
+ * The ground-truth warp itself is never written.
+ * The same launch leaves one partial per CTA (float64 sum of gd over its valid pixels, and the counts of valid, gd < 1, gd < 3,
+ * gd < 5) in partial_sum [batch, RB_DEPTH_WARP_MAX_CTAS] and partial_cnt [batch, RB_DEPTH_WARP_MAX_CTAS, 4]; a second, single-CTA
+ * kernel adds them in a fixed order: pair_sum [batch] float64, pair_cnt [batch, 4] int64 (valid, < 1, < 3, < 5), and over all pairs
+ * pck [3] float32 = (float)count_t * (1.f / (float)count_valid), which is what (gd[prob == 1] < t).float().mean() evaluates to on
+ * the device, and epe [1] float64 = sum * (1 / count_valid).  No pair valid: NaN.  No atomics: the result does not depend on timing. */
+#define RB_DEPTH_WARP_MAX_CTAS 512
+typedef struct {
+    const void* depth0; const void* depth1; int32_t depth_dtype; int32_t h0, w0, h1, w1;
+    const double* T; int32_t T_rows; const double* K0; const double* K1;
+    int32_t batch; double rel_threshold;
+    const float* dense_matches; int64_t dm_sb, dm_sy, dm_sx, dm_sc; int32_t H, W;
+    double* gd; float* prob;
+    double* partial_sum; int32_t* partial_cnt;
+    double* pair_sum; int64_t* pair_cnt; float* pck; double* epe;
+} rb_dense_geometric_dist_args;
+int romab200_dense_geometric_dist(const rb_dense_geometric_dist_args* args, void* stream);
 
 #ifdef __cplusplus
 }

@@ -25,4 +25,7 @@ def __getattr__(name):
     if name in ("estimate_pose", "estimate_pose_batched", "find_homography", "find_homography_batched", "RANSAC"):
         from . import geometry
         return getattr(geometry, name)
+    if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
+        from . import depth_warp
+        return getattr(depth_warp, name)
     raise AttributeError(name)

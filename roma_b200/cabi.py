@@ -18,7 +18,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 HEADER = os.path.join(os.path.dirname(HERE), "include", "romab200.h")
 LIB_PATH = os.path.join(HERE, "lib", "libromab200.so")
 
-RB_F32, RB_F16, RB_BF16, RB_F16S = 0, 1, 2, 3
+RB_F32, RB_F16, RB_BF16, RB_F16S, RB_F64 = 0, 1, 2, 3, 4
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 ROWMAP_NONE, ROWMAP_PAD_KEEP, ROWMAP_PAD_TO_COMPACT, ROWMAP_SEGMENT = 0, 1, 2, 3
 EPI_LINEAR, EPI_COSKERNEL = 0, 1
@@ -104,7 +104,7 @@ launch_count = 0      # number of C-ABI calls made (bench.py reports kernel laun
 
 # ---- argument validation: the C ABI takes raw pointers, so a tensor of the wrong dtype / device / layout would be silent garbage.
 # For every struct: tensor field -> the field that carries its dtype code (or a fixed torch dtype).
-_CODE_DTYPE = {RB_F32: torch.float32, RB_F16: torch.float16, RB_BF16: torch.bfloat16, RB_F16S: torch.float16}
+_CODE_DTYPE = {RB_F32: torch.float32, RB_F16: torch.float16, RB_BF16: torch.bfloat16, RB_F16S: torch.float16, RB_F64: torch.float64}
 _F32 = torch.float32
 _F64 = torch.float64
 _FIELD_DTYPES = {
@@ -157,9 +157,16 @@ _FIELD_DTYPES = {
     "rb_homography_args": {"src": _F32, "dst": _F32, "offsets": torch.int64, "sample": torch.int32, "attempts": torch.int32, "status": torch.int32,
                            "H": _F64, "counts": torch.int32, "state": torch.int32, "best_H": _F64, "running": torch.int32, "out_H": _F64,
                            "ok": torch.uint8, "mask": torch.uint8},
+    "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
+                          "valid": torch.uint8},
+    "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
+                        "x2": _F64, "prob": _F32},
+    "rb_dense_geometric_dist_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "dense_matches": _F32,
+                                     "gd": _F64, "prob": _F32, "partial_sum": _F64, "partial_cnt": torch.int32, "pair_sum": _F64,
+                                     "pair_cnt": torch.int64, "pck": _F32, "epe": _F64},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
-_STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}}
+_STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}, "rb_dense_geometric_dist_args": {"dense_matches"}}
 
 
 def _gemm_min_elems(kw):

@@ -27,6 +27,7 @@ template <typename T> struct DT;
 template <> struct DT<float> { static constexpr int id = RB_F32; };
 template <> struct DT<__half> { static constexpr int id = RB_F16; };
 template <> struct DT<__nv_bfloat16> { static constexpr int id = RB_BF16; };
+template <> struct DT<double> { static constexpr int id = RB_F64; };
 
 // Dtype dispatch of the entry points: returns f(type_tag<T>{}) for the T among Ts whose code is `code`; any other code is refused
 // with "<what>: unsupported dtype <code>" and 1.  List exactly the types the caller has kernels for: a generic lambda instantiates
@@ -94,7 +95,7 @@ __device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint32_t k0, uint32_t k1
 }
 
 // bytes per element of one plane (RB_F16S = two fp16 planes of the same pitch)
-__host__ __device__ __forceinline__ int dtype_size(int dtype) { return dtype == RB_F32 ? 4 : 2; }
+__host__ __device__ __forceinline__ int dtype_size(int dtype) { return dtype == RB_F64 ? 8 : (dtype == RB_F32 ? 4 : 2); }
 
 // ---- split-fp16 pair: x ~ hi + lo * 2^-11 with hi = fp16(x), lo = fp16((x - hi) * 2^11) -------------------------------
 // 22 significand bits, the exponent range of fp16, and no underflow of the low part (it is stored at the magnitude of x).

@@ -310,6 +310,28 @@ def jpeg_edits(seed: int = 0):
     return out
 
 
+def _scene_intrinsics(rng, width, height):
+    """Pinhole intrinsics of a width x height camera: focal length near 3/4 of the width (1100-1300 px at 1600), pixels within 2 %
+    of square, the principal point within width / 80 of the centre."""
+    import numpy as np
+
+    s = width / 1600.0
+    f = rng.uniform(1100.0 * s, 1300.0 * s)
+    return np.array([[f, 0.0, width / 2 + rng.uniform(-20 * s, 20 * s)], [0.0, f * rng.uniform(0.98, 1.02), height / 2 + rng.uniform(-20 * s, 20 * s)],
+                     [0.0, 0.0, 1.0]])
+
+
+def _scene_rotation(rng, deg_lo, deg_hi):
+    """A rotation by deg_lo .. deg_hi degrees about a random axis (Rodrigues)."""
+    import numpy as np
+
+    axis = rng.normal(size=3)
+    axis /= np.linalg.norm(axis)
+    ang = np.deg2rad(rng.uniform(deg_lo, deg_hi))
+    S = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
+    return np.eye(3) + np.sin(ang) * S + (1 - np.cos(ang)) * S @ S
+
+
 def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, width: int = 1600, height: int = 1200):
     """A seeded calibrated two-view scene for the pose estimator: focal lengths near 1200 px, a 5-20 degree rotation about a
     random axis, a unit baseline in a random direction, `n` points seen by camera 0 at depths 6-14, Gaussian pixel noise of
@@ -318,18 +340,8 @@ def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, w
     import numpy as np
 
     rng = np.random.default_rng(seed)
-
-    def intrinsics():
-        f = rng.uniform(1100.0, 1300.0)
-        return np.array([[f, 0.0, width / 2 + rng.uniform(-20, 20)], [0.0, f * rng.uniform(0.98, 1.02), height / 2 + rng.uniform(-20, 20)],
-                         [0.0, 0.0, 1.0]])
-
-    K0, K1 = intrinsics(), intrinsics()
-    axis = rng.normal(size=3)
-    axis /= np.linalg.norm(axis)
-    ang = np.deg2rad(rng.uniform(5.0, 20.0))
-    S = np.array([[0, -axis[2], axis[1]], [axis[2], 0, -axis[0]], [-axis[1], axis[0], 0]])
-    R = np.eye(3) + np.sin(ang) * S + (1 - np.cos(ang)) * S @ S
+    K0, K1 = _scene_intrinsics(rng, width, height), _scene_intrinsics(rng, width, height)
+    R = _scene_rotation(rng, 5.0, 20.0)
     t = rng.normal(size=3)
     t /= np.linalg.norm(t)
     px = np.c_[rng.uniform(0, width, n), rng.uniform(0, height, n), np.ones(n)]
@@ -340,6 +352,65 @@ def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, w
     out = rng.random(n) < outlier_frac
     kpts1[out] = np.c_[rng.uniform(0, width, out.sum()), rng.uniform(0, height, out.sum())]
     return {"kpts0": kpts0, "kpts1": kpts1, "K0": K0, "K1": K1, "R": R, "t": t}
+
+
+def depth_scene(seed: int, batch: int, h0: int, w0: int, h1: int = None, w1: int = None):
+    """Seeded piecewise-planar two-view scenes with exact depth maps, for the depth-based warps (`roma_b200.depth_warp`).  Each pair
+    sees a tilted ground plane 8-13 units away and, in front of it, one occluding quad at 4-5 units; camera 1 is camera 0 moved by
+    a unit baseline, mostly sideways, and rotated by 8-16 degrees (intrinsics and rotation as in `two_view_scene`, scaled to the
+    image size).  The depth of a pixel is the z of the nearest ray-plane intersection through its centre (x + 0.5, y + 0.5) in
+    that view's own camera frame, so the two maps are consistent to rounding; it is stored as float32, like MegaDepth's.  Seven
+    random rectangles per view are holes of zero depth.  The motion is large enough that pixels of view 0 fall in all four classes of
+    `warp_kpts` in quantity: zero depth, not covisible, depth-inconsistent (occluded by the quad, or landing on a hole), valid.
+    h1, w1 default to h0, w0.  Returns torch CPU tensors: depth0 [B, h0, w0] and depth1 [B, h1, w1] float32, T_0to1 [B, 4, 4]
+    (X1 = R X0 + t), K0, K1 [B, 3, 3] float64."""
+    import numpy as np
+
+    h1, w1 = h1 or h0, w1 or w0
+    rng = np.random.default_rng(seed)
+
+    def render(K, R, t, h, w, planes):
+        # rays through the pixel centres of this view; a plane n . X0 = d of frame 0 is (R n) . X = d + (R n) . t in this frame
+        ys, xs = np.meshgrid(np.arange(h) + 0.5, np.arange(w) + 0.5, indexing="ij")
+        rays = np.stack((xs, ys, np.ones_like(xs)), -1) @ np.linalg.inv(K).T
+        depth = np.full((h, w), np.inf)
+        for n, d, centre, axes, half in planes:
+            n1 = R @ n
+            with np.errstate(divide="ignore", invalid="ignore"):
+                z = (d + n1 @ t) / (rays @ n1)
+            hit = np.isfinite(z) & (z > 0)
+            if centre is not None:                   # the quad: bounded in its own plane, tested in frame 0
+                X0 = ((rays * np.where(hit, z, 0.0)[..., None]) - t) @ R
+                for e, a in zip(axes, half):
+                    hit &= np.abs((X0 - centre) @ e) < a
+            depth = np.where(hit & (z < depth), z, depth)
+        depth[~np.isfinite(depth)] = 0.0
+        for _ in range(7):
+            hh, hw = int(h * rng.uniform(0.08, 0.2)), int(w * rng.uniform(0.08, 0.2))
+            y, x = rng.integers(0, h - hh), rng.integers(0, w - hw)
+            depth[y:y + hh, x:x + hw] = 0.0
+        return depth.astype(np.float32)
+
+    out = {k: [] for k in ("depth0", "depth1", "T", "K0", "K1")}
+    for _ in range(batch):
+        K0, K1 = _scene_intrinsics(rng, w0, h0), _scene_intrinsics(rng, w1, h1)
+        R = _scene_rotation(rng, 8.0, 16.0)
+        t = np.array([rng.choice([-1.0, 1.0]), rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3)])
+        t /= np.linalg.norm(t)
+        n = np.array([rng.uniform(-0.15, 0.15), rng.uniform(0.3, 0.5), 1.0])
+        ground = (n / np.linalg.norm(n), rng.uniform(8.0, 11.0), None, None, None)
+        qn = np.array([rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), 1.0])
+        qn /= np.linalg.norm(qn)
+        centre = np.array([rng.uniform(-1.0, 1.0), rng.uniform(-0.7, 0.7), rng.uniform(4.0, 5.0)])
+        e1 = np.cross(qn, [0.0, 1.0, 0.0])
+        e1 /= np.linalg.norm(e1)
+        quad = (qn, qn @ centre, centre, (e1, np.cross(qn, e1)), (rng.uniform(1.0, 1.4), rng.uniform(0.8, 1.2)))
+        T = np.eye(4)
+        T[:3, :3], T[:3, 3] = R, t
+        out["depth0"].append(render(K0, np.eye(3), np.zeros(3), h0, w0, (ground, quad)))
+        out["depth1"].append(render(K1, R, t, h1, w1, (ground, quad)))
+        out["T"].append(T), out["K0"].append(K0), out["K1"].append(K1)
+    return tuple(torch.from_numpy(np.stack(out[k])) for k in ("depth0", "depth1", "T", "K0", "K1"))
 
 
 def planar_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, width: int = 640, height: int = 480):
