@@ -135,6 +135,17 @@ typedef struct {
 } rb_copy2d_args;
 int romab200_copy2d(const rb_copy2d_args* args, void* stream);
 
+/* Indexed copy of whole rows of bytes: for i < count, row dst_index[i] of dst = row src_index[i] of src (a NULL index stands
+ * for i).  Rows are row_bytes long and ld_src / ld_dst bytes apart; row_bytes, both pitches and both pointers are multiples of
+ * 16.  An index outside [0, src_rows) or [0, dst_rows) leaves its destination row unwritten.  The indices are read on the
+ * device, so a captured graph of the call replays for any index list of the same count (match_pairs: images between a
+ * per-image feature bank and the batch buffers of the encoders and of the pair stage). */
+typedef struct {
+    const void* src; void* dst; const int32_t* src_index; const int32_t* dst_index;
+    int32_t count; int64_t row_bytes, ld_src, ld_dst; int32_t src_rows, dst_rows;
+} rb_gather_rows_args;
+int romab200_gather_rows(const rb_gather_rows_args* args, void* stream);
+
 /* fp16 hi/lo operand split for fp32-class accuracy on the f16 tensor pipe:
  * dst[r, 0:C] = hi, dst[r, C:2C] = lo (or hi), dst[r, 2C:3C] = hi (or lo) of x[r,:]/scale[r]
  * layout A: [hi | lo | hi], layout B: [hi | hi | lo]  so that A'.B'^T = hi.hi + lo.hi + hi.lo */

@@ -115,6 +115,7 @@ _FIELD_DTYPES = {
     "rb_flash_attn_args": {"qkv": "dtype", "out": "dtype", "qkv_lo": torch.float16, "out_lo": torch.float16},
     "rb_rownorm_args": {"x": "dtype", "out": _F32},
     "rb_copy2d_args": {"src": "dtype_src", "dst": "dtype_dst", "row_scale": _F32},
+    "rb_gather_rows_args": {"src_index": torch.int32, "dst_index": torch.int32},
     "rb_split_pair_args": {"x": _F32, "hi": torch.float16, "lo": torch.float16, "row_norm": _F32},
     "rb_conv_first_args": {"image": _F32, "out": "dtype_out", "out_lo": torch.float16, "weight": _F32, "bias": _F32},
     "rb_maxpool_args": {"in": "dtype", "out": "dtype", "in_lo": torch.float16, "out_lo": torch.float16},

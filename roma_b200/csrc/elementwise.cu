@@ -243,6 +243,19 @@ __global__ void copy2d_kernel(const void* __restrict__ src, void* __restrict__ d
     }
 }
 
+// dst row dst_index[i] = src row src_index[i] (NULL: i), blockIdx.y = i; 16-byte words, grid-stride along the row
+__global__ void __launch_bounds__(256) gather_rows_kernel(const uint4* __restrict__ src, uint4* __restrict__ dst, const int32_t* __restrict__ src_index,
+                                                          const int32_t* __restrict__ dst_index, int64_t words, int64_t ld_src, int64_t ld_dst,
+                                                          int src_rows, int dst_rows) {
+    rb::pdl_wait();
+    const int i = blockIdx.y;
+    const int s = src_index ? src_index[i] : i, d = dst_index ? dst_index[i] : i;
+    if (s < 0 || s >= src_rows || d < 0 || d >= dst_rows) return;
+    const uint4* sr = src + (int64_t)s * ld_src;
+    uint4* dr = dst + (int64_t)d * ld_dst;
+    for (int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; k < words; k += (int64_t)gridDim.x * blockDim.x) dr[k] = sr[k];
+}
+
 // x / norm -> fp16 hi and lo parts laid out [hi|lo|hi] (A operand) or [hi|hi|lo] (B operand)
 __global__ void split_f16x3_kernel(const float* __restrict__ x, __half* __restrict__ dst, int64_t rows, int cols,
                                    int64_t ldx, int64_t ldd, const float* __restrict__ norm, int layout_b) {
@@ -441,6 +454,19 @@ extern "C" int romab200_copy2d(const rb_copy2d_args* a, void* stream) {
     rb::launch_pdl(copy2d_kernel, dim3(grid1d(a->rows * a->cols, 256, 132 * 32)), dim3(256), 0, st, a->src, a->dst, a->rows, a->cols, a->lds, a->ldd,
                                                                    a->dtype_src, a->dtype_dst, a->row_scale, a->row_scale_reciprocal);
     return check_launch("copy2d");
+}
+
+extern "C" int romab200_gather_rows(const rb_gather_rows_args* a, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    RB_REQUIRE(a->src && a->dst && a->count > 0 && a->count <= 65535 && a->row_bytes > 0 && a->src_rows > 0 && a->dst_rows > 0,
+               "gather_rows: bad shape");
+    RB_REQUIRE(a->row_bytes % 16 == 0 && a->ld_src % 16 == 0 && a->ld_dst % 16 == 0 && a->ld_src >= a->row_bytes && a->ld_dst >= a->row_bytes &&
+               ((uintptr_t)a->src) % 16 == 0 && ((uintptr_t)a->dst) % 16 == 0, "gather_rows: rows, pitches and pointers must be 16-byte multiples");
+    const int64_t words = a->row_bytes / 16;
+    dim3 grid(grid1d(words, 256, 132 * 8 / a->count + 1), a->count);
+    rb::launch_pdl(gather_rows_kernel, grid, dim3(256), 0, st, (const uint4*)a->src, (uint4*)a->dst, a->src_index, a->dst_index, words,
+                   a->ld_src / 16, a->ld_dst / 16, a->src_rows, a->dst_rows);
+    return check_launch("gather_rows");
 }
 
 extern "C" int romab200_split_f16x3(const rb_split_args* a, void* stream) {

@@ -71,6 +71,7 @@ class Engine(BufferArena):
                                                  # flow at r = 2, ties with the per-pixel kernel's L1 hits at r = 3; r = 7 uses the table above)
         self.fused_small_f32 = True              # fp32 modes: stride-1 (C = 24) refiner blocks as one fused fp32 CUDA-core kernel
         self._side = None
+        self._bank, self.bank_version = None, 0  # match_pairs' per-image feature bank: (layout, capacity, {name: buffer})
         self.profile: Optional[dict] = None      # set to {} to collect CUDA-event timings per stage (bench.py)
         self.gemm_profile: Optional[list] = None  # set to [] to time every GEMM launch: (backend, flops, start, end, shape, epilogue)
 
@@ -93,8 +94,6 @@ class Engine(BufferArena):
     def sbuf(self, name, shape, zero=False) -> Split:
         """A cached RB_F16S buffer: two fp16 planes of `shape`."""
         return Split(self.buf(name + ".hi", shape, torch.float16, zero), self.buf(name + ".lo", shape, torch.float16, zero))
-
-    free_buffers = BufferArena.free
 
     def grid_axis(self, n):
         """linspace(-1+1/n, 1-1/n, n): pixel-centre coordinates (matcher.py:365-377)."""
@@ -332,24 +331,33 @@ class Engine(BufferArena):
     # ------------------------------------------------------------------ GP + transformer decoder (scale 16)
     def coarse_match(self, feat16, E, D, b, hp, wp, state):
         """GP posterior (matcher.py:291-323), embedding decoder (transformer/__init__.py:30-46) and
-        cls_to_flow_refine (utils.py:300-322): fills state [D, hp, wp, 3]; returns the projected features."""
+        cls_to_flow_refine (utils.py:300-322): fills state [D, hp, wp, 3]; returns the projected features.
+        The image stage (`gp_project`, `gp_rows`, `gp_solve_images`) reads one image at a time, the pair stage (`corr16_table`,
+        `gp_decode`) the pair; the stride-16 table is issued between the row splits and K_yy, where it always was."""
         n = hp * wp
+        g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
+        self.corr16_table(g, E, D, b, n)
+        Wk, stride_w = self.gp_solve_images(g, E, hp, wp)
+        return self.gp_decode(g, Wk.data_ptr() + n * pad8(n) * 4, stride_w, E, D, b, hp, wp, state)
+
+    def gp_project(self, feat16, E, n):
+        """p16 [E*n, 512] fp32: proj[16] of the DINOv2 patch tokens (the GP runs in fp32: x.float(), matcher.py:296)."""
         cin, cf = arch.PROJ[16]
         P = self.w.proj[16]
-        f32 = cabi.RB_F32
-        p16 = self.buf("gp.p16", (E * n, cf), dtype=torch.float32)      # GP runs in fp32 (x.float(), matcher.py:296)
+        p16 = self.buf("gp.p16", (E * n, cf), dtype=torch.float32)
         with self.stage("  gp.proj16"):
-            self.gemm(feat16, P["w"], p16, E * n, cf, cin, cin, P["w"].shape[1], cf, dtype_c=f32, bias=P["b"])
+            self.gemm(feat16, P["w"], p16, E * n, cf, cin, cin, P["w"].shape[1], cf, dtype_c=cabi.RB_F32, bias=P["b"])
+        return p16
+
+    def gp_rows(self, p16, E, n):
+        """The GP operands of E images' p16 rows: their L2 norms and, for the contractions on the tensor cores, the normalised rows
+        as split-fp16 pairs.  Returns them as a dict the other GP steps take."""
+        cf = arch.PROJ[16][1]
         norms = self.buf("gp.norms", (E * n,), dtype=torch.float32)
-        call("romab200_row_norms", "rb_rownorm_args", x=p16, out=norms, rows=E * n, cols=cf, ldx=cf, dtype=f32)
-        ldw = pad8(n)
-        nrhs = arch.GP_DIM
-        Wk = self.buf("gp.work", (E, n + nrhs, ldw), dtype=torch.float32)
-        stride_w = (n + nrhs) * ldw
-        # K_yy + sigma*I for every image (its own features): exp((cos-1)/T)   (matcher.py:191-200, 298, 301)
+        call("romab200_row_norms", "rb_rownorm_args", x=p16, out=norms, rows=E * n, cols=cf, ldx=cf, dtype=cabi.RB_F32)
         gp_split = self.split or (self.dtype != torch.float32 and self.gp_tensor_core)     # GP contractions as split-fp16 pairs (fp32-class)
         tc_kernel = False                 # (the K' = 3K operand trick of round 1 is superseded by the split back-end)
-        xs = None
+        xs = xa = xb = None
         if gp_split:
             # all-pairs CosKernel on the tensor cores with fp32-class accuracy: the L2-normalised rows as an RB_F16S pair
             with self.stage("  gp.split"):
@@ -362,26 +370,40 @@ class Engine(BufferArena):
             with self.stage("  gp.split"):
                 call("romab200_split_f16x3", "rb_split_args", x=p16, dst=xa, rows=E * n, cols=cf, ldx=cf, ldd=3 * cf, row_norm=norms, layout_b=0)
                 call("romab200_split_f16x3", "rb_split_args", x=p16, dst=xb, rows=E * n, cols=cf, ldx=cf, ldd=3 * cf, row_norm=norms, layout_b=1)
+        return dict(p16=p16, norms=norms, xs=xs, xa=xa, xb=xb, split=gp_split, tc=tc_kernel)
+
+    def corr16_table(self, g, E, D, b, n):
+        """Parity mode: the stride-16 refiner's local correlation (r = 7: 256 dot products of 512 channels per pixel) from ONE
+        all-pairs contraction per direction on the tensor cores: table[i, p, q] = <x_i[p], y_i[q]> / sqrt(512), gathered by the
+        prologue.  Decoder item i pairs image i with image (i + b) % E."""
+        cf, ldw, f32 = arch.PROJ[16][1], pad8(n), cabi.RB_F32
         self._corr16 = None
         if self.split and self.lc_table16:
-            # the stride-16 refiner's local correlation (r = 7: 256 dot products of 512 channels per pixel) from ONE all-pairs
-            # contraction per direction on the tensor cores: table[i, p, q] = <x_i[p], y_i[q]> / sqrt(512), gathered by the prologue
             with self.stage("  gp.corr16"):
-                ps = self.split_pair(p16, E * n, cf, cf, name="gp.p16s")
+                ps = self.split_pair(g["p16"], E * n, cf, cf, name="gp.p16s")
                 tab = self.buf("ref.corr16", (D, n, ldw), dtype=torch.float32)
                 for i0, cnt, y0 in ([(0, b, b)] if D == b else [(0, b, b), (b, b, 0)]):
                     self.gemm(ps.at(i0 * n * cf), ps.at(y0 * n * cf), tab.data_ptr() + i0 * n * ldw * 4, n, n, cf, cf, cf, ldw, dtype_c=f32,
                               batch0=cnt, sa0=n * cf, sb0=n * cf, sc0=n * ldw, alpha=float(torch.rsqrt(torch.tensor(float(cf)))))
                 self._corr16 = (tab, ldw)
+
+    def gp_solve_images(self, g, E, hp, wp):
+        """K_yy + sigma*I of every image with its own features, and the solve against the cosine basis.  Returns the workspace
+        [E, n + 512, ldw] whose rows n.. of every image hold alpha^T, and its per-image stride in elements."""
+        n = hp * wp
+        cf, nrhs, ldw, f32 = arch.PROJ[16][1], arch.GP_DIM, pad8(n), cabi.RB_F32
+        Wk = self.buf("gp.work", (E, n + nrhs, ldw), dtype=torch.float32)
+        stride_w = (n + nrhs) * ldw
+        # K_yy + sigma*I for every image (its own features): exp((cos-1)/T)   (matcher.py:191-200, 298, 301)
         with self.stage("  gp.kyy"):
-            if gp_split:
-                self.gp_kernel_matrix_split(xs, xs, norms, norms, Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
+            if g["split"]:
+                self.gp_kernel_matrix_split(g["xs"], g["xs"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
                                             sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
-            elif tc_kernel:
-                self.gp_kernel_matrix_tc(xa, xb, norms, norms, Wk, n, cf, ldw, batch=E, sa=n * 3 * cf, sb=n * 3 * cf, sc=stride_w,
+            elif g["tc"]:
+                self.gp_kernel_matrix_tc(g["xa"], g["xb"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * 3 * cf, sb=n * 3 * cf, sc=stride_w,
                                          sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
             else:
-                self.gp_kernel_matrix(p16, p16, norms, norms, Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
+                self.gp_kernel_matrix(g["p16"], g["p16"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
                                       sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
         basis_t = self.gp_basis_t(hp, wp)
         for e in range(E):
@@ -394,17 +416,26 @@ class Engine(BufferArena):
             ws = self.buf("gp.solve_ws", (ws_bytes // 4,), dtype=torch.float32)
             call("romab200_gp_solve", "rb_gp_solve_args", W=Wk, n=n, nrhs=nrhs, batch=E, ldw=ldw, stride=stride_w,
                  workspace=ws if self.gp_algo else None, workspace_bytes=ws_bytes if self.gp_algo else 0, algo=self.gp_algo)
+        return Wk, stride_w
+
+    def gp_decode(self, g, alpha_t, stride_a, E, D, b, hp, wp, state):
+        """Pair stage of the coarse match: K_xy and mu = K_xy @ alpha, the decoder and cls_to_flow_refine; fills state [D, hp, wp, 3]
+        and returns the stride-16 refiner features.  `alpha_t` points at image 0's alpha^T [512, ldw] (fp32), the other images follow
+        `stride_a` elements apart."""
+        n = hp * wp
+        cf, nrhs, ldw, f32 = arch.PROJ[16][1], arch.GP_DIM, pad8(n), cabi.RB_F32
+        p16, norms, xs, xa, xb = g["p16"], g["norms"], g["xs"], g["xa"], g["xb"]
         # K_xy and mu = K_xy @ alpha for every decoder item: query image i, support image (i + b) % E
         dim = arch.DEC_DIM
         tokens = self.buf("dec.tokens_in", (D * n, dim))
         es = tokens.element_size()
         halves = [(0, b, b)] if D == b else [(0, b, b), (b, b, 0)]     # (first item, count, first support image)
-        if gp_split:
+        if g["split"]:
             kxy = self.sbuf("gp.kxy", (D, n, ldw))
             alpha = self.sbuf("gp.alpha", (E, nrhs, ldw))
             with self.stage("  gp.kxy+mu"):
-                for e in range(E):          # alpha^T = rows n.. of every solved workspace
-                    call("romab200_split_f16s", "rb_split_pair_args", x=Wk.data_ptr() + (e * stride_w + n * ldw) * 4,
+                for e in range(E):          # alpha^T of every image as an RB_F16S pair
+                    call("romab200_split_f16s", "rb_split_pair_args", x=alpha_t + e * stride_a * 4,
                          hi=alpha.at(e * nrhs * ldw).hi, lo=alpha.at(e * nrhs * ldw).lo, rows=nrhs, cols=n, ldx=ldw, ldd=ldw)
                 for i0, cnt, y0 in halves:
                     self.gp_kernel_matrix_split(xs.at(i0 * n * cf), xs.at(y0 * n * cf), norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
@@ -416,7 +447,7 @@ class Engine(BufferArena):
             kxy = self.buf("gp.kxy", (D, n, ldw), dtype=torch.float32)
         for i0, cnt, y0 in halves:
           with self.stage("  gp.kxy+mu"):
-            if tc_kernel:
+            if g["tc"]:
                 self.gp_kernel_matrix_tc(xa.data_ptr() + i0 * n * 3 * cf * 2, xb.data_ptr() + y0 * n * 3 * cf * 2,
                                          norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
                                          kxy.data_ptr() + i0 * n * ldw * 4, n, cf, ldw, batch=cnt, sa=n * 3 * cf, sb=n * 3 * cf,
@@ -426,9 +457,9 @@ class Engine(BufferArena):
                                       norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
                                       kxy.data_ptr() + i0 * n * ldw * 4, n, cf, ldw, batch=cnt, sa=n * cf, sb=n * cf, sc=n * ldw,
                                       sna=n, snb=n, diag=0.0)
-            self.gemm(kxy.data_ptr() + i0 * n * ldw * 4, Wk.data_ptr() + (y0 * stride_w + n * ldw) * 4,
+            self.gemm(kxy.data_ptr() + i0 * n * ldw * 4, alpha_t + y0 * stride_a * 4,
                       tokens.data_ptr() + i0 * n * dim * es, n, nrhs, n, ldw, ldw, dim, dtype_ab=f32,
-                      batch0=cnt, sa0=n * ldw, sb0=stride_w, sc0=n * dim)
+                      batch0=cnt, sa0=n * ldw, sb0=stride_a, sc0=n * dim)
         # tokens = cat(gp_posterior, f1_s) (transformer/__init__.py:33)
         self.copy2d(p16, tokens.data_ptr() + arch.GP_DIM * es, D * n, cf, cf, dim, f32, self.dt)
         if self.debug is not None:
@@ -576,13 +607,13 @@ class Engine(BufferArena):
             cnn = self.encode_cnn(images, tag)
         feats, sizes = cnn
         sizes = dict(sizes)
-        states = {}
+        feats = dict(feats)
         if not upsample:
             feat16_raw, hp, wp = vit
             sizes[16] = (hp, wp)
             state = self.buf("state.lo.16", (D, hp, wp, 3), dtype=torch.float32)
             with self.stage("gp+decoder"):
-                feat16 = self.coarse_match(feat16_raw, E, D, b, hp, wp, state)
+                feats[16] = (self.coarse_match(feat16_raw, E, D, b, hp, wp, state), arch.PROJ[16][1])
             if self.debug is not None:
                 self.debug["coarse_state"] = state.clone()
             scales = arch.SCALES
@@ -590,15 +621,20 @@ class Engine(BufferArena):
             src, hi, wi = state_in
             state = self.resize_state(src, D, hi, wi, *sizes[8], name="state.up.8")
             scales = arch.UPSAMPLE_SCALES
+        state, states = self.refine_chain(state, scales, feats, sizes, E, D, b, H, W, scale_factor, tag, keep_states, cnn_ready)
+        return state, states, sizes
+
+    def refine_chain(self, state, scales, feats, sizes, E, D, b, H, W, scale_factor, tag, keep_states=False, cnn_ready=None):
+        """The refiners of one pass from `state` [D, h, w, 3] at scale scales[0] on, each followed by the resize to the next scale.
+        feats {s: (features [E, h, w, pitch], pitch)}; H, W: the pass's image size.  Returns (state [D, H, W, 3], {s: state after
+        refiner s} for s = 16, or for every s with keep_states).  `cnn_ready`: event to wait for before the first CNN feature map."""
+        states = {}
         for s in scales:
             h, w = sizes[s]
-            if s == 16:
-                feat, ldf = feat16, arch.PROJ[16][1]
-            else:
-                if cnn_ready is not None:
-                    torch.cuda.current_stream().wait_event(cnn_ready)
-                    cnn_ready = None
-                feat, ldf = feats[s]
+            if s != 16 and cnn_ready is not None:
+                torch.cuda.current_stream().wait_event(cnn_ready)
+                cnn_ready = None
+            feat, ldf = feats[s]
             if self.debug is not None:
                 self.debug[f"{tag}.proj{s}"] = feat.view(E, h, w, -1)[..., :arch.PROJ[s][1]].float().clone()
             with self.stage(f"refine{s}.{tag}"):
@@ -608,16 +644,14 @@ class Engine(BufferArena):
             if s != 1:
                 ho, wo = sizes[s // 2]
                 state = self.resize_state(state, D, h, w, ho, wo, name=f"state.{tag}.{s // 2}")
-        return state, states, sizes
+        return state, states
 
     def run_match(self, images, images_hi, b, symmetric, scale_lo, scale_hi, attenuate, warp, cert):
         """Device side of match(): coarse pass, optional upsample pass, epilogue — no allocation, no host sync.
         The CNN branch (VGG19 + proj of both passes) has no dependency on the ViT / GP / decoder chain, so it runs on a
         side stream and overlaps the latency-bound GP solve and decoder; under CUDA-graph capture this becomes a fork."""
         main = torch.cuda.current_stream()
-        if self._side is None:
-            self._side = torch.cuda.Stream(device=self.device)
-        side = self._side
+        side = self.side_stream()
         overlap = self.overlap_cnn and self.debug is None
         cnn_lo = cnn_hi = ev_lo = ev_hi = vit = None
         if overlap:
@@ -645,6 +679,131 @@ class Engine(BufferArena):
             state, _, _ = self.run_pass(images_hi, b, symmetric, True, scale_hi, (state, hs, ws), cnn=cnn_hi, cnn_ready=ev_hi)
             hs, ws = hh, wh
         self.epilogue(state, coarse, hc, wc, b, hs, ws, symmetric, out=(warp, cert))
+
+    def side_stream(self):
+        if self._side is None:
+            self._side = torch.cuda.Stream(device=self.device)
+        return self._side
+
+    # ------------------------------------------------------------------ match_pairs: encode each image once, then decode pairs
+    def bank_layout(self, hs, ws, hu=0, wu=0):
+        """{name: (per-image shape, dtype)} of everything the pair stage and the refiners read of one image: p16 and alpha^T of the
+        GP solve (fp32), and the projected CNN features at strides 8/4/2/1 of the coarse pass ("lo") and, when hu > 0, of the
+        upsample pass ("up"), in the compute dtype.  The stride-16 refiner features are p16 itself."""
+        n = (hs // arch.VIT_PATCH) * (ws // arch.VIT_PATCH)
+        out = {"p16": ((n, arch.PROJ[16][1]), torch.float32), "alpha": ((arch.GP_DIM, pad8(n)), torch.float32)}
+        for tag, H, W in (("lo", hs, ws), ("up", hu, wu)):
+            if H:
+                for s in (8, 4, 2, 1):
+                    out[f"{tag}.{s}"] = ((H // s, W // s, pad8(arch.PROJ[s][1])), self.dtype)
+        return out
+
+    def feature_bank(self, count, hs, ws, hu=0, wu=0):
+        """The per-image feature bank of match_pairs: {name: [capacity, *per-image shape]} arena buffers, so their addresses are
+        stable for the CUDA graphs that hold them and free_buffers() drops them with those graphs.  The current bank is kept while
+        its layout matches and it has room for `count` images; otherwise it is dropped, one of capacity `count` is made and
+        `bank_version` increases (graphs recorded over the old one must not replay)."""
+        layout = self.bank_layout(hs, ws, hu, wu)
+        cur = self._bank
+        if cur is not None and cur[0] == layout and cur[1] >= count and \
+                all(self._buf.get((f"bank.{k}", tuple(t.shape), t.dtype)) is t for k, t in cur[2].items()):
+            return cur[2]
+        for key in [k for k in self._buf if k[0].startswith("bank.")]:
+            del self._buf[key]
+        bank = {k: self.buf(f"bank.{k}", (count,) + shape, dtype) for k, (shape, dtype) in layout.items()}
+        self._bank = (layout, count, bank)
+        self.bank_version += 1
+        return bank
+
+    def free_buffers(self):
+        self._bank = None
+        self.free()
+
+    def copy_rows(self, src, dst, count, row_bytes, ld_src, ld_dst, src_rows, dst_rows, src_index=None, dst_index=None):
+        """Row dst_index[i] of dst = row src_index[i] of src for i < count (an index left None is i); rows of row_bytes bytes."""
+        call("romab200_gather_rows", "rb_gather_rows_args", src=src, dst=dst, src_index=src_index, dst_index=dst_index, count=count,
+             row_bytes=row_bytes, ld_src=ld_src, ld_dst=ld_dst, src_rows=src_rows, dst_rows=dst_rows)
+
+    def encode_images(self, images, images_hi, slots, bank):
+        """Image stage of match_pairs for E images [E, 3, H, W] (and [E, 3, Hu, Wu] for the upsample pass, else None): DINOv2, p16
+        and the GP solve on the launch stream, the CNN branch of both passes beside them on the side stream as in run_match, then
+        every image's features scattered into the bank rows `slots` (int32 [E] on the device).  No allocation beyond the arena, no
+        host sync."""
+        E, _, H, W = images.shape
+        hp, wp = H // arch.VIT_PATCH, W // arch.VIT_PATCH
+        n, cap = hp * wp, bank["p16"].shape[0]
+        overlap = self.overlap_cnn and self.debug is None
+        cnn, ready = {}, None
+
+        def encode_cnn():
+            cnn["lo"] = self.encode_cnn(images, "lo")[0]
+            if images_hi is not None:
+                cnn["up"] = self.encode_cnn(images_hi, "up")[0]
+        with self.stage("dinov2"):
+            feat16, _, _ = self.dinov2(images)
+        if overlap:
+            main, side = torch.cuda.current_stream(), self.side_stream()
+            side.wait_stream(main)
+            with torch.cuda.stream(side):
+                self._lane = "side"
+                encode_cnn()
+                ready = torch.cuda.Event()
+                ready.record(side)
+                self._lane = "main"
+        else:
+            encode_cnn()
+        with self.stage("gp"):
+            g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
+            Wk, stride_w = self.gp_solve_images(g, E, hp, wp)
+        if ready is not None:
+            main.wait_event(ready)
+        with self.stage("bank.scatter"):
+            row = bank["p16"][0].numel() * 4
+            self.copy_rows(g["p16"], bank["p16"], E, row, row, row, E, cap, dst_index=slots)
+            row = bank["alpha"][0].numel() * 4
+            self.copy_rows(Wk.data_ptr() + n * pad8(n) * 4, bank["alpha"], E, row, stride_w * 4, row, E, cap, dst_index=slots)
+            for tag, feats in cnn.items():
+                for s in (8, 4, 2, 1):
+                    dst = bank[f"{tag}.{s}"]
+                    row = dst[0].numel() * dst.element_size()
+                    self.copy_rows(feats[s][0], dst, E, row, row, row, E, cap, dst_index=slots)
+
+    def decode_pairs(self, bank, index, P, symmetric, scale_lo, scale_hi, attenuate, warp, cert):
+        """Pair stage of match_pairs for P pairs.  The 2P images index[:P] (im_A of every pair) and index[P:] (im_B), int32 bank
+        rows on the device, are gathered into the buffers match() fills for b = P, in its [A_1..A_P | B_1..B_P] layout; then the pair
+        stage of the coarse match, the refiners of both passes and the epilogue run as in run_match, into warp / cert."""
+        E, b = 2 * P, P
+        D = E if symmetric else b
+        cap = bank["p16"].shape[0]
+        passes = [t for t in ("lo", "up") if f"{t}.1" in bank]
+        sizes = {t: {s: tuple(bank[f"{t}.{s}"].shape[1:3]) for s in (8, 4, 2, 1)} for t in passes}
+        hs, ws = sizes["lo"][1]
+        hp, wp = hs // arch.VIT_PATCH, ws // arch.VIT_PATCH
+        n, cf, nrhs = hp * wp, arch.PROJ[16][1], arch.GP_DIM
+        sizes["lo"][16] = (hp, wp)
+
+        def gather(src, dst):
+            row = src[0].numel() * src.element_size()
+            self.copy_rows(src, dst, E, row, row, row, cap, E, src_index=index)
+            return dst
+        with self.stage("bank.gather"):
+            p16 = gather(bank["p16"], self.buf("gp.p16", (E * n, cf), dtype=torch.float32))
+            alpha = gather(bank["alpha"], self.buf("pair.alpha_t", (E, nrhs, pad8(n)), dtype=torch.float32))
+            feats = {t: {s: (gather(bank[f"{t}.{s}"], self.buf(f"proj{t}.{s}", (E,) + tuple(bank[f"{t}.{s}"].shape[1:]), zero=True)),
+                             pad8(arch.PROJ[s][1])) for s in (8, 4, 2, 1)} for t in passes}
+        state = self.buf("state.lo.16", (D, hp, wp, 3), dtype=torch.float32)
+        with self.stage("gp+decoder"):
+            g = self.gp_rows(p16, E, n)
+            self.corr16_table(g, E, D, b, n)
+            feats["lo"][16] = (self.gp_decode(g, alpha.data_ptr(), nrhs * pad8(n), E, D, b, hp, wp, state), cf)
+        state, states = self.refine_chain(state, arch.SCALES, feats["lo"], sizes["lo"], E, D, b, hs, ws, scale_lo, "lo")
+        coarse = states[16] if attenuate else None
+        H, W = hs, ws
+        if "up" in passes:
+            H, W = sizes["up"][1]
+            state = self.resize_state(state, D, hs, ws, *sizes["up"][8], name="state.up.8")
+            state, _ = self.refine_chain(state, arch.UPSAMPLE_SCALES, feats["up"], sizes["up"], E, D, b, H, W, scale_hi, "up")
+        self.epilogue(state, coarse, hp, wp, b, H, W, symmetric, out=(warp, cert))
 
     def epilogue(self, state, coarse_state, hc, wc, b, H, W, symmetric, out=None):
         Wout = 2 * W if symmetric else W

@@ -10,6 +10,7 @@ geometry helpers are plain tensor arithmetic on whatever device their inputs liv
 from __future__ import annotations
 
 import math
+import operator
 import os
 from warnings import warn
 
@@ -43,6 +44,8 @@ class RegressionMatcher:
         self._graphs = GraphCache()
         self._pre = None
         self._sample_graphs = GraphCache()      # static buffers + CUDA graph of the device sampler, per (n, num, mode)
+        self._pair_graphs = GraphCache()        # match_pairs: encode batches and decode chunks, per size
+        self._bank_version = 0                  # the engine's feature bank the match_pairs graphs were recorded over
 
     # ---- nn.Module-ish conveniences callers rely on ------------------------------------------------
     def train(self, mode: bool = True):
@@ -67,6 +70,7 @@ class RegressionMatcher:
         """Release every cached activation buffer and the CUDA graphs recorded over them."""
         self._graphs.clear()
         self._sample_graphs.clear()
+        self._pair_graphs.clear()
         self.engine.free_buffers()
 
     def get_output_resolution(self):
@@ -119,48 +123,161 @@ class RegressionMatcher:
             device = eng.device
         if torch.device(device).type != "cuda":
             raise RuntimeError("roma_b200 computes on CUDA only; device=%r" % (device,))
-        # JPEG paths are decoded on the device (both in one launch set); other paths, PIL images and tensors as before
-        im_A, im_B = open_inputs([im_A_input, im_B_input], eng.device)
-        symmetric = self.symmetric
         ws, hs = self.w_resized, self.h_resized
         scale_factor = math.sqrt(hs * ws / (560 ** 2))
-        pil_route = isinstance(im_A, (Image.Image, DeviceImage)) and isinstance(im_B, (Image.Image, DeviceImage))
+        (a_t, b_t), hi = self._device_inputs([im_A_input, im_B_input], [im_A_high_res, im_B_high_res], ("im_A", "im_B"))
+        a_h, b_h = hi if hi is not None else (None, None)
+        with torch.cuda.device(eng.device):
+            return self._match_device(a_t, b_t, a_h, b_h, b_t.shape[0], self.symmetric, scale_factor)
+
+    def _device_inputs(self, inputs, high_res, names):
+        """The input rules `match` and `match_pairs` share.  `inputs`: paths / PIL images, or tensors [b, 3, h, w] of one size (not a
+        mix); `high_res`: the caller's upsample-resolution tensors, one per input (all None, or all given); `names` name the inputs
+        in error messages.  Returns ([coarse-resolution tensor [b, 3, h, w] per input], [upsample-resolution tensor per input] when
+        upsample_preds, else None).  JPEG paths are decoded on the device in one launch set; path and PIL inputs are resized
+        there (Pillow-exact bicubic, csrc/preprocess.cu) to (h_resized, w_resized) and to upsample_res."""
+        opened = open_inputs(inputs, self.engine.device)
+        hs, ws = self.h_resized, self.w_resized
+        pil_route = all(isinstance(im, (Image.Image, DeviceImage)) for im in opened)
         if pil_route:
-            # raw RGB bytes go up once per image (or were decoded there); Pillow's bicubic resize + normalisation run on the
-            # device (csrc/preprocess.cu)
-            b = 1
+            # raw RGB bytes go up once per image (or were decoded there)
             pre = self._preprocessor()
-            raw_a, raw_b = (im.raw if isinstance(im, DeviceImage) else pre.upload(im) for im in (im_A, im_B))
-            a_t = pre.resize_normalize(raw_a, (hs, ws))[None]
-            b_t = pre.resize_normalize(raw_b, (hs, ws))[None]
-        elif isinstance(im_A, torch.Tensor) and isinstance(im_B, torch.Tensor):
-            b, c, h, w = im_A.shape
-            b, c, h2, w2 = im_B.shape
-            assert w == w2 and h == h2, "For batched images we assume same size"
+            raws = [im.raw if isinstance(im, DeviceImage) else pre.upload(im) for im in opened]
+            lo = [pre.resize_normalize(raw, (hs, ws))[None] for raw in raws]
+        elif all(isinstance(im, torch.Tensor) for im in opened):
+            h, w = opened[0].shape[-2:]
+            assert all(im.shape[-2:] == (h, w) for im in opened), "For batched images we assume same size"
             if h != self.h_resized or self.w_resized != w:
                 warn("Model resolution and batch resolution differ, may produce unexpected results")
-            hs, ws = h, w
-            a_t, b_t = im_A, im_B
+            lo = list(opened)
         else:
-            raise ValueError(f"Unsupported input type: {type(im_A)=} and {type(im_B)=}")
+            raise ValueError("Unsupported input type: " + " and ".join(f"type({nm})={type(im)!r}" for nm, im in zip(names, opened)))
+        if not self.upsample_preds:
+            return lo, None
+        hs, ws = self.upsample_res
+        if all(h is None for h in high_res):
+            # the reference re-opens / re-uses the same images here (matcher.py:855-866): same bytes, already on the device
+            if not isinstance(inputs[0], (str, os.PathLike)):
+                for nm, x in zip(names, inputs):
+                    assert isinstance(x, Image.Image), f"Unsupported input type: type({nm}_input)={type(x)!r}"
+            assert pil_route, "upsample_preds without high-res tensors needs path or PIL inputs"
+            return lo, [pre.resize_normalize(raw, (hs, ws))[None] for raw in raws]
+        if all(h is not None for h in high_res):
+            return lo, list(high_res)
+        parts = [p for nm, im, h in zip(names, opened, high_res) for p in (f"{nm}={im!r}", f"{nm}_high_res={h!r}")]
+        raise ValueError(f"Invalid upsample_preds and high_res inputs with {','.join(parts[:-1])} and {parts[-1]}")
 
-        a_h = b_h = None
+    @torch.inference_mode()
+    def match_pairs(self, images, pairs, images_high_res=None, *, max_batch=8, on_batch=None):
+        """Dense warps of many pairs drawn from one image set, each image encoded once.
+
+        images: a sequence of paths / PIL images (decoded and resized on the device as in `match`), or a tensor [N, 3, h, w]
+        (then `images_high_res` [N, 3, H, W] is required when upsample_preds).  pairs: a [P, 2] integer tensor or a sequence of
+        (i, j); pair k matches im_A = images[i_k] with im_B = images[j_k] (any order, repeats and i == j allowed).
+
+        Returns (warp [P, H, W*(2 if symmetric), 4], certainty [P, H, W*(2)]) in pair order: pair k holds what
+        match(images[i_k], images[j_k]) returns.  With `on_batch`, calls on_batch(first_pair_index, warp, certainty) for consecutive
+        chunks of at most `max_batch` pairs instead and returns None; those tensors are reused by the next chunk, so they stay valid
+        until the callback returns and a caller that keeps them clones them.
+
+        Only the images some pair references are encoded, each once, in batches of at most `max_batch` (which also bounds the
+        decode chunk of path inputs) into a per-image feature bank of the engine (about 0.24 GB per image at 560 -> 864 with fp32
+        maps, computed from the buffer shapes); the bank is kept for later calls until free_buffers()."""
+        eng = self.engine
+        if int(max_batch) < 1:
+            raise ValueError(f"max_batch must be positive, got {max_batch}")
+        max_batch = int(max_batch)
+        if isinstance(images, torch.Tensor):
+            if images.dim() != 4:
+                raise ValueError(f"images must be [N, 3, h, w], got shape {tuple(images.shape)}")
+            n_images = images.shape[0]
+        else:
+            images = list(images)
+            bad = [type(x) for x in images if not isinstance(x, (str, os.PathLike, Image.Image))]
+            if bad:
+                raise ValueError(f"Unsupported input type: images mixes paths / PIL images with {bad[0]!r}")
+            n_images = len(images)
+        pairs = pair_tensor(pairs, n_images)
+        hi_given = images_high_res is not None
+        if hi_given and (images_high_res.dim() != 4 or images_high_res.shape[0] != n_images):
+            raise ValueError(f"images_high_res must be [{n_images}, 3, H, W], got shape {tuple(images_high_res.shape)}")
+        if isinstance(images, torch.Tensor):
+            self._device_inputs([images], [images_high_res], ("images",))      # match()'s checks of tensor inputs; no device work
+            hs, ws = images.shape[-2:]
+        else:
+            hs, ws = self.h_resized, self.w_resized
+        hu, wu = (0, 0)
         if self.upsample_preds:
-            hs, ws = self.upsample_res
-            if im_A_high_res is None and im_B_high_res is None:
-                # the reference re-opens / re-uses the same two images here (matcher.py:855-866): same bytes, already on the device
-                if not isinstance(im_A_input, (str, os.PathLike)):
-                    assert isinstance(im_A_input, Image.Image), f"Unsupported input type: {type(im_A_input)=}"
-                    assert isinstance(im_B_input, Image.Image), f"Unsupported input type: {type(im_B_input)=}"
-                assert pil_route, "upsample_preds without high-res tensors needs path or PIL inputs"
-                a_h = pre.resize_normalize(raw_a, (hs, ws))[None]
-                b_h = pre.resize_normalize(raw_b, (hs, ws))[None]
-            elif im_A_high_res is not None and im_B_high_res is not None:
-                a_h, b_h = im_A_high_res, im_B_high_res
-            else:
-                raise ValueError(f"Invalid upsample_preds and high_res inputs with {im_A=},{im_A_high_res=},{im_B=} and {im_B_high_res=}")
+            hu, wu = images_high_res.shape[-2:] if hi_given else self.upsample_res
+        P = pairs.shape[0]
+        ho, wo = (hu, wu) if self.upsample_preds else (hs, ws)
+        wout = 2 * wo if self.symmetric else wo
+        if P == 0:
+            if on_batch is not None:
+                return None
+            return (torch.empty(0, ho, wout, 4, dtype=torch.float32, device=eng.device),
+                    torch.empty(0, ho, wout, dtype=torch.float32, device=eng.device))
+        plan = plan_pairs(pairs, max_batch)
         with torch.cuda.device(eng.device):
-            return self._match_device(a_t, b_t, a_h, b_h, b, symmetric, scale_factor)
+            return self._match_pairs_device(images, images_high_res, plan, (hs, ws), (hu, wu), (ho, wout), on_batch)
+
+    def _match_pairs_device(self, images, images_high_res, plan, lo_res, hi_res, out_res, on_batch):
+        eng = self.engine
+        dev = eng.device
+        (hs, ws), (hu, wu), (ho, wout) = lo_res, hi_res, out_res
+        used, index = plan["used"], plan["index"].to(dev)
+        symmetric, attenuate = self.symmetric, bool(self.attenuate_cert)
+        scale_lo = math.sqrt(self.h_resized * self.w_resized / (560 ** 2))
+        scale_hi = math.sqrt(self.upsample_res[0] * self.upsample_res[1] / (560 ** 2))
+        use_graph = self.use_cuda_graph and eng.debug is None and eng.profile is None and eng.gemm_profile is None
+        bank = eng.feature_bank(len(used), hs, ws, hu, wu)
+        if eng.bank_version != self._bank_version:
+            self._pair_graphs.clear()           # graphs recorded over a bank that is gone
+            self._bank_version = eng.bank_version
+        cap = bank["p16"].shape[0]
+        slots = torch.arange(len(used), dtype=torch.int32, device=dev)
+        for e0 in range(0, len(used), plan["max_batch"]):
+            sel = used[e0:e0 + plan["max_batch"]]
+            E = len(sel)
+            key = ("encode", E, hs, ws, hu, wu, cap, eng.bank_version)
+            entry = self._pair_graphs.entry(key, lambda: dict(
+                images=torch.empty(E, 3, hs, ws, dtype=torch.float32, device=dev),
+                images_hi=torch.empty(E, 3, hu, wu, dtype=torch.float32, device=dev) if hu else None,
+                slots=torch.empty(E, dtype=torch.int32, device=dev)), use_graph, eng.generation)
+            bufs = entry["bufs"]
+            if isinstance(images, torch.Tensor):
+                lo = [images[sel]]
+                hi = [images_high_res[sel]] if hu else None
+            else:
+                lo, hi = self._device_inputs([images[i] for i in sel], [None] * E if images_high_res is None else
+                                             [images_high_res[i:i + 1] for i in sel], [f"images[{i}]" for i in sel])
+            for name, parts in (("images", lo), ("images_hi", hi if hu else [])):
+                k = 0
+                for t in parts:
+                    bufs[name][k:k + t.shape[0]].copy_(t, non_blocking=True)
+                    k += t.shape[0]
+            bufs["slots"].copy_(slots[e0:e0 + E], non_blocking=True)
+            self._pair_graphs.run(entry, lambda: eng.encode_images(bufs["images"], bufs["images_hi"], bufs["slots"], bank))
+        n_pairs = plan["chunks"][-1][1]
+        outs = None if on_batch is not None else (torch.empty(n_pairs, ho, wout, 4, dtype=torch.float32, device=dev),
+                                                  torch.empty(n_pairs, ho, wout, dtype=torch.float32, device=dev))
+        for k0, k1, i0, i1 in plan["chunks"]:
+            P = k1 - k0
+            key = ("decode", P, hs, ws, hu, wu, symmetric, attenuate, scale_lo, scale_hi, cap, eng.bank_version)
+            entry = self._pair_graphs.entry(key, lambda: dict(
+                index=torch.empty(2 * P, dtype=torch.int32, device=dev),
+                warp=torch.empty(P, ho, wout, 4, dtype=torch.float32, device=dev),
+                cert=torch.empty(P, ho, wout, dtype=torch.float32, device=dev)), use_graph, eng.generation)
+            bufs = entry["bufs"]
+            bufs["index"].copy_(index[i0:i1], non_blocking=True)
+            self._pair_graphs.run(entry, lambda: eng.decode_pairs(bank, bufs["index"], P, symmetric, scale_lo, scale_hi, attenuate,
+                                                                  bufs["warp"], bufs["cert"]))
+            if on_batch is not None:
+                on_batch(k0, bufs["warp"], bufs["cert"])
+            else:
+                outs[0][k0:k1].copy_(bufs["warp"])
+                outs[1][k0:k1].copy_(bufs["cert"])
+        return outs
 
     def _match_device(self, a_t, b_t, a_h, b_h, b, symmetric, scale_factor):
         eng = self.engine
@@ -310,6 +427,45 @@ class RegressionMatcher:
             arr = (arr.clamp(0, 1) * 255).byte().permute(1, 2, 0).cpu().numpy()
             Image.fromarray(arr).save(save_path)
         return vis_im
+
+
+def pair_tensor(pairs, n_images: int) -> torch.Tensor:
+    """`pairs` of match_pairs as an int64 [P, 2] CPU tensor.  ValueError for anything but a [P, 2] integer tensor or a sequence of
+    (i, j) integers, IndexError for an index outside [0, n_images)."""
+    if isinstance(pairs, torch.Tensor):
+        if pairs.dtype.is_floating_point or pairs.dtype.is_complex or pairs.dtype == torch.bool:
+            raise ValueError(f"pairs must hold integers, got {pairs.dtype}")
+        t = pairs.detach().to("cpu", torch.int64)
+    else:
+        rows = []
+        for p in pairs:
+            try:
+                i, j = p
+                rows.append((operator.index(i), operator.index(j)))
+            except (TypeError, ValueError):
+                raise ValueError(f"pairs must be (i, j) pairs of integers, got {p!r}") from None
+        t = torch.tensor(rows, dtype=torch.int64).reshape(-1, 2)
+    if t.dim() != 2 or t.shape[1] != 2:
+        raise ValueError(f"pairs must be [P, 2], got shape {tuple(t.shape)}")
+    if t.numel() and (int(t.min()) < 0 or int(t.max()) >= n_images):
+        bad = t[(t < 0) | (t >= n_images)][0].item()
+        raise IndexError(f"pairs holds image index {bad}, outside [0, {n_images})")
+    return t
+
+
+def plan_pairs(pairs: torch.Tensor, max_batch: int) -> dict:
+    """Schedule of match_pairs for [P, 2] pairs (P > 0): `used`, the referenced images in ascending order (bank row k holds image
+    used[k]; they are encoded in batches of max_batch in that order); `chunks`, (first pair, end pair, first and end entry of
+    `index`) of the decode chunks of at most max_batch pairs; `index`, int32, the bank rows of every chunk's images in
+    [A_1..A_P | B_1..B_P] order, chunk after chunk."""
+    used, rows = torch.unique(pairs.flatten(), return_inverse=True)
+    rows = rows.view(-1, 2).to(torch.int32)
+    index, chunks = [], []
+    for k0 in range(0, pairs.shape[0], max_batch):
+        k1 = min(pairs.shape[0], k0 + max_batch)
+        index += [rows[k0:k1, 0], rows[k0:k1, 1]]
+        chunks.append((k0, k1, 2 * k0, 2 * k1))
+    return dict(used=used.tolist(), index=torch.cat(index), chunks=chunks, max_batch=max_batch)
 
 
 def _keypoints_on_device(x_A, x_B, warp, certainty) -> bool:
