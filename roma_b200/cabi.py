@@ -1,8 +1,10 @@
 """ctypes binding of libromab200.so — the thin shim between PyTorch (device memory, streams) and the C ABI.
 
 The argument structs are generated from `include/romab200.h` itself at import time, so the Python side
-cannot drift from the header.  Every wrapper passes raw device pointers (`tensor.data_ptr()`) and the
-current CUDA stream; a non-zero return code becomes a `RuntimeError` carrying `romab200_last_error()`.
+cannot drift from the header.  Every pointer field takes a tensor (or None), never a raw address: an operand that starts
+inside a buffer is passed as a view (`packing.at`), so its dtype, device, layout and extent are checked against what the call
+describes before the library sees it.  `call` passes the tensors' addresses and the current CUDA stream; a non-zero return
+code becomes a `RuntimeError` carrying `romab200_last_error()`.
 There is no fallback: if the library is missing or the device is not an H100 (sm_90), calls fail loudly.
 """
 from __future__ import annotations
@@ -65,6 +67,7 @@ def _parse_header(path: str):
 
 STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
+_PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
 _lib = None
 
@@ -86,14 +89,6 @@ def load_library(path: str = LIB_PATH) -> ctypes.CDLL:
         getattr(lib, fn)            # AttributeError if the header declares a symbol the library lacks
     _lib = lib
     return lib
-
-
-def _ptr(t):
-    if t is None:
-        return None
-    if isinstance(t, int):
-        return t
-    return t.data_ptr()
 
 
 def _stream():
@@ -128,7 +123,7 @@ _FIELD_DTYPES = {
     "rb_local_corr_args": {"f0": "dtype_f", "f1": "dtype_f", "flow": _F32, "out": "dtype_out", "win_x": _F32, "win_y": _F32},
     "rb_local_corr_warp_args": {"f0": _F32, "f1": _F32, "warp": _F32, "out": _F32},
     "rb_dwconv_args": {"in": "dtype", "weight": _F32, "bias": _F32, "out_lo": torch.float16},
-    "rb_refiner_block_small_args": {"in": "dtype", "out": "dtype", "dw_weight": _F32, "dw_bias": _F32},
+    "rb_refiner_block_small_args": {"in": "dtype", "out": "dtype", "dw_weight": _F32, "dw_bias": _F32, "pw_weight_host": _F32, "pw_bias_host": _F32},
     "rb_refiner_block_c144_args": {"in": "dtype", "out": "dtype", "dw_weight": _F32, "dw_bias": _F32, "pw_weight": "dtype", "pw_bias": _F32},
     "rb_refiner_block_c144_split_args": {"in": _F32, "out": _F32, "dw_weight": _F32, "dw_bias": _F32, "pw_weight": torch.float16,
                                          "pw_weight_lo": torch.float16, "pw_bias": _F32},
@@ -168,6 +163,8 @@ _FIELD_DTYPES = {
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}, "rb_dense_geometric_dist_args": {"dense_matches"}}
+# pointer fields the library reads on the host (the refiner block passes these weights as kernel parameters): CPU tensors
+_HOST_FIELDS = {"rb_refiner_block_small_args": {"pw_weight_host", "pw_bias_host"}}
 
 
 def _gemm_min_elems(kw):
@@ -188,15 +185,39 @@ def _gemm_min_elems(kw):
     return {"A": a, "A_lo": a, "B": b, "B_lo": b, "C": c, "C_lo": c}
 
 
+def _copy2d_min_elems(kw):
+    return {"src": (kw["rows"] - 1) * kw["lds"] + kw["cols"], "dst": (kw["rows"] - 1) * kw["ldd"] + kw["cols"]}
+
+
+def _gather_rows_min_elems(kw):
+    """The row geometry is in bytes; converted to elements of the tensor passed."""
+    out = {}
+    for k, rows, ld in (("src", "src_rows", "ld_src"), ("dst", "dst_rows", "ld_dst")):
+        if isinstance(kw.get(k), torch.Tensor):
+            out[k] = -(-((kw[rows] - 1) * kw[ld] + kw["row_bytes"]) // kw[k].element_size())
+    return out
+
+
+# struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
+_MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems}
+
+
 def _validate(fn_name, struct_name, kw):
     table = _FIELD_DTYPES.get(struct_name, {})
     cur = torch.cuda.current_device() if torch.cuda.is_available() else None
-    mins = _gemm_min_elems(kw) if struct_name == "rb_gemm_args" else {}
+    mins = _MIN_ELEMS[struct_name](kw) if struct_name in _MIN_ELEMS else {}
     strided = _STRIDED_FIELDS.get(struct_name, ())
+    host = _HOST_FIELDS.get(struct_name, ())
     for k, v in kw.items():
         if not isinstance(v, torch.Tensor):
+            if v is not None and k in _PTR_FIELDS[struct_name]:
+                raise TypeError(f"{fn_name}: pointer field `{k}` takes a tensor or None, not {type(v).__name__} "
+                                "(pass an operand that starts inside a buffer as a view, packing.at)")
             continue
-        if not v.is_cuda or (cur is not None and v.device.index != cur):
+        if k in host:
+            if v.device.type != "cpu":
+                raise RuntimeError(f"{fn_name}: argument `{k}` is read on the host, it must be a CPU tensor (got one on {v.device})")
+        elif not v.is_cuda or (cur is not None and v.device.index != cur):
             raise RuntimeError(f"{fn_name}: argument `{k}` lives on {v.device}, expected the current CUDA device cuda:{cur}")
         if k not in strided and not v.is_contiguous():
             raise RuntimeError(f"{fn_name}: argument `{k}` is not contiguous (shape {tuple(v.shape)}, strides {v.stride()})")
@@ -210,7 +231,7 @@ def _validate(fn_name, struct_name, kw):
 
 
 def call(fn_name: str, struct_name: str, **kw) -> None:
-    """Fill `struct_name` from keyword arguments (tensors become device pointers) and call `fn_name`."""
+    """Fill `struct_name` from keyword arguments (a pointer field takes a tensor, passed as its address, or None) and call `fn_name`."""
     global launch_count
     lib = load_library()
     args = STRUCTS[struct_name]()
@@ -220,8 +241,8 @@ def call(fn_name: str, struct_name: str, **kw) -> None:
             raise TypeError(f"{struct_name} has no field {k}")
     _validate(fn_name, struct_name, kw)
     for k, v in kw.items():
-        if isinstance(v, torch.Tensor) or v is None:
-            setattr(args, k, _ptr(v))
+        if k in _PTR_FIELDS[struct_name]:
+            setattr(args, k, None if v is None else v.data_ptr())
         elif isinstance(v, (list, tuple)):
             arr = getattr(args, k)
             for i, x in enumerate(v):

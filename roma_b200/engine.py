@@ -34,7 +34,7 @@ import torch.nn.functional as F
 from . import arch, cabi, sampling
 from .cabi import call
 from .cache import BufferArena
-from .packing import PackedWeights, Split, pad8
+from .packing import PackedWeights, Split, at, pad8
 
 PRECISIONS = {"fp32": torch.float32, "fp32_simt": torch.float32, "fp16": torch.float16, "bf16": torch.bfloat16}
 F16S = cabi.RB_F16S
@@ -261,14 +261,12 @@ class Engine(BufferArena):
             return
         sdt = self.dtype
         S = self.buf(f"attn.scores.{tag}", (Bn, heads, N, npad), dtype=sdt)
-        es = qkv.element_size()
-        q_ptr, k_ptr, v_ptr = qkv.data_ptr(), qkv.data_ptr() + dim * es, qkv.data_ptr() + 2 * dim * es
         # the 1/sqrt(d) scale rides on the QK^T epilogue so that 16-bit scores cannot overflow
         with self.stage(f"  attn.{tag}"):
-            self.gemm(q_ptr, k_ptr, S, N, N, d, ld, ld, npad, batch0=Bn, batch1=heads, alpha=1.0 / math.sqrt(d),
+            self.gemm(qkv, at(qkv, dim), S, N, N, d, ld, ld, npad, batch0=Bn, batch1=heads, alpha=1.0 / math.sqrt(d),
                       sa0=N * ld, sa1=d, sb0=N * ld, sb1=d, sc0=heads * N * npad, sc1=N * npad)
             call("romab200_softmax_rows", "rb_softmax_args", s=S, rows=Bn * heads * N, cols=N, lds=npad, dtype=self.dt, scale=1.0)
-            self.gemm(S, v_ptr, out, N, d, N, npad, ld, dim, trans_b=1, batch0=Bn, batch1=heads,
+            self.gemm(S, at(qkv, 2 * dim), out, N, d, N, npad, ld, dim, trans_b=1, batch0=Bn, batch1=heads,
                       sa0=heads * N * npad, sa1=N * npad, sb0=N * ld, sb1=d, sc0=N * dim, sc1=d)
 
     def block(self, x, blk, Bn, N, dim, heads, mlp, eps, tag):
@@ -313,8 +311,7 @@ class Engine(BufferArena):
         feats = self.buf("vit.feat16", (E, npatch, dim))
         # drop the cls token: rows 1..N of every image
         for e in range(E):
-            self.copy2d(out.data_ptr() + (e * N + 1) * dim * out.element_size(), feats.data_ptr() + e * npatch * dim * feats.element_size(),
-                        npatch, dim, dim, dim, self.dt, self.dt)
+            self.copy2d(at(out, (e * N + 1) * dim), feats[e], npatch, dim, dim, dim, self.dt, self.dt)
         return feats, hp, wp
 
     # ------------------------------------------------------------------ proj (roma_models.py:156-169)
@@ -338,7 +335,7 @@ class Engine(BufferArena):
         g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
         self.corr16_table(g, E, D, b, n)
         Wk, stride_w = self.gp_solve_images(g, E, hp, wp)
-        return self.gp_decode(g, Wk.data_ptr() + n * pad8(n) * 4, stride_w, E, D, b, hp, wp, state)
+        return self.gp_decode(g, at(Wk, n * pad8(n)), stride_w, E, D, b, hp, wp, state)
 
     def gp_project(self, feat16, E, n):
         """p16 [E*n, 512] fp32: proj[16] of the DINOv2 patch tokens (the GP runs in fp32: x.float(), matcher.py:296)."""
@@ -356,21 +353,12 @@ class Engine(BufferArena):
         norms = self.buf("gp.norms", (E * n,), dtype=torch.float32)
         call("romab200_row_norms", "rb_rownorm_args", x=p16, out=norms, rows=E * n, cols=cf, ldx=cf, dtype=cabi.RB_F32)
         gp_split = self.split or (self.dtype != torch.float32 and self.gp_tensor_core)     # GP contractions as split-fp16 pairs (fp32-class)
-        tc_kernel = False                 # (the K' = 3K operand trick of round 1 is superseded by the split back-end)
-        xs = xa = xb = None
+        xs = None
         if gp_split:
             # all-pairs CosKernel on the tensor cores with fp32-class accuracy: the L2-normalised rows as an RB_F16S pair
             with self.stage("  gp.split"):
                 xs = self.split_pair(p16, E * n, cf, cf, name="gp.xs", row_norm=norms)
-        elif tc_kernel:
-            # all-pairs CosKernel on the f16 tensor pipe with fp32-class accuracy: L2-normalised rows split into fp16
-            # hi/lo parts, A' = [hi|lo|hi], B' = [hi|hi|lo]  ->  A'.B'^T = hi.hi + lo.hi + hi.lo  (K' = 3*512)
-            xa = self.buf("gp.split_a", (E * n, 3 * cf), dtype=torch.float16)
-            xb = self.buf("gp.split_b", (E * n, 3 * cf), dtype=torch.float16)
-            with self.stage("  gp.split"):
-                call("romab200_split_f16x3", "rb_split_args", x=p16, dst=xa, rows=E * n, cols=cf, ldx=cf, ldd=3 * cf, row_norm=norms, layout_b=0)
-                call("romab200_split_f16x3", "rb_split_args", x=p16, dst=xb, rows=E * n, cols=cf, ldx=cf, ldd=3 * cf, row_norm=norms, layout_b=1)
-        return dict(p16=p16, norms=norms, xs=xs, xa=xa, xb=xb, split=gp_split, tc=tc_kernel)
+        return dict(p16=p16, norms=norms, xs=xs, split=gp_split)
 
     def corr16_table(self, g, E, D, b, n):
         """Parity mode: the stride-16 refiner's local correlation (r = 7: 256 dot products of 512 channels per pixel) from ONE
@@ -383,7 +371,7 @@ class Engine(BufferArena):
                 ps = self.split_pair(g["p16"], E * n, cf, cf, name="gp.p16s")
                 tab = self.buf("ref.corr16", (D, n, ldw), dtype=torch.float32)
                 for i0, cnt, y0 in ([(0, b, b)] if D == b else [(0, b, b), (b, b, 0)]):
-                    self.gemm(ps.at(i0 * n * cf), ps.at(y0 * n * cf), tab.data_ptr() + i0 * n * ldw * 4, n, n, cf, cf, cf, ldw, dtype_c=f32,
+                    self.gemm(ps.at(i0 * n * cf), ps.at(y0 * n * cf), at(tab, i0 * n * ldw), n, n, cf, cf, cf, ldw, dtype_c=f32,
                               batch0=cnt, sa0=n * cf, sb0=n * cf, sc0=n * ldw, alpha=float(torch.rsqrt(torch.tensor(float(cf)))))
                 self._corr16 = (tab, ldw)
 
@@ -399,15 +387,12 @@ class Engine(BufferArena):
             if g["split"]:
                 self.gp_kernel_matrix_split(g["xs"], g["xs"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
                                             sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
-            elif g["tc"]:
-                self.gp_kernel_matrix_tc(g["xa"], g["xb"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * 3 * cf, sb=n * 3 * cf, sc=stride_w,
-                                         sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
             else:
                 self.gp_kernel_matrix(g["p16"], g["p16"], g["norms"], g["norms"], Wk, n, cf, ldw, batch=E, sa=n * cf, sb=n * cf, sc=stride_w,
                                       sna=n, snb=n, diag=arch.GP_SIGMA_NOISE)
         basis_t = self.gp_basis_t(hp, wp)
         for e in range(E):
-            self.copy2d(basis_t, Wk.data_ptr() + (e * stride_w + n * ldw) * 4, nrhs, n, n, ldw, f32, f32)
+            self.copy2d(basis_t, Wk[e, n:], nrhs, n, n, ldw, f32, f32)
         with self.stage("  gp.solve"):
             # algo 2: 128-wide blocks factored in shared memory + explicit block inverses, everything else K=128 GEMMs
             ws_bytes = max((E * ((n + 31) // 32) * 1024 + 1) * 4, E * ((n + 127) // 128) * 65536)
@@ -420,48 +405,37 @@ class Engine(BufferArena):
 
     def gp_decode(self, g, alpha_t, stride_a, E, D, b, hp, wp, state):
         """Pair stage of the coarse match: K_xy and mu = K_xy @ alpha, the decoder and cls_to_flow_refine; fills state [D, hp, wp, 3]
-        and returns the stride-16 refiner features.  `alpha_t` points at image 0's alpha^T [512, ldw] (fp32), the other images follow
-        `stride_a` elements apart."""
+        and returns the stride-16 refiner features.  `alpha_t` (fp32) starts at image 0's alpha^T [512, ldw] and runs on to the other
+        images, which follow `stride_a` elements apart."""
         n = hp * wp
         cf, nrhs, ldw, f32 = arch.PROJ[16][1], arch.GP_DIM, pad8(n), cabi.RB_F32
-        p16, norms, xs, xa, xb = g["p16"], g["norms"], g["xs"], g["xa"], g["xb"]
+        p16, norms, xs = g["p16"], g["norms"], g["xs"]
         # K_xy and mu = K_xy @ alpha for every decoder item: query image i, support image (i + b) % E
         dim = arch.DEC_DIM
         tokens = self.buf("dec.tokens_in", (D * n, dim))
-        es = tokens.element_size()
         halves = [(0, b, b)] if D == b else [(0, b, b), (b, b, 0)]     # (first item, count, first support image)
         if g["split"]:
             kxy = self.sbuf("gp.kxy", (D, n, ldw))
             alpha = self.sbuf("gp.alpha", (E, nrhs, ldw))
             with self.stage("  gp.kxy+mu"):
                 for e in range(E):          # alpha^T of every image as an RB_F16S pair
-                    call("romab200_split_f16s", "rb_split_pair_args", x=alpha_t + e * stride_a * 4,
-                         hi=alpha.at(e * nrhs * ldw).hi, lo=alpha.at(e * nrhs * ldw).lo, rows=nrhs, cols=n, ldx=ldw, ldd=ldw)
+                    call("romab200_split_f16s", "rb_split_pair_args", x=at(alpha_t, e * stride_a), hi=alpha.hi[e], lo=alpha.lo[e],
+                         rows=nrhs, cols=n, ldx=ldw, ldd=ldw)
                 for i0, cnt, y0 in halves:
-                    self.gp_kernel_matrix_split(xs.at(i0 * n * cf), xs.at(y0 * n * cf), norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
+                    self.gp_kernel_matrix_split(xs.at(i0 * n * cf), xs.at(y0 * n * cf), at(norms, i0 * n), at(norms, y0 * n),
                                                 kxy.at(i0 * n * ldw), n, cf, ldw, batch=cnt, sa=n * cf, sb=n * cf, sc=n * ldw, sna=n, snb=n, diag=0.0)
-                    self.gemm(kxy.at(i0 * n * ldw), alpha.at(y0 * nrhs * ldw), tokens.data_ptr() + i0 * n * dim * es, n, nrhs, n, ldw, ldw, dim,
+                    self.gemm(kxy.at(i0 * n * ldw), alpha.at(y0 * nrhs * ldw), at(tokens, i0 * n * dim), n, nrhs, n, ldw, ldw, dim,
                               batch0=cnt, sa0=n * ldw, sb0=nrhs * ldw, sc0=n * dim)
-            halves = []
         else:
             kxy = self.buf("gp.kxy", (D, n, ldw), dtype=torch.float32)
-        for i0, cnt, y0 in halves:
-          with self.stage("  gp.kxy+mu"):
-            if g["tc"]:
-                self.gp_kernel_matrix_tc(xa.data_ptr() + i0 * n * 3 * cf * 2, xb.data_ptr() + y0 * n * 3 * cf * 2,
-                                         norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
-                                         kxy.data_ptr() + i0 * n * ldw * 4, n, cf, ldw, batch=cnt, sa=n * 3 * cf, sb=n * 3 * cf,
-                                         sc=n * ldw, sna=n, snb=n, diag=0.0)
-            else:
-                self.gp_kernel_matrix(p16.data_ptr() + i0 * n * cf * 4, p16.data_ptr() + y0 * n * cf * 4,
-                                      norms.data_ptr() + i0 * n * 4, norms.data_ptr() + y0 * n * 4,
-                                      kxy.data_ptr() + i0 * n * ldw * 4, n, cf, ldw, batch=cnt, sa=n * cf, sb=n * cf, sc=n * ldw,
-                                      sna=n, snb=n, diag=0.0)
-            self.gemm(kxy.data_ptr() + i0 * n * ldw * 4, alpha_t + y0 * stride_a * 4,
-                      tokens.data_ptr() + i0 * n * dim * es, n, nrhs, n, ldw, ldw, dim, dtype_ab=f32,
-                      batch0=cnt, sa0=n * ldw, sb0=stride_a, sc0=n * dim)
+            for i0, cnt, y0 in halves:
+                with self.stage("  gp.kxy+mu"):
+                    self.gp_kernel_matrix(at(p16, i0 * n * cf), at(p16, y0 * n * cf), at(norms, i0 * n), at(norms, y0 * n),
+                                          at(kxy, i0 * n * ldw), n, cf, ldw, batch=cnt, sa=n * cf, sb=n * cf, sc=n * ldw, sna=n, snb=n, diag=0.0)
+                    self.gemm(at(kxy, i0 * n * ldw), at(alpha_t, y0 * stride_a), at(tokens, i0 * n * dim), n, nrhs, n, ldw, ldw, dim,
+                              dtype_ab=f32, batch0=cnt, sa0=n * ldw, sb0=stride_a, sc0=n * dim)
         # tokens = cat(gp_posterior, f1_s) (transformer/__init__.py:33)
-        self.copy2d(p16, tokens.data_ptr() + arch.GP_DIM * es, D * n, cf, cf, dim, f32, self.dt)
+        self.copy2d(p16, at(tokens, arch.GP_DIM), D * n, cf, cf, dim, f32, self.dt)
         if self.debug is not None:
             self.debug["gp.mu"] = tokens.view(D, n, dim)[:, :, :arch.GP_DIM].float().clone()
         x = self.buf("dec.x", (D * n, dim), dtype=torch.float32)
@@ -499,12 +473,6 @@ class Engine(BufferArena):
                   sa0=sa, sb0=sb, sc0=sc, epi=cabi.EPI_COSKERNEL, norm_a=na, norm_b=nb, sna0=sna, snb0=snb,
                   eps=arch.GP_COS_EPS, inv_t=1.0 / arch.GP_TEMPERATURE, diag_add=diag, cos_normalized=1)
 
-    def gp_kernel_matrix_tc(self, A, B, na, nb, C, n, cf, ldc, batch, sa, sb, sc, sna, snb, diag):
-        """Same contraction on the tensor cores from the split fp16 operands (pre-normalised rows: cos_normalized=1)."""
-        self.gemm(A, B, C, n, n, 3 * cf, 3 * cf, 3 * cf, ldc, dtype_ab=cabi.RB_F16, dtype_c=cabi.RB_F32, batch0=batch,
-                  sa0=sa, sb0=sb, sc0=sc, epi=cabi.EPI_COSKERNEL, norm_a=na, norm_b=nb, sna0=sna, snb0=snb,
-                  eps=arch.GP_COS_EPS, inv_t=1.0 / arch.GP_TEMPERATURE, diag_add=diag, cos_normalized=1)
-
     # ------------------------------------------------------------------ ConvRefiner (matcher.py:124-179)
     def refine(self, s, feat, ldf, E, D, b, h, w, state, scale_factor, h1, w1, tag):
         R = self.w.refiner[s]
@@ -535,7 +503,7 @@ class Engine(BufferArena):
                 t = self.buf(f"ref.t.{tag}", (D * h * w, cp), zero=True)
             for blk in R["blocks"]:
                 call("romab200_refiner_block_small", "rb_refiner_block_small_args", **{"in": d}, out=t, ld=cp, dw_weight=blk["dw_w"],
-                     ldw=cp, dw_bias=blk["dw_b"], pw_weight_host=blk["pw_w_host"].data_ptr(), pw_bias_host=blk["pw_b_host"].data_ptr(), batch=D, h=h, w=w, c=c, dtype=self.dt)
+                     ldw=cp, dw_bias=blk["dw_b"], pw_weight_host=blk["pw_w_host"], pw_bias_host=blk["pw_b_host"], batch=D, h=h, w=w, c=c, dtype=self.dt)
                 d, t = t, d
         elif c == 144 and self.dtype != torch.float32 and self.fused_c144:
             # stride-2 maps: depthwise stage on the CUDA cores feeding a wgmma pointwise GEMM inside one kernel
@@ -761,7 +729,7 @@ class Engine(BufferArena):
             row = bank["p16"][0].numel() * 4
             self.copy_rows(g["p16"], bank["p16"], E, row, row, row, E, cap, dst_index=slots)
             row = bank["alpha"][0].numel() * 4
-            self.copy_rows(Wk.data_ptr() + n * pad8(n) * 4, bank["alpha"], E, row, stride_w * 4, row, E, cap, dst_index=slots)
+            self.copy_rows(at(Wk, n * pad8(n)), bank["alpha"], E, row, stride_w * 4, row, E, cap, dst_index=slots)
             for tag, feats in cnn.items():
                 for s in (8, 4, 2, 1):
                     dst = bank[f"{tag}.{s}"]
@@ -795,7 +763,7 @@ class Engine(BufferArena):
         with self.stage("gp+decoder"):
             g = self.gp_rows(p16, E, n)
             self.corr16_table(g, E, D, b, n)
-            feats["lo"][16] = (self.gp_decode(g, alpha.data_ptr(), nrhs * pad8(n), E, D, b, hp, wp, state), cf)
+            feats["lo"][16] = (self.gp_decode(g, alpha, nrhs * pad8(n), E, D, b, hp, wp, state), cf)
         state, states = self.refine_chain(state, arch.SCALES, feats["lo"], sizes["lo"], E, D, b, hs, ws, scale_lo, "lo")
         coarse = states[16] if attenuate else None
         H, W = hs, ws

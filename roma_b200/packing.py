@@ -25,6 +25,12 @@ def pad8(n: int) -> int:
     return (n + 7) // 8 * 8
 
 
+def at(t: torch.Tensor, elems: int) -> torch.Tensor:
+    """The flat view of contiguous `t` from element `elems` on: an operand that starts inside a buffer, with the buffer's dtype,
+    device and remaining extent for the C-ABI checks (cabi.call)."""
+    return t.view(-1)[elems:]
+
+
 def fold_bn(w: torch.Tensor, b: torch.Tensor, sd: Dict[str, torch.Tensor], bn: str, eps: float = arch.BN_EPS):
     """Fold eval-mode BatchNorm `bn` into the conv (w [cout, ...], b [cout]).  A BatchNorm2d(affine=False) has no
     `weight` / `bias` entries: gamma = 1, beta = 0."""
@@ -38,7 +44,7 @@ def fold_bn(w: torch.Tensor, b: torch.Tensor, sd: Dict[str, torch.Tensor], bn: s
 
 class Split:
     """An RB_F16S matrix (include/romab200.h): fp16 hi plane + fp16 lo plane of identical geometry, value = hi + lo * 2^-11
-    with hi = fp16(x), lo = fp16((x - hi) * 2^11).  `hi` / `lo` are tensors, or raw device pointers (ints) for views."""
+    with hi = fp16(x), lo = fp16((x - hi) * 2^11).  `hi` / `lo` are fp16 tensors of the same shape."""
     __slots__ = ("hi", "lo")
 
     def __init__(self, hi, lo):
@@ -49,9 +55,8 @@ class Split:
         return self.hi.shape
 
     def at(self, elems: int) -> "Split":
-        """The pair of planes starting `elems` elements further (2 bytes per element and plane)."""
-        ptr = lambda t: t if isinstance(t, int) else t.data_ptr()
-        return Split(ptr(self.hi) + 2 * elems, ptr(self.lo) + 2 * elems)
+        """The pair of flat views starting `elems` elements further into both planes."""
+        return Split(at(self.hi, elems), at(self.lo, elems))
 
     def join(self) -> torch.Tensor:
         """fp32 reconstruction (tests / debug)."""

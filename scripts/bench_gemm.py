@@ -144,10 +144,7 @@ def launch_key(kw):
 
 
 def _same(a, b):
-    import torch
-    pa = a.data_ptr() if isinstance(a, torch.Tensor) else a
-    pb = b.data_ptr() if isinstance(b, torch.Tensor) else b
-    return pa == pb
+    return a.data_ptr() == b.data_ptr()
 
 
 def time_launch(kw, reps, trials=5):

@@ -8,6 +8,7 @@ pytestmark = pytest.mark.gpu
 
 from roma_b200 import cabi  # noqa: E402
 from roma_b200.cabi import call  # noqa: E402
+from roma_b200.packing import at  # noqa: E402
 
 DEV = "cuda"
 SENT = -7.0
@@ -145,7 +146,7 @@ def test_epilogue_residual_in_place_split(out):
 
 
 @pytest.mark.parametrize("N", [144, 569])
-def test_split_144_tiles_match_narrow_slices(N):
+def test_split_144_tiles_match_narrow_slice_views(N):
     """N = 144 and 569 run on 144-wide split tiles; the same problem as launches over column slices of at most 128 (128-, 64- and
     32-wide tiles) has the same k order per output, so the results are bit-equal."""
     M, K = 12000, N                                   # enough tiles that the width rule does not fall back to 128 for occupancy
@@ -162,8 +163,8 @@ def test_split_144_tiles_match_narrow_slices(N):
     sliced = torch.full((M, ldc), SENT, device=DEV)
     for n0 in range(0, N, 128):
         w = min(128, N - n0)
-        gemm(A=Ah, A_lo=Al, B=Bh.data_ptr() + n0 * lda * 2, B_lo=Bl.data_ptr() + n0 * lda * 2, dtype_ab=cabi.RB_F16S,
-             C=sliced.data_ptr() + n0 * 4, M=M, N=w, K=K, lda=lda, ldb=lda, ldc=ldc, dtype_c=cabi.RB_F32, bias=bias.data_ptr() + n0 * 4,
+        gemm(A=Ah, A_lo=Al, B=at(Bh, n0 * lda), B_lo=at(Bl, n0 * lda), dtype_ab=cabi.RB_F16S,
+             C=at(sliced, n0), M=M, N=w, K=K, lda=lda, ldb=lda, ldc=ldc, dtype_c=cabi.RB_F32, bias=at(bias, n0),
              act=cabi.ACT_RELU)
     torch.cuda.synchronize()
     ref = torch.relu(joined(Ah, Al) @ joined(Bh, Bl).t() + bias.double())

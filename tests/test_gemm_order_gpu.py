@@ -7,7 +7,7 @@ import torch
 
 pytestmark = pytest.mark.gpu
 
-from roma_b200 import cabi  # noqa: E402
+from roma_b200 import cabi, packing  # noqa: E402
 from roma_b200.cabi import call  # noqa: E402
 
 DEV = "cuda"
@@ -32,8 +32,8 @@ def gemm(**kw):
 
 
 def at(t, elems):
-    """Address of element `elems` of tensor t (None stays None)."""
-    return None if t is None else t.data_ptr() + elems * t.element_size()
+    """Flat view of tensor t from element `elems` on (None stays None)."""
+    return None if t is None else packing.at(t, elems)
 
 
 def full_and_sliced(A, B, outs, N, ldb, ldc, bias=None, col_scale=None, residual=False, **kw):
@@ -63,7 +63,7 @@ def assert_banded(M, k_extent, N, K):
 
 @pytest.mark.parametrize("M", [40000, 38017])          # 313 / 298 M-tiles: the last band is short for every band height here
 @pytest.mark.parametrize("C,max_ctas", [(569, 0), (1137, 0), (569, 40)])
-def test_refiner_pointwise_bands(M, C, max_ctas):
+def test_refiner_pointwise_bands_vs_slice_views(M, C, max_ctas):
     """The refiner's pointwise 1x1 convolution: split operands, fp32 output + bias, N = K = C (4 or 9 N-tiles); max_ctas caps the
     grid and with it the band height."""
     assert_banded(M, C, C, C)
@@ -79,7 +79,7 @@ def test_refiner_pointwise_bands(M, C, max_ctas):
     assert torch.equal(full, sliced)
 
 
-def test_conv3x3_taps_pad_keep_bands():
+def test_conv3x3_taps_pad_keep_bands_vs_slice_views():
     """A 9-tap 3x3 convolution on a zero-padded channels-last map (the VGG pattern): split output, bias + ReLU, PAD_KEEP rows.
     The tap shifts of +-(W + 3) rows reach into neighbouring M-tiles of the same band."""
     E, H, W, cin, cout = 2, 128, 128, 256, 512
@@ -100,7 +100,7 @@ def test_conv3x3_taps_pad_keep_bands():
     assert torch.equal(full[0], sliced[0]) and torch.equal(full[1], sliced[1])
 
 
-def test_residual_in_place_col_scale_bands():
+def test_residual_in_place_col_scale_bands_vs_slice_views():
     """X += (A B^T + bias) * gamma with R == C (the ViT fc2 pattern: M = 3202 tokens, K = 4096, N = 1024)."""
     M, N, K = 3202, 1024, 4096
     assert_banded(M, K, N, K)
@@ -113,7 +113,7 @@ def test_residual_in_place_col_scale_bands():
     assert torch.equal(full, sliced)
 
 
-def test_batched_bands():
+def test_batched_bands_vs_slice_views():
     """Two independent products in one launch (batch0 = 2): bands run inside each z, z outermost."""
     Z, M, N, K = 2, 20000, 569, 576
     assert_banded(M, K, N, K)

@@ -9,6 +9,7 @@ pytestmark = pytest.mark.gpu
 
 from roma_b200 import cabi  # noqa: E402
 from roma_b200.cabi import call  # noqa: E402
+from roma_b200.packing import at  # noqa: E402
 
 DEV = "cuda"
 CODE = cabi.DTYPE_CODE
@@ -67,14 +68,13 @@ def test_tc_epilogues_16bit_out(dt):
 
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("d,N", [(64, 203), (128, 160)])
-def test_tc_attention_shapes(dt, d, N):
+def test_tc_attention_shapes_qkv_views(dt, d, N):
     Bn, H = 2, 3
     dim = H * d
     qkv = rnd(Bn, N, 3 * dim, seed=1, dtype=dt, scale=0.5)
     npad = (N + 7) // 8 * 8
     S = torch.zeros(Bn, H, N, npad, dtype=dt, device=DEV)
-    es = 2
-    gemm(qkv.data_ptr(), qkv.data_ptr() + dim * es, S, N, N, d, 3 * dim, 3 * dim, npad, dt, dt, batch0=Bn, batch1=H,
+    gemm(qkv, at(qkv, dim), S, N, N, d, 3 * dim, 3 * dim, npad, dt, dt, batch0=Bn, batch1=H,
          alpha=1.0 / math.sqrt(d), sa0=N * 3 * dim, sa1=d, sb0=N * 3 * dim, sb1=d, sc0=H * N * npad, sc1=N * npad)
     q, k, v = qkv.float().reshape(Bn, N, 3, H, d).unbind(2)
     ref = torch.einsum("bnhd,bmhd->bhnm", q, k) / math.sqrt(d)
@@ -82,7 +82,7 @@ def test_tc_attention_shapes(dt, d, N):
     call("romab200_softmax_rows", "rb_softmax_args", s=S, rows=Bn * H * N, cols=N, lds=npad, dtype=CODE[dt], scale=1.0)
     P = S[..., :N].float()
     O = torch.zeros(Bn, N, dim, dtype=dt, device=DEV)
-    gemm(S, qkv.data_ptr() + 2 * dim * es, O, N, d, N, npad, 3 * dim, dim, dt, dt, trans_b=1, batch0=Bn, batch1=H,
+    gemm(S, at(qkv, 2 * dim), O, N, d, N, npad, 3 * dim, dim, dt, dt, trans_b=1, batch0=Bn, batch1=H,
          sa0=H * N * npad, sa1=N * npad, sb0=N * 3 * dim, sb1=d, sc0=N * dim, sc1=d)
     ref_o = torch.einsum("bhnm,bmhd->bnhd", P, v).reshape(Bn, N, dim)
     close(O, ref_o, 2e-2 if dt == torch.bfloat16 else 3e-3)
@@ -137,7 +137,7 @@ def test_tc_coskernel_split_f16x3_is_fp32_class():
 
 
 @pytest.mark.parametrize("dt", [torch.float16, torch.bfloat16])
-def test_refiner_block_small_fused_vs_unfused(dt):
+def test_refiner_block_small_fused_vs_unfused_host_tensors(dt):
     """Fused thin-map block (DW5x5+ReLU+PW, C=24) against conv2d on the same 16-bit-rounded tensors."""
     B, C, H, W = 2, 24, 37, 50
     x = rnd(B, C, H, W, seed=1, dtype=dt)
@@ -150,7 +150,7 @@ def test_refiner_block_small_fused_vs_unfused(dt):
     dwt = dw.reshape(C, 25).t().contiguous()
     pw_host, pb_host = pw.float().cpu().contiguous(), pb.cpu().contiguous()       # host arrays: they travel as kernel parameters
     call("romab200_refiner_block_small", "rb_refiner_block_small_args", **{"in": xi}, out=out, ld=C, dw_weight=dwt, ldw=C, dw_bias=db,
-         pw_weight_host=pw_host.data_ptr(), pw_bias_host=pb_host.data_ptr(), batch=B, h=H, w=W, c=C, dtype=CODE[dt])
+         pw_weight_host=pw_host, pw_bias_host=pb_host, batch=B, h=H, w=W, c=C, dtype=CODE[dt])
     close(out, ref, 6e-2 if dt == torch.bfloat16 else 8e-3)
 
 

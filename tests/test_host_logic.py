@@ -8,7 +8,7 @@ import torch
 import torch.nn.functional as F
 
 from roma_b200 import arch, cabi, synthetic
-from roma_b200.packing import PackedWeights, fold_bn, pad8
+from roma_b200.packing import PackedWeights, Split, at, fold_bn, pad8
 
 
 def test_library_exports_every_declared_symbol():
@@ -46,7 +46,8 @@ def test_packing_layouts(weights):
 
 
 class _Recorder:
-    """Stands in for cabi.call: validates field names and that pointer ranges lie inside live tensors."""
+    """Stands in for cabi.call: validates field names, that every pointer field is a tensor (offsets are views) or None, and that
+    pointer ranges lie inside live tensors."""
 
     def __init__(self):
         self.calls = []
@@ -66,6 +67,9 @@ class _Recorder:
     def __call__(self, fn, struct, **kw):
         valid = {f for f, _ in cabi.STRUCT_FIELDS[struct]}
         assert set(kw) <= valid, (fn, set(kw) - valid)
+        ptrs = {f for f, t in cabi.STRUCT_FIELDS[struct] if t is ctypes.c_void_p}
+        raw = {k: type(v).__name__ for k, v in kw.items() if k in ptrs and v is not None and not isinstance(v, torch.Tensor)}
+        assert not raw, (fn, "pointer fields take tensors or None", raw)
         self.calls.append(fn)
         es = {0: 4, 1: 2, 2: 2, 3: 2}
         if fn == "romab200_gemm":
@@ -185,14 +189,6 @@ def test_cabi_call_validates_tensors():
     with pytest.raises(TypeError):
         cabi.call("romab200_gemm", "rb_gemm_args", not_a_field=1)
     # dtype / contiguity / size rules, exercised on the validator itself with the device check satisfied by a stand-in
-    class FakeCuda(torch.Tensor):
-        is_cuda = True
-
-        @property
-        def device(self):
-            return type("D", (), {"index": None})()
-    def fake(t):
-        return t.as_subclass(FakeCuda)
     half, f32 = fake(torch.zeros(8, 8, dtype=torch.float16)), fake(torch.zeros(8, 8))
     kw = dict(A=half, B=half, C=f32, M=8, N=8, K=8, lda=8, ldb=8, ldc=8, dtype_ab=cabi.RB_F32, dtype_c=cabi.RB_F32)
     with pytest.raises(RuntimeError, match="dtype"):
@@ -205,6 +201,76 @@ def test_cabi_call_validates_tensors():
         cabi._validate("romab200_gemm", "rb_gemm_args", kw)
     kw.update(A=f32)
     cabi._validate("romab200_gemm", "rb_gemm_args", kw)
+
+
+class FakeCuda(torch.Tensor):
+    """A host tensor that the shim takes for one on the current CUDA device."""
+    is_cuda = True
+
+    @property
+    def device(self):
+        return type("D", (), {"type": "cuda", "index": torch.cuda.current_device() if torch.cuda.is_available() else None})()
+
+
+def fake(t):
+    return t.as_subclass(FakeCuda)
+
+
+def test_cabi_call_refuses_raw_addresses():
+    """A pointer field takes a tensor or None: an int (a hand-built address) is refused before the library is called."""
+    a = fake(torch.zeros(8, 8))
+    for field in ("A", "bias"):
+        kw = dict(A=a, B=a, C=a, M=8, N=8, K=8, lda=8, ldb=8, ldc=8, dtype_ab=cabi.RB_F32, dtype_c=cabi.RB_F32)
+        kw[field] = a.data_ptr() + 64
+        with pytest.raises(TypeError, match=f"romab200_gemm: pointer field `{field}`"):
+            cabi.call("romab200_gemm", "rb_gemm_args", **kw)
+
+
+def test_cabi_host_fields():
+    """The refiner block's pointwise weights are read on the host: contiguous fp32 CPU tensors; its maps stay device tensors."""
+    m = fake(torch.zeros(2, 16, 16, 24))
+    kw = dict(out=fake(torch.zeros(2, 16, 16, 24)), ld=24, dw_weight=fake(torch.zeros(25, 24)), ldw=24, dw_bias=fake(torch.zeros(24)),
+              pw_weight_host=torch.zeros(24, 24), pw_bias_host=torch.zeros(24), batch=2, h=16, w=16, c=24, dtype=cabi.RB_F32)
+    kw["in"] = m
+    cabi._validate("romab200_refiner_block_small", "rb_refiner_block_small_args", kw)
+    for bad, why in ((fake(torch.zeros(24, 24)), "read on the host"), (torch.zeros(24, 24, dtype=torch.float16), "dtype"),
+                     (torch.zeros(24, 48)[:, :24], "contiguous")):
+        with pytest.raises(RuntimeError, match=why):
+            cabi._validate("romab200_refiner_block_small", "rb_refiner_block_small_args", dict(kw, pw_weight_host=bad))
+    with pytest.raises(RuntimeError, match="expected the current CUDA device"):
+        cabi._validate("romab200_refiner_block_small", "rb_refiner_block_small_args", dict(kw, dw_bias=torch.zeros(24)))
+
+
+def test_split_at_returns_offset_views():
+    hi, lo = torch.arange(24, dtype=torch.float16).view(4, 6), torch.zeros(4, 6, dtype=torch.float16)
+    s = Split(hi, lo).at(7)
+    for view, base in ((s.hi, hi), (s.lo, lo)):
+        assert view.untyped_storage().data_ptr() == base.untyped_storage().data_ptr()
+        assert view.data_ptr() == base.data_ptr() + 7 * 2 and view.numel() == 24 - 7 and view.dtype == torch.float16
+    assert s.hi[0] == 7 and torch.equal(s.at(5).hi, at(hi, 12))
+    with pytest.raises(RuntimeError):
+        at(hi[:, :3], 1)                # only a contiguous buffer has a flat view
+
+
+def test_cabi_offset_views_checked_against_geometry():
+    """An operand that starts inside a buffer must still hold what the described geometry reads (GEMM, copy2d, gather_rows)."""
+    buf = torch.zeros(8, 8)
+    gemm = dict(B=fake(buf), C=fake(buf), M=8, N=8, K=8, lda=8, ldb=8, ldc=8, dtype_ab=cabi.RB_F32, dtype_c=cabi.RB_F32)
+    cabi._validate("romab200_gemm", "rb_gemm_args", dict(gemm, A=fake(at(buf, 0)), M=7))
+    with pytest.raises(RuntimeError, match="`A` holds 56 elements, the described geometry needs 64"):
+        cabi._validate("romab200_gemm", "rb_gemm_args", dict(gemm, A=fake(at(buf, 8))))
+    copy = dict(src=fake(at(buf, 40)), dst=fake(buf), rows=3, cols=8, lds=8, ldd=8, dtype_src=cabi.RB_F32, dtype_dst=cabi.RB_F32)
+    cabi._validate("romab200_copy2d", "rb_copy2d_args", copy)
+    with pytest.raises(RuntimeError, match="`src` holds 23 elements, the described geometry needs 24"):
+        cabi._validate("romab200_copy2d", "rb_copy2d_args", dict(copy, src=fake(at(buf, 41))))
+    with pytest.raises(RuntimeError, match="`dst` holds 15 elements, the described geometry needs 24"):
+        cabi._validate("romab200_copy2d", "rb_copy2d_args", dict(copy, dst=fake(at(buf, 49))))
+    rows = dict(src=fake(at(buf, 16)), dst=fake(buf), count=3, row_bytes=64, ld_src=64, ld_dst=64, src_rows=3, dst_rows=3)
+    cabi._validate("romab200_gather_rows", "rb_gather_rows_args", rows)         # 48 fp32 = 192 bytes = 2 * 64 + 64
+    with pytest.raises(RuntimeError, match="`src` holds 44 elements, the described geometry needs 48"):
+        cabi._validate("romab200_gather_rows", "rb_gather_rows_args", dict(rows, src=fake(at(buf, 20))))
+    with pytest.raises(RuntimeError, match="`dst` holds 48 elements, the described geometry needs 64"):
+        cabi._validate("romab200_gather_rows", "rb_gather_rows_args", dict(rows, dst=fake(at(buf, 16)), ld_dst=96))
 
 
 def test_romatch_import_shim():

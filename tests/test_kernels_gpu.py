@@ -12,6 +12,7 @@ pytestmark = pytest.mark.gpu
 
 from roma_b200 import cabi  # noqa: E402
 from roma_b200.cabi import call  # noqa: E402
+from roma_b200.packing import at  # noqa: E402
 
 DEV = "cuda"
 F32 = cabi.RB_F32
@@ -64,14 +65,13 @@ def test_gemm_layerscale_residual_inplace():
     close(X, ref, 2e-4)
 
 
-def test_gemm_trans_b_and_batched_heads():
+def test_gemm_trans_b_and_batched_heads_qkv_views():
     Bn, H, N, d = 2, 3, 70, 16
     dim = H * d
     qkv = rnd(Bn, N, 3 * dim, seed=1)
     npad = 72
     S = torch.zeros(Bn, H, N, npad, device=DEV)
-    es = 4
-    gemm(qkv.data_ptr(), qkv.data_ptr() + dim * es, S, N, N, d, 3 * dim, 3 * dim, npad, batch0=Bn, batch1=H,
+    gemm(qkv, at(qkv, dim), S, N, N, d, 3 * dim, 3 * dim, npad, batch0=Bn, batch1=H,
          sa0=N * 3 * dim, sa1=d, sb0=N * 3 * dim, sb1=d, sc0=H * N * npad, sc1=N * npad)
     q, k, v = qkv.reshape(Bn, N, 3, H, d).unbind(2)
     ref = torch.einsum("bnhd,bmhd->bhnm", q, k)
@@ -79,7 +79,7 @@ def test_gemm_trans_b_and_batched_heads():
     call("romab200_softmax_rows", "rb_softmax_args", s=S, rows=Bn * H * N, cols=N, lds=npad, dtype=F32, scale=0.25)
     close(S[..., :N], (ref * 0.25).softmax(-1), 1e-5)
     O = torch.zeros(Bn, N, dim, device=DEV)
-    gemm(S, qkv.data_ptr() + 2 * dim * es, O, N, d, N, npad, 3 * dim, dim, trans_b=1, batch0=Bn, batch1=H,
+    gemm(S, at(qkv, 2 * dim), O, N, d, N, npad, 3 * dim, dim, trans_b=1, batch0=Bn, batch1=H,
          sa0=H * N * npad, sa1=N * npad, sb0=N * 3 * dim, sb1=d, sc0=N * dim, sc1=d)
     ref_o = F.scaled_dot_product_attention(q.transpose(1, 2), k.transpose(1, 2), v.transpose(1, 2)).transpose(1, 2).reshape(Bn, N, dim)
     close(O, ref_o, 1e-4)

@@ -31,7 +31,7 @@ class _PairRecorder(_Recorder):
         if fn == "romab200_im2col_patch":
             self.encoded.append(kw["image"].clone())
         if fn == "romab200_gather_rows":
-            base = {k: kw[k].data_ptr() if isinstance(kw[k], torch.Tensor) else kw[k] for k in ("src", "dst")}
+            base = {k: kw[k].data_ptr() for k in ("src", "dst")}
             for i in range(kw["count"]):
                 s = int(kw["src_index"][i]) if kw.get("src_index") is not None else i
                 d = int(kw["dst_index"][i]) if kw.get("dst_index") is not None else i

@@ -257,7 +257,7 @@ def test_split_coskernel_matrix():
 
 
 @pytest.mark.parametrize("B,H,W", [(2, 37, 50), (1, 16, 16), (2, 5, 3)])
-def test_refiner_block_small_fp32(B, H, W):
+def test_refiner_block_small_fp32_host_tensors(B, H, W):
     """Fused thin-map block (DW5x5 + ReLU + PW, C = 24) on fp32 maps: fp32 FFMA throughout, against conv2d in float64."""
     C = 24
     x = rnd(B, C, H, W, seed=1)
@@ -270,7 +270,7 @@ def test_refiner_block_small_fp32(B, H, W):
     dwt = dw.reshape(C, 25).t().contiguous()
     pw_host, pb_host = pw.cpu().contiguous(), pb.cpu().contiguous()       # host arrays: they travel as kernel parameters
     call("romab200_refiner_block_small", "rb_refiner_block_small_args", **{"in": xi}, out=out, ld=C, dw_weight=dwt, ldw=C, dw_bias=db,
-         pw_weight_host=pw_host.data_ptr(), pw_bias_host=pb_host.data_ptr(), batch=B, h=H, w=W, c=C, dtype=F32)
+         pw_weight_host=pw_host, pw_bias_host=pb_host, batch=B, h=H, w=W, c=C, dtype=F32)
     assert rel_err(out, ref) < 2e-6
 
 
