@@ -328,7 +328,12 @@ typedef struct { const float* x; float* density; int32_t n; float std; int32_t h
                  float* workspace; int32_t splits;
                  /* half mode only: evaluate the block pairs (I, J >= I) of 256 x 256 points once and credit both the row and the column sums
                   * (exp(-d2) is symmetric); workspace of (splits + ceil(n / 256)) * n floats, its size in workspace_floats.  0: every pair twice */
-                 int32_t symmetric; int64_t workspace_floats; } rb_kde_args;
+                 int32_t symmetric; int64_t workspace_floats;
+                 /* batch > 1: `batch` independent problems of n points (the per-item KDE of a batched sample(), matcher.py:598-629,
+                  * tiny.py:234-266): item b reads x + b*4n, writes density + b*n and uses its own slice of the workspace (splits * n, or
+                  * (splits + ceil(n/256)) * n floats in the symmetric schedule; workspace_floats covers all items).  Every item runs the
+                  * schedule of a single call of size n, so its densities equal that call's bit for bit.  0 or 1: one problem */
+                 int32_t batch; } rb_kde_args;
 int romab200_kde_density(const rb_kde_args* args, void* stream);
 
 /* sample(): weighted sampling WITHOUT replacement on the device (the two torch.multinomial draws of matcher.py:613-617, 626-628).
@@ -344,8 +349,25 @@ typedef struct {
     int32_t* out_idx; float* out_weights; float* keys;
     void* scratch;   /* batch * 2056 * 4 bytes: histograms and selection state (cleared inside the call) */
     const uint64_t* seed_dev;   /* optional: the seed is read from this DEVICE word instead of `seed` (CUDA-graph replays with fresh seeds) */
+    /* Batches of independent sample() calls (matcher.py:598-629, tiny.py:234-266 run once per item):
+     *   seed_stride > 0 (needs seed_dev): item b reads its own seed seed_dev[b * seed_stride] and keys Philox with it alone, so it draws
+     *     exactly what a batch-1 call with that seed draws; 0: every item shares one seed and b is mixed into the Philox key;
+     *   repeats > 1: item b draws from values + (b / repeats) * stride, so the `repeats` draws of one pair read one map; 0 or 1: row b. */
+    int64_t seed_stride; int32_t repeats;
 } rb_sample_args;
 int romab200_weighted_sample(const rb_sample_args* args, void* stream);
+
+/* The row gathers of sample() after each draw (matches[sel], certainty[sel] and the certainty threshold, matcher.py:604-617, 626-629,
+ * tiny.py:240-266), for `items` draws at once: for item i and j < k, with p = i / repeats (0 or 1 repeats: p = i) and r = idx[i*k + j],
+ *   out_matches[i*k + j] = matches[p*n + r] (4 floats)   out_certainty[i*k + j] = threshold && c > thresh ? 1 : c,  c = certainty[p*n + r].
+ * matches [pairs, n, 4] and out_matches 16-byte aligned; idx [items, k] int32 (the drawn indices, sorted per item by the caller). */
+typedef struct {
+    const float* matches; const float* certainty; int64_t n;
+    const int32_t* idx; int32_t items, k, repeats;
+    int32_t threshold; float thresh;
+    float* out_matches; float* out_certainty;
+} rb_sample_gather_args;
+int romab200_sample_gather(const rb_sample_gather_args* args, void* stream);
 
 /* Image preprocessing in front of match() on the device: RGB uint8 image -> normalised fp32 [3, out_h, out_w]
  * (get_tuple_transform_ops(resize=(h, w), normalize=True), utils.py:164-173 = PIL.Image.resize((w, h), BICUBIC), /255, ImageNet mean/std;

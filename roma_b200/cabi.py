@@ -134,6 +134,7 @@ _FIELD_DTYPES = {
     "rb_preprocess_args": {"in": torch.uint8, "tmp": torch.uint8, "out_u8": torch.uint8, "out": _F32, "bounds_x": torch.int32, "kk_x": torch.int32,
                            "bounds_y": torch.int32, "kk_y": torch.int32},
     "rb_sample_args": {"values": _F32, "out_idx": torch.int32, "out_weights": _F32, "keys": _F32, "scratch": torch.int32, "seed_dev": torch.int64},
+    "rb_sample_gather_args": {"matches": _F32, "certainty": _F32, "idx": torch.int32, "out_matches": _F32, "out_certainty": _F32},
     "rb_tiny_conv_args": {"in": _F32, "out": _F32, "weight": _F32, "bias": _F32, "col_scale": _F32, "R": _F32},
     "rb_tiny_gray_args": {"in": _F32, "out": _F32},
     "rb_tiny_avgpool_args": {"in": _F32, "out": _F32},
@@ -198,8 +199,20 @@ def _gather_rows_min_elems(kw):
     return out
 
 
+def _sample_min_elems(kw):
+    b, n, k, rep = max(kw.get("batch", 1), 1), kw["n"], kw["k"], max(kw.get("repeats", 0), 1)
+    return {"values": ((b - 1) // rep) * (kw.get("stride") or n) + n, "keys": b * n, "scratch": b * 2056, "out_idx": b * k, "out_weights": b * k,
+            "seed_dev": (b - 1) * kw.get("seed_stride", 0) + 1}
+
+
+def _sample_gather_min_elems(kw):
+    items, k, rows = kw["items"], kw["k"], ((kw["items"] - 1) // max(kw.get("repeats", 0), 1) + 1) * kw["n"]
+    return {"matches": 4 * rows, "certainty": rows, "idx": items * k, "out_matches": 4 * items * k, "out_certainty": items * k}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
-_MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems}
+_MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
+              "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -14,8 +14,12 @@ __device__ __forceinline__ float rh(float v) { return __half2float(__float2half_
 // Grid: (row blocks of 256, j-splits).  One thread owns TWO rows (i and i + 128: every staged point is loaded once for both) and
 // the j range of its split; with splits > 1 the fp32 partial sums go to workspace[split][n] and kde_finish_kernel adds them in a
 // fixed order (deterministic), so that the 40000-point problem of sample() is 1256 CTAs instead of 313 (2.1 per SM: 30 % idle).
-__global__ void __launch_bounds__(128) kde_kernel(const float* __restrict__ x, float* __restrict__ out, int n, float two_var, int half, int j_per_split, int final_half) {
+// Batched calls put the items on gridDim.z: item z reads x + z * 4n and writes out + z * out_item; each item runs the single-item schedule.
+__global__ void __launch_bounds__(128) kde_kernel(const float* __restrict__ x, float* __restrict__ out, int n, float two_var, int half, int j_per_split, int final_half,
+                                                  int64_t out_item) {
     rb::pdl_wait();
+    x += (int64_t)blockIdx.z * 4 * n;
+    out += (int64_t)blockIdx.z * out_item;
     __shared__ float4 pts[512];
     __shared__ float nrm[512];
     const int i0 = blockIdx.x * 256 + threadIdx.x, i1 = i0 + 128;
@@ -92,6 +96,8 @@ __global__ void __launch_bounds__(128) kde_kernel(const float* __restrict__ x, f
 
 __global__ void __launch_bounds__(256) kde_finish_kernel(const float* __restrict__ partial, float* __restrict__ density, int n, int splits, int half) {
     rb::pdl_wait();
+    partial += (int64_t)blockIdx.z * splits * n;
+    density += (int64_t)blockIdx.z * n;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     float acc = 0.f;
@@ -123,8 +129,11 @@ __device__ __forceinline__ float kde_transpose_reduce(float (&v)[32], int lane) 
 // row partials (per split) and column partials (per I < block(i)) in a fixed order.  Grid (row blocks, splits): split s owns the J blocks
 // [s * bps, (s + 1) * bps); it writes zeros when none of them is >= I.  6.75 instead of 12 instructions per credited pair.
 __global__ void __launch_bounds__(128) kde_sym_kernel(const float* __restrict__ x, float* __restrict__ ws_row, float* __restrict__ ws_col, int n, float two_var,
-                                                      int blocks_per_split, int nblocks) {
+                                                      int blocks_per_split, int nblocks, int64_t ws_item) {
     rb::pdl_wait();
+    x += (int64_t)blockIdx.z * 4 * n;
+    ws_row += (int64_t)blockIdx.z * ws_item;
+    ws_col += (int64_t)blockIdx.z * ws_item;
     __shared__ float4 pts[256];
     __shared__ float nrm[256];
     __shared__ float colsum[4][256];
@@ -200,8 +209,12 @@ __global__ void __launch_bounds__(128) kde_sym_kernel(const float* __restrict__ 
     if (i1 < n) dst[i1] = acc_b;
 }
 
-__global__ void __launch_bounds__(256) kde_sym_finish_kernel(const float* __restrict__ ws_row, const float* __restrict__ ws_col, float* __restrict__ density, int n, int splits) {
+__global__ void __launch_bounds__(256) kde_sym_finish_kernel(const float* __restrict__ ws_row, const float* __restrict__ ws_col, float* __restrict__ density, int n, int splits,
+                                                             int64_t ws_item) {
     rb::pdl_wait();
+    ws_row += (int64_t)blockIdx.z * ws_item;
+    ws_col += (int64_t)blockIdx.z * ws_item;
+    density += (int64_t)blockIdx.z * n;
     const int i = blockIdx.x * 256 + threadIdx.x;
     if (i >= n) return;
     float acc = 0.f;
@@ -217,6 +230,8 @@ extern "C" int romab200_kde_density(const rb_kde_args* a, void* stream) {
     using namespace rb;
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->n > 0 && ((uintptr_t)a->x) % 16 == 0, "kde_density: n=%d or unaligned input", a->n);
+    RB_REQUIRE(a->batch >= 0 && a->batch <= 65535, "kde_density: batch %d outside [0, 65535]", a->batch);
+    const int batch = a->batch > 0 ? a->batch : 1;
     float two_var = (float)(2.0 * (double)a->std * (double)a->std);
     if (a->symmetric && a->half && a->workspace) {
         // upper-triangle schedule: workspace = (splits + ceil(n / 256)) * n floats
@@ -225,13 +240,15 @@ extern "C" int romab200_kde_density(const rb_kde_args* a, void* stream) {
         if (splits > nblocks) splits = nblocks;
         const int bps = (nblocks + splits - 1) / splits;
         splits = (nblocks + bps - 1) / bps;
-        RB_REQUIRE(a->workspace_floats >= (int64_t)(splits + nblocks) * a->n, "kde_density: the symmetric schedule needs (splits + ceil(n/256)) * n = %lld workspace floats, got %lld",
-                   (long long)(splits + nblocks) * a->n, (long long)a->workspace_floats);
+        const int64_t ws_item = (int64_t)(splits + nblocks) * a->n;
+        RB_REQUIRE(a->workspace_floats >= batch * ws_item, "kde_density: the symmetric schedule needs batch * (splits + ceil(n/256)) * n = %lld workspace floats, got %lld",
+                   (long long)(batch * ws_item), (long long)a->workspace_floats);
         float* ws_row = a->workspace;
         float* ws_col = a->workspace + (int64_t)splits * a->n;
-        rb::launch_pdl(kde_sym_kernel, dim3(nblocks, splits), dim3(128), 0, st, a->x, ws_row, ws_col, a->n, two_var, bps, nblocks);
+        rb::launch_pdl(kde_sym_kernel, dim3(nblocks, splits, batch), dim3(128), 0, st, a->x, ws_row, ws_col, a->n, two_var, bps, nblocks, ws_item);
         if (int rc = check_launch("kde_density(sym)")) return rc;
-        rb::launch_pdl(kde_sym_finish_kernel, dim3((a->n + 255) / 256), dim3(256), 0, st, (const float*)ws_row, (const float*)ws_col, a->density, a->n, splits);
+        rb::launch_pdl(kde_sym_finish_kernel, dim3((a->n + 255) / 256, 1, batch), dim3(256), 0, st, (const float*)ws_row, (const float*)ws_col, a->density, a->n,
+                       splits, ws_item);
         return check_launch("kde_finish(sym)");
     }
     const int chunks = (a->n + 511) / 512;
@@ -239,13 +256,15 @@ extern "C" int romab200_kde_density(const rb_kde_args* a, void* stream) {
     if (splits > chunks) splits = chunks;
     const int per = (chunks + splits - 1) / splits * 512;
     splits = (a->n + per - 1) / per;                                 // no empty split
-    const dim3 grid((a->n + 255) / 256, splits);
+    const dim3 grid((a->n + 255) / 256, splits, batch);
     if (splits == 1) {
-        rb::launch_pdl(kde_kernel, grid, dim3(128), 0, st, a->x, a->density, a->n, two_var, a->half, per, a->half);
+        rb::launch_pdl(kde_kernel, grid, dim3(128), 0, st, a->x, a->density, a->n, two_var, a->half, per, a->half, (int64_t)a->n);
         return check_launch("kde_density");
     }
-    rb::launch_pdl(kde_kernel, grid, dim3(128), 0, st, a->x, a->workspace, a->n, two_var, a->half, per, 0);
+    RB_REQUIRE(batch == 1 || a->workspace_floats >= (int64_t)batch * splits * a->n, "kde_density: %d items of %d splits need %lld workspace floats, got %lld", batch,
+               splits, (long long)batch * splits * a->n, (long long)a->workspace_floats);
+    rb::launch_pdl(kde_kernel, grid, dim3(128), 0, st, a->x, a->workspace, a->n, two_var, a->half, per, 0, (int64_t)splits * a->n);
     if (int rc = check_launch("kde_density")) return rc;
-    rb::launch_pdl(kde_finish_kernel, dim3((a->n + 255) / 256), dim3(256), 0, st, (const float*)a->workspace, a->density, a->n, splits, a->half);
+    rb::launch_pdl(kde_finish_kernel, dim3((a->n + 255) / 256, 1, batch), dim3(256), 0, st, (const float*)a->workspace, a->density, a->n, splits, a->half);
     return check_launch("kde_finish");
 }

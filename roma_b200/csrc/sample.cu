@@ -46,17 +46,20 @@ __device__ __forceinline__ void flush_hist(uint32_t* smem_hist, uint32_t* gh, in
 }
 
 // pass 0: keys (grid-wide) + histogram of bits [31:21]
+// item b: seed from seed_dev[b * seed_stride] (own seed, key as a batch-1 call with it) or, with seed_stride = 0, the shared seed with
+// b mixed into the key; weights from row b / repeats of `values` (the `repeats` draws of one pair read one map)
 __global__ void __launch_bounds__(SMP_THREADS) sample_keys_kernel(const float* __restrict__ values, int64_t n, int64_t stride, uint64_t seed, const uint64_t* __restrict__ seed_dev,
-                                                                  int transform, float param, float* __restrict__ keys_ws, uint32_t* __restrict__ scratch) {
+                                                                  int64_t seed_stride, int repeats, int transform, float param, float* __restrict__ keys_ws,
+                                                                  uint32_t* __restrict__ scratch) {
     rb::pdl_wait();
-    if (seed_dev) seed = *seed_dev;
     __shared__ uint32_t hist[SMP_BINS];
     const int b = blockIdx.y;
+    if (seed_dev) seed = seed_dev[(int64_t)b * seed_stride];
     for (int i = threadIdx.x; i < SMP_BINS; i += SMP_THREADS) hist[i] = 0;
     __syncthreads();
-    const float* v = values + (int64_t)b * stride;
+    const float* v = values + (int64_t)(b / repeats) * stride;
     float* keys = keys_ws + (int64_t)b * n;
-    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32) ^ (uint32_t)b * 0x9E3779B9u;
+    const uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32) ^ (seed_stride ? 0u : (uint32_t)b * 0x9E3779B9u);
     for (int64_t i = (int64_t)blockIdx.x * SMP_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * SMP_THREADS) {
         const float w = sample_weight(v[i], transform, param);
         const uint32_t r = philox_u32((uint32_t)i, (uint32_t)(i >> 32), k0, k1);
@@ -136,14 +139,14 @@ __global__ void __launch_bounds__(SMP_THREADS) sample_hist_kernel(const float* _
 
 // compaction: every key below the k-th smallest, and the ties up to the selected index
 __global__ void __launch_bounds__(SMP_THREADS) sample_compact_kernel(const float* __restrict__ values, const float* __restrict__ keys_ws, int64_t n, int k, int64_t stride,
-                                                                     int transform, float param, uint32_t* __restrict__ scratch, int32_t* __restrict__ out_idx,
-                                                                     float* __restrict__ out_w) {
+                                                                     int repeats, int transform, float param, uint32_t* __restrict__ scratch,
+                                                                     int32_t* __restrict__ out_idx, float* __restrict__ out_w) {
     rb::pdl_wait();
     const int b = blockIdx.y;
     uint32_t* sc = scratch + (int64_t)b * SMP_SCRATCH;
     const uint32_t kth = sc[SMP_BINS + 5], last_tie = sc[SMP_BINS];
     const float* keys = keys_ws + (int64_t)b * n;
-    const float* v = values + (int64_t)b * stride;
+    const float* v = values + (int64_t)(b / repeats) * stride;
     for (int64_t i = (int64_t)blockIdx.x * SMP_THREADS + threadIdx.x; i < n; i += (int64_t)gridDim.x * SMP_THREADS) {
         const uint32_t x = __float_as_uint(keys[i]);
         const bool take = x < kth || (x == kth && (uint32_t)i <= last_tie);
@@ -167,6 +170,9 @@ extern "C" int romab200_weighted_sample(const rb_sample_args* a, void* stream) {
     RB_REQUIRE(a->n > 0 && a->k > 0 && a->k <= a->n && a->n < (1ll << 31) && a->batch > 0 && a->batch <= 65535, "weighted_sample: bad shape n=%lld k=%d batch=%d",
                (long long)a->n, a->k, a->batch);
     RB_REQUIRE(a->transform >= RB_SAMPLE_IDENTITY && a->transform <= RB_SAMPLE_BALANCE, "weighted_sample: unknown transform %d", a->transform);
+    RB_REQUIRE(a->seed_stride >= 0 && (a->seed_stride == 0 || a->seed_dev), "weighted_sample: seed_stride %lld needs seed_dev", (long long)a->seed_stride);
+    RB_REQUIRE(a->repeats >= 0, "weighted_sample: repeats %d < 0", a->repeats);
+    const int repeats = a->repeats > 0 ? a->repeats : 1;
     uint32_t* scratch = reinterpret_cast<uint32_t*>(a->scratch);
     RB_REQUIRE(cudaMemsetAsync(scratch, 0, (size_t)a->batch * SMP_SCRATCH * sizeof(uint32_t), st) == cudaSuccess, "weighted_sample: memset failed");
     const int64_t stride = a->stride > 0 ? a->stride : a->n;
@@ -174,7 +180,8 @@ extern "C" int romab200_weighted_sample(const rb_sample_args* a, void* stream) {
     if (gx > 592) gx = 592;
     if (gx < 1) gx = 1;
     const dim3 grid(gx, a->batch);
-    rb::launch_pdl(sample_keys_kernel, grid, dim3(SMP_THREADS), 0, st, a->values, a->n, stride, a->seed, a->seed_dev, a->transform, a->param, a->keys, scratch);
+    rb::launch_pdl(sample_keys_kernel, grid, dim3(SMP_THREADS), 0, st, a->values, a->n, stride, a->seed, a->seed_dev, a->seed_stride, repeats, a->transform,
+                   a->param, a->keys, scratch);
     if (check_launch("weighted_sample(keys)")) return 1;
     for (int pass = 0; pass < SMP_PASSES; ++pass) {
         rb::launch_pdl(sample_select_kernel, dim3(a->batch), dim3(SMP_THREADS), 0, st, scratch, pass, a->k);
@@ -184,7 +191,38 @@ extern "C" int romab200_weighted_sample(const rb_sample_args* a, void* stream) {
             if (check_launch("weighted_sample(hist)")) return 1;
         }
     }
-    rb::launch_pdl(sample_compact_kernel, grid, dim3(SMP_THREADS), 0, st, a->values, (const float*)a->keys, a->n, a->k, stride, a->transform, a->param, scratch, a->out_idx,
-                   a->out_weights);
+    rb::launch_pdl(sample_compact_kernel, grid, dim3(SMP_THREADS), 0, st, a->values, (const float*)a->keys, a->n, a->k, stride, repeats, a->transform, a->param, scratch,
+                   a->out_idx, a->out_weights);
     return check_launch("weighted_sample(compact)");
+}
+
+namespace rb {
+
+// out[item, j] = row idx[item, j] of pair item / repeats; the certainty thresholded as `c > thresh ? 1 : c` when `threshold`
+__global__ void __launch_bounds__(256) sample_gather_kernel(const float4* __restrict__ matches, const float* __restrict__ certainty, int64_t n,
+                                                            const int32_t* __restrict__ idx, int64_t total, int k, int repeats, int threshold, float thresh,
+                                                            float4* __restrict__ out_m, float* __restrict__ out_c) {
+    rb::pdl_wait();
+    for (int64_t t = (int64_t)blockIdx.x * 256 + threadIdx.x; t < total; t += (int64_t)gridDim.x * 256) {
+        const int64_t row = (int64_t)((int)(t / k) / repeats) * n + idx[t];
+        const float c = certainty[row];
+        out_m[t] = matches[row];
+        out_c[t] = threshold && c > thresh ? 1.0f : c;
+    }
+}
+
+}  // namespace rb
+
+extern "C" int romab200_sample_gather(const rb_sample_gather_args* a, void* stream) {
+    cudaStream_t st = (cudaStream_t)stream;
+    RB_REQUIRE(a->matches && a->certainty && a->idx && a->out_matches && a->out_certainty, "sample_gather: null argument");
+    RB_REQUIRE(a->n > 0 && a->k > 0 && a->items > 0 && a->repeats >= 0, "sample_gather: bad shape n=%lld k=%d items=%d repeats=%d", (long long)a->n, a->k,
+               a->items, a->repeats);
+    RB_REQUIRE(((uintptr_t)a->matches | (uintptr_t)a->out_matches) % 16 == 0, "sample_gather: matches and out_matches must be 16-byte aligned");
+    const int64_t total = (int64_t)a->items * a->k;
+    int64_t blocks = (total + 255) / 256;
+    if (blocks > 4096) blocks = 4096;
+    rb::launch_pdl(sample_gather_kernel, dim3((unsigned)blocks), dim3(256), 0, st, (const float4*)a->matches, a->certainty, a->n, a->idx, total, a->k,
+                   a->repeats > 0 ? a->repeats : 1, a->threshold, a->thresh, (float4*)a->out_matches, a->out_certainty);
+    return check_launch("sample_gather");
 }

@@ -22,6 +22,7 @@ from . import cabi
 from .cache import GraphCache
 from .engine import Engine
 from .preprocess import DeviceImage, DevicePreprocessor, open_inputs
+from . import sampling
 from .sampling import sample_device
 
 
@@ -339,6 +340,21 @@ class RegressionMatcher:
     def _sample_device(self, matches, certainty, num):
         return sample_device(self._sample_graphs, self.engine.kde, matches, certainty, num, self.sample_mode, self.sample_thresh,
                              self.use_cuda_graph)
+
+    def sample_batched(self, matches, certainty, num=10000, *, repeats=1, chunk_bytes=sampling.SAMPLE_CHUNK_BYTES):
+        """`repeats` samples of every pair of a batched warp in one call: matches [B, ..., 4] and certainty [B, ...] (fp32, as `match()`
+        returns them) -> (m [B, repeats, k, 4], c [B, repeats, k]), k being what one `sample(matches[b], certainty[b], num)` returns.
+        After the same `torch.manual_seed` the result equals, element for element, `sample(matches[b], certainty[b], num)` called for
+        b in range(B), r in range(repeats) in that order (the seeds of call b * repeats + r are row b * repeats + r of one CPU
+        `torch.randint(0, 2**62, (B * repeats, 2))`).  The device chain reads the caller's tensors in place, in chunks of whole pairs
+        whose workspace fits `chunk_bytes`, and launches the same kernels for any B and repeats.  With `device_sampler = False` or
+        CPU tensors it is that `sample()` loop."""
+        B = sampling.check_batched(matches, certainty, num, repeats)
+        if not (self.device_sampler and matches.is_cuda):
+            outs = [self.sample(matches[b], certainty[b], num) for b in range(B) for _ in range(repeats)]
+            return (torch.stack([m for m, _ in outs]).view(B, repeats, -1, 4), torch.stack([c for _, c in outs]).view(B, repeats, -1))
+        return sampling.sample_batched(self._sample_graphs, self.engine.kde, matches, certainty, num, repeats, self.sample_mode,
+                                       self.sample_thresh, self.use_cuda_graph, chunk_bytes)
 
     # ---- small geometry helpers (matcher.py:672-773) ---------------------------------------------------
     def _to_pixel_coordinates(self, coords, H, W):

@@ -33,6 +33,7 @@ from .cache import BufferArena, GraphCache
 from .preprocess import DeviceImage, open_inputs
 from .matcher import RegressionMatcher
 from .packing import fold_bn
+from . import sampling
 from .sampling import kde, sample_device
 
 XFEAT_PARTS = ("norm", "skip1", "block1", "block2", "block3", "block4", "block5", "block_fusion")
@@ -412,6 +413,16 @@ class TinyRoMa:
         if not matches.is_cuda:
             raise RuntimeError("roma_b200.sample needs CUDA tensors (no CPU fallback)")
         return sample_device(self._sample_graphs, kde, matches, certainty, num, self.sample_mode, self.sample_thresh, self.use_cuda_graph)
+
+    def sample_batched(self, matches, certainty, num=5000, *, repeats=1, chunk_bytes=sampling.SAMPLE_CHUNK_BYTES):
+        """`repeats` samples of every pair of a batched warp in one call (RegressionMatcher.sample_batched): (m [B, repeats, k, 4],
+        c [B, repeats, k]), equal after the same `torch.manual_seed` to `sample(matches[b], certainty[b], num)` called for b in range(B),
+        r in range(repeats) in that order."""
+        sampling.check_batched(matches, certainty, num, repeats)
+        if not matches.is_cuda:
+            raise RuntimeError("roma_b200.sample needs CUDA tensors (no CPU fallback)")
+        return sampling.sample_batched(self._sample_graphs, kde, matches, certainty, num, repeats, self.sample_mode, self.sample_thresh,
+                                       self.use_cuda_graph, chunk_bytes)
 
     # ---- geometry helpers (identical to RoMa's, tiny.py:102-113) ----------------------------------------
     _to_pixel_coordinates = RegressionMatcher._to_pixel_coordinates
