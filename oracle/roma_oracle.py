@@ -34,13 +34,14 @@ REFINER = {16: (128, 7), 8: (64, 3), 4: (32, 2), 2: (16, 0), 1: (6, 0)}   # scal
 SCALES = (16, 8, 4, 2, 1)
 
 
-def pixel_centre_grid(b: int, h: int, w: int, device="cpu") -> torch.Tensor:
-    """[b,2,h,w] normalised pixel-centre coordinates, channel 0 = x (matcher.py:365-377).  Always built on the CPU (the
-    values the fixtures were pinned with) and then moved: `device` only matters for the stock-PyTorch-CUDA timing leg."""
+def pixel_centre_grid(b: int, h: int, w: int, device="cpu", dtype=torch.float32) -> torch.Tensor:
+    """[b,2,h,w] normalised pixel-centre coordinates, channel 0 = x (matcher.py:365-377).  Always built in fp32 on the CPU (the
+    values the fixtures were pinned with) and then moved: `device` only matters for the stock-PyTorch-CUDA timing leg, `dtype`
+    for the fp64 oracle."""
     ys = torch.linspace(-1 + 1 / h, 1 - 1 / h, h)
     xs = torch.linspace(-1 + 1 / w, 1 - 1 / w, w)
     gy, gx = torch.meshgrid(ys, xs, indexing="ij")
-    return torch.stack((gx, gy))[None].expand(b, 2, h, w).to(device)
+    return torch.stack((gx, gy))[None].expand(b, 2, h, w).to(device, dtype)
 
 
 class RomaOracle:
@@ -48,12 +49,15 @@ class RomaOracle:
 
     def __init__(self, matcher_weights: Dict[str, torch.Tensor], dinov2_weights: Dict[str, torch.Tensor],
                  coarse_res=560, upsample_res=864, symmetric=True, upsample_preds=True,
-                 attenuate_cert=True, sample_thresh=0.05, sample_mode="threshold_balanced", device="cpu"):
+                 attenuate_cert=True, sample_thresh=0.05, sample_mode="threshold_balanced", device="cpu", dtype=torch.float32):
         # device != "cpu" is the stock-PyTorch-on-GPU timing leg of bench.py (`--impl torch_cuda`): the same torch.nn.functional
-        # graph on cuDNN / cuBLAS / SDPA kernels; every parity check uses the CPU default
+        # graph on cuDNN / cuBLAS / SDPA kernels; every parity check uses the CPU default.  dtype=torch.float64 runs the same
+        # graph in double precision (weights, activations and the fp32-built grids cast up): the reference stage checks of the
+        # parity mode compare against, whose own fp32 rounding would be of the size of the errors they bound
         self.device = torch.device(device)
-        self.w = {k: (v.float() if v.is_floating_point() else v).to(self.device) for k, v in matcher_weights.items()}
-        self.d = {k: v.float().to(self.device) for k, v in dinov2_weights.items()}
+        self.dtype = dtype
+        self.w = {k: (v.to(dtype) if v.is_floating_point() else v).to(self.device) for k, v in matcher_weights.items()}
+        self.d = {k: v.to(dtype).to(self.device) for k, v in dinov2_weights.items()}
         cr = (coarse_res, coarse_res) if isinstance(coarse_res, int) else tuple(coarse_res)
         ur = (upsample_res, upsample_res) if isinstance(upsample_res, int) else upsample_res
         self.h_resized, self.w_resized = cr
@@ -78,17 +82,23 @@ class RomaOracle:
     # ------------------------------------------------------------------ encoders
     def vgg(self, x):
         """VGG19-BN features[:40]; taps are the inputs of the four max-pools (encoders.py:17-27)."""
-        feats, scale = {}, 1
-        for idx in range(40):
-            if idx in VGG_POOL_IDX:
-                feats[scale] = x
-                scale *= 2
+        feats = {}
+        for s in (1, 2, 4, 8):
+            if s > 1:
                 x = F.max_pool2d(x, 2, 2)
-            elif idx in VGG_CONV_IDX:
+            x = feats[s] = self.vgg_stage(s, x)
+        return feats
+
+    def vgg_stage(self, s, x):
+        """The conv + BN + ReLU layers of VGG stage `s` (1, 2, 4, 8): the image (s = 1) or the max-pooled tap of the stage before
+        -> the tap at stride s."""
+        k = (1, 2, 4, 8).index(s)
+        for idx in range(VGG_POOL_IDX[k - 1] + 1 if k else 0, VGG_POOL_IDX[k]):
+            if idx in VGG_CONV_IDX:
                 p = f"encoder.cnn.layers.{idx}"
                 x = F.conv2d(x, self.w[f"{p}.weight"], self.w[f"{p}.bias"], padding=1)
                 x = F.relu(self._bn(x, f"encoder.cnn.layers.{idx + 1}"))
-        return feats
+        return x
 
     def dinov2_pos_embed(self, hp, wp):
         """Bicubic resize of the 37x37 positional grid with the `+0.1` scale-factor quirk
@@ -154,13 +164,13 @@ class RomaOracle:
         b, c, h1, w1 = x.shape
         _, _, h2, w2 = y.shape
         w = self.w
-        f = torch.cos(8 * math.pi * F.conv2d(pixel_centre_grid(b, h2, w2, x.device),
+        f = torch.cos(8 * math.pi * F.conv2d(pixel_centre_grid(b, h2, w2, x.device, self.dtype),
                                               w["decoder.gps.16.pos_conv.weight"], w["decoder.gps.16.pos_conv.bias"]))
         flat = lambda t: t.flatten(2).transpose(1, 2)
-        x, y, f = flat(x.float()), flat(y.float()), flat(f)
+        x, y, f = flat(x.to(self.dtype)), flat(y.to(self.dtype)), flat(f)
         k_yy = self.cos_kernel(y, y)
         k_xy = self.cos_kernel(x, y)
-        noise = 0.1 * torch.eye(h2 * w2)[None].to(x.device)
+        noise = 0.1 * torch.eye(h2 * w2, dtype=self.dtype)[None].to(x.device)
         chol = torch.linalg.cholesky(k_yy + noise)
         alpha = torch.cholesky_solve(f, chol, upper=False)
         mu = k_xy @ alpha
@@ -187,7 +197,7 @@ class RomaOracle:
         res = round(math.sqrt(c))
         lin = torch.linspace(-1 + 1 / res, 1 - 1 / res, res)
         gy, gx = torch.meshgrid(lin, lin, indexing="ij")
-        anchors = torch.stack((gx, gy), dim=-1).reshape(c, 2).to(cls.device)
+        anchors = torch.stack((gx, gy), dim=-1).reshape(c, 2).to(cls.device, cls.dtype)
         p = cls.softmax(dim=1)
         mode = p.max(dim=1).indices
         idx = torch.stack((mode - 1, mode, mode + 1, mode - res, mode + res), dim=1).clamp(0, c - 1)
@@ -205,14 +215,17 @@ class RomaOracle:
         wy = torch.linspace(-2 * r / h, 2 * r / h, 2 * r + 1)
         wx = torch.linspace(-2 * r / w, 2 * r / w, 2 * r + 1)
         oy, ox = torch.meshgrid(wy, wx, indexing="ij")
-        window = torch.stack((ox, oy), dim=-1).reshape(1, k, 2).to(f0.device)
+        window = torch.stack((ox, oy), dim=-1).reshape(1, k, 2).to(f0.device, f0.dtype)
         flow = flow.permute(0, 2, 3, 1)
-        corr = torch.empty(b, k, h, w, device=f0.device)
+        corr = torch.empty(b, k, h, w, device=f0.device, dtype=f0.dtype)
+        band = max(1, (1 << 27) // (c * w * k * f0.element_size()))      # rows per grid_sample: bounds the [c, rows, w, k] samples
         for i in range(b):
-            coords = (flow[i, :, :, None] + window[:, None, None]).reshape(1, h, w * k, 2)
-            samp = F.grid_sample(f1[i:i + 1], coords, padding_mode="zeros", align_corners=False,
-                                 mode="bilinear").reshape(c, h, w, k)
-            corr[i] = (f0[i, ..., None] / (c ** 0.5) * samp).sum(dim=0).permute(2, 0, 1)
+            for y0 in range(0, h, band):
+                y1 = min(h, y0 + band)
+                coords = (flow[i, y0:y1, :, None] + window[:, None, None]).reshape(1, y1 - y0, w * k, 2)
+                samp = F.grid_sample(f1[i:i + 1], coords, padding_mode="zeros", align_corners=False,
+                                     mode="bilinear").reshape(c, y1 - y0, w, k)
+                corr[i, :, y0:y1] = (f0[i, :, y0:y1, :, None] / (c ** 0.5) * samp).sum(dim=0).permute(2, 0, 1)
         return corr
 
     def refiner_input(self, s, x, y, flow, scale_factor):
@@ -221,7 +234,7 @@ class RomaOracle:
         emb_dim, r = REFINER[s]
         p = f"decoder.conv_refiner.{s}"
         x_hat = F.grid_sample(y, flow.permute(0, 2, 3, 1), align_corners=False, mode="bilinear")
-        disp = flow - pixel_centre_grid(b, hs, ws, flow.device)
+        disp = flow - pixel_centre_grid(b, hs, ws, flow.device, self.dtype)
         emb = F.conv2d(40 / 32 * scale_factor * disp, self.w[f"{p}.disp_emb.weight"], self.w[f"{p}.disp_emb.bias"])
         parts = [x, x_hat, emb]
         if r:
@@ -255,13 +268,13 @@ class RomaOracle:
         b = f1[1].shape[0]
         tag = "up" if upsample else "lo"
         if not upsample:
-            flow, certainty = pixel_centre_grid(b, *sizes[16], device=f1[1].device), 0.0
+            flow, certainty = pixel_centre_grid(b, *sizes[16], device=f1[1].device, dtype=self.dtype), 0.0
         else:
             flow = F.interpolate(flow, size=sizes[8], align_corners=False, mode="bilinear")
             certainty = F.interpolate(certainty, size=sizes[8], align_corners=False, mode="bilinear")
         corresps = {}
         for s in scales:
-            x, y = self.proj(s, f1[s].float()), self.proj(s, f2[s].float())
+            x, y = self.proj(s, f1[s].to(self.dtype)), self.proj(s, f2[s].to(self.dtype))
             self._rec(f"{tag}.proj{s}.x", x)
             if s == 16:
                 post = self.gp(x, y)
@@ -301,23 +314,28 @@ class RomaOracle:
     @torch.inference_mode()
     def match(self, im_a, im_b, im_a_high=None, im_b_high=None):
         """Tensor-input `match` (matcher.py:779-934): returns (warp [b,H,W(*2),4], certainty [b,H,W(*2)])."""
-        b, _, hs, ws = im_a.shape
         scale_factor = math.sqrt(self.h_resized * self.w_resized / 560 ** 2)
         corresps = self.forward(im_a, im_b, scale_factor=scale_factor)
-        if self.upsample_preds:
-            hs, ws = self.upsample_res
-        low = 0
-        if self.attenuate_cert:
-            low = F.interpolate(corresps[16]["certainty"], size=(hs, ws), align_corners=False, mode="bilinear")
-            low = 0.5 * low * (low < 0)
+        coarse_certainty = corresps[16]["certainty"] if self.attenuate_cert else None
         if self.upsample_preds:
             scale_factor = math.sqrt(self.upsample_res[0] * self.upsample_res[1] / 560 ** 2)
             corresps = self.forward(im_a_high, im_b_high, upsample=True, scale_factor=scale_factor,
                                     corresps=corresps[1])
-        flow = corresps[1]["flow"].permute(0, 2, 3, 1)
-        cert = (corresps[1]["certainty"] - low).sigmoid()
-        self._rec("final.flow", flow), self._rec("final.logit", corresps[1]["certainty"] - low)
-        grid = pixel_centre_grid(b, hs, ws, flow.device).permute(0, 2, 3, 1)
+        return self.epilogue(corresps[1]["flow"], corresps[1]["certainty"], coarse_certainty)
+
+    def epilogue(self, flow, certainty, coarse_certainty=None):
+        """The end of `match` (matcher.py:868-934): final flow [D,2,H,W] and certainty logit [D,1,H,W], attenuated by the coarse
+        pass's stride-16 certainty [D,1,h,w] unless it is None -> (warp [b,H,W(*2),4], certainty [b,H,W(*2)])."""
+        hs, ws = flow.shape[-2:]
+        b = flow.shape[0] // (2 if self.symmetric else 1)
+        low = 0
+        if coarse_certainty is not None:
+            low = F.interpolate(coarse_certainty, size=(hs, ws), align_corners=False, mode="bilinear")
+            low = 0.5 * low * (low < 0)
+        flow = flow.permute(0, 2, 3, 1)
+        cert = (certainty - low).sigmoid()
+        self._rec("final.flow", flow), self._rec("final.logit", certainty - low)
+        grid = pixel_centre_grid(b, hs, ws, flow.device, self.dtype).permute(0, 2, 3, 1)
         if (flow.abs() > 1).any():
             wrong = (flow.abs() > 1).sum(dim=-1) > 0
             cert[wrong[:, None]] = 0

@@ -214,6 +214,8 @@ class Engine(BufferArena):
                           rowmap=cabi.ROWMAP_PAD_KEEP, pad_h=h + 2, pad_w=w + 2)
                 cur = nxt
             taps[scale] = (cur, h, w)
+            if self.debug is not None:
+                self.debug[f"{tag}.vgg{scale}"] = (cur.join() if self.split else cur.float())[:, 1:h + 1, 1:w + 1].clone()
             if scale == 8:
                 break
             c = layers[li - 1]["cout"]
@@ -312,6 +314,8 @@ class Engine(BufferArena):
         # drop the cls token: rows 1..N of every image
         for e in range(E):
             self.copy2d(at(out, (e * N + 1) * dim), feats[e], npatch, dim, dim, dim, self.dt, self.dt)
+        if self.debug is not None:
+            self.debug["vit.feat16"] = feats.float().clone()
         return feats, hp, wp
 
     # ------------------------------------------------------------------ proj (roma_models.py:156-169)
@@ -344,6 +348,8 @@ class Engine(BufferArena):
         p16 = self.buf("gp.p16", (E * n, cf), dtype=torch.float32)
         with self.stage("  gp.proj16"):
             self.gemm(feat16, P["w"], p16, E * n, cf, cin, cin, P["w"].shape[1], cf, dtype_c=cabi.RB_F32, bias=P["b"])
+        if self.debug is not None:
+            self.debug["gp.p16"] = p16.view(E, n, cf).clone()
         return p16
 
     def gp_rows(self, p16, E, n):
@@ -437,7 +443,8 @@ class Engine(BufferArena):
         # tokens = cat(gp_posterior, f1_s) (transformer/__init__.py:33)
         self.copy2d(p16, at(tokens, arch.GP_DIM), D * n, cf, cf, dim, f32, self.dt)
         if self.debug is not None:
-            self.debug["gp.mu"] = tokens.view(D, n, dim)[:, :, :arch.GP_DIM].float().clone()
+            self.debug["tokens"] = tokens.view(D, n, dim).float().clone()
+            self.debug["gp.mu"] = self.debug["tokens"][:, :, :arch.GP_DIM].clone()
         x = self.buf("dec.x", (D * n, dim), dtype=torch.float32)
         self.copy2d(tokens, x, D * n, dim, dim, dim, self.dt, f32)
         with self.stage("  dec.blocks"):
@@ -485,6 +492,8 @@ class Engine(BufferArena):
         if r in self.lc_tile_radii and self.dt == cabi.RB_F32 and table is None:
             # workspace of the tile-cooperative pass (coherent flow: one CTA per 8x2 / 8x4 pixels stages the union of their windows)
             tiles = self.buf(f"ref.tiles.{tag}", (D * cabi.prologue_tiles(r, h, w),), dtype=torch.uint8, zero=True)
+        if self.debug is not None:
+            self.debug[f"{tag}.state_in"] = state.clone()
         with self.stage(f"  prologue{s}.{tag[:2]}"):
           call("romab200_refiner_prologue", "rb_refiner_prologue_args", feat=feat, ldf=ldf, n_img=E, y_shift=b,
              tile_done=tiles, tile_done_len=tiles.numel() if tiles is not None else 0, corr_table=table, ld_corr_table=ld_table,
@@ -538,6 +547,7 @@ class Engine(BufferArena):
              dtype=self.dt, delta_out=delta)
         if self.debug is not None:
             self.debug[f"{tag}.delta"] = delta.view(D, h, w, 3).clone()
+            self.debug[f"{tag}.state_out"] = state.clone()
 
     def resize_state(self, src, D, hi, wi, ho, wo, name):
         dst = self.buf(name, (D, ho, wo, 3), dtype=torch.float32)

@@ -40,15 +40,18 @@ class _PairRecorder(_Recorder):
                 self._inside(base["dst"] + d * kw["ld_dst"], kw["row_bytes"], "gather_rows.dst")
 
 
-def _engine(weights, monkeypatch, split):
+def _engine(weights, monkeypatch, precision):
+    """A host-only Engine of `precision` whose C-ABI calls go to a _PairRecorder."""
     import roma_b200.engine as engine_mod
     rec = _PairRecorder()
     eng = engine_mod.Engine.__new__(engine_mod.Engine)
     eng.device = torch.device("cpu")
-    eng.precision, eng.dtype, eng.dt = "fp32" if split else "fp32_simt", torch.float32, cabi.RB_F32
-    eng.split, eng._lane, eng.generation = split, "main", 0
-    eng.w = PackedWeights(weights[0], weights[1], eng.device, torch.float32, split=split)
-    eng._buf, eng._const, eng.debug, eng.profile, eng.gemm_profile, eng.use_flash_attn, eng.gp_algo = {}, {}, None, None, None, True, (3 if split else 2)
+    eng.precision = precision
+    eng.dtype = engine_mod.PRECISIONS[eng.precision]
+    eng.dt = cabi.DTYPE_CODE[eng.dtype]
+    eng.split, eng._lane, eng.generation = precision == "fp32", "main", 0
+    eng.w = PackedWeights(weights[0], weights[1], eng.device, eng.dtype, split=eng.split)
+    eng._buf, eng._const, eng.debug, eng.profile, eng.gemm_profile, eng.use_flash_attn, eng.gp_algo = {}, {}, None, None, None, True, (2 if eng.precision == "fp32_simt" else 3)
     eng.overlap_cnn, eng._side, eng.gp_tensor_core, eng.fused_c144, eng.fused_small_f32 = False, None, True, True, True
     eng.lc_table16, eng.lc_tile_radii, eng.side_ctas = True, (2,), 0
     eng._bank, eng.bank_version = None, 0
@@ -88,7 +91,7 @@ class _TrackingCache(GraphCache):
 
 @pytest.mark.parametrize("symmetric,upsample,split", [(True, True, True), (False, True, False), (True, False, False)])
 def test_match_pairs_dry_run(weights, monkeypatch, symmetric, upsample, split):
-    eng, rec = _engine(weights, monkeypatch, split)
+    eng, rec = _engine(weights, monkeypatch, "fp32" if split else "fp32_simt")
     coarse, up = 112, 168
     A, B, Ah, Bh = synthetic.make_pair(3, coarse, up, 2)
     images, images_hi = torch.cat((A, B)), torch.cat((Ah, Bh))         # 6 images; image 5 is in no pair
@@ -152,3 +155,36 @@ def test_pair_arguments():
             pair_tensor(bad, 3)
     plan = plan_pairs(torch.tensor([[3, 1], [1, 3], [5, 5]]), 8)
     assert plan["used"] == [1, 3, 5] and plan["index"].tolist() == [1, 0, 2, 0, 1, 2] and plan["chunks"] == [(0, 3, 0, 6)]
+
+
+@pytest.mark.parametrize("precision,symmetric", [("fp16", True), ("bf16", False), ("fp32", True)])
+def test_debug_captures_are_inert(weights, monkeypatch, precision, symmetric):
+    """`engine.debug = {}` only clones stage tensors: a dry run of both passes and the epilogue makes the same C-ABI calls, in the
+    same order and with the same scalar arguments, as with `debug = None` (the CNN overlap is off in both), and keeps every stage
+    tensor tests/test_fast_mode_stages_gpu.py reads, in its documented shape."""
+    b, coarse, up = 2, 112, 168
+    A, B, Ah, Bh = synthetic.make_pair(b, coarse, up, 2)
+    logs = {}
+    for debug in (None, {}):
+        eng, rec = _engine(weights, monkeypatch, precision)
+        eng.debug = debug
+        images, hi = torch.cat((A, B)), torch.cat((Ah, Bh))
+        rec.track(images), rec.track(hi)
+        state, states, sizes = eng.run_pass(images, b, symmetric, False, coarse / 560)
+        state, _, _ = eng.run_pass(hi, b, symmetric, True, up / 560, (state, coarse, coarse))
+        wout = 2 * up if symmetric else up
+        out = (torch.empty(b, up, wout, 4), torch.empty(b, up, wout))
+        rec.track(out[0]), rec.track(out[1])
+        eng.epilogue(state, states[16], *sizes[16], b, up, up, symmetric, out=out)
+        logs[debug is None] = [(fn, sc) for fn, _, sc, _ in rec.log]
+    assert logs[True] == logs[False] and len(logs[True]) > 300
+    dbg, E, D, n = eng.debug, 2 * b, (2 * b if symmetric else b), (coarse // 14) ** 2
+    assert dbg["vit.feat16"].shape == (E, n, arch.VIT_DIM) and dbg["gp.p16"].shape == (E, n, arch.PROJ[16][1])
+    assert dbg["tokens"].shape == (D, n, arch.DEC_DIM) and dbg["gp.mu"].shape == (D, n, arch.GP_DIM)
+    for tag, res in (("lo", coarse), ("up", up)):
+        for s in (1, 2, 4, 8):
+            assert dbg[f"{tag}.vgg{s}"].shape == (E, res // s, res // s, arch.PROJ[s][0]) and dbg[f"{tag}.vgg{s}"].dtype == torch.float32
+        for s in ((16, 8, 4, 2, 1) if tag == "lo" else (8, 4, 2, 1)):
+            h = res // s if s < 16 else coarse // 14
+            for k in ("state_in", "state_out", "delta"):
+                assert dbg[f"{tag}{s}.{k}"].shape == (D, h, h, 3), (tag, s, k)
