@@ -3,7 +3,9 @@
 One `Engine` owns the packed weights, the per-resolution constants and a cache of activation buffers,
 and enqueues the whole of `forward_symmetric` / `forward` (`romatch/models/matcher.py:631-670`) plus the
 `match()` epilogue on the current CUDA stream through the C ABI.  PyTorch is used for device memory
-(`torch.empty/zeros`) and streams only; every arithmetic step is one of our kernels.
+(`torch.empty/zeros`) and streams only; every arithmetic step is one of our kernels.  `match()`, `forward()` and `match_pairs()`
+share one pipeline in two halves: `image_stage` does what each image needs on its own (DINOv2, the GP solve, the CNN branch) and
+`pair_stage` what each pair needs from it (the GP posterior, the decoder, the refiners and the epilogue).
 
 Precision regimes (`precision=`):
   "fp32"        parity mode on the tensor cores: activations stay fp32 in HBM, every GEMM operand is carried as an
@@ -26,7 +28,7 @@ from __future__ import annotations
 import math
 import os
 from contextlib import contextmanager
-from typing import Optional, Tuple
+from typing import Optional
 
 import torch
 import torch.nn.functional as F
@@ -329,18 +331,8 @@ class Engine(BufferArena):
                   rowmap=cabi.ROWMAP_PAD_TO_COMPACT, pad_h=h + 2, pad_w=w + 2)
         return out
 
-    # ------------------------------------------------------------------ GP + transformer decoder (scale 16)
-    def coarse_match(self, feat16, E, D, b, hp, wp, state):
-        """GP posterior (matcher.py:291-323), embedding decoder (transformer/__init__.py:30-46) and
-        cls_to_flow_refine (utils.py:300-322): fills state [D, hp, wp, 3]; returns the projected features.
-        The image stage (`gp_project`, `gp_rows`, `gp_solve_images`) reads one image at a time, the pair stage (`corr16_table`,
-        `gp_decode`) the pair; the stride-16 table is issued between the row splits and K_yy, where it always was."""
-        n = hp * wp
-        g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
-        self.corr16_table(g, E, D, b, n)
-        Wk, stride_w = self.gp_solve_images(g, E, hp, wp)
-        return self.gp_decode(g, at(Wk, n * pad8(n)), stride_w, E, D, b, hp, wp, state)
-
+    # ------------------------------------------------------------------ GP (matcher.py:291-323) + transformer decoder (scale 16)
+    # per image: gp_project, gp_rows, gp_solve_images; per pair: corr16_table, gp_decode
     def gp_project(self, feat16, E, n):
         """p16 [E*n, 512] fp32: proj[16] of the DINOv2 patch tokens (the GP runs in fp32: x.float(), matcher.py:296)."""
         cin, cf = arch.PROJ[16]
@@ -410,9 +402,9 @@ class Engine(BufferArena):
         return Wk, stride_w
 
     def gp_decode(self, g, alpha_t, stride_a, E, D, b, hp, wp, state):
-        """Pair stage of the coarse match: K_xy and mu = K_xy @ alpha, the decoder and cls_to_flow_refine; fills state [D, hp, wp, 3]
-        and returns the stride-16 refiner features.  `alpha_t` (fp32) starts at image 0's alpha^T [512, ldw] and runs on to the other
-        images, which follow `stride_a` elements apart."""
+        """Pair stage of the coarse match: K_xy and mu = K_xy @ alpha, the embedding decoder (transformer/__init__.py:30-46) and
+        cls_to_flow_refine (utils.py:300-322); fills state [D, hp, wp, 3] and returns the stride-16 refiner features.  `alpha_t`
+        (fp32) starts at image 0's alpha^T [512, ldw] and runs on to the other images, which follow `stride_a` elements apart."""
         n = hp * wp
         cf, nrhs, ldw, f32 = arch.PROJ[16][1], arch.GP_DIM, pad8(n), cabi.RB_F32
         p16, norms, xs = g["p16"], g["norms"], g["xs"]
@@ -554,7 +546,7 @@ class Engine(BufferArena):
         call("romab200_bilinear_resize", "rb_resize_args", **{"in": src}, out=dst, batch=D, hi=hi, wi=wi, ho=ho, wo=wo, c=3)
         return dst
 
-    # ------------------------------------------------------------------ one pass of the matcher
+    # ------------------------------------------------------------------ the pipeline: an image stage, then a pair stage
     def encode_cnn(self, images: torch.Tensor, tag: str):
         """VGG19 pyramid + proj[s] of one pass: {s: (projected channels-last features, pitch)}, {s: (h, w)}."""
         E = images.shape[0]
@@ -568,39 +560,66 @@ class Engine(BufferArena):
                 feats[s] = (self.proj_from_padded(s, taps[s][0], E, h, w, tag), pad8(arch.PROJ[s][1]))
         return feats, sizes
 
-    def run_pass(self, images: torch.Tensor, b: int, symmetric: bool, upsample: bool, scale_factor: float,
-                 state_in: Optional[Tuple[torch.Tensor, int, int]] = None, keep_states=False, cnn=None, cnn_ready=None, vit=None):
-        """images [2b,3,H,W] fp32 (A batch then B batch).  Returns (state [D,H,W,3], states per scale, sizes).
-        `cnn` = result of `encode_cnn` computed elsewhere (side stream); `cnn_ready` = event to wait for before use."""
-        tag = "up" if upsample else "lo"
-        E = 2 * b
-        D = E if symmetric else b
-        _, _, H, W = images.shape
-        if cnn is None and (upsample or vit is None):
-            cnn = self.encode_cnn(images, tag)
-        if not upsample and vit is None:
-            with self.stage("dinov2"):
-                vit = self.dinov2(images)
-        if cnn is None:
-            cnn = self.encode_cnn(images, tag)
-        feats, sizes = cnn
-        sizes = dict(sizes)
-        feats = dict(feats)
-        if not upsample:
-            feat16_raw, hp, wp = vit
-            sizes[16] = (hp, wp)
-            state = self.buf("state.lo.16", (D, hp, wp, 3), dtype=torch.float32)
-            with self.stage("gp+decoder"):
-                feats[16] = (self.coarse_match(feat16_raw, E, D, b, hp, wp, state), arch.PROJ[16][1])
-            if self.debug is not None:
-                self.debug["coarse_state"] = state.clone()
-            scales = arch.SCALES
+    def image_stage(self, images: torch.Tensor, images_hi: Optional[torch.Tensor] = None):
+        """Everything the matcher computes of each image on its own, for E images [E, 3, H, W] fp32 and, when there is an upsample
+        pass, their copies at its resolution [E, 3, Hu, Wu]: DINOv2, the GP operands of its tokens and the GP solve against the
+        cosine basis on the launch stream, and the CNN branch (VGG19 + proj) of each pass.
+        The CNN branch depends on none of the rest.  With `overlap_cnn` (and no debug capture) it is released onto a side stream once
+        DINOv2, which saturates the tensor pipe by itself, is enqueued, so that it fills the SMs left idle by the latency-bound GP
+        solve and the small decoder GEMMs; under CUDA-graph capture this is a fork.  Each pass records its own event, so the coarse
+        refiners can start before the upsample CNN finishes.  Otherwise the CNN runs inline on the launch stream after DINOv2.
+        Returns {"g": the GP operands of `gp_rows`, "alpha": fp32 alpha^T of image 0 [512, ldw], image e's `e * stride_a` elements
+        on, "stride_a", "hp", "wp": the stride-14 grid, "cnn": {"lo" / "up": (features, sizes) of `encode_cnn`}, "ready": {pass:
+        event to wait for before reading its CNN features, None when they were made on the launch stream}}."""
+        E = images.shape[0]
+        with self.stage("dinov2"):
+            feat16, hp, wp = self.dinov2(images)
+        passes = {"lo": images} if images_hi is None else {"lo": images, "up": images_hi}
+        cnn, ready = {}, dict.fromkeys(passes)
+        if self.overlap_cnn and self.debug is None:
+            side = self.side_stream()
+            side.wait_stream(torch.cuda.current_stream())
+            with torch.cuda.stream(side):
+                self._lane = "side"
+                for tag, x in passes.items():
+                    cnn[tag] = self.encode_cnn(x, tag)
+                    ready[tag] = torch.cuda.Event()
+                    ready[tag].record(side)
+                self._lane = "main"
         else:
-            src, hi, wi = state_in
-            state = self.resize_state(src, D, hi, wi, *sizes[8], name="state.up.8")
-            scales = arch.UPSAMPLE_SCALES
-        state, states = self.refine_chain(state, scales, feats, sizes, E, D, b, H, W, scale_factor, tag, keep_states, cnn_ready)
-        return state, states, sizes
+            for tag, x in passes.items():
+                cnn[tag] = self.encode_cnn(x, tag)
+        n = hp * wp
+        with self.stage("gp"):
+            g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
+            Wk, stride_a = self.gp_solve_images(g, E, hp, wp)
+        return dict(g=g, alpha=at(Wk, n * pad8(n)), stride_a=stride_a, hp=hp, wp=wp, cnn=cnn, ready=ready)
+
+    def coarse_pass(self, enc, b, symmetric, scale_factor, keep_states=False):
+        """The coarse pass of b pairs from what `image_stage` returned for their 2b images [A_1..A_b | B_1..B_b]: the stride-16
+        table and `gp_decode` (K_xy, mu, the decoder, cls_to_flow), then the refiners at strides 16 to 1.  Returns refine_chain's
+        (state [D, H, W, 3], states)."""
+        E, D = 2 * b, (2 * b if symmetric else b)
+        hp, wp = enc["hp"], enc["wp"]
+        state = self.buf("state.lo.16", (D, hp, wp, 3), dtype=torch.float32)
+        with self.stage("gp+decoder"):
+            self.corr16_table(enc["g"], E, D, b, hp * wp)
+            feat16 = self.gp_decode(enc["g"], enc["alpha"], enc["stride_a"], E, D, b, hp, wp, state)
+        if self.debug is not None:
+            self.debug["coarse_state"] = state.clone()
+        feats, sizes = enc["cnn"]["lo"]
+        feats, sizes = {**feats, 16: (feat16, arch.PROJ[16][1])}, {**sizes, 16: (hp, wp)}
+        return self.refine_chain(state, arch.SCALES, feats, sizes, E, D, b, *sizes[1], scale_factor, "lo", keep_states,
+                                 enc["ready"].get("lo"))
+
+    def upsample_pass(self, state, cnn, b, symmetric, scale_factor, keep_states=False, ready=None):
+        """The upsample pass of b pairs: `state` [D, h, w, 3] of the coarse pass resized to stride 8 of the upsample resolution,
+        then the refiners at strides 8 to 1 on cnn = (features, sizes) of `encode_cnn` at that resolution, which wait for the event
+        `ready` if given.  Returns refine_chain's (state [D, Hu, Wu, 3], states)."""
+        feats, sizes = cnn
+        E, D = 2 * b, (2 * b if symmetric else b)
+        state = self.resize_state(state, D, *state.shape[1:3], *sizes[8], name="state.up.8")
+        return self.refine_chain(state, arch.UPSAMPLE_SCALES, feats, sizes, E, D, b, *sizes[1], scale_factor, "up", keep_states, ready)
 
     def refine_chain(self, state, scales, feats, sizes, E, D, b, H, W, scale_factor, tag, keep_states=False, cnn_ready=None):
         """The refiners of one pass from `state` [D, h, w, 3] at scale scales[0] on, each followed by the resize to the next scale.
@@ -624,39 +643,18 @@ class Engine(BufferArena):
                 state = self.resize_state(state, D, h, w, ho, wo, name=f"state.{tag}.{s // 2}")
         return state, states
 
+    def pair_stage(self, enc, b, symmetric, scale_lo, scale_hi, attenuate, warp, cert):
+        """Everything the matcher computes of b pairs from what `image_stage` returned for their 2b images: the coarse pass, the
+        upsample pass when the images have an upsample-resolution copy, and the match() epilogue into warp / cert."""
+        state, states = self.coarse_pass(enc, b, symmetric, scale_lo)
+        if "up" in enc["cnn"]:
+            state, _ = self.upsample_pass(state, enc["cnn"]["up"], b, symmetric, scale_hi, ready=enc["ready"].get("up"))
+        self.epilogue(state, states[16] if attenuate else None, enc["hp"], enc["wp"], b, *state.shape[1:3], symmetric, out=(warp, cert))
+
     def run_match(self, images, images_hi, b, symmetric, scale_lo, scale_hi, attenuate, warp, cert):
-        """Device side of match(): coarse pass, optional upsample pass, epilogue — no allocation, no host sync.
-        The CNN branch (VGG19 + proj of both passes) has no dependency on the ViT / GP / decoder chain, so it runs on a
-        side stream and overlaps the latency-bound GP solve and decoder; under CUDA-graph capture this becomes a fork."""
-        main = torch.cuda.current_stream()
-        side = self.side_stream()
-        overlap = self.overlap_cnn and self.debug is None
-        cnn_lo = cnn_hi = ev_lo = ev_hi = vit = None
-        if overlap:
-            # the ViT saturates the tensor pipe by itself; the CNN branch is released when it finishes, so that it
-            # fills the SMs left idle by the latency-bound GP solve and the small decoder GEMMs that follow
-            with self.stage("dinov2"):
-                vit = self.dinov2(images)
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                self._lane = "side"
-                cnn_lo = self.encode_cnn(images, "lo")
-                ev_lo = torch.cuda.Event()
-                ev_lo.record(side)
-                if images_hi is not None:
-                    cnn_hi = self.encode_cnn(images_hi, "up")
-                    ev_hi = torch.cuda.Event()
-                    ev_hi.record(side)
-                self._lane = "main"
-        hs, ws = images.shape[-2:]
-        state, states, sizes = self.run_pass(images, b, symmetric, False, scale_lo, cnn=cnn_lo, cnn_ready=ev_lo, vit=vit)
-        coarse = states[16] if attenuate else None
-        hc, wc = sizes[16]
-        if images_hi is not None:
-            hh, wh = images_hi.shape[-2:]
-            state, _, _ = self.run_pass(images_hi, b, symmetric, True, scale_hi, (state, hs, ws), cnn=cnn_hi, cnn_ready=ev_hi)
-            hs, ws = hh, wh
-        self.epilogue(state, coarse, hc, wc, b, hs, ws, symmetric, out=(warp, cert))
+        """Device side of match() for images [2b, 3, H, W] fp32 (A batch then B batch) and their upsample-resolution copies (or
+        None): the image stage, then the pair stage into warp / cert.  No allocation beyond the arena, no host sync."""
+        self.pair_stage(self.image_stage(images, images_hi), b, symmetric, scale_lo, scale_hi, attenuate, warp, cert)
 
     def side_stream(self):
         if self._side is None:
@@ -703,44 +701,20 @@ class Engine(BufferArena):
              row_bytes=row_bytes, ld_src=ld_src, ld_dst=ld_dst, src_rows=src_rows, dst_rows=dst_rows)
 
     def encode_images(self, images, images_hi, slots, bank):
-        """Image stage of match_pairs for E images [E, 3, H, W] (and [E, 3, Hu, Wu] for the upsample pass, else None): DINOv2, p16
-        and the GP solve on the launch stream, the CNN branch of both passes beside them on the side stream as in run_match, then
-        every image's features scattered into the bank rows `slots` (int32 [E] on the device).  No allocation beyond the arena, no
-        host sync."""
-        E, _, H, W = images.shape
-        hp, wp = H // arch.VIT_PATCH, W // arch.VIT_PATCH
-        n, cap = hp * wp, bank["p16"].shape[0]
-        overlap = self.overlap_cnn and self.debug is None
-        cnn, ready = {}, None
-
-        def encode_cnn():
-            cnn["lo"] = self.encode_cnn(images, "lo")[0]
-            if images_hi is not None:
-                cnn["up"] = self.encode_cnn(images_hi, "up")[0]
-        with self.stage("dinov2"):
-            feat16, _, _ = self.dinov2(images)
-        if overlap:
-            main, side = torch.cuda.current_stream(), self.side_stream()
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                self._lane = "side"
-                encode_cnn()
-                ready = torch.cuda.Event()
-                ready.record(side)
-                self._lane = "main"
-        else:
-            encode_cnn()
-        with self.stage("gp"):
-            g = self.gp_rows(self.gp_project(feat16, E, n), E, n)
-            Wk, stride_w = self.gp_solve_images(g, E, hp, wp)
+        """Image stage of match_pairs for E images [E, 3, H, W] (and [E, 3, Hu, Wu] for the upsample pass, else None): `image_stage`,
+        then every image's p16, alpha^T and CNN features scattered into the bank rows `slots` (int32 [E] on the device).  No
+        allocation beyond the arena, no host sync."""
+        E, cap = images.shape[0], bank["p16"].shape[0]
+        enc = self.image_stage(images, images_hi)
+        ready = list(enc["ready"].values())[-1]         # the last pass's CNN event: the side stream records them in order
         if ready is not None:
-            main.wait_event(ready)
+            torch.cuda.current_stream().wait_event(ready)
         with self.stage("bank.scatter"):
             row = bank["p16"][0].numel() * 4
-            self.copy_rows(g["p16"], bank["p16"], E, row, row, row, E, cap, dst_index=slots)
+            self.copy_rows(enc["g"]["p16"], bank["p16"], E, row, row, row, E, cap, dst_index=slots)
             row = bank["alpha"][0].numel() * 4
-            self.copy_rows(at(Wk, n * pad8(n)), bank["alpha"], E, row, stride_w * 4, row, E, cap, dst_index=slots)
-            for tag, feats in cnn.items():
+            self.copy_rows(enc["alpha"], bank["alpha"], E, row, enc["stride_a"] * 4, row, E, cap, dst_index=slots)
+            for tag, (feats, _) in enc["cnn"].items():
                 for s in (8, 4, 2, 1):
                     dst = bank[f"{tag}.{s}"]
                     row = dst[0].numel() * dst.element_size()
@@ -748,40 +722,31 @@ class Engine(BufferArena):
 
     def decode_pairs(self, bank, index, P, symmetric, scale_lo, scale_hi, attenuate, warp, cert):
         """Pair stage of match_pairs for P pairs.  The 2P images index[:P] (im_A of every pair) and index[P:] (im_B), int32 bank
-        rows on the device, are gathered into the buffers match() fills for b = P, in its [A_1..A_P | B_1..B_P] layout; then the pair
-        stage of the coarse match, the refiners of both passes and the epilogue run as in run_match, into warp / cert."""
-        E, b = 2 * P, P
-        D = E if symmetric else b
-        cap = bank["p16"].shape[0]
-        passes = [t for t in ("lo", "up") if f"{t}.1" in bank]
-        sizes = {t: {s: tuple(bank[f"{t}.{s}"].shape[1:3]) for s in (8, 4, 2, 1)} for t in passes}
-        hs, ws = sizes["lo"][1]
+        rows on the device, are gathered into the buffers match() fills for b = P, in its [A_1..A_P | B_1..B_P] layout.  With
+        `gp_rows` of the gathered p16 that is what `image_stage` returns for those images, and `pair_stage` runs on it into
+        warp / cert."""
+        E, cap = 2 * P, bank["p16"].shape[0]
+        hs, ws = bank["lo.1"].shape[1:3]
         hp, wp = hs // arch.VIT_PATCH, ws // arch.VIT_PATCH
-        n, cf, nrhs = hp * wp, arch.PROJ[16][1], arch.GP_DIM
-        sizes["lo"][16] = (hp, wp)
+        n, nrhs = hp * wp, arch.GP_DIM
 
         def gather(src, dst):
             row = src[0].numel() * src.element_size()
             self.copy_rows(src, dst, E, row, row, row, cap, E, src_index=index)
             return dst
         with self.stage("bank.gather"):
-            p16 = gather(bank["p16"], self.buf("gp.p16", (E * n, cf), dtype=torch.float32))
+            p16 = gather(bank["p16"], self.buf("gp.p16", (E * n, arch.PROJ[16][1]), dtype=torch.float32))
             alpha = gather(bank["alpha"], self.buf("pair.alpha_t", (E, nrhs, pad8(n)), dtype=torch.float32))
-            feats = {t: {s: (gather(bank[f"{t}.{s}"], self.buf(f"proj{t}.{s}", (E,) + tuple(bank[f"{t}.{s}"].shape[1:]), zero=True)),
-                             pad8(arch.PROJ[s][1])) for s in (8, 4, 2, 1)} for t in passes}
-        state = self.buf("state.lo.16", (D, hp, wp, 3), dtype=torch.float32)
-        with self.stage("gp+decoder"):
+            cnn = {}
+            for t in [t for t in ("lo", "up") if f"{t}.1" in bank]:
+                src = {s: bank[f"{t}.{s}"] for s in (8, 4, 2, 1)}
+                feats = {s: (gather(x, self.buf(f"proj{t}.{s}", (E,) + tuple(x.shape[1:]), zero=True)), pad8(arch.PROJ[s][1]))
+                         for s, x in src.items()}
+                cnn[t] = (feats, {s: tuple(x.shape[1:3]) for s, x in src.items()})
+        with self.stage("gp+decoder"):                 # profiled as part of the pair work it feeds
             g = self.gp_rows(p16, E, n)
-            self.corr16_table(g, E, D, b, n)
-            feats["lo"][16] = (self.gp_decode(g, alpha, nrhs * pad8(n), E, D, b, hp, wp, state), cf)
-        state, states = self.refine_chain(state, arch.SCALES, feats["lo"], sizes["lo"], E, D, b, hs, ws, scale_lo, "lo")
-        coarse = states[16] if attenuate else None
-        H, W = hs, ws
-        if "up" in passes:
-            H, W = sizes["up"][1]
-            state = self.resize_state(state, D, hs, ws, *sizes["up"][8], name="state.up.8")
-            state, _ = self.refine_chain(state, arch.UPSAMPLE_SCALES, feats["up"], sizes["up"], E, D, b, H, W, scale_hi, "up")
-        self.epilogue(state, coarse, hp, wp, b, H, W, symmetric, out=(warp, cert))
+        enc = dict(g=g, alpha=alpha, stride_a=nrhs * pad8(n), hp=hp, wp=wp, cnn=cnn, ready={})
+        self.pair_stage(enc, P, symmetric, scale_lo, scale_hi, attenuate, warp, cert)
 
     def epilogue(self, state, coarse_state, hc, wc, b, H, W, symmetric, out=None):
         Wout = 2 * W if symmetric else W

@@ -98,14 +98,14 @@ class RegressionMatcher:
         im_a = batch["im_A"].to(eng.device, torch.float32)
         im_b = batch["im_B"].to(eng.device, torch.float32)
         images = torch.cat((im_a, im_b)).contiguous()
-        state_in = None
-        if upsample:
-            c = batch["corresps"]
-            st = torch.cat((c["flow"], c["certainty"]), dim=1).permute(0, 2, 3, 1).contiguous().float()
-            state_in = (st, st.shape[1], st.shape[2])
+        b, scale_factor = im_a.shape[0], float(scale_factor)
         with torch.cuda.device(eng.device):
-            _, states, _ = eng.run_pass(images, im_a.shape[0], symmetric, upsample, float(scale_factor), state_in,
-                                        keep_states=True)
+            if upsample:
+                c = batch["corresps"]
+                state = torch.cat((c["flow"], c["certainty"]), dim=1).permute(0, 2, 3, 1).contiguous().float()
+                _, states = eng.upsample_pass(state, eng.encode_cnn(images, "up"), b, symmetric, scale_factor, keep_states=True)
+            else:
+                _, states = eng.coarse_pass(eng.image_stage(images), b, symmetric, scale_factor, keep_states=True)
         return self._states_to_corresps(states)
 
     def _preprocessor(self) -> DevicePreprocessor:

@@ -112,18 +112,19 @@ class _Recorder:
                 self._inside(v, 1, f"{fn}.{k}")
 
 
-@pytest.mark.parametrize("symmetric,upsample,split", [(True, True, True), (True, True, False), (False, True, True), (True, False, False)])
-def test_engine_dry_run(weights, monkeypatch, symmetric, upsample, split):
+def host_engine(weights, monkeypatch, precision, rec):
+    """A host-only Engine of `precision` (CPU tensors, CNN inline) whose C-ABI calls go to the recording stand-in `rec`, which
+    tracks every weight, arena buffer and constant of the engine."""
     import roma_b200.engine as engine_mod
-    rec = _Recorder()
     eng = engine_mod.Engine.__new__(engine_mod.Engine)
-    eng.device = torch.device("cpu")
-    eng.precision, eng.dtype, eng.dt = "fp32" if split else "fp32_simt", torch.float32, cabi.RB_F32
-    eng.split, eng._lane, eng.generation = split, "main", 0
-    eng.w = PackedWeights(weights[0], weights[1], eng.device, torch.float32, split=split)
-    eng._buf, eng._const, eng.debug, eng.profile, eng.gemm_profile, eng.use_flash_attn, eng.gp_algo = {}, {}, None, None, None, True, (3 if split else 2)
+    engine_mod.BufferArena.__init__(eng, "cpu")
+    eng.precision, eng.dtype = precision, engine_mod.PRECISIONS[precision]
+    eng.dt, eng.split, eng._lane = cabi.DTYPE_CODE[eng.dtype], precision == "fp32", "main"
+    eng.w = PackedWeights(weights[0], weights[1], eng.device, eng.dtype, split=eng.split)
+    eng.debug, eng.profile, eng.gemm_profile, eng.use_flash_attn, eng.gp_algo = None, None, None, True, (2 if precision == "fp32_simt" else 3)
     eng.overlap_cnn, eng._side, eng.gp_tensor_core, eng.fused_c144, eng.fused_small_f32 = False, None, True, True, True
     eng.lc_table16, eng.lc_tile_radii, eng.side_ctas = True, (2,), 0
+    eng._bank, eng.bank_version = None, 0
     for t in _tensors(eng.w):
         rec.track(t)
     orig_buf, orig_const = eng.buf, eng.const
@@ -135,16 +136,37 @@ def test_engine_dry_run(weights, monkeypatch, symmetric, upsample, split):
         t = orig_const(*a, **k); rec.track(t); return t
     eng.buf, eng.const = buf, const
     monkeypatch.setattr(engine_mod, "call", rec)
+    return eng
+
+
+@pytest.mark.parametrize("symmetric,upsample,split", [(True, True, True), (True, True, False), (False, True, True), (True, False, False),
+                                                      (False, True, False), (False, False, True), (False, False, False), (True, False, True)])
+def test_engine_dry_run(weights, monkeypatch, symmetric, upsample, split):
+    rec = _Recorder()
+    eng = host_engine(weights, monkeypatch, "fp32" if split else "fp32_simt", rec)
+    chains, orig_chain = [], eng.refine_chain
+
+    def refine_chain(state, scales, feats, sizes, *a, **k):
+        out = orig_chain(state, scales, feats, sizes, *a, **k)
+        chains.append((sizes, out))
+        return out
+    eng.refine_chain = refine_chain
     b, coarse, up = 1, 112, 168
     A, B, Ah, Bh = synthetic.make_pair(b, coarse, up, 1)
-    images = torch.cat((A, B)); rec.track(images)
-    state, states, sizes = eng.run_pass(images, b, symmetric, False, coarse / 560)
+    images, hi = torch.cat((A, B)), (torch.cat((Ah, Bh)) if upsample else None)
+    D, H = (2 * b if symmetric else b), (up if upsample else coarse)
+    wout = 2 * H if symmetric else H
+    warp, cert = torch.empty(b, H, wout, 4), torch.empty(b, H, wout)
+    for t in (images, hi, warp, cert):
+        if t is not None:
+            rec.track(t)
+    eng.run_match(images, hi, b, symmetric, coarse / 560, up / 560, False, warp, cert)
+    assert len(chains) == (2 if upsample else 1)
+    sizes, (state, states) = chains[0]
     assert sizes == {1: (112, 112), 2: (56, 56), 4: (28, 28), 8: (14, 14), 16: (8, 8)}
-    D = 2 * b if symmetric else b
     assert state.shape == (D, 112, 112, 3) and states[16].shape == (D, 8, 8, 3)
     if upsample:
-        hi = torch.cat((Ah, Bh)); rec.track(hi)
-        state, _, sizes = eng.run_pass(hi, b, symmetric, True, up / 560, (state, 112, 112))
+        state = chains[1][1][0]
         assert state.shape == (D, 168, 168, 3)
     n_gemm = rec.calls.count("romab200_gemm")
     per_pass_refiner = 9 * (5 if not upsample else 5 + 4)

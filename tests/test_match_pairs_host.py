@@ -10,9 +10,9 @@ import torch
 from roma_b200 import arch, cabi, synthetic
 from roma_b200.cache import GraphCache
 from roma_b200.matcher import RegressionMatcher, pair_tensor, plan_pairs
-from roma_b200.packing import PackedWeights
-from test_host_logic import _Recorder, _tensors
+from test_host_logic import _Recorder, _tensors, host_engine
 
+# the calls of Engine.image_stage other than gp_rows, which a decode chunk runs again on the gathered p16
 IMAGE_STAGE = ("dinov2", "encode_cnn", "gp_project", "gp_solve_images")
 
 
@@ -42,29 +42,8 @@ class _PairRecorder(_Recorder):
 
 def _engine(weights, monkeypatch, precision):
     """A host-only Engine of `precision` whose C-ABI calls go to a _PairRecorder."""
-    import roma_b200.engine as engine_mod
     rec = _PairRecorder()
-    eng = engine_mod.Engine.__new__(engine_mod.Engine)
-    eng.device = torch.device("cpu")
-    eng.precision = precision
-    eng.dtype = engine_mod.PRECISIONS[eng.precision]
-    eng.dt = cabi.DTYPE_CODE[eng.dtype]
-    eng.split, eng._lane, eng.generation = precision == "fp32", "main", 0
-    eng.w = PackedWeights(weights[0], weights[1], eng.device, eng.dtype, split=eng.split)
-    eng._buf, eng._const, eng.debug, eng.profile, eng.gemm_profile, eng.use_flash_attn, eng.gp_algo = {}, {}, None, None, None, True, (2 if eng.precision == "fp32_simt" else 3)
-    eng.overlap_cnn, eng._side, eng.gp_tensor_core, eng.fused_c144, eng.fused_small_f32 = False, None, True, True, True
-    eng.lc_table16, eng.lc_tile_radii, eng.side_ctas = True, (2,), 0
-    eng._bank, eng.bank_version = None, 0
-    for t in _tensors(eng.w):
-        rec.track(t)
-    orig_buf, orig_const = eng.buf, eng.const
-
-    def buf(*a, **k):
-        t = orig_buf(*a, **k); rec.track(t); return t
-
-    def const(*a, **k):
-        t = orig_const(*a, **k); rec.track(t); return t
-    eng.buf, eng.const = buf, const
+    eng = host_engine(weights, monkeypatch, precision, rec)
     for name in IMAGE_STAGE:           # mark the calls of the per-image stage
         def wrapped(*a, _f=getattr(eng, name), **k):
             rec.image_stage += 1
@@ -73,7 +52,6 @@ def _engine(weights, monkeypatch, precision):
             finally:
                 rec.image_stage -= 1
         setattr(eng, name, wrapped)
-    monkeypatch.setattr(engine_mod, "call", rec)
     return eng, rec
 
 
@@ -89,7 +67,8 @@ class _TrackingCache(GraphCache):
         return e
 
 
-@pytest.mark.parametrize("symmetric,upsample,split", [(True, True, True), (False, True, False), (True, False, False)])
+@pytest.mark.parametrize("symmetric,upsample,split", [(True, True, True), (False, True, False), (True, False, False), (True, True, False),
+                                                      (False, True, True), (True, False, True), (False, False, True), (False, False, False)])
 def test_match_pairs_dry_run(weights, monkeypatch, symmetric, upsample, split):
     eng, rec = _engine(weights, monkeypatch, "fp32" if split else "fp32_simt")
     coarse, up = 112, 168
@@ -116,21 +95,19 @@ def test_match_pairs_dry_run(weights, monkeypatch, symmetric, upsample, split):
     first_decode = next(i for i, (fn, stage, _, _) in enumerate(rec.log) if fn == "romab200_gather_rows" and (rec.log[i][3].get("src_index") is not None))
     assert "romab200_refiner_prologue" not in [fn for fn, _, _, _ in rec.log[:first_decode]]
 
-    # decode: after its gathers, every chunk launches the pair work of match(b = P): run_pass (+ the upsample pass) and the epilogue
-    # with the image stage left out, call for call with the same scalar arguments
+    # decode: after its gathers, every chunk launches the pair work of match(b = P), i.e. the calls of run_match outside the
+    # image stage, call for call with the same scalar arguments
     decode = [(fn, sc) for fn, _, sc, _ in rec.log[first_decode:] if fn != "romab200_gather_rows"]
     expect = []
     for b in (2, 2, 1):
         n0 = len(rec.log)
         imgs = torch.cat((images[:b], images[b:2 * b])); rec.track(imgs)
-        state, states, sizes = eng.run_pass(imgs, b, symmetric, False, math.sqrt(coarse * coarse / 560 ** 2))
-        H = coarse
-        if upsample:
-            hi = torch.cat((images_hi[:b], images_hi[b:2 * b])); rec.track(hi)
-            state, _, _ = eng.run_pass(hi, b, symmetric, True, math.sqrt(up * up / 560 ** 2), (state, coarse, coarse))
-            H = up
-        out = (torch.empty(b, H, wout, 4), torch.empty(b, H, wout)); rec.track(out[0]); rec.track(out[1])
-        eng.epilogue(state, None, *sizes[16], b, H, H, symmetric, out=out)
+        hi = torch.cat((images_hi[:b], images_hi[b:2 * b])) if upsample else None
+        out = (torch.empty(b, ho, wout, 4), torch.empty(b, ho, wout))
+        for t in (hi, *out):
+            if t is not None:
+                rec.track(t)
+        eng.run_match(imgs, hi, b, symmetric, math.sqrt(coarse * coarse / 560 ** 2), math.sqrt(up * up / 560 ** 2), False, *out)
         expect += [(fn, sc) for fn, stage, sc, _ in rec.log[n0:] if not stage]
     # the one difference: mu = K_xy @ alpha reads alpha^T from the gathered [2P, 512, ldw] rows rather than from rows n.. of the
     # solve's [2P, n + 512, ldw] workspace, so its per-image B stride differs
@@ -157,11 +134,12 @@ def test_pair_arguments():
     assert plan["used"] == [1, 3, 5] and plan["index"].tolist() == [1, 0, 2, 0, 1, 2] and plan["chunks"] == [(0, 3, 0, 6)]
 
 
-@pytest.mark.parametrize("precision,symmetric", [("fp16", True), ("bf16", False), ("fp32", True)])
+@pytest.mark.parametrize("precision,symmetric", [("fp16", True), ("bf16", False), ("fp32", True), ("fp16", False), ("bf16", True),
+                                               ("fp32", False), ("fp32_simt", True), ("fp32_simt", False)])
 def test_debug_captures_are_inert(weights, monkeypatch, precision, symmetric):
-    """`engine.debug = {}` only clones stage tensors: a dry run of both passes and the epilogue makes the same C-ABI calls, in the
-    same order and with the same scalar arguments, as with `debug = None` (the CNN overlap is off in both), and keeps every stage
-    tensor tests/test_fast_mode_stages_gpu.py reads, in its documented shape."""
+    """`engine.debug = {}` only clones stage tensors: a dry run of match()'s device side (`run_match`: both passes and the
+    epilogue) makes the same C-ABI calls, in the same order and with the same scalar arguments, as with `debug = None` (the CNN
+    overlap is off in both), and keeps every stage tensor tests/test_fast_mode_stages_gpu.py reads, in its documented shape."""
     b, coarse, up = 2, 112, 168
     A, B, Ah, Bh = synthetic.make_pair(b, coarse, up, 2)
     logs = {}
@@ -169,13 +147,11 @@ def test_debug_captures_are_inert(weights, monkeypatch, precision, symmetric):
         eng, rec = _engine(weights, monkeypatch, precision)
         eng.debug = debug
         images, hi = torch.cat((A, B)), torch.cat((Ah, Bh))
-        rec.track(images), rec.track(hi)
-        state, states, sizes = eng.run_pass(images, b, symmetric, False, coarse / 560)
-        state, _, _ = eng.run_pass(hi, b, symmetric, True, up / 560, (state, coarse, coarse))
         wout = 2 * up if symmetric else up
         out = (torch.empty(b, up, wout, 4), torch.empty(b, up, wout))
-        rec.track(out[0]), rec.track(out[1])
-        eng.epilogue(state, states[16], *sizes[16], b, up, up, symmetric, out=out)
+        for t in (images, hi, *out):
+            rec.track(t)
+        eng.run_match(images, hi, b, symmetric, coarse / 560, up / 560, True, *out)
         logs[debug is None] = [(fn, sc) for fn, _, sc, _ in rec.log]
     assert logs[True] == logs[False] and len(logs[True]) > 300
     dbg, E, D, n = eng.debug, 2 * b, (2 * b if symmetric else b), (coarse // 14) ** 2
