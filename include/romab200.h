@@ -198,7 +198,7 @@ typedef struct {
                        2: 128-wide blocks factored in shared memory with explicit block inverses, all O(n^2) work as K=128
                           GEMMs; workspace >= batch*ceil(n/128)*65536 bytes (receives the diagonal-block inverses)
                        3: the schedule of 2 with those GEMMs on the tensor cores (split-fp16 operand pairs, fp32-class; the symmetric
-                          trailing update is an in-place TMA reduce-add); n % 4 == 0, ldw % 8 == 0, stride % 8 == 0; workspace >=
+                          trailing update is an in-place TMA reduce-add); ldw % 8 == 0, stride % 8 == 0; workspace >=
                           batch * (ceil(n/128)*65536 + 4*max((n+nrhs)*128 + 16384, nrhs*128 + 16384 + 128*ldw)) bytes */
 } rb_gp_solve_args;
 int romab200_gp_solve(const rb_gp_solve_args* args, void* stream);

@@ -91,10 +91,12 @@ __global__ void __launch_bounds__(128) layernorm_vec_kernel(const float* __restr
 }
 
 // ------------------------------------------------------------------------------------------------
-// softmax over rows (attention scores), in place: one block of 256 threads per row
+// softmax over rows (attention scores), in place: one block of 256 threads per row.  With `oh` (fp32 scores only) the result
+// goes to an RB_F16S pair [rows, ldo] instead, for rows too long for softmax_rows_split_kernel.
 // ------------------------------------------------------------------------------------------------
 template <typename T>
-__global__ void softmax_rows_kernel(T* __restrict__ s, int64_t rows, int cols, int64_t lds, float scale) {
+__global__ void softmax_rows_kernel(T* __restrict__ s, int64_t rows, int cols, int64_t lds, float scale, __half* __restrict__ oh,
+                                    __half* __restrict__ ol, int64_t ldo) {
     rb::pdl_wait();
     __shared__ float red[8];
     int64_t row = blockIdx.x;
@@ -118,6 +120,12 @@ __global__ void softmax_rows_kernel(T* __restrict__ s, int64_t rows, int cols, i
 #pragma unroll
     for (int i = 0; i < 8; ++i) sum += red[i];
     float inv = 1.0f / sum;
+    if (oh) {
+        // the pad columns of the last 4-element group receive 0, as from the warp kernel
+        for (int c = tid; c < (cols + 3) / 4 * 4; c += 256)
+            split_f16s(c < cols ? expf(to_f(sr[c]) * scale - m) * inv : 0.f, oh[row * ldo + c], ol[row * ldo + c]);
+        return;
+    }
     for (int c = tid; c < cols; c += 256) sr[c] = from_f<T>(expf(to_f(sr[c]) * scale - m) * inv);
 }
 
@@ -292,14 +300,20 @@ __global__ void __launch_bounds__(256) split_f16s_vec_kernel(const float* __rest
         *reinterpret_cast<uint2*>(lo + r * ldd + c) = *reinterpret_cast<uint2*>(l);
     }
 }
-// batched variant (blockIdx.y = matrix): used by the tensor-core GP solve for its strided panels
+// batched variant (blockIdx.y = matrix): used by the tensor-core GP solve for its strided panels.  Columns [0, cols) only: a last
+// group of fewer than 4 columns (the GP's last diagonal block at n % 4 != 0) is read and written element by element, so that
+// nothing beyond `cols` is read (the source pad may hold anything) or written.
 __global__ void __launch_bounds__(256) split_f16s_batched_kernel(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, int64_t rows, int cols4,
-                                                                 int64_t ldx, int64_t ldd, int64_t sx, int64_t sd) {
+                                                                 int cols, int64_t ldx, int64_t ldd, int64_t sx, int64_t sd) {
     rb::pdl_wait();
     x += blockIdx.y * sx; hi += blockIdx.y * sd; lo += blockIdx.y * sd;
     const int64_t total = rows * cols4;
     for (int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (int64_t)gridDim.x * blockDim.x) {
         const int64_t r = idx / cols4; const int c = (int)(idx - r * cols4) * 4;
+        if (c + 4 > cols) {
+            for (int j = c; j < cols; ++j) split_f16s(x[r * ldx + j], hi[r * ldd + j], lo[r * ldd + j]);
+            continue;
+        }
         const float4 v = *reinterpret_cast<const float4*>(x + r * ldx + c);
         __half h[4], l[4];
         split_f16s(v.x, h[0], l[0]); split_f16s(v.y, h[1], l[1]); split_f16s(v.z, h[2], l[2]); split_f16s(v.w, h[3], l[3]);
@@ -371,14 +385,14 @@ __global__ void transpose_kernel(const T* __restrict__ src, T* __restrict__ dst,
     }
 }
 
-// fp32 [batch][rows, cols] (pitch ldx, matrix stride sx) -> RB_F16S planes [batch][rows, ldd] (matrix stride sd); cols % 4 == 0,
-// 16-byte aligned rows
+// fp32 [batch][rows, cols] (pitch ldx, matrix stride sx) -> RB_F16S planes [batch][rows, ldd] (matrix stride sd); 16-byte aligned rows
 int split_f16s_batched(const float* x, void* hi, void* lo, int64_t rows, int cols, int64_t ldx, int64_t ldd, int batch, int64_t sx, int64_t sd, cudaStream_t st) {
-    RB_REQUIRE(cols % 4 == 0 && ldx % 4 == 0 && ldd % 4 == 0 && sx % 4 == 0 && sd % 4 == 0 && ((uintptr_t)x) % 16 == 0 && ((uintptr_t)hi) % 8 == 0 && ((uintptr_t)lo) % 8 == 0,
+    RB_REQUIRE(ldx % 4 == 0 && ldd % 4 == 0 && sx % 4 == 0 && sd % 4 == 0 && ((uintptr_t)x) % 16 == 0 && ((uintptr_t)hi) % 8 == 0 && ((uintptr_t)lo) % 8 == 0,
                "split_f16s_batched: alignment");
-    RB_REQUIRE(batch > 0 && batch <= 65535 && rows > 0, "split_f16s_batched: bad shape");
-    dim3 grid(grid1d(rows * (cols / 4), 256, 132 * 8), batch);
-    rb::launch_pdl(split_f16s_batched_kernel, grid, dim3(256), 0, st, x, (__half*)hi, (__half*)lo, rows, cols / 4, ldx, ldd, sx, sd);
+    RB_REQUIRE(batch > 0 && batch <= 65535 && rows > 0 && cols > 0 && cols <= ldx && cols <= ldd, "split_f16s_batched: bad shape");
+    const int cols4 = (cols + 3) / 4;
+    dim3 grid(grid1d(rows * cols4, 256, 132 * 8), batch);
+    rb::launch_pdl(split_f16s_batched_kernel, grid, dim3(256), 0, st, x, (__half*)hi, (__half*)lo, rows, cols4, cols, ldx, ldd, sx, sd);
     return check_launch("split_f16s_batched");
 }
 
@@ -419,11 +433,15 @@ extern "C" int romab200_softmax_rows(const rb_softmax_args* a, void* stream) {
     cudaStream_t st = (cudaStream_t)stream;
     RB_REQUIRE(a->rows > 0 && a->cols > 0 && a->rows < (1ll << 31), "softmax: bad shape");
     if (a->out_hi) {
-        RB_REQUIRE(a->dtype == RB_F32 && a->out_lo && a->cols <= 2048 && a->lds % 4 == 0 && a->ldo % 4 == 0 && (a->cols + 3) / 4 * 4 <= a->ldo &&
+        RB_REQUIRE(a->dtype == RB_F32 && a->out_lo && a->lds % 4 == 0 && a->ldo % 4 == 0 && (a->cols + 3) / 4 * 4 <= a->ldo &&
                    (a->cols + 3) / 4 * 4 <= a->lds && ((uintptr_t)a->s) % 16 == 0 && ((uintptr_t)a->out_hi) % 8 == 0 && ((uintptr_t)a->out_lo) % 8 == 0,
-                   "softmax: split output needs fp32 scores, <= 2048 columns and 4-element aligned pitches");
-        rb::launch_pdl(softmax_rows_split_kernel, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, (const float*)a->s, (__half*)a->out_hi, (__half*)a->out_lo,
-                       a->rows, a->cols, a->lds, a->ldo, a->scale);
+                   "softmax: split output needs fp32 scores and 4-element aligned pitches");
+        if (a->cols <= 2048)
+            rb::launch_pdl(softmax_rows_split_kernel, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, (const float*)a->s, (__half*)a->out_hi, (__half*)a->out_lo,
+                           a->rows, a->cols, a->lds, a->ldo, a->scale);
+        else
+            rb::launch_pdl(softmax_rows_kernel<float>, dim3((unsigned)a->rows), dim3(256), 0, st, (float*)a->s, a->rows, a->cols, a->lds, a->scale,
+                           (__half*)a->out_hi, (__half*)a->out_lo, a->ldo);
         return check_launch("softmax_rows");
     }
     return with_dtype<float, __half, __nv_bfloat16>(a->dtype, "softmax_rows", [&](auto t) {
@@ -431,8 +449,11 @@ extern "C" int romab200_softmax_rows(const rb_softmax_args* a, void* stream) {
         constexpr int vn = 16 / sizeof(T);
         // warp per row when the rows are padded to whole 16-byte vectors (the pad columns are rewritten with zeros), else block per row
         const bool warp = a->cols <= 2048 && (a->lds * (int)sizeof(T)) % 16 == 0 && ((uintptr_t)a->s) % 16 == 0 && (a->cols + vn - 1) / vn * vn <= a->lds;
-        rb::launch_pdl(warp ? softmax_rows_warp_kernel<T> : softmax_rows_kernel<T>, dim3((unsigned)(warp ? (a->rows + 7) / 8 : a->rows)), dim3(256), 0, st,
-                       (T*)a->s, a->rows, a->cols, a->lds, a->scale);
+        if (warp)
+            rb::launch_pdl(softmax_rows_warp_kernel<T>, dim3((unsigned)((a->rows + 7) / 8)), dim3(256), 0, st, (T*)a->s, a->rows, a->cols, a->lds, a->scale);
+        else
+            rb::launch_pdl(softmax_rows_kernel<T>, dim3((unsigned)a->rows), dim3(256), 0, st, (T*)a->s, a->rows, a->cols, a->lds, a->scale,
+                           (__half*)nullptr, (__half*)nullptr, (int64_t)0);
         return check_launch("softmax_rows");
     });
 }

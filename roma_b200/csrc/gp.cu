@@ -731,7 +731,7 @@ extern "C" int romab200_gp_solve(const rb_gp_solve_args* a, void* stream) {
     RB_REQUIRE(a->batch <= 65535, "gp_solve: batch too large");
     if (a->workspace && a->algo == 3) {
         const int64_t nblk128 = (a->n + BB - 1) / BB;
-        RB_REQUIRE(a->ldw % 8 == 0 && a->stride % 8 == 0 && a->n % 4 == 0 && ((uintptr_t)a->W) % 16 == 0 && ((uintptr_t)a->workspace) % 16 == 0, "gp_solve: alignment (algo 3)");
+        RB_REQUIRE(a->ldw % 8 == 0 && a->stride % 8 == 0 && ((uintptr_t)a->W) % 16 == 0 && ((uintptr_t)a->workspace) % 16 == 0, "gp_solve: alignment (algo 3)");
         const int64_t need = (int64_t)a->batch * (nblk128 * BB * BB * 4 + 4 * gp_tc_scratch_halves(a->n, a->nrhs, a->ldw));
         RB_REQUIRE(a->workspace_bytes >= need, "gp_solve: workspace too small for algo 3 (%lld < %lld bytes)", (long long)a->workspace_bytes, (long long)need);
         return gp_solve_tc(a, st);

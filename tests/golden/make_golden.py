@@ -99,6 +99,9 @@ if __name__ == "__main__":
     run("small_b2_sym_up", 112, 168, batch=2, seed=7, step=2, hooks=False)
     run("small_pil_sym_up", 112, 168, pil=True, hooks=False, seed=3)
     run("rect_sym_up", (112, 168), (168, 224), hooks=False, seed=5)
+    # coarse grids of an odd token count (9 x 13 = 117) and of more than 2048 tokens (40 x 56 = 2240)
+    run("odd_sym_up", (126, 182), (182, 238), step=2, hooks=False, seed=11)
+    run("wide_sym_noup", (560, 784), None, upsample_preds=False, step=8, hooks=False, seed=12)
     run("full_sym_up", 560, 864, step=8, hooks=False)
     run("full_nosym_up", 560, 864, symmetric=False, step=8, hooks=False, seed=2)
     run("small_indoor_sym_up", 112, 168, hooks=False, seed=9, factory=roma_indoor)

@@ -73,6 +73,33 @@ def test_match_rectangular_vs_reference_golden(weights, backend):
 
 
 @pytest.mark.parametrize("backend", BACKENDS)
+@pytest.mark.parametrize("name", ["odd_sym_up", "wide_sym_noup"])
+def test_match_token_grids_vs_reference_golden(weights, name, backend):
+    """Coarse grids of an odd token count (126 x 182 -> 182 x 238: 9 x 13 = 117 tokens, the GP solve's last block of odd size)
+    and of more than 2048 tokens (560 x 784: 40 x 56 = 2240, decoder rows longer than the warp-per-row softmax holds)."""
+    from roma_b200 import model_zoo, roma_outdoor
+    g = load_golden(name)
+    ch, cw, uh, uw = (int(v) for v in g["res"])
+    sym, upp, batch, seed, step = (int(v) for v in g["meta"][2:])
+    model_zoo.fp32_backend = backend
+    try:
+        model = roma_outdoor("cuda", weights=weights[0], dinov2_weights=weights[1], coarse_res=(ch, cw),
+                             upsample_res=(uh, uw) if upp else (ch, cw), symmetric=bool(sym), upsample_preds=bool(upp), amp_dtype=torch.float32)
+    finally:
+        model_zoo.fp32_backend = None
+    A, B, Ah, Bh = synthetic.make_pair(batch, (ch, cw), (uh, uw) if upp else None, seed)
+    warp, cert = model.match(A.cuda(), B.cuda(), im_A_high_res=None if Ah is None else Ah.cuda(),
+                             im_B_high_res=None if Bh is None else Bh.cuda())
+    assert warp[:, ::step, ::step].shape == g["warp"].shape and cert[:, ::step, ::step].shape == g["certainty"].shape
+    ew, ec = report(f"{name} {backend}", warp, cert, g, step)
+    assert ew <= TOL and ec <= TOL
+    # the pixels the sub-sampled golden leaves out, through the full-tensor checksums: within TOL per element on average
+    assert abs(warp.double().sum().item() - g["warp_checksum"][0]) <= TOL * warp.numel()
+    assert abs(cert.double().abs().sum().item() - g["certainty_checksum"][1]) <= TOL * cert.numel()
+    model.free_buffers()
+
+
+@pytest.mark.parametrize("backend", BACKENDS)
 def test_stagewise_vs_reference_hooks(weights, backend):
     """Stage tensors of the coarse pass against the tensors hooked out of the reference's own modules."""
     g = load_golden("small_sym_up")

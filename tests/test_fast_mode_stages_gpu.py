@@ -36,8 +36,10 @@ CONFIGS = {
     "sym_b2": ((112, 112), (168, 168), True, 2),
     "nosym": ((112, 112), (168, 168), False, 1),
     "rect": ((112, 168), (168, 224), True, 1),
+    "odd": ((126, 182), (182, 238), True, 1),        # 9 x 13 = 117 tokens: the GP solve's last block of odd size
 }
 FULL = ((560, 560), (864, 864), True, 1)
+WIDE = ((560, 784), (560, 784), True, 1)             # 40 x 56 = 2240 tokens: decoder rows longer than 2048
 SEED = 1
 PRECISIONS = ("fp16", "bf16", "fp32", "fp32_simt")
 U = {"fp16": 2.0 ** -11, "bf16": 2.0 ** -8, "fp32": 2.0 ** -22, "fp32_simt": 2.0 ** -22}
@@ -69,6 +71,15 @@ CEIL_PARITY = {k: 4 * v + KSUM.get(k, 0) / 64 for k, v in CEIL16.items()}
 CEIL_PARITY["gp"] = 256          # the solve's error grows with cond(K_yy + 0.1 I) <= 10 n + 1
 CEIL_F32 = {"cls_to_flow": 16, "update": 4, "resize": 4, "epilogue": 4}
 CEILING = {p: {**(CEIL16 if p in ("fp16", "bf16") else CEIL_PARITY), **CEIL_F32} for p in PRECISIONS}
+
+
+def ceilings(precision, cfg):
+    """CEILING of a configuration: the solve's share of the gp ceiling is one fp32 rounding (2^-24) amplified by the bound
+    cond(K_yy + 0.1 I) <= 10 n + 1 of its n coarse tokens, on top of the storage of mu (1 u in the 16-bit modes).  The constant
+    above covers it up to about 100 tokens (parity) and 200 (fp16); the 2240 tokens of 560 x 784 were measured above it."""
+    n = (cfg[0][0] // arch.VIT_PATCH) * (cfg[0][1] // arch.VIT_PATCH)
+    solve = (10 * n + 1) * 2.0 ** -24 / U[precision]
+    return {**CEILING[precision], "gp": max(CEILING[precision]["gp"], solve + (1.0 if precision in ("fp16", "bf16") else 0.0))}
 
 # (rel, mx) bars in units of u per precision and stage kind: min(ceiling, ~3x the largest value measured on an NVIDIA H100 80GB
 # HBM3 at a 700 W power limit over seeds 1-3 of every configuration; DINOv2 and the first VGG stage: seed 1), measured in comments
@@ -140,6 +151,15 @@ FULL_BARS = {
         # gp 0.426/0.843, decoder 1.3/1.43, cls_to_flow 0.035/0.098, update 0.125/0.238, resize 3.98/23.9, epilogue 0.438/1.68,
         # prologue16-1 0.439/0.675, 0.42/0.923, 0.337/0.979, 0.364/0.65, 0.383/0.852, blocks16-1 1.53/3.54, 4.24/5.69, 2.09/4.56, 2.28/5.19, 1.05/2.87
     },
+}
+
+# 560 x 784, seed 1: min(ceiling, 3x the measured value; measured rel/mx in the comments).  The parity decoder's error grows with
+# the PV contraction over 2240 tokens (measured 3x the small configurations'), the gp error with the condition bound (see ceilings)
+WIDE_BARS = {
+    "fp16": {"gp": (2.0, 3.73), "decoder": (3.7, 4.3), "cls_to_flow": (0.11, 0.3)},         # gp 0.675/2.31, decoder 1.24/1.42, cls_to_flow 0.036/0.098
+    "bf16": {"gp": (1.29, 1.34), "decoder": (3.9, 4.3), "cls_to_flow": (0.11, 0.3)},        # gp 0.430/0.773, decoder 1.29/1.44, cls_to_flow 0.038/0.098
+    "fp32": {"gp": (3200.0, 5600.0), "decoder": (200.0, 180.0), "cls_to_flow": (0.11, 0.3)},  # gp 1073/4422, decoder 66.5/59.3, cls_to_flow 0.036/0.098
+    "fp32_simt": {"gp": (1850.0, 5600.0), "decoder": (17.0, 36.0), "cls_to_flow": (0.11, 0.3)},  # gp 616/3753, decoder 5.50/11.9, cls_to_flow 0.035/0.098
 }
 
 
@@ -216,9 +236,9 @@ def metrics(y, ref, unit):
     return (d.norm() / ref.norm()).item() / unit, (d.abs().max() / ref.abs().max()).item() / unit
 
 
-def stage_errors(precision, cfg, dbg, warp, cert, images, oracles, image_cache, attenuate=True, encoders=True):
+def stage_errors(precision, cfg, dbg, warp, cert, images, oracles, image_cache, attenuate=True, encoders=True, refiners=True):
     """{stage name: (kind, rel / u, mx / u, position term of the ceiling / u)} for every stage of both passes of one debug run.  encoders=False leaves out DINOv2,
-    VGG and proj (the oracle's encoders are too slow on the CPU at full resolution)."""
+    VGG and proj (the oracle's encoders are too slow on the CPU at full resolution); refiners=False stops after cls_to_flow."""
     (hs, ws), (hu, wu), symmetric, b = cfg
     E = 2 * b
     D = E if symmetric else b
@@ -270,6 +290,8 @@ def stage_errors(precision, cfg, dbg, warp, cert, images, oracles, image_cache, 
     check("cls_to_flow", "coarse_state", dbg["coarse_state"],
           torch.cat((o64.cls_to_flow_refine(logits[:, :-1]), nhwc(logits[:, -1:])), -1))
     assert torch.equal(dbg["lo16.state_in"], dbg["coarse_state"])
+    if not refiners:
+        return errs
 
     for tag, (H, W), scales in (("lo", (hs, ws), arch.SCALES), ("up", (hu, wu), arch.UPSAMPLE_SCALES)):
         scale_factor = math.sqrt(H * W / 560 ** 2)
@@ -321,8 +343,8 @@ def test_stages_vs_oracle(weights, models, oracles, image_cache, precision, conf
     dbg, warp, cert, images = run_engine(model, cfg, SEED)
     errs = stage_errors(precision, cfg, dbg, warp, cert, images, oracles, image_cache, attenuate=bool(model.attenuate_cert))
     assert len(errs) == 1 + 16 + 1 + 1 + 1 + 1 + 9 * 3 + 8 + 2
-    report(f"{precision} {config}", errs, BARS[precision], CEILING[precision])
-    assert_within(errs, BARS[precision], CEILING[precision])
+    report(f"{precision} {config}", errs, BARS[precision], ceilings(precision, cfg))
+    assert_within(errs, BARS[precision], ceilings(precision, cfg))
 
 
 @pytest.mark.slow
@@ -334,5 +356,18 @@ def test_stages_vs_oracle_full(weights, models, oracles, image_cache, precision)
     dbg, warp, cert, images = run_engine(model, FULL, SEED)
     errs = stage_errors(precision, FULL, dbg, warp, cert, images, oracles, image_cache, attenuate=bool(model.attenuate_cert),
                         encoders=False)
-    report(f"{precision} full", errs, FULL_BARS[precision], CEILING[precision])
-    assert_within(errs, FULL_BARS[precision], CEILING[precision])
+    report(f"{precision} full", errs, FULL_BARS[precision], ceilings(precision, FULL))
+    assert_within(errs, FULL_BARS[precision], ceilings(precision, FULL))
+
+
+@pytest.mark.slow
+@pytest.mark.parametrize("precision", PRECISIONS)
+def test_stages_vs_oracle_wide(weights, models, oracles, image_cache, precision):
+    """560 x 784: 2240 tokens, more than the warp-per-row softmax holds, and cond(K_yy + 0.1 I) up to 22401.  The coarse stages
+    from the GP on (DINOv2's oracle is too slow on the CPU here; the refiners are the small configurations' business)."""
+    model = models(precision)
+    dbg, warp, cert, images = run_engine(model, WIDE, SEED)
+    errs = stage_errors(precision, WIDE, dbg, warp, cert, images, oracles, image_cache, encoders=False, refiners=False)
+    assert sorted(errs) == ["cls", "coarse_state", "gp.mu"]
+    report(f"{precision} wide", errs, WIDE_BARS[precision], ceilings(precision, WIDE))
+    assert_within(errs, WIDE_BARS[precision], ceilings(precision, WIDE))

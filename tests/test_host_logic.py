@@ -112,6 +112,18 @@ class _Recorder:
                 self._inside(v, 1, f"{fn}.{k}")
 
 
+class _ArgRecorder(_Recorder):
+    """_Recorder that also keeps the arguments of every call"""
+
+    def __init__(self):
+        super().__init__()
+        self.args = []
+
+    def __call__(self, fn, struct, **kw):
+        self.args.append((fn, kw))
+        super().__call__(fn, struct, **kw)
+
+
 def host_engine(weights, monkeypatch, precision, rec):
     """A host-only Engine of `precision` (CPU tensors, CNN inline) whose C-ABI calls go to the recording stand-in `rec`, which
     tracks every weight, arena buffer and constant of the engine."""
@@ -174,6 +186,36 @@ def test_engine_dry_run(weights, monkeypatch, symmetric, upsample, split):
     assert n_gemm > per_pass_refiner * 4 // 5 + 24 * 4
     assert rec.calls.count("romab200_gp_solve") == 1
     assert rec.calls.count("romab200_refiner_prologue") == (9 if upsample else 5)
+
+
+@pytest.mark.parametrize("precision", ["fp32", "fp32_simt", "fp16", "bf16"])
+@pytest.mark.parametrize("coarse,up", [((126, 182), (182, 238)), ((560, 784), None)])
+def test_engine_dry_run_token_grids(weights, monkeypatch, precision, coarse, up):
+    """Coarse grids of 9 x 13 = 117 tokens (odd: the GP solve's last block) and of 40 x 56 = 2240 tokens (decoder rows longer than
+    2048) through run_match under the recorder's bounds checks, symmetric, with the GP solve and the softmax calls they reach."""
+    rec = _ArgRecorder()
+    eng = host_engine(weights, monkeypatch, precision, rec)
+    b = 1
+    A, B, Ah, Bh = synthetic.make_pair(b, coarse, up, 1)
+    images, hi = torch.cat((A, B)), (torch.cat((Ah, Bh)) if up else None)
+    H, W = up or coarse
+    warp, cert = torch.empty(b, H, 2 * W, 4), torch.empty(b, H, 2 * W)
+    for t in (images, hi, warp, cert):
+        if t is not None:
+            rec.track(t)
+    scale = lambda r: (r[0] * r[1] / 560 ** 2) ** 0.5    # noqa: E731
+    eng.run_match(images, hi, b, True, scale(coarse), scale(up or coarse), False, warp, cert)
+    n = (coarse[0] // 14) * (coarse[1] // 14)
+    solves = [kw for fn, kw in rec.args if fn == "romab200_gp_solve"]
+    assert len(solves) == 1 and solves[0]["n"] == n and solves[0]["batch"] == 2 * b
+    s = solves[0]
+    assert s["ldw"] == pad8(n) and s["stride"] == (n + s["nrhs"]) * s["ldw"] and s["algo"] == (2 if precision == "fp32_simt" else 3)
+    if s["algo"] == 3:                   # the workspace the header asks of algo 3
+        need = s["batch"] * (-(-n // 128) * 65536 + 4 * max((n + s["nrhs"]) * 128 + 16384, s["nrhs"] * 128 + 16384 + 128 * s["ldw"]))
+        assert s["workspace_bytes"] >= need
+    long_rows = [kw for fn, kw in rec.args if fn == "romab200_softmax_rows" and kw["cols"] == n]
+    if precision == "fp32":              # the parity decoder: QK^T, the split-output softmax, PV in each of its 5 blocks
+        assert len(long_rows) == 5 and all(kw["out_hi"] is not None and kw["ldo"] == pad8(n) for kw in long_rows)
 
 
 def _tensors(obj):

@@ -150,6 +150,33 @@ def test_layernorm(rows, cols, out_dt):
     close(y[:, :cols], ref, tol)
 
 
+@pytest.mark.parametrize("cols", [1600, 2047, 2048, 2049, 2240, 2304, 4100])
+@pytest.mark.parametrize("extra", [0, 12])
+def test_softmax_split_rows(cols, extra):
+    """Softmax of fp32 scores written as an RB_F16S pair (the parity mode's attention probabilities), up to 2048 columns by the
+    warp-per-row kernel, beyond by the block-per-row one (decoders of coarse grids with more than 2048 tokens); `extra` makes
+    the pitches ragged.  hi + lo 2^-11 against fp64, the pad columns of the last 4-element group zero and the rest of the pitch
+    untouched, and bit for bit the in-place fp32 softmax of the same scores, split."""
+    rows, c4 = 37, (cols + 3) // 4 * 4
+    lds, ldo = c4 + extra, c4 + 2 * extra
+    s = rnd(rows, lds, seed=cols, scale=3.0)
+    hi = torch.full((rows, ldo), 7.0, dtype=torch.float16, device=DEV)
+    lo = torch.full((rows, ldo), 7.0, dtype=torch.float16, device=DEV)
+    call("romab200_softmax_rows", "rb_softmax_args", s=s, rows=rows, cols=cols, lds=lds, dtype=F32, scale=1.0, out_hi=hi, out_lo=lo, ldo=ldo)
+    ref = torch.softmax(s[:, :cols].double(), -1).cpu()
+    got = (hi[:, :cols].double() + lo[:, :cols].double() * 2.0 ** -11).cpu()
+    err = ((got - ref).abs() - (2.0 ** -19 * ref + 2.0 ** -34)).max().item()
+    assert err <= 0, f"split softmax off fp64 by {err:.3e} beyond the bar"
+    for plane in (hi, lo):
+        assert (plane[:, cols:c4] == 0).all() and (plane[:, c4:] == 7.0).all()
+    inplace = s.clone()
+    call("romab200_softmax_rows", "rb_softmax_args", s=inplace, rows=rows, cols=cols, lds=lds, dtype=F32, scale=1.0)
+    p = inplace[:, :cols]
+    p_hi = p.half()
+    p_lo = ((p - p_hi.float()) * 2048.0).half()
+    assert torch.equal(hi[:, :cols], p_hi) and torch.equal(lo[:, :cols], p_lo)
+
+
 def test_copy_split_transpose_tokens_im2col():
     x = rnd(33, 20, seed=1)
     d = torch.zeros(33, 24, dtype=torch.float16, device=DEV)

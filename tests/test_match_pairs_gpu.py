@@ -47,9 +47,19 @@ def _err(a, b):
 
 @pytest.mark.parametrize("mode", list(MODES))
 def test_match_pairs_equals_match(weights, images, mode):
-    model = _model(weights, mode)
+    _check_equals_match(_model(weights, mode), *images, mode)
+
+
+@pytest.mark.parametrize("mode", list(MODES))
+def test_match_pairs_equals_match_odd_grid(weights, mode):
+    """126 x 182 -> 182 x 238: a coarse grid of 9 x 13 = 117 tokens, an odd size for the per-image GP solve."""
+    A, B, Ah, Bh = synthetic.make_pair(3, (126, 182), (182, 238), seed=7)
+    model = _model(weights, mode, (126, 182), (182, 238))
+    _check_equals_match(model, torch.cat((A, B))[:5].cuda(), torch.cat((Ah, Bh))[:5].cuda(), mode)
+
+
+def _check_equals_match(model, ims, his, mode):
     model.use_cuda_graph = False          # eager on both sides; graph replays are covered below
-    ims, his = images
     for symmetric in (True, False):
         for upsample in (True, False):
             model.symmetric, model.upsample_preds = symmetric, upsample

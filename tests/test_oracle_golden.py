@@ -53,6 +53,22 @@ def test_oracle_matches_reference_rectangular(weights):
     _check(warp, cert, g)
 
 
+@pytest.mark.parametrize("name", ["odd_sym_up", pytest.param("wide_sym_noup", marks=pytest.mark.slow)])
+def test_oracle_matches_reference_token_grids(weights, name):
+    """Coarse grids of 9 x 13 = 117 tokens (126 x 182 -> 182 x 238) and of 40 x 56 = 2240 tokens (560 x 784), sub-sampled
+    goldens + full-tensor checksums."""
+    g = load_golden(name)
+    ch, cw, uh, uw = (int(v) for v in g["res"])
+    sym, upp, batch, seed, step = (int(v) for v in g["meta"][2:])
+    up = (uh, uw) if upp else None
+    orc = RomaOracle(weights[0], weights[1], (ch, cw), up or (ch, cw), symmetric=bool(sym), upsample_preds=bool(upp))
+    A, B, Ah, Bh = synthetic.make_pair(batch, (ch, cw), up, seed)
+    warp, cert = orc.match(A, B, Ah, Bh)
+    _check(warp, cert, g, step)
+    assert abs(warp.double().sum().item() - g["warp_checksum"][0]) <= 1e-3 * max(1.0, abs(g["warp_checksum"][0]))
+    assert abs(cert.double().abs().sum().item() - g["certainty_checksum"][1]) <= 1e-4 * g["certainty_checksum"][1]
+
+
 def test_oracle_stage_tensors(weights):
     g = load_golden("small_sym_up")
     st = load_golden("small_sym_up_stages")          # x[:, ::cs, ::ss, ::ss] with [cs, ss] = st[key + "__step"]
