@@ -631,6 +631,77 @@ int romab200_homography_score(const rb_homography_args* args, void* stream);
 int romab200_homography_select(const rb_homography_args* args, void* stream);
 int romab200_homography_refine(const rb_homography_args* args, void* stream);
 
+/* ---- fundamental matrix: cv2.findFundamentalMat(kptsA, kptsB, ransacReprojThreshold, cv2.USAC_MAGSAC, confidence, maxIters) of the
+ *      reference's usage example (README.md:62-78, demo/demo_fundamental.py): MAGSAC++ over seven-point samples ----
+ * B pairs with ragged point counts, packed: pair b owns points [offsets[b], offsets[b+1]).  x1^T F x0 = 0.  All arithmetic is float64
+ * and, where a stage is restated bit for bit (oracle/fundamental_ransac.py), every operation is rounded separately.
+ *   romab200_fund_hypotheses  round 0 first normalises every pair (one CTA per pair; the rows whose four coordinates are finite give
+ *                             centroids and mean distances to them through fixed-order sums, scale = sqrt(2) / mean distance; norm[b] =
+ *                             (cx0, cy0, s0, cx1, cy1, s1), xn = ((x - c) s) per image).  Then one thread per hypothesis of the round:
+ *                             hypothesis h of every pair takes 7 distinct indices from Philox4x32-10 with key (seed lo, seed hi) and
+ *                             counter (h, s, 0, RB_FUND_CTR), s = 0, 1, ...; words in order, index (w * n) >> 32, repeats skipped.  The
+ *                             counter does not name the pair, so a pair's result does not depend on its place in the batch.  The 7x9 system
+ *                             of the normalised points is reduced by Gauss-Jordan with partial pivoting (no model on a pivot that is not
+ *                             finite or below 1e-12 of the first), giving the pencil F2 + l (F1 - F2); the real roots of the cubic
+ *                             det(F2 + l (F1 - F2)) are bracketed by the critical points and the Cauchy bound and bisected to adjacent
+ *                             doubles.  A root is kept if (e' x x_i) . (F x_i) has the same strict sign on all 7 points (the oriented
+ *                             epipolar constraint; e' the largest of the three cross products of F's columns).  The kept models, in
+ *                             ascending l, are de-normalised (T1^T F T0) and scaled to unit Frobenius norm.  A pair with n == 7 solves
+ *                             its 7 points once (hypothesis 0).
+ *   romab200_fund_score       thread = (hypothesis, model slot).  Per point the squared Sampson distance r2 = (x1^T F x0)^2 /
+ *                             ((F x0)_0^2 + (F x0)_1^2 + (F^T x1)_0^2 + (F^T x1)_1^2); the MAGSAC++ loss (sigma_max = thresh) is 1
+ *                             unless r2 < l2 = RB_FUND_K2 thresh^2, then table[0] interpolated linearly at p = r2 (RB_FUND_TABLE / l2):
+ *                             t[i] + (p - i) (t[i + 1] - t[i]), i = min(floor(p), RB_FUND_TABLE - 1).  Slice y holds points
+ *                             [y RB_FUND_SLICE, (y + 1) RB_FUND_SLICE) of its pair, whatever the batch; its loss is the sequential sum
+ *                             over them in index order and its count the points with r2 < thresh^2.
+ *   romab200_fund_select      one warp per pair replays the sequential loop: the slices of a model add up in slice order, a model
+ *                             replaces the best iff its loss is lower, then niters = RANSACUpdateNumIters(conf, (n - count) / n, 7,
+ *                             niters); the loop stops at iter >= niters.  Sets running[0] when a pair needs another round.
+ *   romab200_fund_refine      one CTA per pair, sigma-consensus++: (n >= 8) at most RB_FUND_REFINE_ITERS times, weights table[1]
+ *                             interpolated as above, the weighted normalised eight-point fit (the smallest eigenvector of the 9x9 sum
+ *                             of w a a^T, cyclic Jacobi), rank 2 by a 3x3 SVD, de-normalised; the fit is kept while the loss (summed
+ *                             over the CTA in a fixed order) decreases.  mask = r2 < thresh^2 under the returned F, which has unit
+ *                             Frobenius norm and its largest-magnitude entry positive.  ok[b] = 0, F and mask zero, when no model.
+ * `table` is [2, RB_FUND_TABLE + 1] float64: the normalised MAGSAC++ loss and weight at r^2 = (i / RB_FUND_TABLE) RB_FUND_K2 thresh^2
+ * (roma_b200/geometry.py, DESIGN.md); RB_FUND_K2 is the 0.99 quantile of chi^2 with 4 degrees of freedom.  The caller zero-fills `state` before round 0 and calls hypotheses / score / select for rounds
+ * 0, 1, ... while running[0] != 0 and round * RB_FUND_ROUND < max_iters, then refine once. */
+#define RB_FUND_ROUND 1024
+#define RB_FUND_MODELS 3
+#define RB_FUND_SLICE 512
+#define RB_FUND_TABLE 1024
+#define RB_FUND_REFINE_ITERS 10
+#define RB_FUND_CTR 0x46370000u
+#define RB_FUND_K2 13.276704135987622
+#define RB_FUND_STATE 8       /* state[b, :]: iter, niters, best hypothesis, best slot, running, n, unused, unused */
+typedef struct {
+    int32_t batch;
+    const double* x0; const double* x1;   /* [total, 2] points in image A / image B */
+    const int64_t* offsets;               /* [batch + 1] */
+    int64_t max_n;                        /* largest pair (sizes the grid of the score) */
+    double thresh, conf;
+    int32_t max_iters, round;
+    uint64_t seed;
+    const double* table;                  /* [2, RB_FUND_TABLE + 1] loss, weight */
+    double* norm;                         /* [batch, 6] */
+    double* xn;                           /* [total, 4] normalised (x0, y0, x1, y1) */
+    int32_t* sample;                      /* [batch, RB_FUND_ROUND, 7] drawn indices of the round */
+    int32_t* nmod;                        /* [batch, RB_FUND_ROUND] models of each hypothesis */
+    double* F;                            /* [batch, RB_FUND_ROUND, RB_FUND_MODELS, 9] models of the round, row-major */
+    int32_t* counts;                      /* [batch, ceil(max_n / RB_FUND_SLICE), RB_FUND_ROUND * RB_FUND_MODELS] */
+    double* losses;                       /* [batch, ceil(max_n / RB_FUND_SLICE), RB_FUND_ROUND * RB_FUND_MODELS] */
+    int32_t* state;                       /* [batch, RB_FUND_STATE] */
+    double* best_F;                       /* [batch, 9] the best model of the loop */
+    double* best_loss;                    /* [batch] its loss */
+    int32_t* running;                     /* [1] */
+    double* out_F;                        /* [batch, 9] the refined model */
+    uint8_t* ok;                          /* [batch] */
+    uint8_t* mask;                        /* [total] */
+} rb_fund_args;
+int romab200_fund_hypotheses(const rb_fund_args* args, void* stream);
+int romab200_fund_score(const rb_fund_args* args, void* stream);
+int romab200_fund_select(const rb_fund_args* args, void* stream);
+int romab200_fund_refine(const rb_fund_args* args, void* stream);
+
 /* ---- depth-based ground-truth warps and the MegaDepth dense metric: `warp_kpts`, `get_gt_warp` (romatch/utils/utils.py:325-454)
  *      and `MegadepthDenseBenchmark.geometric_dist` (romatch/benchmarks/megadepth_dense_benchmark.py:17-42) ----
  * One float64 statement of the geometry, shared by the three entry points.  For a normalised point (x, y) of view 0 of pair b:

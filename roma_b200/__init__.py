@@ -22,7 +22,8 @@ def __getattr__(name):
     if name == "decode_jpeg":
         from .jpeg import decode_jpeg
         return decode_jpeg
-    if name in ("estimate_pose", "estimate_pose_batched", "find_homography", "find_homography_batched", "RANSAC"):
+    if name in ("estimate_pose", "estimate_pose_batched", "find_homography", "find_homography_batched", "RANSAC", "find_fundamental",
+                "find_fundamental_batched", "USAC_MAGSAC"):
         from . import geometry
         return getattr(geometry, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):

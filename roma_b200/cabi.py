@@ -154,6 +154,9 @@ _FIELD_DTYPES = {
     "rb_homography_args": {"src": _F32, "dst": _F32, "offsets": torch.int64, "sample": torch.int32, "attempts": torch.int32, "status": torch.int32,
                            "H": _F64, "counts": torch.int32, "state": torch.int32, "best_H": _F64, "running": torch.int32, "out_H": _F64,
                            "ok": torch.uint8, "mask": torch.uint8},
+    "rb_fund_args": {"x0": _F64, "x1": _F64, "offsets": torch.int64, "table": _F64, "norm": _F64, "xn": _F64, "sample": torch.int32,
+                     "nmod": torch.int32, "F": _F64, "counts": torch.int32, "losses": _F64, "state": torch.int32, "best_F": _F64,
+                     "best_loss": _F64, "running": torch.int32, "out_F": _F64, "ok": torch.uint8, "mask": torch.uint8},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,

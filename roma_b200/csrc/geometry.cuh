@@ -1,4 +1,4 @@
-// Helpers shared by the two-view geometry estimators (pose.cu, homography.cu).
+// Helpers shared by the two-view geometry estimators (pose.cu, homography.cu, fundamental.cu).
 #pragma once
 #include "common.cuh"
 
@@ -43,13 +43,12 @@ __device__ __forceinline__ void ransac_draw(int (&id)[M], int64_t n, uint64_t se
     }
 }
 
-// Inliers of this thread's model among the points of score slice blockIdx.y (per_split points each, n in all).  The CTA of
-// THREADS threads stages the points through `tile`, load(j) giving point j; inlier(p) tests one.  Every thread must call
-// it; the count is meaningful for the threads with act set.  Integer counts: the slices add up in any order.
-template <int THREADS, typename T, int TILE, typename Load, typename Inlier>
-__device__ __forceinline__ int ransac_count(T (&tile)[TILE], int64_t n, int per_split, bool act, Load load, Inlier inlier) {
+// Visits the points of score slice blockIdx.y (per_split points each, n in all) in index order: the CTA of THREADS threads
+// stages them through `tile`, load(j) giving point j, and every thread with act set calls visit(p) on each.  Every thread must
+// call it.
+template <int THREADS, typename T, int TILE, typename Load, typename Visit>
+__device__ __forceinline__ void ransac_scan(T (&tile)[TILE], int64_t n, int per_split, bool act, Load load, Visit visit) {
     const int64_t j0 = (int64_t)blockIdx.y * per_split, j1 = min(n, j0 + per_split);
-    int cnt = 0;
     for (int64_t t0 = j0; t0 < j1; t0 += TILE) {
         const int m = (int)min((int64_t)TILE, j1 - t0);
         __syncthreads();
@@ -57,9 +56,17 @@ __device__ __forceinline__ int ransac_count(T (&tile)[TILE], int64_t n, int per_
         __syncthreads();
         if (act) {
 #pragma unroll 4
-            for (int j = 0; j < m; ++j) cnt += inlier(tile[j]);
+            for (int j = 0; j < m; ++j) visit(tile[j]);
         }
     }
+}
+
+// Inliers of this thread's model among the points of score slice blockIdx.y; inlier(p) tests one.  The count is meaningful
+// for the threads with act set.  Integer counts: the slices add up in any order.
+template <int THREADS, typename T, int TILE, typename Load, typename Inlier>
+__device__ __forceinline__ int ransac_count(T (&tile)[TILE], int64_t n, int per_split, bool act, Load load, Inlier inlier) {
+    int cnt = 0;
+    ransac_scan<THREADS>(tile, n, per_split, act, load, [&](const T& p) { cnt += inlier(p); });
     return cnt;
 }
 
@@ -166,6 +173,70 @@ __device__ __forceinline__ void jacobi_eig_warp(double (*A)[N], double (*V)[N], 
                 __syncwarp();
             }
     }
+}
+
+// 3x3 SVD M = sum_k s_k u_k v_k^T from cyclic Jacobi on M^T M: v[k] is the k-th right singular vector by descending singular
+// value with det [v0 v1 v2] = +1, u[k] = M v_k / s_k and s[k] = |M v_k| for k < 2, u[2] = u[0] x u[1] (M row-major)
+__device__ __forceinline__ void svd3(const double* M, double (&u)[3][3], double (&v)[3][3], double (&s)[2]) {
+    double A[3][3], V[3][3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i)
+#pragma unroll
+        for (int j = 0; j < 3; ++j) A[i][j] = M[i] * M[j] + M[3 + i] * M[3 + j] + M[6 + i] * M[6 + j];   // M^T M
+    jacobi_eig<3>(A, V, 12);
+    // order the eigenvalues descending: columns i0 (largest), i1, i2 (smallest)
+    double e0 = A[0][0], e1 = A[1][1], e2 = A[2][2];
+    int i0 = 0, i1 = 1, i2 = 2;
+    if (e1 > e0) { const double t = e0; e0 = e1; e1 = t; const int k = i0; i0 = i1; i1 = k; }
+    if (e2 > e1) { const double t = e1; e1 = e2; e2 = t; const int k = i1; i1 = i2; i2 = k; }
+    if (e1 > e0) { const double t = e0; e0 = e1; e1 = t; const int k = i0; i0 = i1; i1 = k; }
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+        v[0][i] = i0 == 0 ? V[i][0] : (i0 == 1 ? V[i][1] : V[i][2]);
+        v[1][i] = i1 == 0 ? V[i][0] : (i1 == 1 ? V[i][1] : V[i][2]);
+        v[2][i] = i2 == 0 ? V[i][0] : (i2 == 1 ? V[i][1] : V[i][2]);
+    }
+    const double dv = v[0][0] * (v[1][1] * v[2][2] - v[1][2] * v[2][1]) - v[0][1] * (v[1][0] * v[2][2] - v[1][2] * v[2][0]) +
+                      v[0][2] * (v[1][0] * v[2][1] - v[1][1] * v[2][0]);
+    if (dv < 0.0) { v[2][0] = -v[2][0]; v[2][1] = -v[2][1]; v[2][2] = -v[2][2]; }
+#pragma unroll
+    for (int k = 0; k < 2; ++k) {
+        double nn = 0.0;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) { u[k][i] = M[3 * i] * v[k][0] + M[3 * i + 1] * v[k][1] + M[3 * i + 2] * v[k][2]; nn += u[k][i] * u[k][i]; }
+        nn = sqrt(nn);
+        s[k] = nn;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) u[k][i] /= nn;
+    }
+    u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
+    u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
+    u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+}
+
+// Sums of v[0..N) over a CTA of THREADS threads: per-warp butterfly, then the warp partials added in warp order.  Fixed order,
+// so the result does not depend on the batch.  Leaves the totals in tot[0..N) (visible to every thread on return).
+template <int N, int THREADS, int M, int W>
+__device__ __forceinline__ void cta_sum(double (&v)[M], double (*red)[W], double* tot) {
+    static_assert(N <= M && N <= W && N <= THREADS, "cta_sum: too many sums");
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+    for (int k = 0; k < N; ++k) {
+#pragma unroll
+        for (int d = 16; d; d >>= 1) v[k] += __shfl_xor_sync(0xffffffffu, v[k], d);
+    }
+    __syncthreads();
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < N; ++k) red[w][k] = v[k];
+    }
+    __syncthreads();
+    if (threadIdx.x < N) {
+        double s = 0.0;
+        for (int q = 0; q < THREADS / 32; ++q) s += red[q][threadIdx.x];
+        tot[threadIdx.x] = s;
+    }
+    __syncthreads();
 }
 
 }  // namespace rb

@@ -317,31 +317,6 @@ __global__ void __launch_bounds__(128) homog_select_kernel(rb_homography_args a,
 }
 
 // ---------------------------------------------------------------------------------------------------------------- refine
-// Sums of v[0..N) over the CTA: per-warp butterfly, then warp partials added in warp order.  Fixed order, so the result does not
-// depend on the batch.  Leaves the totals in tot[0..N) (visible to every thread on return).
-template <int N, int M>
-__device__ __forceinline__ void cta_sum(double (&v)[M], double (*red)[HG_NRED], double* tot) {
-    static_assert(N <= M && N <= HG_NRED, "cta_sum: too many sums");
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-#pragma unroll
-    for (int k = 0; k < N; ++k) {
-#pragma unroll
-        for (int d = 16; d; d >>= 1) v[k] += __shfl_xor_sync(HG_FULL, v[k], d);
-    }
-    __syncthreads();
-    if (lane == 0) {
-#pragma unroll
-        for (int k = 0; k < N; ++k) red[w][k] = v[k];
-    }
-    __syncthreads();
-    if (threadIdx.x < N) {
-        double s = 0.0;
-        for (int q = 0; q < HG_REFINE_THREADS / 32; ++q) s += red[q][threadIdx.x];
-        tot[threadIdx.x] = s;
-    }
-    __syncthreads();
-}
-
 // maximum of v over the CTA into *out (visible to every thread on return)
 __device__ __forceinline__ void cta_max(double v, double (*red)[HG_NRED], double* out) {
 #pragma unroll
@@ -498,9 +473,9 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
             s4[0] += d.x; s4[1] += d.y; s4[2] += s.x; s4[3] += s.y;
             cnt[0] += 1.0;
         }
-        cta_sum<1>(cnt, sm.red, sm.tot);
+        cta_sum<1, HG_REFINE_THREADS>(cnt, sm.red, sm.tot);
         const double count = sm.tot[0];
-        cta_sum<4>(s4, sm.red, sm.tot);
+        cta_sum<4, HG_REFINE_THREADS>(s4, sm.red, sm.tot);
         const double cmx = sm.tot[0] / count, cmy = sm.tot[1] / count, cMx = sm.tot[2] / count, cMy = sm.tot[3] / count;
         double a4[4] = {0.0, 0.0, 0.0, 0.0};
         for (int64_t i = tid; i < n; i += HG_REFINE_THREADS) {
@@ -508,7 +483,7 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
             const float2 s = S[i], d = Dp[i];
             a4[0] += fabs(d.x - cmx); a4[1] += fabs(d.y - cmy); a4[2] += fabs(s.x - cMx); a4[3] += fabs(s.y - cMy);
         }
-        cta_sum<4>(a4, sm.red, sm.tot);
+        cta_sum<4, HG_REFINE_THREADS>(a4, sm.red, sm.tot);
         const bool degenerate = !(fabs(sm.tot[0]) >= HG_DBL_EPS && fabs(sm.tot[1]) >= HG_DBL_EPS && fabs(sm.tot[2]) >= HG_DBL_EPS &&
                                   fabs(sm.tot[3]) >= HG_DBL_EPS);
         if (degenerate) {
@@ -544,7 +519,7 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
                         acc[15 + 3 * u + w] -= pp * y;
                     }
             }
-            cta_sum<LM_SUMS>(acc, sm.red, sm.tot);
+            cta_sum<LM_SUMS, HG_REFINE_THREADS>(acc, sm.red, sm.tot);
             if (tid == 0) {
                 const int pi[3][3] = {{0, 1, 2}, {1, 3, 4}, {2, 4, 5}};
                 for (int r = 0; r < 9; ++r)
@@ -587,7 +562,7 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
     __syncthreads();
     lm_partials(sm.x, S, Dp, mask, n, acc);
     cta_max(acc[LM_SUMS], sm.red, &sm.rinf_d);
-    cta_sum<LM_SUMS>(acc, sm.red, sm.tot);
+    cta_sum<LM_SUMS, HG_REFINE_THREADS>(acc, sm.red, sm.tot);
     if (tid == 0) {
         lm_assemble(sm.tot, sm.A, sm.v, sm.S);
         for (int r = 0; r < 8; ++r) sm.D[r] = sm.A[r][r];
@@ -610,7 +585,7 @@ __global__ void __launch_bounds__(HG_REFINE_THREADS, 1) homog_refine_kernel(rb_h
         // the residual at xd, and (used only if the step is taken) J^T J and J^T r there
         lm_partials(sm.xd, S, Dp, mask, n, acc);
         cta_max(acc[LM_SUMS], sm.red, &sm.rinf_d);
-        cta_sum<LM_SUMS>(acc, sm.red, sm.tot);
+        cta_sum<LM_SUMS, HG_REFINE_THREADS>(acc, sm.red, sm.tot);
         if (tid == 0) {
             const double Sd = sm.tot[29];
             double dS = 0.0, dv = 0.0, dinf = 0.0;

@@ -541,40 +541,8 @@ __global__ void __launch_bounds__(128) pose_select_kernel(rb_pose_args a, int sp
 // ---------------------------------------------------------------------------------------------------------------- recover
 // cv::decomposeEssentialMat: E = U diag V^T with det U = det V = 1, R1 = U W V^T, R2 = U W^T V^T, t = U[:, 2]
 __device__ void decompose_essential(const double* E, double (&R1)[9], double (&R2)[9], double (&tv)[3]) {
-    double A[3][3], V[3][3];
-#pragma unroll
-    for (int i = 0; i < 3; ++i)
-#pragma unroll
-        for (int j = 0; j < 3; ++j) A[i][j] = E[i] * E[j] + E[3 + i] * E[3 + j] + E[6 + i] * E[6 + j];   // E^T E
-    jacobi_eig<3>(A, V, 12);
-    // order the eigenvalues descending: columns i0 (largest), i1, i2 (smallest)
-    double e0 = A[0][0], e1 = A[1][1], e2 = A[2][2];
-    int i0 = 0, i1 = 1, i2 = 2;
-    if (e1 > e0) { const double t = e0; e0 = e1; e1 = t; const int k = i0; i0 = i1; i1 = k; }
-    if (e2 > e1) { const double t = e1; e1 = e2; e2 = t; const int k = i1; i1 = i2; i2 = k; }
-    if (e1 > e0) { const double t = e0; e0 = e1; e1 = t; const int k = i0; i0 = i1; i1 = k; }
-    double v[3][3], u[3][3];                    // v[k] = k-th right singular vector
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        v[0][i] = i0 == 0 ? V[i][0] : (i0 == 1 ? V[i][1] : V[i][2]);
-        v[1][i] = i1 == 0 ? V[i][0] : (i1 == 1 ? V[i][1] : V[i][2]);
-        v[2][i] = i2 == 0 ? V[i][0] : (i2 == 1 ? V[i][1] : V[i][2]);
-    }
-    const double dv = v[0][0] * (v[1][1] * v[2][2] - v[1][2] * v[2][1]) - v[0][1] * (v[1][0] * v[2][2] - v[1][2] * v[2][0]) +
-                      v[0][2] * (v[1][0] * v[2][1] - v[1][1] * v[2][0]);
-    if (dv < 0.0) { v[2][0] = -v[2][0]; v[2][1] = -v[2][1]; v[2][2] = -v[2][2]; }
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-        double nn = 0.0;
-#pragma unroll
-        for (int i = 0; i < 3; ++i) { u[k][i] = E[3 * i] * v[k][0] + E[3 * i + 1] * v[k][1] + E[3 * i + 2] * v[k][2]; nn += u[k][i] * u[k][i]; }
-        nn = sqrt(nn);
-#pragma unroll
-        for (int i = 0; i < 3; ++i) u[k][i] /= nn;
-    }
-    u[2][0] = u[0][1] * u[1][2] - u[0][2] * u[1][1];
-    u[2][1] = u[0][2] * u[1][0] - u[0][0] * u[1][2];
-    u[2][2] = u[0][0] * u[1][1] - u[0][1] * u[1][0];
+    double v[3][3], u[3][3], sv[2];             // v[k] = k-th right singular vector
+    svd3(E, u, v, sv);
     // U W V^T with W = [[0 1 0] [-1 0 0] [0 0 1]]: columns of U W are (-u1, u0, u2); of U W^T: (u1, -u0, u2)
 #pragma unroll
     for (int i = 0; i < 3; ++i)

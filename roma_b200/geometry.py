@@ -16,6 +16,13 @@ the final model.  Again only the stream of minimal samples differs (Philox4x32-1
 
     from roma_b200 import find_homography, RANSAC
     H, mask = find_homography(pos_a, pos_b, RANSAC, 3.0, confidence=0.99999)
+
+`find_fundamental` replaces the `cv2.findFundamentalMat(..., cv2.USAC_MAGSAC, ...)` call of the reference's usage example with
+MAGSAC++ over seven-point samples in `csrc/fundamental.cu`.  OpenCV's USAC internals are not restated; the estimator is defined
+in include/romab200.h and DESIGN.md and agrees with cv2 statistically.
+
+    from roma_b200 import find_fundamental, USAC_MAGSAC
+    F, mask = find_fundamental(kptsA, kptsB, ransacReprojThreshold=0.2, method=USAC_MAGSAC, confidence=0.999999, maxIters=10000)
 """
 from __future__ import annotations
 
@@ -239,3 +246,145 @@ def find_homography(srcPoints, dstPoints, method=0, ransacReprojThreshold=3, mas
     if not bool(ok[0]):
         return None, masks[0]
     return H[0], masks[0]
+
+
+# ---- fundamental matrices ------------------------------------------------------------------------------------------------
+USAC_MAGSAC = 38                # cv2.USAC_MAGSAC
+# include/romab200.h: RB_FUND_ROUND, RB_FUND_MODELS, RB_FUND_SLICE, RB_FUND_TABLE, RB_FUND_STATE
+FUND_ROUND, FUND_MODELS, FUND_SLICE, FUND_TABLE, FUND_STATE = 1024, 3, 512, 1024, 8
+# cv2's other findFundamentalMat methods, which are not restated here
+_FUND_UNSUPPORTED = {1: "FM_7POINT", 2: "FM_8POINT", 4: "FM_LMEDS", 8: "FM_RANSAC", 32: "USAC_DEFAULT", 33: "USAC_PARALLEL",
+                     34: "USAC_FM_8PTS", 35: "USAC_FAST", 36: "USAC_ACCURATE", 37: "USAC_PROSAC"}
+# MAGSAC++ with 4 degrees of freedom (a point correspondence) and sigma_max = ransacReprojThreshold: the loss reaches its outlier
+# value at k sigma_max, k^2 the 0.99 quantile of chi^2 with 4 degrees of freedom (include/romab200.h: RB_FUND_K2)
+MAGSAC_K2 = 13.276704135987622
+
+
+def _gamma_upper_3_2(x):
+    """Gamma(3/2, x), the upper incomplete gamma function (not regularised)."""
+    return math.sqrt(x) * math.exp(-x) + 0.5 * math.sqrt(math.pi) * math.erfc(math.sqrt(x))
+
+
+def _gamma_lower_5_2(x):
+    """gamma(5/2, x), the lower incomplete gamma function (not regularised)."""
+    return 0.75 * math.sqrt(math.pi) - (1.5 * _gamma_upper_3_2(x) + x * math.sqrt(x) * math.exp(-x))
+
+
+def magsac_tables():
+    """The MAGSAC++ loss and weight of a residual r at q = r^2 / (k sigma_max)^2 = i / FUND_TABLE, i = 0 .. FUND_TABLE: float64
+    [2, FUND_TABLE + 1].  With x = r^2 / (2 sigma_max^2) = q k^2 / 2 and x_k = k^2 / 2 (DESIGN.md):
+        loss(q)   = (gamma(5/2, x) + x (Gamma(3/2, x) - Gamma(3/2, x_k))) / gamma(5/2, x_k)     0 at r = 0, 1 at r = k sigma_max
+        weight(q) = (Gamma(3/2, x) - Gamma(3/2, x_k)) / (Gamma(3/2, 0) - Gamma(3/2, x_k))        1 at r = 0, 0 at r = k sigma_max
+    which are the paper's sigma-marginalised loss and weight, each divided by its value at the end of its range."""
+    xk = 0.5 * MAGSAC_K2
+    gk, lk = _gamma_upper_3_2(xk), _gamma_lower_5_2(xk)
+    g0 = 0.5 * math.sqrt(math.pi)
+    out = np.empty((2, FUND_TABLE + 1))
+    for i in range(FUND_TABLE + 1):
+        x = xk * i / FUND_TABLE
+        g = _gamma_upper_3_2(x)
+        out[0, i] = (_gamma_lower_5_2(x) + x * (g - gk)) / lk
+        out[1, i] = (g - gk) / (g0 - gk)
+    out[:, 0] = (0.0, 1.0)
+    out[:, -1] = (1.0, 0.0)
+    return out
+
+
+_TABLES = {}
+
+
+def _magsac_tables_on(dev):
+    """magsac_tables() on `dev`, uploaded once per device (so that a CUDA graph can capture the estimate)."""
+    if dev not in _TABLES:
+        _TABLES[dev] = torch.tensor(magsac_tables(), dtype=torch.float64, device=dev)
+    return _TABLES[dev]
+
+
+def _fund_points(p, dev):
+    """[N, 2] or [N, 1, 2] real points -> float64 [N, 2] on `dev`."""
+    t = p if isinstance(p, torch.Tensor) else torch.as_tensor(np.asarray(p))
+    if t.dim() == 3 and t.shape[1] == 1:
+        t = t[:, 0]
+    if t.dim() != 2 or t.shape[1] != 2:
+        raise ValueError(f"points must be [N, 2] or [N, 1, 2], got {tuple(t.shape)}")
+    if t.dtype.is_complex or t.dtype == torch.bool:
+        raise TypeError(f"points must be real numbers, got {t.dtype}")
+    return t.to(torch.float64).to(dev).contiguous()
+
+
+def _fund_args(method, thr, conf, max_iters):
+    """Mirrors cv2.findFundamentalMat's argument checks for USAC_MAGSAC; returns (threshold, confidence, maxIters)."""
+    method = int(method)
+    if method in _FUND_UNSUPPORTED:
+        raise NotImplementedError(f"find_fundamental implements USAC_MAGSAC only, not {_FUND_UNSUPPORTED[method]}")
+    if method != USAC_MAGSAC:
+        raise ValueError(f"unknown estimation method {method}")
+    thr, conf = float(thr), float(conf)
+    if not (math.isfinite(thr) and thr > 0):
+        raise ValueError(f"ransacReprojThreshold must be positive, got {thr}")
+    if not 0 < conf < 1:
+        raise ValueError(f"confidence must lie in (0, 1), got {conf}")
+    if int(max_iters) < 1:
+        raise ValueError(f"maxIters must be >= 1, got {max_iters}")
+    return thr, conf, int(max_iters)
+
+
+def _fund_launch(x0, x1, offsets, max_n, thr, conf, max_iters, seed):
+    """Enqueues the whole estimate on the current stream.  x0, x1: float64 [total, 2] device tensors, offsets: int64 [B + 1].
+    With max_iters <= FUND_ROUND this is one round and reads nothing back, so it can be captured in a CUDA graph; each further
+    round costs one 4-byte read of the `running` flag.  Returns the buffers (out_F, ok, mask, state, best_F, best_loss, norm, xn,
+    sample, nmod, F, counts, losses)."""
+    dev = x0.device
+    B = offsets.numel() - 1
+    total = x0.shape[0]
+    S = max(1, -(-int(max_n) // FUND_SLICE))
+    f64, i32 = dict(device=dev, dtype=torch.float64), dict(device=dev, dtype=torch.int32)
+    buf = dict(
+        norm=torch.empty(B, 6, **f64), xn=torch.empty(max(total, 1), 4, **f64), sample=torch.empty(B, FUND_ROUND, 7, **i32),
+        nmod=torch.empty(B, FUND_ROUND, **i32), F=torch.empty(B, FUND_ROUND, FUND_MODELS, 9, **f64),
+        counts=torch.empty(B, S, FUND_ROUND * FUND_MODELS, **i32), losses=torch.empty(B, S, FUND_ROUND * FUND_MODELS, **f64),
+        state=torch.zeros(B, FUND_STATE, **i32), best_F=torch.zeros(B, 9, **f64), best_loss=torch.zeros(B, **f64),
+        running=torch.zeros(1, **i32), out_F=torch.empty(B, 9, **f64), ok=torch.empty(B, device=dev, dtype=torch.uint8),
+        mask=torch.empty(max(total, 1), device=dev, dtype=torch.uint8))
+    kw = dict(batch=B, x0=x0, x1=x1, offsets=offsets, max_n=int(max_n), thresh=float(thr), conf=float(conf), max_iters=int(max_iters),
+              seed=int(seed) & (2 ** 64 - 1), round=0, table=_magsac_tables_on(dev), **buf)
+    _ransac_rounds("fund", "rb_fund_args", kw, FUND_ROUND)
+    cabi.call("romab200_fund_refine", "rb_fund_args", **kw)
+    return buf
+
+
+def find_fundamental_batched(points1_list, points2_list, method=USAC_MAGSAC, ransacReprojThreshold=3, confidence=0.99, maxIters=1000,
+                             *, seed=0):
+    """`find_fundamental` for B pairs in one launch set.  points*_list: B arrays / tensors [N_b, 2] or [N_b, 1, 2] (ragged N).
+    Every pair draws from the stream keyed by `seed` alone and nothing of pair b depends on the other pairs, so pair b is
+    bit-identical to `find_fundamental` of that pair alone.  Returns (F [B, 3, 3] float64, ok [B] bool, masks: list of uint8
+    [N_b, 1]); numpy inputs give numpy outputs, tensors give device tensors.  ok[b] is False, F[b] zero and the mask all zero
+    where `find_fundamental` returns None, and for pairs of fewer than 7 points."""
+    thr, conf, max_iters = _fund_args(method, ransacReprojThreshold, confidence, maxIters)
+    x0, x1, offsets, ns = _pack_pairs(points1_list, points2_list, _fund_points, "find_fundamental", ("points1_list", "points2_list"),
+                                      ("points1", "points2"))
+    buf = _fund_launch(x0, x1, offsets, max(ns), thr, conf, max_iters, seed)
+    masks = [m.view(-1, 1) for m in buf["mask"][:sum(ns)].split(ns)]
+    return _outputs(not isinstance(points1_list[0], torch.Tensor), buf["out_F"].view(len(ns), 3, 3), buf["ok"].bool(), masks)
+
+
+def find_fundamental(points1, points2, method=USAC_MAGSAC, ransacReprojThreshold=3, confidence=0.99, maxIters=1000, mask=None, *, seed=0):
+    """Drop-in for `cv2.findFundamentalMat` with method USAC_MAGSAC: the same keywords and return form.  points2^T F points1 = 0.
+    MAGSAC++ over seven-point samples (csrc/fundamental.cu, DESIGN.md): the best model by the sigma-marginalised loss with
+    sigma_max = ransacReprojThreshold, at most maxIters hypotheses (fewer as `confidence` allows, from the inlier ratio at
+    the threshold), then sigma-consensus++.  Returns (F float64 [3, 3], mask uint8 [N, 1]): F has unit Frobenius norm and its
+    largest-magnitude entry positive (cv2 fixes neither, so compare up to scale and sign); the mask holds the points whose Sampson
+    distance to F is below ransacReprojThreshold.  `mask` is accepted and ignored, as in cv2's Python binding.  numpy in gives
+    numpy out (float32 points are accepted); tensors give device tensors.
+    Rows with a NaN or infinite coordinate are never inliers and do not enter the normalisation; a sample that draws one gives no
+    model.  When no sample gives a model (all points identical, all on one line in both images, ...) the result is (None, all-zero
+    mask).  Raises ValueError for fewer than 7 points and NotImplementedError for every other cv2 method."""
+    del mask
+    thr, conf, max_iters = _fund_args(method, ransacReprojThreshold, confidence, maxIters)
+    n = len(points1)
+    if n < 7 or len(points2) != n:
+        raise ValueError(f"find_fundamental needs the same number (>= 7) of points in both images, got {n} and {len(points2)}")
+    F, ok, masks = find_fundamental_batched([points1], [points2], USAC_MAGSAC, thr, conf, max_iters, seed=seed)
+    if not bool(ok[0]):
+        return None, masks[0]
+    return F[0], masks[0]

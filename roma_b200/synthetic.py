@@ -336,7 +336,8 @@ def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, w
     """A seeded calibrated two-view scene for the pose estimator: focal lengths near 1200 px, a 5-20 degree rotation about a
     random axis, a unit baseline in a random direction, `n` points seen by camera 0 at depths 6-14, Gaussian pixel noise of
     `noise` px in both images, and a fraction `outlier_frac` of correspondences whose second point is uniform in image 1.
-    Returns float64 numpy arrays: kpts0, kpts1 [n, 2], K0, K1 [3, 3], R [3, 3], t [3] (x1 ~ K1 (R X + t))."""
+    Returns float64 numpy arrays: kpts0, kpts1 [n, 2], K0, K1 [3, 3], R [3, 3], t [3] (x1 ~ K1 (R X + t)), and outlier bool [n]
+    marking the replaced correspondences."""
     import numpy as np
 
     rng = np.random.default_rng(seed)
@@ -351,7 +352,7 @@ def two_view_scene(seed: int, n: int, outlier_frac: float, noise: float = 0.5, w
     kpts1 = x1[:, :2] / x1[:, 2:] + rng.normal(scale=noise, size=(n, 2))
     out = rng.random(n) < outlier_frac
     kpts1[out] = np.c_[rng.uniform(0, width, out.sum()), rng.uniform(0, height, out.sum())]
-    return {"kpts0": kpts0, "kpts1": kpts1, "K0": K0, "K1": K1, "R": R, "t": t}
+    return {"kpts0": kpts0, "kpts1": kpts1, "K0": K0, "K1": K1, "R": R, "t": t, "outlier": out}
 
 
 def depth_scene(seed: int, batch: int, h0: int, w0: int, h1: int = None, w1: int = None):
