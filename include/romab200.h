@@ -766,6 +766,59 @@ typedef struct {
 } rb_dense_geometric_dist_args;
 int romab200_dense_geometric_dist(const rb_dense_geometric_dist_args* args, void* stream);
 
+/* ---- structure-from-motion match graph: per-image keypoints and one-to-one pair matches from sampled dense matches ----
+ * Not in the reference (its users snap `sample()` output to pixels on the host).  For pair k = (i, j) = pairs[k] and sample s < n,
+ * side 0 is (u, v) = matches[k, s, 0:2] in image i and side 1 is matches[k, s, 2:4] in image j, both with certainty[k, s].  For an
+ * image of image_sizes[img] = (H, W): x = (W / 2) * (u + 1), y = (H / 2) * (v + 1), each operation rounded to fp32 (matcher.py:713-717);
+ * the side is ignored unless certainty > min_certainty (>= 0) and u, v and the certainty are finite.
+ * cell (cx, cy) = (min(max(floor(x), 0), W - 1) / cell_size, the same for y) (integer division), index cy * gw + cx with
+ * gw = ceil(W / cell_size), gh = ceil(H / cell_size).  The winner of a cell is the side landing in it with the largest certainty,
+ * ties to the smallest g = (k * n + s) * 2 + side; it gives the keypoint's position (x, y) and score.  Ids: occupied cells in raster
+ * order within each image.  Everything is exact and order-free (integer atomics on monotone keys only), so the result does not
+ * depend on timing or on how images and pairs are grouped.
+ *
+ * romab200_match_graph_keypoints: the images [img_begin, img_end) (one group) in one call.  cell_start / tile_start [num_images + 1]
+ * int64 are the cumulative cell and tile counts over all images (an image no pair references has none); the group's grid is
+ * grid_bits [cells] (uint32, the winning certainty's bits, then the cell's id) and grid_g [cells] (uint64, the winning g), cells =
+ * cell_start[img_end] - cell_start[img_begin] = grid_cells; tile_scan [grid_tiles + 1] int64, grid_tiles the same difference of
+ * tile_start (a tile is RB_MG_TILE consecutive cells of one image).  The caller passes the two extents it built the tables with.  kp_offsets [num_images + 1] int64: entry img_begin must hold the keypoints of the
+ * images before the group (0 for the first); the call writes entries img_begin + 1 .. img_end, and the keypoints [kp_capacity, 2],
+ * kp_scores [kp_capacity] of the group's images at those offsets.  sid [num_pairs, n, 2] int32 receives, for every side whose image
+ * is in the group, its keypoint id, or -1 when ignored.
+ *
+ * romab200_match_graph_count + romab200_match_graph_emit: the one-to-one matches of pairs [pair_begin, pair_end) from sid, one CTA
+ * per pair.  A sample is used iff both sides have an id (a, b).  best_b(a) = b of the used sample with that a of the largest
+ * certainty, ties to the smallest s; best_a(b) likewise; (a, best_b(a)) is kept iff best_a(best_b(a)) == a, with that certainty as
+ * its score, in ascending a.  A CTA sorts 64-bit keys three times (certainty rank, then (b, rank), then (a, rank)).  It needs
+ * pair_bytes = 8 * n2 + 5 * n rounded up to a multiple of 16 (n2 the smallest power of two >= n): shared memory when
+ * pair_bytes <= RB_MG_PAIR_SMEM, otherwise scratch of pair_bytes per pair of the call.
+ * count writes pair k's match count to match_offsets[k]; the call with pair_end == num_pairs then turns match_offsets [num_pairs + 1]
+ * into exclusive offsets with the total last.  emit (after the caller has sized the outputs) writes matches [match_capacity, 2]
+ * int32 (a, b) and match_scores at those offsets. */
+#define RB_MG_TILE 2048
+#define RB_MG_PAIR_SMEM 230400
+typedef struct {
+    const int64_t* pairs; int32_t num_pairs, n;
+    const float* matches; const float* certainty;
+    const int32_t* image_sizes; int32_t num_images, cell_size; float min_certainty;
+    const int64_t* cell_start; const int64_t* tile_start; int32_t img_begin, img_end;
+    uint32_t* grid_bits; uint64_t* grid_g; int64_t grid_cells;
+    int64_t* tile_scan; int64_t grid_tiles;
+    int64_t* kp_offsets; float* keypoints; float* kp_scores; int64_t kp_capacity;
+    int32_t* sid;
+} rb_match_graph_keypoints_args;
+int romab200_match_graph_keypoints(const rb_match_graph_keypoints_args* args, void* stream);
+
+typedef struct {
+    const int32_t* sid; const float* certainty; int32_t num_pairs, n;
+    int32_t pair_begin, pair_end;
+    uint8_t* scratch; int64_t scratch_bytes;
+    int64_t* match_offsets;
+    int32_t* matches; float* match_scores; int64_t match_capacity;   /* emit only */
+} rb_match_graph_pairs_args;
+int romab200_match_graph_count(const rb_match_graph_pairs_args* args, void* stream);
+int romab200_match_graph_emit(const rb_match_graph_pairs_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

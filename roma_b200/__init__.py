@@ -26,6 +26,9 @@ def __getattr__(name):
                 "find_fundamental_batched", "USAC_MAGSAC"):
         from . import geometry
         return getattr(geometry, name)
+    if name in ("consolidate_matches", "MatchGraph"):
+        from . import match_graph
+        return getattr(match_graph, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
         from . import depth_warp
         return getattr(depth_warp, name)

@@ -66,6 +66,9 @@ def _parse_header(path: str):
 
 
 STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
+# integer constants of the header that the host side sizes buffers with
+RB_MG_TILE, RB_MG_PAIR_SMEM = (int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+                               for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -157,6 +160,11 @@ _FIELD_DTYPES = {
     "rb_fund_args": {"x0": _F64, "x1": _F64, "offsets": torch.int64, "table": _F64, "norm": _F64, "xn": _F64, "sample": torch.int32,
                      "nmod": torch.int32, "F": _F64, "counts": torch.int32, "losses": _F64, "state": torch.int32, "best_F": _F64,
                      "best_loss": _F64, "running": torch.int32, "out_F": _F64, "ok": torch.uint8, "mask": torch.uint8},
+    "rb_match_graph_keypoints_args": {"pairs": torch.int64, "matches": _F32, "certainty": _F32, "image_sizes": torch.int32, "cell_start": torch.int64,
+                                      "tile_start": torch.int64, "grid_bits": torch.int32, "grid_g": torch.int64, "tile_scan": torch.int64,
+                                      "kp_offsets": torch.int64, "keypoints": _F32, "kp_scores": _F32, "sid": torch.int32},
+    "rb_match_graph_pairs_args": {"sid": torch.int32, "certainty": _F32, "scratch": torch.uint8, "match_offsets": torch.int64,
+                                  "matches": torch.int32, "match_scores": _F32},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -213,9 +221,23 @@ def _sample_gather_min_elems(kw):
     return {"matches": 4 * rows, "certainty": rows, "idx": items * k, "out_matches": 4 * items * k, "out_certainty": items * k}
 
 
+def _match_graph_keypoints_min_elems(kw):
+    sides, img = kw["num_pairs"] * kw["n"], kw["num_images"] + 1
+    return {"pairs": 2 * kw["num_pairs"], "matches": 4 * sides, "certainty": sides, "image_sizes": 2 * kw["num_images"], "cell_start": img,
+            "tile_start": img, "grid_bits": kw["grid_cells"], "grid_g": kw["grid_cells"], "tile_scan": kw["grid_tiles"] + 1, "kp_offsets": img,
+            "keypoints": 2 * kw["kp_capacity"], "kp_scores": kw["kp_capacity"], "sid": 2 * sides}
+
+
+def _match_graph_pairs_min_elems(kw):
+    sides, cap = kw["num_pairs"] * kw["n"], kw.get("match_capacity", 0)
+    return {"sid": 2 * sides, "certainty": sides, "scratch": kw.get("scratch_bytes", 0), "match_offsets": kw["num_pairs"] + 1,
+            "matches": 2 * cap, "match_scores": cap}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
-              "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems}
+              "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
+              "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -207,6 +207,45 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     return cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);
 }
 
+// In place: v[0..n) counts -> exclusive prefix sums, v[n] = total.  One CTA of 1024 threads, a contiguous chunk per thread.  A
+// template so that every translation unit that launches it carries its own copy.
+template <typename T>
+__global__ void __launch_bounds__(1024) scan_counts_kernel(T* __restrict__ v, int n) {
+    pdl_wait();
+    __shared__ T warp_tot[32];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const int per = (n + 1023) / 1024;
+    const int b = min(n, (int)threadIdx.x * per), e = min(n, b + per);
+    T s = 0;
+    for (int k = b; k < e; ++k) s += v[k];
+    T incl = s;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const T u = __shfl_up_sync(0xffffffffu, incl, d);
+        if (lane >= d) incl += u;
+    }
+    if (lane == 31) warp_tot[wid] = incl;
+    __syncthreads();
+    if (wid == 0) {
+        const T t = warp_tot[lane];
+        T wi = t;
+#pragma unroll
+        for (int d = 1; d < 32; d <<= 1) {
+            const T u = __shfl_up_sync(0xffffffffu, wi, d);
+            if (lane >= d) wi += u;
+        }
+        warp_tot[lane] = wi - t;
+    }
+    __syncthreads();
+    T run = warp_tot[wid] + incl - s;
+    for (int k = b; k < e; ++k) {
+        const T c = v[k];
+        v[k] = run;
+        run += c;
+    }
+    if (threadIdx.x == 1023) v[n] = run;
+}
+
 int gemm_simt(const rb_gemm_args* a, cudaStream_t stream, int lower_only = 0);
 int gemm_tc(const rb_gemm_args* a, cudaStream_t stream);
 int dwconv_tma(const rb_dwconv_args* a, cudaStream_t stream);     // dwconv_tma.cu: TMA-fed persistent depthwise kernel (16-bit maps)

@@ -10,7 +10,7 @@
 //   count    one thread per row: rows failing the certainty or the max_dist test are skipped, the others count the columns j
 //            with colmin[j] == rowmin[i] and D[i,j] == rowmin[i] (the two minimum conditions; D[i,j] is only evaluated on the
 //            rare column whose minimum equals the row's);
-//   scan     exclusive scan of the counts in one CTA -> offsets[0..n_a], offsets[n_a] = number of matches;
+//   scan     exclusive scan of the counts in one CTA (scan_counts_kernel) -> offsets[0..n_a], offsets[n_a] = number of matches;
 //   emit     the same sweep writes (i, j) at the row's offset, j ascending: the order of torch.nonzero.
 #include "common.cuh"
 #include "tma.cuh"
@@ -161,43 +161,6 @@ __global__ void __launch_bounds__(KP_THREADS) kp_pairs_kernel(const float* __res
     if (!EMIT) offsets[i] = c;
 }
 
-// in place: offsets[0..n) counts -> exclusive prefix sums, offsets[n] = total.  One CTA, a contiguous chunk per thread.
-__global__ void __launch_bounds__(1024) kp_scan_kernel(int64_t* __restrict__ offsets, int n) {
-    rb::pdl_wait();
-    __shared__ int64_t warp_tot[32];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    const int per = (n + 1023) / 1024;
-    const int b = min(n, (int)threadIdx.x * per), e = min(n, b + per);
-    int64_t s = 0;
-    for (int k = b; k < e; ++k) s += offsets[k];
-    int64_t incl = s;
-#pragma unroll
-    for (int d = 1; d < 32; d <<= 1) {
-        const int64_t v = __shfl_up_sync(0xffffffffu, incl, d);
-        if (lane >= d) incl += v;
-    }
-    if (lane == 31) warp_tot[wid] = incl;
-    __syncthreads();
-    if (wid == 0) {
-        const int64_t t = warp_tot[lane];
-        int64_t wi = t;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) {
-            const int64_t v = __shfl_up_sync(0xffffffffu, wi, d);
-            if (lane >= d) wi += v;
-        }
-        warp_tot[lane] = wi - t;
-    }
-    __syncthreads();
-    int64_t run = warp_tot[wid] + incl - s;
-    for (int k = b; k < e; ++k) {
-        const int64_t c = offsets[k];
-        offsets[k] = run;
-        run += c;
-    }
-    if (threadIdx.x == 1023) offsets[n] = run;
-}
-
 // slices of the other set for a min sweep over n_own points: enough CTAs to fill the GPU several times, at least one tile per slice
 static int kp_splits(int n_own, int n_other) {
     const int ctas = (n_own + KP_THREADS * KP_ROWS - 1) / (KP_THREADS * KP_ROWS);
@@ -247,7 +210,7 @@ extern "C" int romab200_keypoints_mnn_count(const rb_keypoints_mnn_args* a, void
     rb::launch_pdl(kp_pairs_kernel<false>, dim3((n_a + KP_THREADS - 1) / KP_THREADS), dim3(KP_THREADS), 0, st, a->x_A_to_B, a->cert_A, a->x_B,
                    (const float*)mins, (const float*)(mins + n_a), n_a, n_b, a->cert_th, a->max_dist, a->offsets, (int64_t*)nullptr, (int64_t*)nullptr);
     if (check_launch("keypoints_mnn_count(count)")) return 1;
-    rb::launch_pdl(kp_scan_kernel, dim3(1), dim3(1024), 0, st, a->offsets, n_a);
+    rb::launch_pdl(scan_counts_kernel<int64_t>, dim3(1), dim3(1024), 0, st, a->offsets, n_a);
     return check_launch("keypoints_mnn_count(scan)");
 }
 

@@ -222,6 +222,46 @@ class RegressionMatcher:
         with torch.cuda.device(eng.device):
             return self._match_pairs_device(images, images_high_res, plan, (hs, ws), (hu, wu), (ho, wout), on_batch)
 
+    @torch.inference_mode()
+    def match_graph(self, images, pairs, images_high_res=None, *, num=10000, cell_size=1, image_sizes=None, max_batch=8):
+        """Keypoints and one-to-one matches of an image set for a structure-from-motion back end, without holding dense warps: runs
+        `match_pairs(images, pairs, images_high_res, max_batch=max_batch)` chunk by chunk, draws `sample_batched(warp, certainty, num)`
+        from each chunk into one [P, k, 4] buffer, and returns `consolidate_matches(pairs, matches, certainty, image_sizes,
+        cell_size=cell_size)` (a `MatchGraph`).  After the same `torch.manual_seed` the result equals that loop written out by hand.
+
+        image_sizes [N, 2] (H, W) is the pixel frame of the keypoints; it defaults to each file's own size for paths (read from the
+        header) and PIL images, and is required for tensor images."""
+        from .match_graph import consolidate_matches
+        if not isinstance(num, int) or num < 1:
+            raise ValueError(f"match_graph: num must be a positive int, got {num!r}")
+        if isinstance(images, torch.Tensor):
+            if image_sizes is None:
+                raise ValueError("match_graph: image_sizes [N, 2] (H, W) is required for tensor images")
+            if images.dim() != 4:
+                raise ValueError(f"images must be [N, 3, h, w], got shape {tuple(images.shape)}")
+            n_images = images.shape[0]
+        else:
+            images = list(images)
+            n_images = len(images)
+            if image_sizes is None:
+                image_sizes = [_image_size(x) for x in images]
+        if len(image_sizes) != n_images:
+            raise ValueError(f"match_graph: image_sizes holds {len(image_sizes)} sizes for {n_images} images")
+        pairs = pair_tensor(pairs, n_images)
+        P, buf = pairs.shape[0], []
+
+        def on_batch(k0, warp, cert):
+            m, c = self.sample_batched(warp, cert, num)
+            if not buf:
+                buf.extend((torch.empty(P, m.shape[2], 4, device=m.device), torch.empty(P, m.shape[2], device=m.device)))
+            buf[0][k0:k0 + m.shape[0]].copy_(m[:, 0])
+            buf[1][k0:k0 + m.shape[0]].copy_(c[:, 0])
+
+        self.match_pairs(images, pairs, images_high_res, max_batch=max_batch, on_batch=on_batch)
+        if not buf:
+            buf = [torch.empty(0, 0, 4, device=self.engine.device), torch.empty(0, 0, device=self.engine.device)]
+        return consolidate_matches(pairs, buf[0], buf[1], image_sizes, cell_size=cell_size)
+
     def _match_pairs_device(self, images, images_high_res, plan, lo_res, hi_res, out_res, on_batch):
         eng = self.engine
         dev = eng.device
@@ -467,6 +507,18 @@ def pair_tensor(pairs, n_images: int) -> torch.Tensor:
         bad = t[(t < 0) | (t >= n_images)][0].item()
         raise IndexError(f"pairs holds image index {bad}, outside [0, {n_images})")
     return t
+
+
+def _image_size(x):
+    """(H, W) of a path (from the file header: `Image.open` is lazy) or of a PIL image."""
+    if isinstance(x, (str, os.PathLike)):
+        with Image.open(x) as im:
+            w, h = im.size
+    elif isinstance(x, Image.Image):
+        w, h = x.size
+    else:
+        raise ValueError(f"Unsupported input type: {type(x)!r}")
+    return h, w
 
 
 def plan_pairs(pairs: torch.Tensor, max_batch: int) -> dict:
