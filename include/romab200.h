@@ -819,6 +819,54 @@ typedef struct {
 int romab200_match_graph_count(const rb_match_graph_pairs_args* args, void* stream);
 int romab200_match_graph_emit(const rb_match_graph_pairs_args* args, void* stream);
 
+/* ---- feature tracks of a match graph: connected components of its keypoint matches ----
+ * Not in the reference.  The input is a match graph as consolidate_matches returns it, with pairs [num_pairs, 2] int64 (the pairs
+ * it was built from), kp_offsets [num_images + 1] int64, match_offsets [num_pairs + 1] int64, matches [num_matches, 2] int32 (a, b)
+ * and match_scores [num_matches] fp32.  The rules:
+ * 1. Vertices.  Row r of the keypoints is a vertex.  Keypoint a of image i has row r = kp_offsets[i] + a.  K = kp_offsets[N] =
+ *    num_rows, where N = num_images.
+ * 2. Edges.  Each match (a, b) of pair k = (i, j) whose match_scores value is > min_score joins row kp_offsets[i] + a to row
+ *    kp_offsets[j] + b.  The comparison is in fp32, with min_score rounded to fp32, so a NaN score is never an edge.  Repeated
+ *    pairs, reversed pairs and i == j pairs all just add edges.
+ * 3. Components.  Take the connected components of that graph on the K rows.  A component has a conflict when two distinct rows
+ *    in it belong to one image.  num_conflicting counts those components, whatever their size.
+ * 4. Tracks.  A component is a track when it has at least min_length rows (an int, at least 2) and has no conflict.  With
+ *    drop_conflicts = 0, conflicts are allowed, and the elements of a track may then repeat an image.
+ * 5. Order.  Tracks are numbered in ascending order of their smallest row.  The elements of a track are in ascending row order,
+ *    which is image ascending, then keypoint id ascending.  kp_track[r] is the track of row r, or -1.
+ * 6. Determinism.  The result is bit-identical from run to run, and it depends on no timing.
+ * Every match's ids are checked, 0 <= a < K_i and 0 <= b < K_j (K_i = kp_offsets[i + 1] - kp_offsets[i]), before any access that
+ * depends on them; an out-of-range match sets RB_TRACKS_BAD_ID in info[0] and is skipped.  A walk of parent pointers longer than
+ * K steps (which the invariant parent[r] <= r rules out) sets RB_TRACKS_WALK and stops.  The caller checks the offsets on the host:
+ * both start at 0 and do not decrease, pairs hold image indices < N, num_rows < 2^31, num_matches = match_offsets[num_pairs].
+ *
+ * romab200_tracks_link: parent[r] = r, then a lock-free union-find over the matches (path halving; a link is
+ * atomicCAS(&parent[larger root], larger root, smaller root), so the root of a component is its smallest row), then
+ * parent[r] = root(r) and size[root] = the component's size (integer atomics).  kp_track [num_rows] is set to -1.  The rows of
+ * components of at least 2 rows are counted per tile of RB_TRACKS_TILE rows into tile_scan [ceil(num_rows / RB_TRACKS_TILE) + 1]
+ * and scanned; info [5] int64 = {status, kept rows, T, E, num_conflicting} receives the status and the kept rows.
+ * romab200_tracks_build (after the caller has read info[0..1] and sized the buffers by num_kept = info[1] > 0): the kept rows in
+ * ascending order as keys (root << 32 | row), a stable LSD radix sort on the ceil(log2 num_rows) bits of the root in 8-bit digits
+ * (keys and keys_alt [num_kept] uint64, hist [256 * ceil(num_kept / RB_TRACKS_TILE) + 1] int32), the conflict flags (bit 31 of
+ * size[root]), then track_offsets [T + 1] int64 (capacity num_kept / 2 + 1), elements [E, 2] int32 (image, keypoint id; capacity
+ * num_kept) and kp_track, and info[2..4].  tile_scan is reused for the sorted tiles.  Workspace: 8 bytes per row (parent, size),
+ * 16.25 bytes per kept row, 8 bytes per tile. */
+#define RB_TRACKS_TILE 4096
+#define RB_TRACKS_BAD_ID 1
+#define RB_TRACKS_WALK 2
+typedef struct {
+    const int64_t* pairs; int32_t num_pairs, num_images;
+    const int64_t* kp_offsets; int32_t num_rows;
+    const int64_t* match_offsets; const int32_t* matches; const float* match_scores; int64_t num_matches;
+    float min_score; int32_t min_length, drop_conflicts;
+    int32_t* parent; int32_t* size; int64_t* tile_scan; int64_t* info; int32_t* kp_track;
+    int64_t num_kept;                                                   /* build only: */
+    uint64_t* keys; uint64_t* keys_alt; int32_t* hist;
+    int64_t* track_offsets; int32_t* elements;
+} rb_tracks_args;
+int romab200_tracks_link(const rb_tracks_args* args, void* stream);
+int romab200_tracks_build(const rb_tracks_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,6 +29,9 @@ def __getattr__(name):
     if name in ("consolidate_matches", "MatchGraph"):
         from . import match_graph
         return getattr(match_graph, name)
+    if name in ("build_tracks", "Tracks"):
+        from . import tracks
+        return getattr(tracks, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
         from . import depth_warp
         return getattr(depth_warp, name)

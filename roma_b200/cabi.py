@@ -67,8 +67,9 @@ def _parse_header(path: str):
 
 STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
 # integer constants of the header that the host side sizes buffers with
-RB_MG_TILE, RB_MG_PAIR_SMEM = (int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
-                               for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM"))
+RB_MG_TILE, RB_MG_PAIR_SMEM, RB_TRACKS_TILE, RB_TRACKS_BAD_ID, RB_TRACKS_WALK = (
+    int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+    for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM", "RB_TRACKS_TILE", "RB_TRACKS_BAD_ID", "RB_TRACKS_WALK"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -165,6 +166,9 @@ _FIELD_DTYPES = {
                                       "kp_offsets": torch.int64, "keypoints": _F32, "kp_scores": _F32, "sid": torch.int32},
     "rb_match_graph_pairs_args": {"sid": torch.int32, "certainty": _F32, "scratch": torch.uint8, "match_offsets": torch.int64,
                                   "matches": torch.int32, "match_scores": _F32},
+    "rb_tracks_args": {"pairs": torch.int64, "kp_offsets": torch.int64, "match_offsets": torch.int64, "matches": torch.int32, "match_scores": _F32,
+                       "parent": torch.int32, "size": torch.int32, "tile_scan": torch.int64, "info": torch.int64, "kp_track": torch.int32,
+                       "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32, "track_offsets": torch.int64, "elements": torch.int32},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -234,10 +238,18 @@ def _match_graph_pairs_min_elems(kw):
             "matches": 2 * cap, "match_scores": cap}
 
 
+def _tracks_min_elems(kw):
+    K, kept, tile = kw["num_rows"], kw.get("num_kept", 0), RB_TRACKS_TILE
+    return {"pairs": 2 * kw["num_pairs"], "kp_offsets": kw["num_images"] + 1, "match_offsets": kw["num_pairs"] + 1, "matches": 2 * kw["num_matches"],
+            "match_scores": kw["num_matches"], "parent": K, "size": K, "tile_scan": (K + tile - 1) // tile + 1, "info": 5, "kp_track": K,
+            "keys": kept, "keys_alt": kept, "hist": 256 * ((kept + tile - 1) // tile) + 1, "track_offsets": kept // 2 + 1, "elements": 2 * kept}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
-              "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems}
+              "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
+              "rb_tracks_args": _tracks_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -465,3 +465,77 @@ def homography_auc(errors, thresholds=(3, 5, 10)):
         e = np.r_[errors[:last], th]
         out.append(float(np.trapezoid(r, x=e) / th))
     return out
+
+
+def planted_views(seed: int, n_images: int, n_points: int, *, size=(768, 1024), cell_size: int = 1, visibility: float = 0.5,
+                  outlier_frac: float = 0.0, device="cpu"):
+    """Seeded multi-view samples with planted tracks, for `consolidate_matches` and `build_tracks`.  Each of `n_images` images of
+    `size` (H, W) sees each of `n_points` scene points with probability `visibility`, at a cell of `cell_size` px of its own (the
+    points take distinct cells in every image).  Every pair (i, j), i < j, of the exhaustive graph gets one sample per point both
+    images see: each side at its cell's centre plus uniform noise of up to a quarter cell, drawn per sample, with certainty in
+    [0.5, 1).  On top of a pair's m such samples come round(m * outlier_frac / (1 - outlier_frac)) outliers, so that a fraction
+    `outlier_frac` of its samples are outliers: both sides uniform in their images, certainty in [0.05, 0.5).  Pairs with fewer
+    samples than the largest are padded with certainty 0, which consolidate_matches ignores.
+    Returns, on `device`: pairs [P, 2] int64, matches [P, n, 4] fp32 (normalised (xA, yA, xB, yB), as sample_batched returns them),
+    certainty [P, n] fp32, image_sizes [N, 2] int64, and views [n_points, N] int64, the cell cy * gw + cx of each point in each
+    image (gw = ceil(W / cell_size)), -1 where the image does not see it."""
+    H, W = size
+    cs = int(cell_size)
+    gh, gw = -(-H // cs), -(-W // cs)
+    if n_points > gh * gw:
+        raise ValueError(f"planted_views: {n_points} points do not fit in {gh * gw} cells")
+    g = torch.Generator(device=device).manual_seed(seed)
+    vis = torch.rand(n_images, n_points, generator=g, device=device) < visibility
+    cells = torch.stack([torch.randperm(gh * gw, generator=g, device=device)[:n_points] for _ in range(n_images)])
+    pairs = torch.triu_indices(n_images, n_images, 1, device=device).T.contiguous()
+    P = pairs.shape[0]
+    co = vis[pairs[:, 0]] & vis[pairs[:, 1]]
+    n_in = co.sum(1)
+    n_out = torch.round(n_in * (outlier_frac / (1.0 - outlier_frac))).long() if outlier_frac > 0 else torch.zeros_like(n_in)
+    n = int((n_in + n_out).max()) if P else 0
+    matches = torch.zeros(P, n, 4, device=device)
+    certainty = torch.zeros(P, n, device=device)
+
+    def start(counts):
+        return torch.cumsum(counts, 0) - counts
+
+    def side(cell, count):
+        """Normalised (u, v) of `count` positions in the given cells: the centre of the cell's pixels plus uniform noise."""
+        lo_x, lo_y = (cell % gw) * cs, (cell // gw) * cs
+        hi_x, hi_y = torch.clamp(lo_x + cs, max=W), torch.clamp(lo_y + cs, max=H)
+        noise = torch.rand(count, 2, generator=g, device=device, dtype=torch.float64) - 0.5
+        x = (lo_x + hi_x) / 2 + (hi_x - lo_x) * noise[:, 0] / 2
+        y = (lo_y + hi_y) / 2 + (hi_y - lo_y) * noise[:, 1] / 2
+        return torch.stack((2 * x / W - 1, 2 * y / H - 1), 1).float()
+
+    k, p = co.nonzero(as_tuple=True)
+    slot = torch.arange(k.numel(), device=device) - start(n_in)[k]
+    matches[k, slot, 0:2] = side(cells[pairs[k, 0], p], k.numel())
+    matches[k, slot, 2:4] = side(cells[pairs[k, 1], p], k.numel())
+    certainty[k, slot] = 0.5 + 0.5 * torch.rand(k.numel(), generator=g, device=device)
+    k = torch.repeat_interleave(torch.arange(P, device=device), n_out)
+    slot = n_in[k] + torch.arange(k.numel(), device=device) - start(n_out)[k]
+    matches[k, slot] = torch.rand(k.numel(), 4, generator=g, device=device) * 2 - 1
+    certainty[k, slot] = 0.05 + 0.45 * torch.rand(k.numel(), generator=g, device=device)
+    sizes = torch.tensor([[H, W]] * n_images, dtype=torch.int64, device=device)
+    return pairs, matches, certainty, sizes, torch.where(vis, cells, -1).T.contiguous()
+
+
+def planted_tracks(views, min_length: int = 2):
+    """The planted tracks of `planted_views` with at least `min_length` views, as a set of tuples ((image, cell), ...) in image order."""
+    v = views.cpu().numpy()
+    return {tuple((i, int(c)) for i, c in enumerate(row) if c >= 0) for row in v if (row >= 0).sum() >= min_length}
+
+
+def track_cells(track_offsets, elements, kp_offsets, keypoints, width: int, cell_size: int = 1):
+    """Tracks (offsets and (image, keypoint id) elements) as the tuples of `planted_tracks`: each element's keypoint mapped to its
+    cell, for images `width` px wide."""
+    import numpy as np
+
+    off, el = track_offsets.cpu().numpy(), elements.cpu().numpy().astype(np.int64)
+    kp, kpo = keypoints.cpu().numpy(), kp_offsets.cpu().numpy()
+    xy = kp[kpo[el[:, 0]] + el[:, 1]] if el.size else np.zeros((0, 2), np.float32)
+    gw = -(-width // cell_size)
+    cell = (np.floor(xy[:, 1]).astype(np.int64) // cell_size) * gw + np.floor(xy[:, 0]).astype(np.int64) // cell_size
+    pairs = list(zip(el[:, 0].tolist(), cell.tolist()))
+    return {tuple(pairs[off[t]:off[t + 1]]) for t in range(len(off) - 1)}
