@@ -867,6 +867,65 @@ typedef struct {
 int romab200_tracks_link(const rb_tracks_args* args, void* stream);
 int romab200_tracks_build(const rb_tracks_args* args, void* stream);
 
+/* ---- geometric verification of a match graph: a MAGSAC++ fundamental matrix per pair, only its inlier matches kept ----
+ * Not in the reference.  The input is a match graph as consolidate_matches returns it (kp_offsets [num_images + 1] int64, keypoints
+ * [K, 2] fp32, match_offsets [num_pairs + 1] int64, matches [num_matches, 2] int32, match_scores [num_matches] fp32) with the pairs
+ * [num_pairs, 2] int64 it was built from.  The rules:
+ * 1. Points.  Pair k = (i, j) has matches (a, b).  Its points are x0 = keypoints[kp_offsets[i] + a] and x1 = keypoints[kp_offsets[j] + b],
+ *    widened exactly to float64, in match order.
+ * 2. Estimate.  F, ok and the per-match mask are what find_fundamental_batched([x0], [x1], USAC_MAGSAC, threshold, confidence,
+ *    max_iters, seed=seed) returns for that pair.  The Philox counter of fundamental.cu does not name the pair, so every pair draws
+ *    the stream keyed by seed alone.  Pair k is therefore bit-identical to that single call, whatever the chunking and pair order.
+ *    Pairs with fewer than 7 matches get ok = 0.
+ * 3. Accept.  num_inliers[k] is the sum of the mask.  accepted[k] = ok[k] and num_inliers[k] >= min_inliers.
+ * 4. Output.  For an accepted pair, keep the matches whose mask is 1, in their original order (ascending a), with their scores
+ *    unchanged.  A rejected pair keeps no matches.  match_offsets keeps num_pairs + 1 entries, so pair indices do not change.
+ * 5. No special cases.  i == j and repeated pairs get exactly what rule 2 gives.
+ * 6. Determinism.  Integer work only outside the estimator.  The result is bit-identical from run to run, for any workspace_bytes
+ *    and under any pair order.
+ * Every match's ids are checked, 0 <= a < K_i and 0 <= b < K_j, before any access that depends on them; an out-of-range match sets
+ * RB_VERIFY_BAD_ID in info[0].  The caller checks the offsets on the host (both start at 0 and do not decrease, pairs hold image
+ * indices < num_images, num_matches = match_offsets[num_pairs]).
+ *
+ * romab200_verify_check: every match's ids; info [2] int64 = {status, kept matches} is zeroed first.  The caller reads info[0] and
+ *   launches no estimator when it is set.
+ * romab200_verify_gather: the pairs [pair_begin, pair_end) of one chunk, whose matches are [match_offsets[pair_begin],
+ *   match_offsets[pair_end]): x0, x1 [max(total, 1), 2] float64 (rule 1; zero for a bad id) and chunk_offsets [pair_end - pair_begin
+ *   + 1] int64, starting at 0: the x0 / x1 / offsets layout of rb_fund_args.  The estimator then runs on the chunk (romab200_fund_*).
+ *   Its device bytes, with B pairs, total matches and S = max(1, ceil(max_n / RB_FUND_SLICE)) score slices (max_n the chunk's
+ *   largest pair), are the buffers it allocates plus the gathered points:
+ *     B (RB_VERIFY_PAIR_BYTES + RB_VERIFY_SLICE_BYTES S) + RB_VERIFY_POINT_BYTES max(total, 1) + RB_VERIFY_CHUNK_BYTES
+ *   per pair norm 48, sample 28 672, nmod 4 096, F 221 184, state 32, best_F 72, best_loss 8, out_F 72, ok 1, chunk_offsets 8;
+ *   per pair and slice counts 12 288 and losses 24 576; per match xn 32, mask 1, x0 16, x1 16; once running 4 and chunk_offsets 8.
+ * romab200_verify_count (after every chunk's F, ok and mask are in the whole-call ok [num_pairs] uint8 and mask [num_matches]
+ *   uint8): one CTA per pair sums its mask (integers) into num_inliers [num_pairs] int64 and sets accepted [num_pairs] uint8 (rule 3);
+ *   out_offsets [num_pairs + 1] int64 becomes the exclusive scan of the kept counts (num_inliers where accepted, else 0), total
+ *   last; the kept matches (mask set and pair accepted) are counted per tile of RB_VERIFY_TILE matches into tile_scan
+ *   [ceil(num_matches / RB_VERIFY_TILE) + 1] and scanned; info[1] = the total.
+ * romab200_verify_emit (after the caller has sized the outputs by num_kept = info[1] > 0): out_matches [num_kept, 2] int32 and
+ *   out_scores [num_kept] fp32, the kept matches in their original order (rule 4). */
+#define RB_VERIFY_TILE 4096
+#define RB_VERIFY_BAD_ID 1
+#define RB_VERIFY_PAIR_BYTES 254193
+#define RB_VERIFY_SLICE_BYTES 36864
+#define RB_VERIFY_POINT_BYTES 65
+#define RB_VERIFY_CHUNK_BYTES 12
+typedef struct {
+    const int64_t* pairs; int32_t num_pairs, num_images;
+    const int64_t* kp_offsets; const float* keypoints; int64_t num_rows;
+    const int64_t* match_offsets; const int32_t* matches; const float* match_scores; int64_t num_matches;
+    int64_t* info;
+    int32_t pair_begin, pair_end;                                       /* gather only: */
+    double* x0; double* x1; int64_t* chunk_offsets;
+    const uint8_t* ok; const uint8_t* mask; int64_t min_inliers;        /* count and emit: */
+    int64_t* num_inliers; uint8_t* accepted; int64_t* tile_scan; int64_t* out_offsets;
+    int64_t num_kept; int32_t* out_matches; float* out_scores;          /* emit only */
+} rb_verify_args;
+int romab200_verify_check(const rb_verify_args* args, void* stream);
+int romab200_verify_gather(const rb_verify_args* args, void* stream);
+int romab200_verify_count(const rb_verify_args* args, void* stream);
+int romab200_verify_emit(const rb_verify_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -67,9 +67,11 @@ def _parse_header(path: str):
 
 STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
 # integer constants of the header that the host side sizes buffers with
-RB_MG_TILE, RB_MG_PAIR_SMEM, RB_TRACKS_TILE, RB_TRACKS_BAD_ID, RB_TRACKS_WALK = (
+(RB_MG_TILE, RB_MG_PAIR_SMEM, RB_TRACKS_TILE, RB_TRACKS_BAD_ID, RB_TRACKS_WALK, RB_VERIFY_TILE, RB_VERIFY_BAD_ID, RB_VERIFY_PAIR_BYTES,
+ RB_VERIFY_SLICE_BYTES, RB_VERIFY_POINT_BYTES, RB_VERIFY_CHUNK_BYTES) = (
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
-    for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM", "RB_TRACKS_TILE", "RB_TRACKS_BAD_ID", "RB_TRACKS_WALK"))
+    for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM", "RB_TRACKS_TILE", "RB_TRACKS_BAD_ID", "RB_TRACKS_WALK", "RB_VERIFY_TILE", "RB_VERIFY_BAD_ID",
+                 "RB_VERIFY_PAIR_BYTES", "RB_VERIFY_SLICE_BYTES", "RB_VERIFY_POINT_BYTES", "RB_VERIFY_CHUNK_BYTES"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -169,6 +171,10 @@ _FIELD_DTYPES = {
     "rb_tracks_args": {"pairs": torch.int64, "kp_offsets": torch.int64, "match_offsets": torch.int64, "matches": torch.int32, "match_scores": _F32,
                        "parent": torch.int32, "size": torch.int32, "tile_scan": torch.int64, "info": torch.int64, "kp_track": torch.int32,
                        "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32, "track_offsets": torch.int64, "elements": torch.int32},
+    "rb_verify_args": {"pairs": torch.int64, "kp_offsets": torch.int64, "keypoints": _F32, "match_offsets": torch.int64, "matches": torch.int32,
+                       "match_scores": _F32, "info": torch.int64, "x0": _F64, "x1": _F64, "chunk_offsets": torch.int64, "ok": torch.uint8,
+                       "mask": torch.uint8, "num_inliers": torch.int64, "accepted": torch.uint8, "tile_scan": torch.int64,
+                       "out_offsets": torch.int64, "out_matches": torch.int32, "out_scores": _F32},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -245,11 +251,21 @@ def _tracks_min_elems(kw):
             "keys": kept, "keys_alt": kept, "hist": 256 * ((kept + tile - 1) // tile) + 1, "track_offsets": kept // 2 + 1, "elements": 2 * kept}
 
 
+def _verify_min_elems(kw):
+    P, M, kept, tiles = kw["num_pairs"], kw["num_matches"], kw.get("num_kept", 0), (kw["num_matches"] + RB_VERIFY_TILE - 1) // RB_VERIFY_TILE
+    out = {"pairs": 2 * P, "kp_offsets": kw["num_images"] + 1, "keypoints": 2 * kw["num_rows"], "match_offsets": P + 1, "matches": 2 * M,
+           "match_scores": M, "info": 2, "ok": P, "mask": M, "num_inliers": P, "accepted": P, "tile_scan": tiles + 1, "out_offsets": P + 1,
+           "out_matches": 2 * kept, "out_scores": kept}
+    if "chunk_offsets" in kw:
+        out["chunk_offsets"] = kw["pair_end"] - kw["pair_begin"] + 1
+    return out
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
-              "rb_tracks_args": _tracks_min_elems}
+              "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -487,6 +487,14 @@ def planted_views(seed: int, n_images: int, n_points: int, *, size=(768, 1024), 
     g = torch.Generator(device=device).manual_seed(seed)
     vis = torch.rand(n_images, n_points, generator=g, device=device) < visibility
     cells = torch.stack([torch.randperm(gh * gw, generator=g, device=device)[:n_points] for _ in range(n_images)])
+    return _planted_samples(g, vis, cells, H, W, cs, outlier_frac, device)
+
+
+def _planted_samples(g, vis, cells, H, W, cs, outlier_frac, device):
+    """The samples of `planted_views` from g's stream for points seen where vis [N, n_points] is set, at cells [N, n_points] of cs px:
+    returns (pairs, matches, certainty, image_sizes, views)."""
+    n_images = vis.shape[0]
+    gw = -(-W // cs)
     pairs = torch.triu_indices(n_images, n_images, 1, device=device).T.contiguous()
     P = pairs.shape[0]
     co = vis[pairs[:, 0]] & vis[pairs[:, 1]]
@@ -519,6 +527,60 @@ def planted_views(seed: int, n_images: int, n_points: int, *, size=(768, 1024), 
     certainty[k, slot] = 0.05 + 0.45 * torch.rand(k.numel(), generator=g, device=device)
     sizes = torch.tensor([[H, W]] * n_images, dtype=torch.int64, device=device)
     return pairs, matches, certainty, sizes, torch.where(vis, cells, -1).T.contiguous()
+
+
+def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024), cell_size: int = 1, noise: float = 0.5,
+                    visibility: float = 0.5, outlier_frac: float = 0.0, device="cpu"):
+    """Seeded multi-view samples of a real scene, for geometric verification (`verify_matches`): `planted_views` with geometry.  A
+    cloud of `n_points` scene points fills a 8 x 6 x 6 box around the origin; `n_images` pinhole cameras of `size` (H, W) with the
+    intrinsics of `_scene_intrinsics` stand 8-10 units from the origin at azimuths of -40..40 degrees and heights of -1..1 and look at
+    a point near the origin, so depths vary from about 5 to 13 and no pair's F is degenerate.  A point's observed position in an
+    image is its projection plus Gaussian noise of `noise` px, drawn once per (point, image), so every pair puts the point in the same
+    cell.  The observation is dropped when it lies outside the image or behind the camera, when a draw with probability
+    `visibility` fails, or when its cell (the fp32 rule of `consolidate_matches` applied to the normalised coordinates) is already
+    taken by a lower-indexed point.  Samples, outliers, certainties and padding are those of `planted_views` for these cells.
+    Returns, on `device`: what `planted_views` returns (pairs, matches, certainty, image_sizes, views), then K [N, 3, 3], R [N, 3, 3]
+    and t [N, 3] float64 (x ~ K (R X + t)) and X [n_points, 3] float64."""
+    import numpy as np
+
+    H, W = size
+    cs = int(cell_size)
+    gw = -(-W // cs)
+    rng = np.random.default_rng(seed)
+    X = rng.uniform(-1.0, 1.0, (n_points, 3)) * np.array([4.0, 3.0, 3.0])
+    K = np.stack([_scene_intrinsics(rng, W, H) for _ in range(n_images)])
+    az = np.deg2rad(rng.uniform(-40.0, 40.0, n_images))
+    r, h = rng.uniform(8.0, 10.0, n_images), rng.uniform(-1.0, 1.0, n_images)
+    C = np.stack((r * np.sin(az), h, -r * np.cos(az)), 1)
+    target = rng.uniform(-0.5, 0.5, (n_images, 3))
+    R = np.empty((n_images, 3, 3))
+    for c in range(n_images):
+        z = (target[c] - C[c]) / np.linalg.norm(target[c] - C[c])
+        x = np.cross([0.0, 1.0, 0.0], z)
+        x /= np.linalg.norm(x)
+        R[c] = np.stack((x, np.cross(z, x), z))
+    t = -np.einsum("cij,cj->ci", R, C)
+    p = np.einsum("cij,cjk,pk->cpi", K, R, X) + np.einsum("cij,cj->ci", K, t)[:, None]        # [N, n_points, 3]
+    depth = p[..., 2]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        xy = p[..., :2] / depth[..., None] + rng.normal(scale=noise, size=(n_images, n_points, 2))
+    vis = (depth > 0) & (xy[..., 0] >= 0) & (xy[..., 0] < W) & (xy[..., 1] >= 0) & (xy[..., 1] < H)
+    vis &= rng.random((n_images, n_points)) < visibility
+    u = np.where(vis, 2 * xy[..., 0] / W - 1, 0.0).astype(np.float32)
+    v = np.where(vis, 2 * xy[..., 1] / H - 1, 0.0).astype(np.float32)
+    px = np.float32(W / 2) * (u + np.float32(1))
+    py = np.float32(H / 2) * (v + np.float32(1))
+    cx = np.clip(np.floor(px), 0, W - 1).astype(np.int64) // cs
+    cy = np.clip(np.floor(py), 0, H - 1).astype(np.int64) // cs
+    cells = cy * gw + cx
+    for c in range(n_images):
+        seen = np.flatnonzero(vis[c])
+        first = np.zeros(n_points, bool)
+        first[seen[np.unique(cells[c, seen], return_index=True)[1]]] = True
+        vis[c] &= first
+    g = torch.Generator(device=device).manual_seed(seed)
+    out = _planted_samples(g, torch.from_numpy(vis).to(device), torch.from_numpy(cells).to(device), H, W, cs, outlier_frac, device)
+    return out + tuple(torch.from_numpy(a).to(device) for a in (K, R, t, X))
 
 
 def planted_tracks(views, min_length: int = 2):
