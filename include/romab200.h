@@ -926,6 +926,58 @@ int romab200_verify_gather(const rb_verify_args* args, void* stream);
 int romab200_verify_count(const rb_verify_args* args, void* stream);
 int romab200_verify_emit(const rb_verify_args* args, void* stream);
 
+/* ---- triangulation of feature tracks with known cameras: two-view RANSAC over each track's observations, multi-view refinement,
+ *      reprojection and angle filters ----
+ * Not in the reference.  The input is a match graph's kp_offsets [num_images + 1] int64 and keypoints [K, 2] fp32, the tracks built
+ * from it (track_offsets [num_tracks + 1] int64, elements [num_elements, 2] int32 (image, keypoint id)) and per image i a camera
+ * x ~ K_i (R_i X + t_i) in pixels.  All arithmetic is float64.  The rules:
+ * 1. Observations.  Element (i, a) of track k is observed at x = keypoints[kp_offsets[i] + a], widened to float64.  The host builds a
+ *    float64 camera table once: P_i = K_i [R_i | t_i] and C_i = -R_i^T t_i.  An observation's depth is (R_i X + t_i)_z.
+ * 2. Hypotheses.  Let the track have L elements.  If L (L - 1) / 2 <= max_hypotheses, take every pair p < q in lexicographic order.
+ *    Otherwise take max_hypotheses pairs: pair h is the two distinct indices in [0, L) that ransac_draw<2> gives under key seed and
+ *    counter (h, s, k, RB_TRI_CTR), s = 0, 1, ..., in the order drawn.  A pair whose two elements share an image is skipped but keeps
+ *    its index h (this can only happen with drop_conflicts = 0).
+ * 3. Two-view point.  Triangulate each pair by DLT: the point is the eigenvector of the smallest eigenvalue of the 4 x 4 A^T A, where
+ *    A has rows x P^3 - P^1 and y P^3 - P^2 per observation (P^r row r of P), dehomogenised.  The hypothesis is skipped if the point
+ *    is not finite or either depth is <= 0.
+ * 4. Support.  Element e is an inlier of X when its depth is > 0 and |pi(P_i X) - x_e|^2 <= max_error^2 (pi(p) = (p_0 / p_2,
+ *    p_1 / p_2)).  The best hypothesis has the most inliers, ties to the smallest h.  If no hypothesis has 2 inliers, the track is
+ *    not ok.
+ * 5. Refine.  A multi-view DLT over the best hypothesis's inliers (the same rows, summed over them; the hypothesis's own point is
+ *    kept if it is not finite), then Gauss-Newton on their summed squared reprojection error: at most RB_TRI_GN_ITERS steps, a step
+ *    kept only if it lowers the cost, stopping at the first rejected step.  Then the inlier set is recomputed once against the
+ *    refined X by rule 4.
+ * 6. Accept.  A track is ok when it has at least 2 inliers in distinct images and the largest angle between X - C_i and X - C_j over
+ *    its inlier pairs in distinct images (atan2(|a x b|, a . b)) is >= min_angle (radians, min_angle_deg pi / 180 on the host).
+ * 7. Determinism.  The result is bit-identical from run to run: no float atomics, every reduction in a fixed order.
+ * Outputs, zero where the track is not ok: X [num_tracks, 3], num_inliers [num_tracks] int32, error [num_tracks] (the mean
+ * reprojection error in px of the inliers), inlier [num_elements] uint8; ok [num_tracks] uint8.
+ * Every element's ids are checked, 0 <= i < num_images and 0 <= a < K_i, before any access that depends on them; a bad element sets
+ * RB_TRI_BAD_ID in info[0] (zeroed by the call) and its track is left not ok.  The caller checks on the host: track_offsets start at 0,
+ * never decrease and end at num_elements < 2^31; kp_offsets likewise; the cameras are finite; max_error2 > 0; 1 <= max_hypotheses.
+ *
+ * romab200_triangulate: one warp per track.  The lanes split the hypotheses (lane l takes h = l, l + 32, ...), each solving its DLT
+ * by cyclic Jacobi (10 sweeps); the best is the warp maximum of (count << 32) | ~h.  The refinement sums the 4 x 4 DLT matrix, the
+ * 3 x 3 normal equations and the cost over the lanes (each lane its elements e = l, l + 32, ... in order, then a xor butterfly);
+ * the lanes split the angle test over the inlier pairs.  Observations are read through global memory, so any L is supported.
+ * cameras [num_images, RB_TRI_CAM] float64 per image: P (12, row-major), row 2 of R (3), t_z, C (3), unused. */
+#define RB_TRI_CTR 0x54524900u
+#define RB_TRI_GN_ITERS 10
+#define RB_TRI_CAM 20
+#define RB_TRI_BAD_ID 1
+typedef struct {
+    int32_t num_tracks, num_images;
+    const int64_t* track_offsets; const int32_t* elements; int64_t num_elements;
+    const int64_t* kp_offsets; const float* keypoints; int64_t num_rows;
+    const double* cameras;
+    double max_error2, min_angle;
+    int32_t max_hypotheses;
+    uint64_t seed;
+    int64_t* info;                                                      /* [1] status */
+    double* X; uint8_t* ok; int32_t* num_inliers; double* error; uint8_t* inlier;
+} rb_tri_args;
+int romab200_triangulate(const rb_tri_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -68,10 +68,12 @@ def _parse_header(path: str):
 STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
 # integer constants of the header that the host side sizes buffers with
 (RB_MG_TILE, RB_MG_PAIR_SMEM, RB_TRACKS_TILE, RB_TRACKS_BAD_ID, RB_TRACKS_WALK, RB_VERIFY_TILE, RB_VERIFY_BAD_ID, RB_VERIFY_PAIR_BYTES,
- RB_VERIFY_SLICE_BYTES, RB_VERIFY_POINT_BYTES, RB_VERIFY_CHUNK_BYTES) = (
+ RB_VERIFY_SLICE_BYTES, RB_VERIFY_POINT_BYTES, RB_VERIFY_CHUNK_BYTES, RB_TRI_GN_ITERS, RB_TRI_CAM, RB_TRI_BAD_ID) = (
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
     for name in ("RB_MG_TILE", "RB_MG_PAIR_SMEM", "RB_TRACKS_TILE", "RB_TRACKS_BAD_ID", "RB_TRACKS_WALK", "RB_VERIFY_TILE", "RB_VERIFY_BAD_ID",
-                 "RB_VERIFY_PAIR_BYTES", "RB_VERIFY_SLICE_BYTES", "RB_VERIFY_POINT_BYTES", "RB_VERIFY_CHUNK_BYTES"))
+                 "RB_VERIFY_PAIR_BYTES", "RB_VERIFY_SLICE_BYTES", "RB_VERIFY_POINT_BYTES", "RB_VERIFY_CHUNK_BYTES", "RB_TRI_GN_ITERS",
+                 "RB_TRI_CAM", "RB_TRI_BAD_ID"))
+RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEADER).read()).group(1), 16)
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -175,6 +177,8 @@ _FIELD_DTYPES = {
                        "match_scores": _F32, "info": torch.int64, "x0": _F64, "x1": _F64, "chunk_offsets": torch.int64, "ok": torch.uint8,
                        "mask": torch.uint8, "num_inliers": torch.int64, "accepted": torch.uint8, "tile_scan": torch.int64,
                        "out_offsets": torch.int64, "out_matches": torch.int32, "out_scores": _F32},
+    "rb_tri_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "cameras": _F64,
+                    "info": torch.int64, "X": _F64, "ok": torch.uint8, "num_inliers": torch.int32, "error": _F64, "inlier": torch.uint8},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -261,11 +265,17 @@ def _verify_min_elems(kw):
     return out
 
 
+def _tri_min_elems(kw):
+    T, N, E = kw["num_tracks"], kw["num_images"], kw["num_elements"]
+    return {"track_offsets": T + 1, "elements": 2 * E, "kp_offsets": N + 1, "keypoints": 2 * kw["num_rows"], "cameras": N * RB_TRI_CAM,
+            "info": 1, "X": 3 * T, "ok": T, "num_inliers": T, "error": T, "inlier": E}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
-              "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems}
+              "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -601,3 +601,33 @@ def track_cells(track_offsets, elements, kp_offsets, keypoints, width: int, cell
     cell = (np.floor(xy[:, 1]).astype(np.int64) // cell_size) * gw + np.floor(xy[:, 0]).astype(np.int64) // cell_size
     pairs = list(zip(el[:, 0].tolist(), cell.tolist()))
     return {tuple(pairs[off[t]:off[t + 1]]) for t in range(len(off) - 1)}
+
+
+def track_points(track_offsets, elements, kp_offsets, keypoints, views, width: int, cell_size: int = 1):
+    """The planted point of every track, int64 [T]: each element's keypoint mapped to its cell by the rule of `track_cells`, then to
+    the point whose view in that image (`views` [n_points, N] of `planted_views` or `planted_cameras`) is that cell.  -1 for a track
+    whose elements are not all views of one point."""
+    import numpy as np
+
+    off, el = track_offsets.cpu().numpy(), elements.cpu().numpy().astype(np.int64)
+    kp, kpo, v = keypoints.cpu().numpy(), kp_offsets.cpu().numpy(), views.cpu().numpy()
+    T = len(off) - 1
+    if el.size == 0:
+        return np.full(T, -1, np.int64)
+    xy = kp[kpo[el[:, 0]] + el[:, 1]]
+    gw = -(-width // cell_size)
+    cell = (np.floor(xy[:, 1]).astype(np.int64) // cell_size) * gw + np.floor(xy[:, 0]).astype(np.int64) // cell_size
+    span = int(max(v.max(), cell.max())) + 1
+    p, i = np.nonzero(v >= 0)
+    keys = i * span + v[p, i]                               # (image, cell) of every planted view
+    order = np.argsort(keys)
+    keys, p = np.r_[keys[order], -1], np.r_[p[order], -1]   # a sentinel, so that a miss finds a key that differs
+    q = el[:, 0] * span + cell
+    at = np.minimum(np.searchsorted(keys[:-1], q), keys.size - 1)
+    point = np.where(keys[at] == q, p[at], -1)
+    out = np.full(T, -1, np.int64)
+    for k in range(T):
+        pk = point[off[k]:off[k + 1]]
+        if pk.size and pk[0] >= 0 and (pk == pk[0]).all():
+            out[k] = pk[0]
+    return out
