@@ -978,6 +978,106 @@ typedef struct {
 } rb_tri_args;
 int romab200_triangulate(const rb_tri_args* args, void* stream);
 
+/* ---- bundle adjustment: Levenberg-Marquardt over the cameras' poses and the tracks' points, with a Schur-reduced camera system ----
+ * Not in the reference.  The input is what triangulation takes and gives: kp_offsets and keypoints of a match graph, the tracks
+ * (track_offsets, elements), per track ok [num_tracks] uint8 and per element inlier [num_elements] uint8, the points X
+ * [num_tracks, 3], and per image i a camera x ~ K_i (R_i X + t_i) in pixels; K stays fixed.  All arithmetic is float64.  The rules:
+ * 1. Observations.  The used observations are the elements e with inlier[e] set, in tracks with ok set.  Element (i, a) of track k
+ *    is observed at x_e = keypoints[kp_offsets[i] + a], widened to float64.  A track that is not ok is not touched: its X stays as
+ *    given (zero).
+ * 2. Residual and cost.  r_e = pi(K_i (R_i X_k + t_i)) - x_e in px, and s_e = |r_e|^2.  The cost is F = 1/2 sum_e rho(s_e).
+ *    rho(s) = s without a loss scale.  Otherwise rho(s) = c^2 log(1 + s / c^2) with c the loss scale (Cauchy), which is scipy's
+ *    loss="cauchy", f_scale=c cost.
+ * 3. Linearisation.  Parameters are d_omega_i, d_t_i per camera and d_X_k per ok track.  The update is R_i <- Exp(d_omega_i) R_i,
+ *    t_i <- t_i + d_t_i and X_k <- X_k + d_X_k.  Exp is Rodrigues in float64: with theta^2 = |w|^2 > 2^-52, Exp(w) = cos theta I +
+ *    (1 - cos theta) k k^T + sin theta [k]x with k = w / theta; otherwise the small-angle branch Exp(w) = I + [w]x.  Each
+ *    observation's Jacobian block is weighted by w_e = rho'(s_e) (1 without a loss scale, 1 / (1 + s_e / c^2) with one): this is
+ *    IRLS, with no second-order corrector.  H = J^T W J and g = J^T W r.
+ * 4. Gauge.  The cameras in fixed_poses get d_omega = d_t = 0.  The cameras in fixed_tx get d_t_x = 0: in the reduced system, that
+ *    row and column become the identity and the right-hand side becomes 0.  This is COLMAP's default, which holds the first pose
+ *    and the second camera's x-translation constant.
+ * 5. Damped step.  D is the diagonal of H, each entry clamped to [1e-6, 1e32].  Solve (H + lambda D) d = -g by the Schur complement
+ *    on the cameras.  V_k is the damped 3 x 3 block of track k.  S = U - W V^-1 W^T, restricted to free cameras, is factored by
+ *    dense Cholesky.  Back-substitution then gives d_X_k.  A non-positive or non-finite pivot makes the trial a rejected step.
+ * 6. Trial.  pred = 1/2 d^T (lambda D d - g) and rho = (F(x) - F(x + d)) / pred.  The step is kept when rho > 1e-3, F(x + d) is
+ *    finite and every used observation has depth > 0 at x + d.  When kept: lambda <- lambda max(1/3, 1 - (2 rho - 1)^3) and
+ *    nu <- 2.  When not kept: lambda <- lambda nu and nu <- 2 nu.  Start from lambda = 1e-4 and nu = 2.  This is Ceres'
+ *    Levenberg-Marquardt with radius 1 / lambda.
+ * 7. Stop.  Each trial counts against max_iterations.  The run also stops after a kept step that lowered F by at most
+ *    function_tolerance F ("function_tolerance"), or when lambda > 1e32 ("no_progress").  With no used observations or no free
+ *    parameters, it returns the inputs ("nothing_to_adjust").
+ * 8. Determinism.  There are no float atomics and every reduction runs in a fixed order, so reruns are bit-identical.
+ * A track whose used observations repeat an image (possible with drop_conflicts = 0) is refused: it sets RB_BA_REPEATED in info[0].
+ * Every used element's ids are checked, 0 <= i < num_images and 0 <= a < K_i, before any access that depends on them; a bad one
+ * sets RB_BA_BAD_ID in info[0].
+ * The caller checks on the host: the offsets as for triangulation, the cameras and points finite.  It builds the compact index of
+ * the free cameras (those not in fixed_poses): free_index [num_images] int32 (-1 for a fixed camera), free_cams [num_free] int32
+ * (their images, ascending) and fixed_tx [num_free] uint8 (1 for a camera in fixed_tx).
+ *
+ * The host drives the loop of rules 6-7 and reads result [RB_BA_RESULT] once per trial: F(x + d), pred, the number of used
+ * observations with depth <= 0 at x + d, and the pivot flag.  The cameras are cams [num_images, RB_BA_CAM] float64: R (9,
+ * row-major), t (3), K (9, row-major).  One trial is linearize, cameras, cholesky, solve, step; an accepted trial swaps the
+ * (cams, X) and (cams_trial, X_trial) buffers.
+ * romab200_ba_setup: info [2] int64 = {status, used observations} is zeroed; a warp per track checks its used elements' ids and
+ *   writes elem_track [num_elements] int32 and keys (image << 32 | e, image = num_images for an unused element) [num_elements];
+ *   radix_sort_hi32 (common.cuh) sorts them stably by image (keys_alt, hist RADIX_DIGITS ceil(num_elements / RB_TRACKS_TILE) + 1 int32);
+ *   obs_offsets [num_images + 1] int64 is the start of each image's observations in obs [num_elements] int32 (element ids in
+ *   ascending order per image); info[1] = obs_offsets[num_images].
+ * romab200_ba_linearize: a warp per track at lambda: track_sys [num_tracks, RB_BA_TRACK] = V^-1 of the damped block (00, 01, 02, 11,
+ *   12, 22), g_X (3), D_X (3), the track's cost 1/2 sum rho(s_e); W [num_elements, 18] = w_e J_c^T J_X (6 x 3 row-major) of every
+ *   used element.  result[0..3] are zeroed.
+ * romab200_ba_cameras: a CTA per free camera fills the 6 rows of S [6 num_free, 6 num_free] (row-major, the blocks (i, j) with j <= i;
+ *   the Cholesky reads the lower triangle), rhs [6 num_free] and cam_sys [num_free, 12] = g_c (6), D_c (6).
+ * romab200_ba_cholesky: S = L L^T in place (lower triangle), right-looking with RB_BA_NB-wide panels: panel, triangular solve and
+ *   trailing update kernels; a pivot that is not > 0 and finite sets result[3].  Then the forward and backward substitutions turn
+ *   rhs into the camera step.
+ * romab200_ba_step: the trial cameras cams_trial, cam_pred [num_images] (1/2 d_c^T (lambda D_c d_c - g_c)), then a warp per track:
+ *   d_X, X_trial, track_part [num_tracks, 3] = the trial cost, 1/2 d_X^T (lambda D_X d_X - g_X), and the count of depths <= 0;
+ *   then result[0..2] as fixed-order tree sums.  Without free cameras, pass num_free = 0 and skip cameras and cholesky.
+ * romab200_ba_cost: result[0] = the sum of the tracks' costs in track_sys (after linearize), result[1] = 0.
+ * romab200_ba_error: error [num_tracks] = the mean |r_e| of the used observations of every ok track (0 for the others).
+ * Device bytes, with N images, F free cameras, T tracks and E elements (the buffers bundle.py allocates):
+ *   RB_BA_ELEMENT_BYTES E + RB_BA_TRACK_BYTES T + RB_BA_IMAGE_BYTES N + RB_BA_FREE_BYTES F + 288 F^2
+ *   + 1024 ceil(E / RB_TRACKS_TILE) + RB_BA_ONCE_BYTES
+ *   per element keys 8, keys_alt 8, elem_track 4, obs 4, W 144, inlier 1; per track track_sys 104, X 24, X_trial 24, track_part 24,
+ *   error 8, track_offsets 8, track_ok 1; per image cams 168, cams_trial 168, cam_pred 8, free_index 4, obs_offsets 8, kp_offsets 8;
+ *   per free camera cam_sys 96, rhs 48, free_cams 4, fixed_tx 1; S 288 F^2; once hist 4, obs_offsets 8, kp_offsets 8, track_offsets
+ *   8, info 16, result 32.  W is stored rather than recomputed by the camera kernel: 144 B per element is 576 MB at 4 M elements. */
+#define RB_BA_BAD_ID 1
+#define RB_BA_REPEATED 2
+#define RB_BA_CAM 21
+#define RB_BA_TRACK 13
+#define RB_BA_RESULT 4
+#define RB_BA_NB 32
+#define RB_BA_ELEMENT_BYTES 169
+#define RB_BA_TRACK_BYTES 193
+#define RB_BA_IMAGE_BYTES 364
+#define RB_BA_FREE_BYTES 149
+#define RB_BA_ONCE_BYTES 76
+typedef struct {
+    int32_t num_tracks, num_images, num_free;
+    const int64_t* track_offsets; const int32_t* elements; int64_t num_elements;
+    const int64_t* kp_offsets; const float* keypoints; int64_t num_rows;
+    const uint8_t* track_ok; const uint8_t* inlier;
+    const int32_t* free_index; const int32_t* free_cams; const uint8_t* fixed_tx;
+    double loss_scale2;                                                 /* c^2, or 0 for the squared loss */
+    double lambda;
+    int64_t* info;                                                      /* [2] status, used observations */
+    int32_t* elem_track; uint64_t* keys; uint64_t* keys_alt; int32_t* hist; int64_t* obs_offsets; int32_t* obs;
+    const double* cams; const double* X;                                /* the current state */
+    double* cams_trial; double* X_trial;
+    double* W; double* track_sys; double* cam_sys; double* S; double* rhs;
+    double* cam_pred; double* track_part; double* result;
+    double* error;
+} rb_ba_args;
+int romab200_ba_setup(const rb_ba_args* args, void* stream);
+int romab200_ba_linearize(const rb_ba_args* args, void* stream);
+int romab200_ba_cameras(const rb_ba_args* args, void* stream);
+int romab200_ba_cholesky(const rb_ba_args* args, void* stream);
+int romab200_ba_step(const rb_ba_args* args, void* stream);
+int romab200_ba_cost(const rb_ba_args* args, void* stream);
+int romab200_ba_error(const rb_ba_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -38,6 +38,9 @@ def __getattr__(name):
     if name in ("triangulate_tracks", "Points3D"):
         from . import triangulate
         return getattr(triangulate, name)
+    if name in ("bundle_adjust", "BundleResult"):
+        from . import bundle
+        return getattr(bundle, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
         from . import depth_warp
         return getattr(depth_warp, name)

@@ -74,6 +74,11 @@ STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
                  "RB_VERIFY_PAIR_BYTES", "RB_VERIFY_SLICE_BYTES", "RB_VERIFY_POINT_BYTES", "RB_VERIFY_CHUNK_BYTES", "RB_TRI_GN_ITERS",
                  "RB_TRI_CAM", "RB_TRI_BAD_ID"))
 RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEADER).read()).group(1), 16)
+(RB_BA_BAD_ID, RB_BA_REPEATED, RB_BA_CAM, RB_BA_TRACK, RB_BA_RESULT, RB_BA_NB, RB_BA_ELEMENT_BYTES, RB_BA_TRACK_BYTES, RB_BA_IMAGE_BYTES,
+ RB_BA_FREE_BYTES, RB_BA_ONCE_BYTES) = (
+    int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+    for name in ("RB_BA_BAD_ID", "RB_BA_REPEATED", "RB_BA_CAM", "RB_BA_TRACK", "RB_BA_RESULT", "RB_BA_NB", "RB_BA_ELEMENT_BYTES",
+                 "RB_BA_TRACK_BYTES", "RB_BA_IMAGE_BYTES", "RB_BA_FREE_BYTES", "RB_BA_ONCE_BYTES"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -179,6 +184,11 @@ _FIELD_DTYPES = {
                        "out_offsets": torch.int64, "out_matches": torch.int32, "out_scores": _F32},
     "rb_tri_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "cameras": _F64,
                     "info": torch.int64, "X": _F64, "ok": torch.uint8, "num_inliers": torch.int32, "error": _F64, "inlier": torch.uint8},
+    "rb_ba_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "track_ok": torch.uint8,
+                   "inlier": torch.uint8, "free_index": torch.int32, "free_cams": torch.int32, "fixed_tx": torch.uint8, "info": torch.int64,
+                   "elem_track": torch.int32, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32, "obs_offsets": torch.int64,
+                   "obs": torch.int32, "cams": _F64, "X": _F64, "cams_trial": _F64, "X_trial": _F64, "W": _F64, "track_sys": _F64,
+                   "cam_sys": _F64, "S": _F64, "rhs": _F64, "cam_pred": _F64, "track_part": _F64, "result": _F64, "error": _F64},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -271,11 +281,22 @@ def _tri_min_elems(kw):
             "info": 1, "X": 3 * T, "ok": T, "num_inliers": T, "error": T, "inlier": E}
 
 
+def _ba_min_elems(kw):
+    T, N, F, E = kw["num_tracks"], kw["num_images"], kw.get("num_free", 0), kw["num_elements"]
+    n = 6 * F
+    return {"track_offsets": T + 1, "elements": 2 * E, "kp_offsets": N + 1, "keypoints": 2 * kw["num_rows"], "track_ok": T, "inlier": E,
+            "free_index": N, "free_cams": F, "fixed_tx": F, "info": 2, "elem_track": E, "keys": E, "keys_alt": E,
+            "hist": 256 * ((E + RB_TRACKS_TILE - 1) // RB_TRACKS_TILE) + 1, "obs_offsets": N + 1, "obs": E, "cams": N * RB_BA_CAM,
+            "X": 3 * T, "cams_trial": N * RB_BA_CAM, "X_trial": 3 * T, "W": 18 * E, "track_sys": T * RB_BA_TRACK, "cam_sys": 12 * F,
+            "S": n * n, "rhs": n, "cam_pred": N, "track_part": 3 * T, "result": RB_BA_RESULT, "error": T}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
-              "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems}
+              "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
+              "rb_ba_args": _ba_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -246,6 +246,89 @@ __global__ void __launch_bounds__(1024) scan_counts_kernel(T* __restrict__ v, in
     if (threadIdx.x == 1023) v[n] = run;
 }
 
+// ---- stable LSD radix sort of 64-bit keys by their high 32 bits, 8-bit digits, tiles of TILE keys --------------------------------
+// Templates, so that every translation unit that launches them carries its own copy.
+constexpr int RADIX_THREADS = 256;
+constexpr int RADIX_WARPS = RADIX_THREADS / 32;
+constexpr int RADIX_DIGITS = 256;
+static_assert(RADIX_DIGITS == RADIX_THREADS, "the radix kernels give one digit to each thread");
+
+// hist[d * tiles + t] = keys of tile t whose high word has digit d at `shift`
+template <int TILE>
+__global__ void __launch_bounds__(RADIX_THREADS) radix_hist_kernel(const uint64_t* __restrict__ keys, int64_t n, int shift, int32_t* hist) {
+    pdl_wait();
+    __shared__ int h[RADIX_DIGITS];
+    h[threadIdx.x] = 0;
+    __syncthreads();
+    const int64_t q0 = (int64_t)blockIdx.x * TILE;
+    for (int k = 0; k < TILE / RADIX_THREADS; ++k) {
+        const int64_t q = q0 + k * RADIX_THREADS + threadIdx.x;
+        if (q < n) atomicAdd(&h[(keys[q] >> (32 + shift)) & (RADIX_DIGITS - 1)], 1);
+    }
+    __syncthreads();
+    hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
+}
+
+// Stable scatter of tile t: rounds of RADIX_THREADS consecutive keys; within a warp, the rank among equal digits from
+// __match_any_sync; across warps and rounds, a running offset per digit that starts at the scanned hist entry of (digit, tile).
+template <int TILE>
+__global__ void __launch_bounds__(RADIX_THREADS) radix_scatter_kernel(const uint64_t* __restrict__ in, uint64_t* __restrict__ out, int64_t n,
+                                                                      int shift, const int32_t* __restrict__ hist) {
+    pdl_wait();
+    __shared__ int base[RADIX_DIGITS];
+    __shared__ int wcnt[RADIX_WARPS][RADIX_DIGITS];
+    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    base[threadIdx.x] = hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x];
+    const int64_t q0 = (int64_t)blockIdx.x * TILE;
+    for (int k = 0; k < TILE / RADIX_THREADS; ++k) {
+#pragma unroll
+        for (int w = 0; w < RADIX_WARPS; ++w) wcnt[w][threadIdx.x] = 0;
+        __syncthreads();
+        const int64_t q = q0 + k * RADIX_THREADS + threadIdx.x;
+        const bool valid = q < n;
+        const uint64_t key = valid ? in[q] : 0;
+        const int d = valid ? (int)((key >> (32 + shift)) & (RADIX_DIGITS - 1)) : RADIX_DIGITS;
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        const int rank = __popc(peers & ((1u << lane) - 1u));
+        if (valid && rank == 0) wcnt[wid][d] = __popc(peers);
+        __syncthreads();
+        int run = base[threadIdx.x];                     // column of digit threadIdx.x: exclusive over the warps, from base
+#pragma unroll
+        for (int w = 0; w < RADIX_WARPS; ++w) {
+            const int c = wcnt[w][threadIdx.x];
+            wcnt[w][threadIdx.x] = run;
+            run += c;
+        }
+        base[threadIdx.x] = run;
+        __syncthreads();
+        if (valid) out[wcnt[wid][d] + rank] = key;
+        __syncthreads();
+    }
+}
+
+// Sorts keys[0, n) stably by the low `bits` bits of their high words, ping-ponging between keys and keys_alt; hist holds
+// RADIX_DIGITS ceil(n / TILE) + 1 ints.  *sorted receives the buffer that holds the result.  0, or 1 after a failed launch.
+template <int TILE>
+inline int radix_sort_hi32(uint64_t* keys, uint64_t* keys_alt, int32_t* hist, int64_t n, int bits, cudaStream_t st, const char* what,
+                           uint64_t** sorted) {
+    const int tiles = (int)((n + TILE - 1) / TILE);
+    uint64_t* in = keys;
+    uint64_t* out = keys_alt;
+    for (int shift = 0; shift < bits; shift += 8) {
+        launch_pdl(radix_hist_kernel<TILE>, dim3(tiles), dim3(RADIX_THREADS), 0, st, (const uint64_t*)in, n, shift, hist);
+        if (check_launch(what)) return 1;
+        launch_pdl(scan_counts_kernel<int32_t>, dim3(1), dim3(1024), 0, st, hist, RADIX_DIGITS * tiles);
+        if (check_launch(what)) return 1;
+        launch_pdl(radix_scatter_kernel<TILE>, dim3(tiles), dim3(RADIX_THREADS), 0, st, (const uint64_t*)in, out, n, shift, (const int32_t*)hist);
+        if (check_launch(what)) return 1;
+        uint64_t* t = in;
+        in = out;
+        out = t;
+    }
+    *sorted = in;
+    return 0;
+}
+
 int gemm_simt(const rb_gemm_args* a, cudaStream_t stream, int lower_only = 0);
 int gemm_tc(const rb_gemm_args* a, cudaStream_t stream);
 int dwconv_tma(const rb_dwconv_args* a, cudaStream_t stream);     // dwconv_tma.cu: TMA-fed persistent depthwise kernel (16-bit maps)

@@ -7,8 +7,8 @@
 //           flatten    parent[r] = root(r) (walks that store nothing else), size[root] += 1 (integer atomics);
 //           rows       a CTA per RB_TRACKS_TILE rows counts the rows of components of >= 2 rows; scan; info[1] = the total.
 //   build   rows       the same tiles write those rows as keys (root << 32 | row) in ascending row order;
-//           radix      per 8-bit digit of the root: tile histograms, a scan over (digit, tile), a stable scatter with in-tile ranks;
-//                      the input is in row order, so the output is in (root, row) order;
+//           radix      radix_sort_hi32 (common.cuh) by root: per 8-bit digit, tile histograms, a scan over (digit, tile), a stable
+//                      scatter with in-tile ranks; the input is in row order, so the output is in (root, row) order;
 //           conflict   an element whose predecessor has the same root and the same image flags its root (bit 31 of size[root]);
 //           segments   per tile: kept track heads and kept elements (packed into one int64), scan, then track_offsets, elements
 //                      and kp_track at the scanned offsets.
@@ -20,9 +20,7 @@ namespace rb {
 constexpr int TR_THREADS = 256;
 constexpr int TR_IPT = RB_TRACKS_TILE / TR_THREADS;   // consecutive items per thread in the tile kernels
 constexpr int TR_WARPS = TR_THREADS / 32;
-constexpr int TR_DIGITS = 256;
 constexpr uint32_t TR_CONFLICT = 0x80000000u;         // bit 31 of size[root]: the component has a conflict
-static_assert(TR_DIGITS == TR_THREADS, "the radix kernels give one digit to each thread");
 
 __device__ __forceinline__ void tr_status(int64_t* info, int bit) { atomicOr((unsigned long long*)info, (unsigned long long)bit); }
 __device__ __forceinline__ int tr_load(const int32_t* p) { return *(const volatile int32_t*)p; }
@@ -160,57 +158,6 @@ __global__ void __launch_bounds__(TR_THREADS) tr_rows_kernel(rb_tracks_args a) {
     }
 }
 
-// hist[d * tiles + t] = keys of tile t whose root has digit d at `shift`
-__global__ void __launch_bounds__(TR_THREADS) tr_hist_kernel(const uint64_t* __restrict__ keys, int64_t n, int shift, int32_t* hist) {
-    pdl_wait();
-    __shared__ int h[TR_DIGITS];
-    h[threadIdx.x] = 0;
-    __syncthreads();
-    const int64_t q0 = (int64_t)blockIdx.x * RB_TRACKS_TILE;
-    for (int k = 0; k < TR_IPT; ++k) {
-        const int64_t q = q0 + k * TR_THREADS + threadIdx.x;
-        if (q < n) atomicAdd(&h[(keys[q] >> (32 + shift)) & (TR_DIGITS - 1)], 1);
-    }
-    __syncthreads();
-    hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x] = h[threadIdx.x];
-}
-
-// Stable scatter of tile t: rounds of TR_THREADS consecutive keys; within a warp, the rank among equal digits from __match_any_sync;
-// across warps and rounds, a running offset per digit that starts at the scanned hist entry of (digit, tile).
-__global__ void __launch_bounds__(TR_THREADS) tr_scatter_kernel(const uint64_t* __restrict__ in, uint64_t* __restrict__ out, int64_t n,
-                                                                 int shift, const int32_t* __restrict__ hist) {
-    pdl_wait();
-    __shared__ int base[TR_DIGITS];
-    __shared__ int wcnt[TR_WARPS][TR_DIGITS];
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    base[threadIdx.x] = hist[(int64_t)threadIdx.x * gridDim.x + blockIdx.x];
-    const int64_t q0 = (int64_t)blockIdx.x * RB_TRACKS_TILE;
-    for (int k = 0; k < TR_IPT; ++k) {
-#pragma unroll
-        for (int w = 0; w < TR_WARPS; ++w) wcnt[w][threadIdx.x] = 0;
-        __syncthreads();
-        const int64_t q = q0 + k * TR_THREADS + threadIdx.x;
-        const bool valid = q < n;
-        const uint64_t key = valid ? in[q] : 0;
-        const int d = valid ? (int)((key >> (32 + shift)) & (TR_DIGITS - 1)) : TR_DIGITS;
-        const unsigned peers = __match_any_sync(0xffffffffu, d);
-        const int rank = __popc(peers & ((1u << lane) - 1u));
-        if (valid && rank == 0) wcnt[wid][d] = __popc(peers);
-        __syncthreads();
-        int run = base[threadIdx.x];                     // column of digit threadIdx.x: exclusive over the warps, from base
-#pragma unroll
-        for (int w = 0; w < TR_WARPS; ++w) {
-            const int c = wcnt[w][threadIdx.x];
-            wcnt[w][threadIdx.x] = run;
-            run += c;
-        }
-        base[threadIdx.x] = run;
-        __syncthreads();
-        if (valid) out[wcnt[wid][d] + rank] = key;
-        __syncthreads();
-    }
-}
-
 __global__ void __launch_bounds__(TR_THREADS) tr_conflict_kernel(rb_tracks_args a, const uint64_t* __restrict__ keys, int64_t n) {
     pdl_wait();
     for (int64_t q = 1 + blockIdx.x * (int64_t)TR_THREADS + threadIdx.x; q < n; q += (int64_t)gridDim.x * TR_THREADS) {
@@ -320,19 +267,8 @@ extern "C" int romab200_tracks_build(const rb_tracks_args* a, void* stream) {
     const int64_t n = a->num_kept;
     const int tiles = (int)((n + RB_TRACKS_TILE - 1) / RB_TRACKS_TILE);
     const int bits = 32 - __builtin_clz((unsigned)(a->num_rows - 1));        // roots lie in [0, num_rows), num_rows >= 2
-    uint64_t* in = a->keys;
-    uint64_t* out = a->keys_alt;
-    for (int shift = 0; shift < bits; shift += 8) {
-        launch_pdl(tr_hist_kernel, dim3(tiles), dim3(TR_THREADS), 0, st, (const uint64_t*)in, n, shift, a->hist);
-        if (check_launch("tracks_build(histogram)")) return 1;
-        launch_pdl(scan_counts_kernel<int32_t>, dim3(1), dim3(1024), 0, st, a->hist, TR_DIGITS * tiles);
-        if (check_launch("tracks_build(digit scan)")) return 1;
-        launch_pdl(tr_scatter_kernel, dim3(tiles), dim3(TR_THREADS), 0, st, (const uint64_t*)in, out, n, shift, (const int32_t*)a->hist);
-        if (check_launch("tracks_build(scatter)")) return 1;
-        uint64_t* t = in;
-        in = out;
-        out = t;
-    }
+    uint64_t* in = nullptr;
+    if (radix_sort_hi32<RB_TRACKS_TILE>(a->keys, a->keys_alt, a->hist, n, bits, st, "tracks_build(radix)", &in)) return 1;
     launch_pdl(tr_conflict_kernel, dim3(grid1d(n, TR_THREADS, 16 * 1024)), dim3(TR_THREADS), 0, st, *a, (const uint64_t*)in, n);
     if (check_launch("tracks_build(conflicts)")) return 1;
     launch_pdl(tr_segments_kernel<false>, dim3(tiles), dim3(TR_THREADS), 0, st, *a, (const uint64_t*)in, n);

@@ -583,6 +583,34 @@ def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024)
     return out + tuple(torch.from_numpy(a).to(device) for a in (K, R, t, X))
 
 
+def perturb_cameras(seed: int, R, t, rot_deg: float, centre: float):
+    """Seeded noise on cameras x ~ K (R X + t): each rotation turned by `rot_deg` degrees about a uniformly random axis (R' = Q R)
+    and each centre C = -R^T t moved by `centre` units in a uniformly random direction.  R [N, 3, 3] and t [N, 3] are tensors or
+    arrays; returns float64 (R', t') of the same kind, on the same device."""
+    import numpy as np
+
+    dev = R.device if isinstance(R, torch.Tensor) else None
+    Rn = R.detach().cpu().double().numpy() if dev is not None else np.asarray(R, np.float64)
+    tn = t.detach().cpu().double().numpy() if dev is not None else np.asarray(t, np.float64)
+    rng = np.random.default_rng(seed)
+    N = Rn.shape[0]
+    axis = rng.normal(size=(N, 3))
+    axis /= np.linalg.norm(axis, axis=1, keepdims=True)
+    step = rng.normal(size=(N, 3))
+    step /= np.linalg.norm(step, axis=1, keepdims=True)
+    th = np.deg2rad(rot_deg)
+    Kx = np.zeros((N, 3, 3))
+    Kx[:, 0, 1], Kx[:, 0, 2], Kx[:, 1, 2] = -axis[:, 2], axis[:, 1], -axis[:, 0]
+    Kx -= Kx.transpose(0, 2, 1)
+    Q = np.eye(3) + np.sin(th) * Kx + (1 - np.cos(th)) * Kx @ Kx
+    C = -np.einsum("nji,nj->ni", Rn, tn) + centre * step
+    R2 = Q @ Rn
+    t2 = -np.einsum("nij,nj->ni", R2, C)
+    if dev is None:
+        return R2, t2
+    return torch.from_numpy(R2).to(dev), torch.from_numpy(t2).to(dev)
+
+
 def planted_tracks(views, min_length: int = 2):
     """The planted tracks of `planted_views` with at least `min_length` views, as a set of tuples ((image, cell), ...) in image order."""
     v = views.cpu().numpy()

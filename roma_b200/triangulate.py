@@ -28,21 +28,21 @@ class Points3D:
     inlier: torch.Tensor
 
 
-def _float64(name, v, shape):
+def _float64(name, v, shape, what="triangulate_tracks"):
     """A float camera array (tensor on any device, or array-like) widened to a float64 numpy array of `shape`, all finite."""
     if isinstance(v, torch.Tensor):
         if not v.dtype.is_floating_point:
-            raise ValueError(f"triangulate_tracks: {name} must have a float dtype, got {v.dtype}")
+            raise ValueError(f"{what}: {name} must have a float dtype, got {v.dtype}")
         v = v.detach().cpu().double().numpy()
     else:
         v = np.asarray(v)
         if v.dtype.kind != "f":
-            raise ValueError(f"triangulate_tracks: {name} must have a float dtype, got {v.dtype}")
+            raise ValueError(f"{what}: {name} must have a float dtype, got {v.dtype}")
         v = v.astype(np.float64)
     if v.shape != shape:
-        raise ValueError(f"triangulate_tracks: {name} must have shape {list(shape)}, got {list(v.shape)}")
+        raise ValueError(f"{what}: {name} must have shape {list(shape)}, got {list(v.shape)}")
     if not np.isfinite(v).all():
-        raise ValueError(f"triangulate_tracks: {name} has values that are not finite")
+        raise ValueError(f"{what}: {name} has values that are not finite")
     return v
 
 
@@ -57,67 +57,72 @@ def camera_table(K, R, t) -> np.ndarray:
     return tab
 
 
-def _check(graph, tracks, K, R, t, max_error, min_angle, max_hypotheses, seed):
-    """Argument rules, checked before any device work.  Returns (kp_offsets list, track_offsets list, camera table, max_error^2,
-    min_angle in radians, max_hypotheses, seed)."""
+def _check(graph, tracks, K, R, t, max_error, min_angle, max_hypotheses, seed, what="triangulate_tracks", device=True):
+    """Argument rules, checked before any device work; `what` names the caller in the messages, and `device=False` leaves the
+    device rule to the caller.  Returns (kp_offsets list, track_offsets list, camera table, max_error^2, min_angle in radians,
+    max_hypotheses, seed)."""
     if not isinstance(graph, MatchGraph):
-        raise ValueError(f"triangulate_tracks: graph must be a MatchGraph, got {type(graph).__name__}")
+        raise ValueError(f"{what}: graph must be a MatchGraph, got {type(graph).__name__}")
     if not isinstance(tracks, Tracks):
-        raise ValueError(f"triangulate_tracks: tracks must be Tracks, got {type(tracks).__name__}")
+        raise ValueError(f"{what}: tracks must be Tracks, got {type(tracks).__name__}")
     kp_off = graph._kp_off
     for name, tv in (("graph.kp_offsets", graph.kp_offsets), ("tracks.track_offsets", tracks.track_offsets)):
         if not isinstance(tv, torch.Tensor) or tv.dtype != torch.int64 or tv.dim() != 1 or tv.numel() < 1:
-            raise ValueError(f"triangulate_tracks: {name} must be a 1-D int64 tensor of at least one entry, got "
+            raise ValueError(f"{what}: {name} must be a 1-D int64 tensor of at least one entry, got "
                              f"{getattr(tv, 'dtype', type(tv).__name__)} {tuple(getattr(tv, 'shape', ()))}")
     tr_off = tracks.track_offsets.tolist()
     for name, off in (("graph.kp_offsets", kp_off), ("tracks.track_offsets", tr_off)):
         if off[0] != 0 or any(b < a for a, b in zip(off, off[1:])):
-            raise ValueError(f"triangulate_tracks: {name} must start at 0 and never decrease")
+            raise ValueError(f"{what}: {name} must start at 0 and never decrease")
     N, Kr, T, E = len(kp_off) - 1, kp_off[-1], len(tr_off) - 1, tr_off[-1]
     if not isinstance(graph.keypoints, torch.Tensor) or graph.keypoints.dtype != torch.float32 or tuple(graph.keypoints.shape) != (Kr, 2):
-        raise ValueError(f"triangulate_tracks: graph.keypoints must be fp32 [{Kr}, 2], got {getattr(graph.keypoints, 'dtype', None)} "
+        raise ValueError(f"{what}: graph.keypoints must be fp32 [{Kr}, 2], got {getattr(graph.keypoints, 'dtype', None)} "
                          f"{tuple(getattr(graph.keypoints, 'shape', ()))}")
     el = tracks.elements
     if not isinstance(el, torch.Tensor) or el.dtype != torch.int32 or tuple(el.shape) != (E, 2):
-        raise ValueError(f"triangulate_tracks: tracks.elements must be int32 [{E}, 2], got {getattr(el, 'dtype', None)} "
+        raise ValueError(f"{what}: tracks.elements must be int32 [{E}, 2], got {getattr(el, 'dtype', None)} "
                          f"{tuple(getattr(el, 'shape', ()))}")
     if E >= 1 << 31:
-        raise ValueError(f"triangulate_tracks: {E} elements, at most 2^31 - 1 are supported")
+        raise ValueError(f"{what}: {E} elements, at most 2^31 - 1 are supported")
     if T >= 1 << 31:
-        raise ValueError(f"triangulate_tracks: {T} tracks, at most 2^31 - 1 are supported")
+        raise ValueError(f"{what}: {T} tracks, at most 2^31 - 1 are supported")
     if N < 1:
-        raise ValueError("triangulate_tracks: the graph has no images")
-    K = _float64("K", K, (N, 3, 3))
-    R = _float64("R", R, (N, 3, 3))
-    t = _float64("t", t, (N, 3))
+        raise ValueError(f"{what}: the graph has no images")
+    K = _float64("K", K, (N, 3, 3), what)
+    R = _float64("R", R, (N, 3, 3), what)
+    t = _float64("t", t, (N, 3), what)
     try:
         max_error, min_angle = float(max_error), float(min_angle)
     except (TypeError, ValueError):
-        raise ValueError(f"triangulate_tracks: max_error and min_angle must be numbers, got {max_error!r} and {min_angle!r}") from None
+        raise ValueError(f"{what}: max_error and min_angle must be numbers, got {max_error!r} and {min_angle!r}") from None
     if not (math.isfinite(max_error) and max_error > 0):
-        raise ValueError(f"triangulate_tracks: max_error must be finite and > 0, got {max_error!r}")
+        raise ValueError(f"{what}: max_error must be finite and > 0, got {max_error!r}")
     if not 0 <= min_angle < 180:
-        raise ValueError(f"triangulate_tracks: min_angle must lie in [0, 180) degrees, got {min_angle!r}")
+        raise ValueError(f"{what}: min_angle must lie in [0, 180) degrees, got {min_angle!r}")
     bad = isinstance(max_hypotheses, bool)
     try:
         max_hypotheses = operator.index(max_hypotheses)
     except TypeError:
         bad = True
     if bad or not 1 <= max_hypotheses < 1 << 31:
-        raise ValueError(f"triangulate_tracks: max_hypotheses must be an int in [1, 2^31), got {max_hypotheses!r}")
+        raise ValueError(f"{what}: max_hypotheses must be an int in [1, 2^31), got {max_hypotheses!r}")
     try:
         seed = operator.index(seed)
     except TypeError:
-        raise ValueError(f"triangulate_tracks: seed must be an int, got {seed!r}") from None
+        raise ValueError(f"{what}: seed must be an int, got {seed!r}") from None
     if isinstance(seed, bool) or not 0 <= seed < 1 << 64:
-        raise ValueError(f"triangulate_tracks: seed must be an int in [0, 2^64), got {seed!r}")
+        raise ValueError(f"{what}: seed must be an int in [0, 2^64), got {seed!r}")
     if Kr == 0 and E > 0:
-        raise ValueError("triangulate_tracks: the graph has no keypoints, so every element id is out of range")
-    tensors = [graph.kp_offsets, graph.keypoints, tracks.track_offsets, el]
-    dev = graph.kp_offsets.device
-    if not all(tv.is_cuda and tv.device == dev for tv in tensors):
-        raise ValueError(f"triangulate_tracks: the graph's and tracks' tensors must be on one CUDA device, got {[tv.device for tv in tensors]}")
+        raise ValueError(f"{what}: the graph has no keypoints, so every element id is out of range")
+    if device:
+        _check_device([graph.kp_offsets, graph.keypoints, tracks.track_offsets, el], what)
     return kp_off, tr_off, camera_table(K, R, t), max_error * max_error, min_angle * (math.pi / 180.0), max_hypotheses, seed
+
+
+def _check_device(tensors, what):
+    dev = tensors[0].device
+    if not all(tv.is_cuda and tv.device == dev for tv in tensors):
+        raise ValueError(f"{what}: the graph's and tracks' tensors must be on one CUDA device, got {[tv.device for tv in tensors]}")
 
 
 def triangulate_tracks(graph: MatchGraph, tracks: Tracks, K, R, t, *, max_error=4.0, min_angle=1.5, max_hypotheses=256,
