@@ -960,7 +960,10 @@ int romab200_verify_emit(const rb_verify_args* args, void* stream);
  * by cyclic Jacobi (10 sweeps); the best is the warp maximum of (count << 32) | ~h.  The refinement sums the 4 x 4 DLT matrix, the
  * 3 x 3 normal equations and the cost over the lanes (each lane its elements e = l, l + 32, ... in order, then a xor butterfly);
  * the lanes split the angle test over the inlier pairs.  Observations are read through global memory, so any L is supported.
- * cameras [num_images, RB_TRI_CAM] float64 per image: P (12, row-major), row 2 of R (3), t_z, C (3), unused. */
+ * cameras [num_images, RB_TRI_CAM] float64 per image: P (12, row-major), row 2 of R (3), t_z, C (3), and the exclusion flag: 0, or
+ * 1 for an image that is not among the registered `images` of triangulate_tracks.  An element of an excluded image is not an
+ * observation: a pair that contains it is skipped but keeps its index h (as a pair within one image is in rule 2), and it is never an
+ * inlier.  The other entries of an excluded image's row are not read. */
 #define RB_TRI_CTR 0x54524900u
 #define RB_TRI_GN_ITERS 10
 #define RB_TRI_CAM 20
@@ -1077,6 +1080,123 @@ int romab200_ba_cholesky(const rb_ba_args* args, void* stream);
 int romab200_ba_step(const rb_ba_args* args, void* stream);
 int romab200_ba_cost(const rb_ba_args* args, void* stream);
 int romab200_ba_error(const rb_ba_args* args, void* stream);
+
+/* ---- absolute pose: batched P3P RANSAC and Gauss-Newton refinement (COLMAP's EstimateAbsolutePose + RefineAbsolutePose) ----
+ * Not in the reference.  B items with ragged point counts, packed: item b owns points [offsets[b], offsets[b+1]), each a pixel x
+ * [total, 2] and a world point X [total, 3], and its intrinsics K [batch, 3, 3], with the camera model x ~ K (R X + t).  All
+ * arithmetic is float64.  The rules:
+ * 1. Bearings.  For each point, f = normalise(K^-1 [x, y, 1]), K^-1 by cofactors over the determinant.
+ * 2. Samples.  Hypothesis h draws 3 distinct indices with ransac_draw<3> (geometry.cuh) under key seed and counter
+ *    (h, s, 0, RB_ABS_CTR), s = 0, 1, ...  The counter does not name the item, so item b is bit-identical to a call on that item
+ *    alone, whatever the batch and its order.
+ * 3. Minimal solver.  Lambda Twist P3P (Persson & Nordberg, ECCV 2018) on the three bearings f_i and world points X_i: with
+ *    a_ij = |X_i - X_j|^2 and b_ij = f_i . f_j, D1 = a23 M12 - a12 M23 and D2 = a23 M13 - a13 M23 (M_ij the quadratic form of
+ *    l_i^2 + l_j^2 - 2 b_ij l_i l_j), of the real roots g of det(D1 + g D2) = 0 (Cardano or the trigonometric form, two Newton
+ *    steps each; descending) whose D0 = D1 + g D2 is indefinite (cyclic Jacobi; its two eigenvalues of largest magnitude have
+ *    opposite signs), the one with the largest ratio of their magnitudes is used, the first on a tie: it keeps clear of a
+ *    semidefinite D0, whose lines are complex.  Let sigma1 > 0 > sigma2 be those eigenvalues, with eigenvectors u1, u2 signed so that
+ *    their first largest-magnitude entry is positive.  Its lines n = u1 - s u2, then u1 + s u2 (s = sqrt(-sigma2 / sigma1)) give
+ *    l1 = w0 l2 + w1 l3 (w = -(n1, n2) / n0); on each, the roots tau > 0 of the quadratic v^T D2 v, v = (w0 + w1 tau, 1, tau), in
+ *    ascending order, give l2 = sqrt(a23 / (tau^2 - 2 b23 tau + 1)), l3 = tau l2, kept when l1 > 0.  The depths are then polished
+ *    by at most RB_ABS_POLISH_ITERS Newton steps on the three residuals l_i^2 + l_j^2 - 2 b_ij l_i l_j - a_ij (a step kept only if
+ *    it lowers their sum of squares), and with Y_i = l_i f_i, R = [Y1 - Y2, Y1 - Y3, (Y1 - Y2) x (Y1 - Y3)] [X1 - X2, X1 - X3,
+ *    (X1 - X2) x (X1 - X3)]^-1 and t = Y1 - R X1.  A solution that is not finite is dropped; every other one is a model, so a
+ *    sample gives up to RB_ABS_MAX_SOL models.  The 4th-point disambiguation of OpenCV's P3P is not used.
+ * 4. Support.  Point j is an inlier of (R, t) when its depth (R X_j + t)_z > 0 and |pi(K (R X_j + t)) - x_j|^2 <= max_error2
+ *    (pi(p) = (p_0 / p_2, p_1 / p_2)).  The best model has the most inliers, and at least 3; ties go to the smallest
+ *    (h, solution index).  The loop is OpenCV's: the best changes iff count > max(best, 2), then niters =
+ *    RANSACUpdateNumIters(conf, (n - count) / n, 3, niters) (ransac_update_num_iters<3>), and it stops at h >= niters; it is
+ *    replayed one hypothesis at a time, so the stopping point does not depend on the round size.
+ * 5. Refine.  Over the best model's inliers, at most RB_ABS_GN_ITERS Gauss-Newton steps on their summed squared reprojection
+ *    error: the update is R <- Exp(d_omega) R, t <- t + d_t, with Exp as in bundle rule 3, and (J^T J) d = -J^T r is solved by
+ *    Cholesky.  A step is kept only if it lowers the cost and every used depth stays > 0; the first rejected step (or a pivot that
+ *    is not > 0 and finite) stops.  Then the inlier set is recomputed once against the refined pose by rule 4.
+ * 6. Output.  ok[b] = 1 when a model exists; an item with fewer than 3 points has none.  R [batch, 3, 3], t [batch, 3], num_inliers
+ *    [batch] int64 and mask [total] uint8 are zero where ok is 0.
+ * 7. Determinism.  Integer counts, no float atomics, and every reduction in a fixed order, so reruns are byte-identical.
+ *   romab200_abspose_hypotheses  one thread per hypothesis of round `round`: rules 1-3.
+ *   romab200_abspose_score       thread = (hypothesis, solution slot), the model in registers, the item's points streamed through
+ *                                shared memory; grid.y cuts the points into slices whose integer partial counts `select` adds.
+ *   romab200_abspose_select      one thread per item replays rule 4's loop over the round and sets running[0] when an item needs
+ *                                another round.
+ *   romab200_abspose_refine      one CTA per item: rule 5, the 6 x 6 normal equations and the cost summed by cta_sum (a fixed
+ *                                order), then rule 6.
+ * The caller zero-fills `state` before round 0 and calls hypotheses / score / select for rounds 0, 1, ... while running[0] != 0 and
+ * round * RB_ABS_ROUND < max_iters, then refine once.  With max_iters <= RB_ABS_ROUND nothing is read back. */
+#define RB_ABS_ROUND 256
+#define RB_ABS_MAX_SOL 4
+#define RB_ABS_MAX_SPLITS 16
+#define RB_ABS_SLICE 1024
+#define RB_ABS_GN_ITERS 10
+#define RB_ABS_POLISH_ITERS 5
+#define RB_ABS_CTR 0x41425300u
+#define RB_ABS_MAX_BATCH 16383  /* the score's grid.z holds batch * RB_ABS_MAX_SOL */
+#define RB_ABS_STATE 8        /* state[b, :]: iter, niters, best count, best hypothesis, best solution, running, n, unused */
+typedef struct {
+    int32_t batch;
+    const double* x;                      /* [total, 2] pixels */
+    const double* X;                      /* [total, 3] world points */
+    const int64_t* offsets;               /* [batch + 1] */
+    const double* K;                      /* [batch, 3, 3] */
+    int64_t max_n;                        /* largest item (sizes the point slices of the score) */
+    double max_error2, conf;
+    int32_t max_iters, round;
+    uint64_t seed;
+    int32_t* sample;                      /* [batch, RB_ABS_ROUND, 3] drawn indices of the round */
+    double* models;                       /* [batch, RB_ABS_ROUND, RB_ABS_MAX_SOL, 12] R (row-major), t of the round */
+    int32_t* nsol;                        /* [batch, RB_ABS_ROUND] */
+    int32_t* counts;                      /* [batch, splits, RB_ABS_MAX_SOL, RB_ABS_ROUND] partial inlier counts, splits =
+                                             max(1, min(RB_ABS_MAX_SPLITS, ceil(max_n / RB_ABS_SLICE))) */
+    int32_t* state;                       /* [batch, RB_ABS_STATE] */
+    double* best;                         /* [batch, 12] the best model of the loop */
+    int32_t* running;                     /* [1] */
+    double* R; double* t;                 /* [batch, 3, 3], [batch, 3] */
+    uint8_t* ok;                          /* [batch] */
+    int64_t* num_inliers;                 /* [batch] */
+    uint8_t* mask;                        /* [total] */
+} rb_abspose_args;
+int romab200_abspose_hypotheses(const rb_abspose_args* args, void* stream);
+int romab200_abspose_score(const rb_abspose_args* args, void* stream);
+int romab200_abspose_select(const rb_abspose_args* args, void* stream);
+int romab200_abspose_refine(const rb_abspose_args* args, void* stream);
+
+/* ---- image registration: the correspondences of listed images against triangulated tracks, gathered for the absolute-pose
+ *      estimator ----
+ * Not in the reference.  The input is a match graph's kp_offsets [num_images + 1] int64 and keypoints [K, 2] fp32, the tracks
+ * (track_offsets, elements) and per track ok [num_tracks] uint8 and X [num_tracks, 3] float64.  The correspondences of image i are the
+ * elements (i, a) of tracks k with ok[k], in element order; each has x = keypoints[kp_offsets[i] + a] widened to float64 and X = X[k].
+ * Every element's ids are checked, 0 <= i < num_images and 0 <= a < K_i, and a bad one sets RB_REG_BAD_ID in info[0]; the caller reads
+ * it before any kernel indexes with the ids.
+ * romab200_register_setup: info [1] int64 is zeroed; a warp per track checks its elements and writes keys (image << 32 | e, image =
+ *   num_images for an element of a track that is not ok or of a bad id) [num_elements]; radix_sort_hi32 (common.cuh) sorts them stably
+ *   by image (keys_alt, hist RADIX_DIGITS ceil(num_elements / RB_TRACKS_TILE) + 1 int32); image_offsets [num_images + 1] int64 is the
+ *   start of each image's correspondences, elem [num_elements] int32 the element ids in sorted order and track [num_elements] int32
+ *   the track of every element (by element id).
+ * romab200_register_gather: for the chunk's images `images` [num_list] int32, packed at out_offsets [num_list + 1] int64 (the host's
+ *   exclusive scan of their counts), x [total, 2] and X [total, 3] float64: the x / X / offsets layout of rb_abspose_args.
+ * Device bytes of one estimator chunk of B images with `total` correspondences and S = max(1, min(RB_ABS_MAX_SPLITS,
+ * ceil(max_n / RB_ABS_SLICE))) score slices (max_n its largest image), the buffers register.py allocates per chunk:
+ *   B (RB_REG_ITEM_BYTES + RB_REG_SLICE_BYTES S) + RB_REG_POINT_BYTES max(total, 1) + RB_REG_CHUNK_BYTES
+ *   per item sample 3 072, models 98 304, nsol 1 024, state 32, best 96, R 72, t 24, ok 1, num_inliers 8, K 72, images 4, offsets 8;
+ *   per item and slice counts 4 096; per point x 16, X 24, mask 1; once running 4 and offsets 8. */
+#define RB_REG_BAD_ID 1
+#define RB_REG_ITEM_BYTES 102717
+#define RB_REG_SLICE_BYTES 4096
+#define RB_REG_POINT_BYTES 41
+#define RB_REG_CHUNK_BYTES 12
+typedef struct {
+    int32_t num_tracks, num_images;
+    const int64_t* track_offsets; const int32_t* elements; int64_t num_elements;
+    const int64_t* kp_offsets; const float* keypoints; int64_t num_rows;
+    const uint8_t* track_ok; const double* points;                     /* [num_tracks], [num_tracks, 3] */
+    int64_t* info;                                                      /* [1] status */
+    uint64_t* keys; uint64_t* keys_alt; int32_t* hist;
+    int64_t* image_offsets; int32_t* elem; int32_t* track;
+    int32_t num_list; const int32_t* images; const int64_t* out_offsets;  /* gather only: */
+    double* x; double* X;
+} rb_register_args;
+int romab200_register_setup(const rb_register_args* args, void* stream);
+int romab200_register_gather(const rb_register_args* args, void* stream);
 
 #ifdef __cplusplus
 }

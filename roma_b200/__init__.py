@@ -23,7 +23,7 @@ def __getattr__(name):
         from .jpeg import decode_jpeg
         return decode_jpeg
     if name in ("estimate_pose", "estimate_pose_batched", "find_homography", "find_homography_batched", "RANSAC", "find_fundamental",
-                "find_fundamental_batched", "USAC_MAGSAC"):
+                "find_fundamental_batched", "USAC_MAGSAC", "estimate_absolute_pose", "estimate_absolute_pose_batched"):
         from . import geometry
         return getattr(geometry, name)
     if name in ("consolidate_matches", "MatchGraph"):
@@ -38,6 +38,9 @@ def __getattr__(name):
     if name in ("triangulate_tracks", "Points3D"):
         from . import triangulate
         return getattr(triangulate, name)
+    if name in ("register_images", "Registration"):
+        from . import register
+        return getattr(register, name)
     if name in ("bundle_adjust", "BundleResult"):
         from . import bundle
         return getattr(bundle, name)

@@ -79,6 +79,11 @@ RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEA
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
     for name in ("RB_BA_BAD_ID", "RB_BA_REPEATED", "RB_BA_CAM", "RB_BA_TRACK", "RB_BA_RESULT", "RB_BA_NB", "RB_BA_ELEMENT_BYTES",
                  "RB_BA_TRACK_BYTES", "RB_BA_IMAGE_BYTES", "RB_BA_FREE_BYTES", "RB_BA_ONCE_BYTES"))
+(RB_ABS_ROUND, RB_ABS_MAX_SOL, RB_ABS_MAX_SPLITS, RB_ABS_SLICE, RB_ABS_STATE, RB_ABS_MAX_BATCH, RB_REG_BAD_ID, RB_REG_ITEM_BYTES, RB_REG_SLICE_BYTES,
+ RB_REG_POINT_BYTES, RB_REG_CHUNK_BYTES) = (
+    int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+    for name in ("RB_ABS_ROUND", "RB_ABS_MAX_SOL", "RB_ABS_MAX_SPLITS", "RB_ABS_SLICE", "RB_ABS_STATE", "RB_ABS_MAX_BATCH", "RB_REG_BAD_ID", "RB_REG_ITEM_BYTES",
+                 "RB_REG_SLICE_BYTES", "RB_REG_POINT_BYTES", "RB_REG_CHUNK_BYTES"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -189,6 +194,13 @@ _FIELD_DTYPES = {
                    "elem_track": torch.int32, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32, "obs_offsets": torch.int64,
                    "obs": torch.int32, "cams": _F64, "X": _F64, "cams_trial": _F64, "X_trial": _F64, "W": _F64, "track_sys": _F64,
                    "cam_sys": _F64, "S": _F64, "rhs": _F64, "cam_pred": _F64, "track_part": _F64, "result": _F64, "error": _F64},
+    "rb_abspose_args": {"x": _F64, "X": _F64, "offsets": torch.int64, "K": _F64, "sample": torch.int32, "models": _F64, "nsol": torch.int32,
+                        "counts": torch.int32, "state": torch.int32, "best": _F64, "running": torch.int32, "R": _F64, "t": _F64, "ok": torch.uint8,
+                        "num_inliers": torch.int64, "mask": torch.uint8},
+    "rb_register_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "track_ok": torch.uint8,
+                         "points": _F64, "info": torch.int64, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32,
+                         "image_offsets": torch.int64, "elem": torch.int32, "track": torch.int32, "images": torch.int32,
+                         "out_offsets": torch.int64, "x": _F64, "X": _F64},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -291,12 +303,36 @@ def _ba_min_elems(kw):
             "S": n * n, "rhs": n, "cam_pred": N, "track_part": 3 * T, "result": RB_BA_RESULT, "error": T}
 
 
+def abspose_splits(max_n) -> int:
+    """Score slices of an absolute-pose launch whose largest item has max_n points (include/romab200.h)."""
+    return max(1, min(RB_ABS_MAX_SPLITS, -(-int(max_n) // RB_ABS_SLICE)))
+
+
+def _abspose_min_elems(kw):
+    B, total = kw["batch"], kw["x"].numel() // 2
+    splits = abspose_splits(kw["max_n"])
+    return {"x": 2 * total, "X": 3 * total, "offsets": B + 1, "K": 9 * B, "sample": 3 * B * RB_ABS_ROUND, "models": 12 * B * RB_ABS_ROUND * RB_ABS_MAX_SOL,
+            "nsol": B * RB_ABS_ROUND, "counts": B * splits * RB_ABS_MAX_SOL * RB_ABS_ROUND,
+            "state": B * RB_ABS_STATE, "best": 12 * B, "running": 1, "R": 9 * B, "t": 3 * B, "ok": B, "num_inliers": B, "mask": total}
+
+
+def _register_min_elems(kw):
+    T, N, E = kw["num_tracks"], kw["num_images"], kw["num_elements"]
+    out = {"track_offsets": T + 1, "elements": 2 * E, "kp_offsets": N + 1, "keypoints": 2 * kw["num_rows"], "track_ok": T, "points": 3 * T,
+           "info": 1, "keys": E, "keys_alt": E, "hist": 256 * ((E + RB_TRACKS_TILE - 1) // RB_TRACKS_TILE) + 1, "image_offsets": N + 1,
+           "elem": E, "track": E}
+    if kw.get("num_list"):
+        total = kw["x"].numel() // 2
+        out.update(images=kw["num_list"], out_offsets=kw["num_list"] + 1, X=3 * total)
+    return out
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
               "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
-              "rb_ba_args": _ba_min_elems}
+              "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

@@ -9,7 +9,6 @@
 //   step       the trial cameras (Rodrigues), then a warp per track: d_X, the trial cost and the depth check; fixed-order tree sums.
 // No float atomics and a fixed order in every reduction, so the result is bit-identical from run to run.
 #include "common.cuh"
-#include <math_constants.h>
 
 namespace rb {
 
@@ -406,24 +405,6 @@ __global__ void __launch_bounds__(1024) ba_potrs_kernel(const double* __restrict
 }
 
 // ---- step ---------------------------------------------------------------------------------------------------------------------
-// rule 3: Exp(w) by Rodrigues, with the small-angle branch I + [w]x for theta^2 <= 2^-52
-__device__ __forceinline__ void ba_exp(const double (&w)[3], double (&E)[3][3]) {
-    const double t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
-    if (t2 > 0x1p-52) {
-        const double th = sqrt(t2), k0 = w[0] / th, k1 = w[1] / th, k2 = w[2] / th;
-        double s, c;
-        sincospi(th * (1.0 / CUDART_PI), &s, &c);      // sincospi: its argument reduction is exact and needs no stack
-        const double c1 = 1.0 - c;
-        E[0][0] = c + c1 * k0 * k0;      E[0][1] = c1 * k0 * k1 - s * k2; E[0][2] = c1 * k0 * k2 + s * k1;
-        E[1][0] = c1 * k1 * k0 + s * k2; E[1][1] = c + c1 * k1 * k1;      E[1][2] = c1 * k1 * k2 - s * k0;
-        E[2][0] = c1 * k2 * k0 - s * k1; E[2][1] = c1 * k2 * k1 + s * k0; E[2][2] = c + c1 * k2 * k2;
-    } else {
-        E[0][0] = 1.0;   E[0][1] = -w[2]; E[0][2] = w[1];
-        E[1][0] = w[2];  E[1][1] = 1.0;   E[1][2] = -w[0];
-        E[2][0] = -w[1]; E[2][1] = w[0];  E[2][2] = 1.0;
-    }
-}
-
 __global__ void __launch_bounds__(128) ba_step_cameras_kernel(rb_ba_args a) {
     pdl_wait();
     const int i = blockIdx.x * 128 + threadIdx.x;
@@ -443,7 +424,7 @@ __global__ void __launch_bounds__(128) ba_step_cameras_kernel(rb_ba_args a) {
     for (int j = 0; j < 6; ++j) pred += d[j] * (a.lambda * a.cam_sys[12 * (int64_t)fi + 6 + j] * d[j] - a.cam_sys[12 * (int64_t)fi + j]);
     const double w[3] = {d[0], d[1], d[2]};
     double E[3][3];
-    ba_exp(w, E);
+    so3_exp(w, E);
 #pragma unroll
     for (int r = 0; r < 3; ++r)
 #pragma unroll

@@ -8,6 +8,7 @@
 #include <stdio.h>
 #include <stdarg.h>
 #include <type_traits>
+#include <math_constants.h>
 #include "../../include/romab200.h"
 
 namespace rb {
@@ -244,6 +245,24 @@ __global__ void __launch_bounds__(1024) scan_counts_kernel(T* __restrict__ v, in
         run += c;
     }
     if (threadIdx.x == 1023) v[n] = run;
+}
+
+// Exp(w) by Rodrigues (bundle rule 3, absolute-pose rule 5), with the small-angle branch I + [w]x for theta^2 <= 2^-52
+__device__ __forceinline__ void so3_exp(const double (&w)[3], double (&E)[3][3]) {
+    const double t2 = w[0] * w[0] + w[1] * w[1] + w[2] * w[2];
+    if (t2 > 0x1p-52) {
+        const double th = sqrt(t2), k0 = w[0] / th, k1 = w[1] / th, k2 = w[2] / th;
+        double s, c;
+        sincospi(th * (1.0 / CUDART_PI), &s, &c);      // sincospi: its argument reduction is exact and needs no stack
+        const double c1 = 1.0 - c;
+        E[0][0] = c + c1 * k0 * k0;      E[0][1] = c1 * k0 * k1 - s * k2; E[0][2] = c1 * k0 * k2 + s * k1;
+        E[1][0] = c1 * k1 * k0 + s * k2; E[1][1] = c + c1 * k1 * k1;      E[1][2] = c1 * k1 * k2 - s * k0;
+        E[2][0] = c1 * k2 * k0 - s * k1; E[2][1] = c1 * k2 * k1 + s * k0; E[2][2] = c + c1 * k2 * k2;
+    } else {
+        E[0][0] = 1.0;   E[0][1] = -w[2]; E[0][2] = w[1];
+        E[1][0] = w[2];  E[1][1] = 1.0;   E[1][2] = -w[0];
+        E[2][0] = -w[1]; E[2][1] = w[0];  E[2][2] = 1.0;
+    }
 }
 
 // ---- stable LSD radix sort of 64-bit keys by their high 32 bits, 8-bit digits, tiles of TILE keys --------------------------------

@@ -32,9 +32,17 @@ __device__ __forceinline__ double tri_depth(const double* c, const double (&X)[3
     return c[12] * X[0] + c[13] * X[1] + c[14] * X[2] + c[15];
 }
 
-// rule 4: depth > 0 and squared reprojection error <= max_error2; *err2 receives the squared error
+// the observation's image is not among the registered images: it is not an observation (its other camera entries are not read)
+__device__ __forceinline__ bool tri_excluded(const TriObs& o) { return o.cam[19] != 0.0; }
+
+// rule 4: depth > 0 and squared reprojection error <= max_error2; *err2 receives the squared error.  An observation of an excluded
+// image is never an inlier.
 __device__ __forceinline__ bool tri_inlier(const TriObs& o, const double (&X)[3], double max_error2, double* err2) {
     const double* c = o.cam;
+    if (tri_excluded(o)) {
+        *err2 = 0.0;
+        return false;
+    }
     const double p0 = c[0] * X[0] + c[1] * X[1] + c[2] * X[2] + c[3];
     const double p1 = c[4] * X[0] + c[5] * X[1] + c[6] * X[2] + c[7];
     const double p2 = c[8] * X[0] + c[9] * X[1] + c[10] * X[2] + c[11];
@@ -192,7 +200,7 @@ __device__ void tri_track(const rb_tri_args& a, int k, int lane) {
                 q = id[1];
             }
             const TriObs op = tri_obs(a, base + p), oq = tri_obs(a, base + q);
-            if (op.img == oq.img) continue;
+            if (op.img == oq.img || tri_excluded(op) || tri_excluded(oq)) continue;
             double M[4][4] = {}, Xh[3];
             tri_dlt_add(op, M);
             tri_dlt_add(oq, M);

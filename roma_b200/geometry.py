@@ -388,3 +388,96 @@ def find_fundamental(points1, points2, method=USAC_MAGSAC, ransacReprojThreshold
     if not bool(ok[0]):
         return None, masks[0]
     return F[0], masks[0]
+
+
+# ---- absolute pose -------------------------------------------------------------------------------------------------------
+# include/romab200.h: RB_ABS_ROUND, RB_ABS_MAX_SOL, RB_ABS_STATE, RB_ABS_MAX_BATCH
+ABS_ROUND, ABS_MAX_SOL, ABS_STATE, ABS_MAX_BATCH = cabi.RB_ABS_ROUND, cabi.RB_ABS_MAX_SOL, cabi.RB_ABS_STATE, cabi.RB_ABS_MAX_BATCH
+
+
+def _abs_points(p, dev, width, name):
+    """[n, width] real points of any float dtype -> float64 [n, width] on `dev`."""
+    t = p if isinstance(p, torch.Tensor) else torch.as_tensor(np.asarray(p))
+    if t.dim() != 2 or t.shape[1] != width:
+        raise ValueError(f"{name} must be [n, {width}], got {tuple(t.shape)}")
+    if not t.dtype.is_floating_point:
+        raise TypeError(f"{name} must have a float dtype, got {t.dtype}")
+    return t.to(dev, torch.float64).contiguous()
+
+
+def _abs_args(max_error, confidence, max_iters, seed):
+    """Checks the estimator's scalar arguments; returns (max_error^2, confidence, max_iters, seed)."""
+    max_error, confidence = float(max_error), float(confidence)
+    if not (math.isfinite(max_error) and max_error > 0):
+        raise ValueError(f"max_error must be finite and > 0, got {max_error!r}")
+    if not 0 < confidence < 1:
+        raise ValueError(f"confidence must lie in (0, 1), got {confidence!r}")
+    if isinstance(max_iters, bool) or not 1 <= int(max_iters) < 1 << 31 or int(max_iters) != max_iters:
+        raise ValueError(f"max_iters must be an int in [1, 2^31), got {max_iters!r}")
+    if isinstance(seed, bool) or int(seed) != seed or not 0 <= int(seed) < 1 << 64:
+        raise ValueError(f"seed must be an int in [0, 2^64), got {seed!r}")
+    return max_error * max_error, confidence, int(max_iters), int(seed)
+
+
+def _abs_launch(x, X, offsets, K, max_n, max_error2, conf, max_iters, seed):
+    """Enqueues the whole absolute-pose estimate on the current stream.  x: float64 [total, 2], X: float64 [total, 3] device tensors
+    (total >= 1), offsets: int64 [B + 1], K: float64 [B, 3, 3].  With max_iters <= ABS_ROUND this is one round and reads nothing
+    back; each further round costs one 4-byte read of the `running` flag.  Returns the buffers (R, t, ok, num_inliers, mask, ...);
+    their bytes are include/romab200.h's per-chunk formula of image registration, less the gathered points and image list."""
+    dev = x.device
+    B = offsets.numel() - 1
+    total = x.shape[0]
+    S = cabi.abspose_splits(max_n)
+    f64, i32 = dict(device=dev, dtype=torch.float64), dict(device=dev, dtype=torch.int32)
+    buf = dict(sample=torch.empty(B, ABS_ROUND, 3, **i32), models=torch.empty(B, ABS_ROUND, ABS_MAX_SOL, 12, **f64),
+               nsol=torch.empty(B, ABS_ROUND, **i32), counts=torch.empty(B, S, ABS_MAX_SOL, ABS_ROUND, **i32),
+               state=torch.zeros(B, ABS_STATE, **i32), best=torch.zeros(B, 12, **f64), running=torch.zeros(1, **i32),
+               R=torch.empty(B, 3, 3, **f64), t=torch.empty(B, 3, **f64), ok=torch.empty(B, device=dev, dtype=torch.uint8),
+               num_inliers=torch.empty(B, device=dev, dtype=torch.int64), mask=torch.empty(total, device=dev, dtype=torch.uint8))
+    kw = dict(batch=B, x=x, X=X, offsets=offsets, K=K, max_n=int(max_n), max_error2=float(max_error2), conf=float(conf),
+              max_iters=int(max_iters), seed=int(seed) & (2 ** 64 - 1), round=0, **buf)
+    _ransac_rounds("abspose", "rb_abspose_args", kw, ABS_ROUND)
+    cabi.call("romab200_abspose_refine", "rb_abspose_args", **kw)
+    return buf
+
+
+def estimate_absolute_pose_batched(points2D_list, points3D_list, K, *, max_error=12.0, confidence=0.9999, max_iters=10000, seed=0):
+    """Absolute pose of B cameras x ~ K (R X + t) from ragged sets of pixels points2D_list[b] [n_b, 2] and world points
+    points3D_list[b] [n_b, 3] of any float dtype (widened to float64); K is one [3, 3] for every item or [B, 3, 3].  COLMAP's
+    EstimateAbsolutePose + RefineAbsolutePose on the device (csrc/absolute_pose.cu, the rules in include/romab200.h): Lambda Twist
+    P3P on Philox-drawn samples, the model with the most points within `max_error` px and in front of the camera (OpenCV's RANSAC
+    loop and stopping rule at `confidence`, at most `max_iters` hypotheses), then Gauss-Newton on its inliers and the inliers
+    recomputed once.  Every item draws the stream keyed by `seed` alone, so item b is bit-identical to a call on that item alone.
+    Returns (R [B, 3, 3] float64, t [B, 3] float64, ok [B] bool, num_inliers [B] int64, masks: list of bool [n_b]); numpy inputs give
+    numpy outputs, tensors give device tensors.  ok[b] is False, and R, t, the mask zero, where no model was found or n_b < 3.
+    Host reads: the `running` flag once per round of RB_ABS_ROUND hypotheses before the last."""
+    max_error2, conf, max_iters, seed = _abs_args(max_error, confidence, max_iters, seed)
+    if len(points2D_list) != len(points3D_list) or len(points2D_list) == 0:
+        raise ValueError("points2D_list and points3D_list must be non-empty and of the same length")
+    if len(points2D_list) > ABS_MAX_BATCH:
+        raise ValueError(f"at most {ABS_MAX_BATCH} items per call, got {len(points2D_list)}")
+    dev = _device("estimate_absolute_pose")
+    xs = [_abs_points(p, dev, 2, "points2D") for p in points2D_list]
+    Xs = [_abs_points(p, dev, 3, "points3D") for p in points3D_list]
+    for a, b in zip(xs, Xs):
+        if a.shape[0] != b.shape[0]:
+            raise ValueError(f"points2D and points3D differ in length: {a.shape[0]} vs {b.shape[0]}")
+    ns = [a.shape[0] for a in xs]
+    B = len(ns)
+    offsets = torch.tensor(np.concatenate([[0], np.cumsum(ns)]), dtype=torch.int64, device=dev)
+    if not sum(ns):
+        xs, Xs = [torch.zeros(1, 2, dtype=torch.float64, device=dev)], [torch.zeros(1, 3, dtype=torch.float64, device=dev)]
+    Kt = _intrinsics(K, B, dev).contiguous()
+    buf = _abs_launch(torch.cat(xs), torch.cat(Xs), offsets, Kt, max(ns), max_error2, conf, max_iters, seed)
+    masks = list(buf["mask"][:sum(ns)].bool().split(ns))
+    return _outputs(not isinstance(points2D_list[0], torch.Tensor), buf["R"], buf["t"], buf["ok"].bool(), buf["num_inliers"], masks)
+
+
+def estimate_absolute_pose(points2D, points3D, K, *, max_error=12.0, confidence=0.9999, max_iters=10000, seed=0):
+    """`estimate_absolute_pose_batched` for one camera: None when no model is found (or fewer than 3 points), otherwise
+    (R float64 [3, 3], t float64 [3], mask bool [n]) with x ~ K (R X + t).  numpy in gives numpy out; tensors give device tensors."""
+    R, t, ok, _, masks = estimate_absolute_pose_batched([points2D], [points3D], K, max_error=max_error, confidence=confidence,
+                                                        max_iters=max_iters, seed=seed)
+    if not bool(ok[0]):
+        return None
+    return R[0], t[0], masks[0]

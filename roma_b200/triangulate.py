@@ -47,7 +47,8 @@ def _float64(name, v, shape, what="triangulate_tracks"):
 
 
 def camera_table(K, R, t) -> np.ndarray:
-    """The float64 camera table of rule 1, [N, RB_TRI_CAM] per image: P = K [R | t] (12, row-major), row 2 of R, t_z, C = -R^T t, 0."""
+    """The float64 camera table of rule 1, [N, RB_TRI_CAM] per image: P = K [R | t] (12, row-major), row 2 of R, t_z, C = -R^T t, and
+    the exclusion flag 0 (triangulate_tracks sets it to 1 for the images not among `images`)."""
     N = K.shape[0]
     tab = np.zeros((N, cabi.RB_TRI_CAM))
     tab[:, :12] = (K @ np.concatenate((R, t[:, :, None]), 2)).reshape(N, 12)
@@ -55,6 +56,22 @@ def camera_table(K, R, t) -> np.ndarray:
     tab[:, 15] = t[:, 2]
     tab[:, 16:19] = -np.einsum("nji,nj->ni", R, t)
     return tab
+
+
+def image_list(images, N, what):
+    """`images`: distinct ints in [0, N), as a list, or ValueError."""
+    images = images.tolist() if isinstance(images, (torch.Tensor, np.ndarray)) else list(images)
+    try:
+        if any(isinstance(i, (bool, np.bool_)) for i in images):
+            raise TypeError
+        out = [operator.index(i) for i in images]
+    except TypeError:
+        raise ValueError(f"{what}: images must hold ints, got {images!r}") from None
+    if any(not 0 <= i < N for i in out):
+        raise ValueError(f"{what}: images must lie in [0, {N}), got {out}")
+    if len(set(out)) != len(out):
+        raise ValueError(f"{what}: images must be distinct, got {out}")
+    return out
 
 
 def _check(graph, tracks, K, R, t, max_error, min_angle, max_hypotheses, seed, what="triangulate_tracks", device=True):
@@ -126,7 +143,7 @@ def _check_device(tensors, what):
 
 
 def triangulate_tracks(graph: MatchGraph, tracks: Tracks, K, R, t, *, max_error=4.0, min_angle=1.5, max_hypotheses=256,
-                       seed=0) -> Points3D:
+                       seed=0, images=None) -> Points3D:
     """The 3-D point of every track of `tracks` (built from `graph`) seen by cameras x ~ K[i] (R[i] X + t[i]) in pixels of the
     image_sizes frame (x = (W / 2) (u + 1), `synthetic.planted_cameras`' convention).  K, R [N, 3, 3] and t [N, 3] are tensors or
     arrays of any float dtype, widened to float64 on the host.  Only graph.kp_offsets and graph.keypoints are read.
@@ -135,6 +152,9 @@ def triangulate_tracks(graph: MatchGraph, tracks: Tracks, K, R, t, *, max_error=
     when it has more; the point with the most observations within `max_error` px (and in front of their cameras) wins, ties to the
     first; a multi-view DLT and at most RB_TRI_GN_ITERS Gauss-Newton steps over those inliers refine it; the inliers are recomputed
     once, and the track is ok when two of them, in distinct images, see the point under an angle of at least `min_angle` degrees.
+    `images` (distinct ints in [0, N), or None for all) lists the registered cameras: an element of any other image is not an
+    observation, a pair that contains it is skipped but keeps its index, and it is never an inlier, so the cameras of the other images
+    are not used (they must still be finite).  With images=None the result is byte-identical to the call without the argument.
     The defaults of max_error (4 px) and min_angle (1.5 degrees) are COLMAP's triangulator.  With keypoints snapped to 1 px cells
     (`consolidate_matches`) and 0.5 px noise, the largest reprojection error of a true observation is about 2 px, so 4 px keeps them
     all; the cell's quantisation grows with cell_size, and at cell_size 4 it reaches about 4 px, so the default cuts a few true
@@ -145,6 +165,10 @@ def triangulate_tracks(graph: MatchGraph, tracks: Tracks, K, R, t, *, max_error=
     kp_off, tr_off, table, max_error2, min_angle, max_hypotheses, seed = _check(graph, tracks, K, R, t, max_error, min_angle,
                                                                                 max_hypotheses, seed)
     N, T, E = len(kp_off) - 1, len(tr_off) - 1, tr_off[-1]
+    if images is not None:
+        registered = np.zeros(N, bool)
+        registered[image_list(images, N, "triangulate_tracks")] = True
+        table[:, 19] = np.where(registered, 0.0, 1.0)
     dev = graph.kp_offsets.device
     with torch.cuda.device(dev):
         X = torch.zeros(T, 3, dtype=torch.float64, device=dev)
