@@ -49,9 +49,12 @@ def _rho(s, c2):
 
 
 def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier, K, R, t, *, fixed_poses=(0,), fixed_tx=(1,),
-                  loss_scale=None, max_iterations=50, function_tolerance=1e-6):
+                  loss_scale=None, max_iterations=50, function_tolerance=1e-6, systems=None):
     """Rules 1-7.  Returns dict(R, t, X, cost [n + 1], accepted [n], termination, trials: per trial F, F_new, pred, rho, margin
-    (rho - 1e-3), step (the largest |d| entry))."""
+    (rho - 1e-3), step (the largest |d| entry)).  A list `systems` receives one dict per trial: lam, the reduced camera system S
+    [6F, 6F] and b [6F] after rule 4, the step dc [6F], Dc [F, 6] (the clamped diagonal of U) and S_abs, b_abs: the same assembly
+    over the absolute value of every term, the scale of the rounding error of any summation order (zero on the rows and
+    columns rule 4 sets)."""
     kpo, xy = _arr(kp_offsets, np.int64), _arr(keypoints, np.float64)
     off, el = _arr(track_offsets, np.int64), _arr(elements, np.int64).reshape(-1, 2)
     X, okb, inl = _arr(X, np.float64).copy(), _arr(ok, bool), _arr(inlier, bool)
@@ -115,6 +118,17 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
         for fi, i in enumerate(free):
             S[6 * fi:6 * fi + 6, 6 * fi:6 * fi + 6] = U[i] + lam * np.diag(Dc[i])
             b[6 * fi:6 * fi + 6] = -gc[i]
+        if systems is not None:
+            aJc, aJX, ar = np.abs(Jc), np.abs(JX), np.abs(r)                 # w > 0
+            Uabs, gcabs, gpabs = np.zeros((N, 6, 6)), np.zeros((N, 6)), np.zeros((T, 3))
+            np.add.at(Uabs, img, np.einsum("m,mai,maj->mij", w, aJc, aJc))
+            np.add.at(gcabs, img, np.einsum("m,mai,ma->mi", w, aJc, ar))
+            np.add.at(gpabs, trk, np.einsum("m,mai,ma->mi", w, aJX, ar))
+            Wabs, Vabs = np.einsum("m,mai,maj->mij", w, aJc, aJX), np.abs(Vinv)
+            S_abs, b_abs = np.zeros((n, n)), np.zeros(n)
+            for fi, i in enumerate(free):
+                S_abs[6 * fi:6 * fi + 6, 6 * fi:6 * fi + 6] = Uabs[i] + lam * np.diag(Dc[i])
+                b_abs[6 * fi:6 * fi + 6] = gcabs[i]
         order = np.argsort(trk, kind="stable")
         bounds = np.searchsorted(trk[order], np.arange(T + 1))
         for k in range(T):
@@ -129,12 +143,21 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
             for a_ in range(m.size):                                       # a track's images are distinct
                 b[6 * f[a_]:6 * f[a_] + 6] += Ak[a_] @ gp[k]
                 S4[f[a_], :, f, :] -= blocks[a_]
+            if systems is not None:
+                Aabs = Wabs[m] @ Vabs[k]
+                S4abs = S_abs.reshape(F_, 6, F_, 6)
+                blocks_abs = np.einsum("arm,bcm->abrc", Aabs, Wabs[m])
+                for a_ in range(m.size):
+                    b_abs[6 * f[a_]:6 * f[a_] + 6] += Aabs[a_] @ gpabs[k]
+                    S4abs[f[a_], :, f, :] += blocks_abs[a_]
         for fi in tx:
             j = 6 * fi + 3
             S[j, :] = 0.0
             S[:, j] = 0.0
             S[j, j] = 1.0
             b[j] = 0.0
+            if systems is not None:
+                S_abs[j, :] = S_abs[:, j] = b_abs[j] = 0.0
         dc = np.zeros(n)
         pivot_ok = True
         if n:
@@ -143,6 +166,8 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
                 dc = np.linalg.solve(L.T, np.linalg.solve(L, b))
             except np.linalg.LinAlgError:
                 pivot_ok = False
+        if systems is not None:
+            systems.append(dict(lam=lam, S=S, b=b, dc=dc, Dc=Dc[free], S_abs=S_abs, b_abs=b_abs))
         dC = np.zeros((N, 6))
         dC[free] = dc.reshape(F_, 6)
         bX = np.zeros((T, 3))

@@ -1,6 +1,7 @@
 """CPU tests of bundle adjustment (`bundle_adjust`): the numpy oracle against `scipy.optimize.least_squares` on perturbed
-`planted_cameras` scenes with both losses, Rodrigues and its small-angle branch, the camera-major list, `perturb_cameras`, every
-argument rule (raised before any device work), the gauge defaults and the workspace formula."""
+`planted_cameras` scenes with both losses, the oracle's reduced camera system against a dense Schur complement, Rodrigues and its
+small-angle branch, the camera-major list, `perturb_cameras`, every argument rule (raised before any device work), the gauge
+defaults and the workspace formula."""
 import math
 
 import numpy as np
@@ -222,3 +223,80 @@ def test_entry_points_and_exports():
     assert roma_b200.bundle_adjust is rb_ba.bundle_adjust and roma_b200.BundleResult is rb_ba.BundleResult
     assert cabi.RB_BA_CAM == 21 and cabi.RB_BA_TRACK == 13 and cabi.RB_BA_NB == 32
     assert not any(f.startswith("dtype") for f, _ in cabi.STRUCT_FIELDS["rb_ba_args"])
+
+
+def test_oracle_system_equals_the_dense_schur_complement():
+    """The oracle's reduced camera system (`systems`) against one built without its block assembly: the dense Jacobian of every
+    used observation (checked against central differences), the damped H = J^T W J + lambda D, and H_cc - H_cp H_pp^-1 H_pc on the
+    free cameras with rule 4 applied, under a gauge with a gap in the free cameras and a fixed_tx camera that is also fixed."""
+    g, tr, tri, K, R, t, Rt, tt = oracle_scene(5, 4, 50)
+    fixed_poses, fixed_tx, c2 = (1,), (0, 1, 3), 1.0
+    systems = []
+    ref = oracle_ba(g["kp_offsets"], g["keypoints"], tr["track_offsets"], tr["elements"], tri["X"], tri["ok"], tri["inlier"], K, R, t,
+                    fixed_poses=fixed_poses, fixed_tx=fixed_tx, loss_scale=1.0, max_iterations=1, systems=systems)
+    assert len(systems) == 1 and len(ref["trials"]) == 1
+    off, el = tr["track_offsets"], tr["elements"].astype(np.int64)
+    N, T = K.shape[0], off.size - 1
+    track = np.repeat(np.arange(T), np.diff(off))
+    e = np.flatnonzero(np.repeat(tri["ok"], np.diff(off)) & tri["inlier"])
+    img, trk = el[e, 0], track[e]
+    obs = g["keypoints"].astype(np.float64)[g["kp_offsets"][img] + el[e, 1]]
+    X = tri["X"]
+    nc, M = 6 * N, e.size
+
+    def residuals(p):
+        """r [M, 2] at parameters p = (d_omega, d_t) per camera, then d_X per track, applied as R = Exp(d_omega) R_0."""
+        Rs = np.einsum("nij,njk->nik", Rotation.from_rotvec(p[:nc].reshape(N, 6)[:, :3]).as_matrix(), R)
+        ts, Xs = t + p[:nc].reshape(N, 6)[:, 3:], X + p[nc:].reshape(T, 3)
+        q = np.einsum("mij,mj->mi", K[img], np.einsum("mij,mj->mi", Rs[img], Xs[trk]) + ts[img])
+        return q[:, :2] / q[:, 2:3] - obs
+
+    J = np.zeros((2 * M, nc + 3 * T))
+    for m in range(M):
+        i, k = img[m], trk[m]
+        pc = R[i] @ X[k] + t[i]
+        q = K[i] @ pc
+        dq = np.array([[1 / q[2], 0, -q[0] / q[2] ** 2], [0, 1 / q[2], -q[1] / q[2] ** 2]]) @ K[i]
+        a = R[i] @ X[k]
+        skew = np.array([[0, -a[2], a[1]], [a[2], 0, -a[0]], [-a[1], a[0], 0]])
+        J[2 * m:2 * m + 2, 6 * i:6 * i + 3] = -dq @ skew
+        J[2 * m:2 * m + 2, 6 * i + 3:6 * i + 6] = dq
+        J[2 * m:2 * m + 2, nc + 3 * k:nc + 3 * k + 3] = dq @ R[i]
+    h = 1e-6
+    cols = np.r_[np.arange(nc), (nc + 3 * np.unique(trk)[:5, None] + np.arange(3)).ravel()]
+    for c in cols:
+        d = np.zeros(nc + 3 * T)
+        d[c] = h
+        num = (residuals(d) - residuals(-d)).reshape(-1) / (2 * h)
+        assert np.abs(num - J[:, c]).max() <= 1e-5 * max(1.0, np.abs(J[:, c]).max()), c
+    r = residuals(np.zeros(nc + 3 * T)).reshape(-1)
+    s = (r.reshape(M, 2) ** 2).sum(1)
+    w = np.repeat(1.0 / (1.0 + s / c2), 2)                                  # rule 2: rho'(s) of the Cauchy loss
+    H = J.T @ (w[:, None] * J)
+    grad = J.T @ (w * r)
+    lam = systems[0]["lam"]
+    D = np.clip(np.diag(H), 1e-6, 1e32)
+    H += lam * np.diag(D)
+    free = [i for i in range(N) if i not in fixed_poses]
+    c = (6 * np.asarray(free)[:, None] + np.arange(6)).ravel()
+    p = np.arange(nc, nc + 3 * T)
+    Hpp_inv = np.linalg.inv(H[np.ix_(p, p)])
+    S = H[np.ix_(c, c)] - H[np.ix_(c, p)] @ Hpp_inv @ H[np.ix_(p, c)]
+    b = -grad[c] + H[np.ix_(c, p)] @ Hpp_inv @ grad[p]
+    for fi, i in enumerate(free):
+        if i in fixed_tx:
+            j = 6 * fi + 3
+            S[j], S[:, j], b[j] = 0.0, 0.0, 0.0
+            S[j, j] = 1.0
+    sy = systems[0]
+    assert lam == 1e-4 and sy["S"].shape == (18, 18) and np.allclose(sy["Dc"], D[c].reshape(-1, 6), rtol=1e-12, atol=0)
+    scale = np.abs(S).max()
+    print(f"S: largest difference {np.abs(sy['S'] - S).max() / scale:.1e} of max |S|, b: {np.abs(sy['b'] - b).max() / np.abs(b).max():.1e}")
+    assert np.abs(sy["S"] - S).max() <= 1e-12 * scale and np.abs(sy["b"] - b).max() <= 1e-12 * np.abs(b).max()
+    assert np.allclose(sy["dc"], np.linalg.solve(S, b), rtol=1e-9, atol=1e-12 * np.abs(sy["dc"]).max())
+    # the summation-error bars bound the terms they stand for, and rule 4's entries are exact
+    off_tx = np.ones(18, bool)
+    off_tx[[6 * fi + 3 for fi, i in enumerate(free) if i in fixed_tx]] = False
+    assert (np.abs(S)[np.ix_(off_tx, off_tx)] <= sy["S_abs"][np.ix_(off_tx, off_tx)] * (1 + 1e-12)).all()
+    assert (np.abs(b)[off_tx] <= sy["b_abs"][off_tx] * (1 + 1e-12)).all()
+    assert (sy["S_abs"][~off_tx] == 0).all() and (sy["S_abs"][:, ~off_tx] == 0).all() and (sy["b_abs"][~off_tx] == 0).all()
