@@ -891,7 +891,9 @@ int romab200_tracks_build(const rb_tracks_args* args, void* stream);
  *   launches no estimator when it is set.
  * romab200_verify_gather: the pairs [pair_begin, pair_end) of one chunk, whose matches are [match_offsets[pair_begin],
  *   match_offsets[pair_end]): x0, x1 [max(total, 1), 2] float64 (rule 1; zero for a bad id) and chunk_offsets [pair_end - pair_begin
- *   + 1] int64, starting at 0: the x0 / x1 / offsets layout of rb_fund_args.  The estimator then runs on the chunk (romab200_fund_*).
+ *   + 1] int64, starting at 0: the x0 / x1 / offsets layout of rb_fund_args.  With pair_list set, [pair_begin, pair_end) index
+ *   pair_list instead, and the listed pairs pair_list[pair_begin], ... are packed in list order in the same layout (their pair
+ *   indices must lie in [0, num_pairs); a pair may be listed twice); with pair_list null the call is unchanged.  The estimator then runs on the chunk (romab200_fund_*).
  *   Its device bytes, with B pairs, total matches and S = max(1, ceil(max_n / RB_FUND_SLICE)) score slices (max_n the chunk's
  *   largest pair), are the buffers it allocates plus the gathered points:
  *     B (RB_VERIFY_PAIR_BYTES + RB_VERIFY_SLICE_BYTES S) + RB_VERIFY_POINT_BYTES max(total, 1) + RB_VERIFY_CHUNK_BYTES
@@ -920,6 +922,7 @@ typedef struct {
     const uint8_t* ok; const uint8_t* mask; int64_t min_inliers;        /* count and emit: */
     int64_t* num_inliers; uint8_t* accepted; int64_t* tile_scan; int64_t* out_offsets;
     int64_t num_kept; int32_t* out_matches; float* out_scores;          /* emit only */
+    const int32_t* pair_list;                                           /* gather only: null, or the pairs to pack */
 } rb_verify_args;
 int romab200_verify_check(const rb_verify_args* args, void* stream);
 int romab200_verify_gather(const rb_verify_args* args, void* stream);
@@ -1197,6 +1200,42 @@ typedef struct {
 } rb_register_args;
 int romab200_register_setup(const rb_register_args* args, void* stream);
 int romab200_register_gather(const rb_register_args* args, void* stream);
+
+/* ---- two-view initialisation: statistics of a candidate pair's relative pose (COLMAP's EstimateInitialTwoViewGeometry) ----
+ * Not in the reference.  It runs after the relative-pose estimator (romab200_pose_*) on a batch of candidate pairs and reads that
+ * call's buffers: offsets [batch + 1], xn [total, 4] (the normalised points the estimator wrote), mask [total], R [batch, 3, 3],
+ * t [batch, 3] (unit length), ok [batch] and K [batch, 2, 3, 3], with the gathered pixels x0, x1 [total, 2].  All arithmetic is
+ * float64.  The rules:
+ * 1. Points.  Only the matches with mask set are used: the RANSAC inliers that passed recoverPose's chirality test.  Each is
+ *    triangulated by the DLT of the chirality test (dlt_two_view, geometry.cuh) with P0 = [I | 0] and P1 = [R | t] on xn: the
+ *    homogeneous Q, and X = Q.xyz / Q.w.
+ * 2. Good point.  A point is good when Q.w != 0 and X is finite, X.z > 0 and (R X + t).z > 0, and the squared reprojection error in
+ *    pixels is <= max_error2 in both images: |pi(K_0 X) - x0|^2 and |pi(K_1 (R X + t)) - x1|^2, pi(p) = (p_0 / p_2, p_1 / p_2).
+ * 3. Angle.  The triangulation angle of a good point is atan2(|a x b|, a . b) with a = X - C0 = X and b = X - C1, C1 = -R^T t
+ *    (triangulation rule 6's formula), in degrees (times 180 / pi).
+ * 4. Outputs per candidate.  num_good [batch] int64, median_angle [batch] float64 degrees and forward [batch] = |t_z|.
+ *    median_angle is the median of the good points' angles: the mean of the two middle values for an even count (numpy's and
+ *    COLMAP's Median), and 0 when there are none.  A candidate with ok = 0 has no masked matches, so num_good = 0 there.
+ * 5. Median without a sort.  The k-th smallest angle is found exactly by a radix select on its IEEE-754 bits: the angles are
+ *    non-negative, so their bit patterns order like their values.  8-bit digits from the top, one shared-memory histogram of
+ *    integer counts per digit over the per-point scratch angle [max(total, 1)] float64 that the first pass writes (-1 for a point
+ *    that is not good).
+ * 6. Determinism.  No float atomics and integer counts only, so reruns are byte-identical.
+ * romab200_twoview_score: one CTA of 256 threads per candidate. */
+typedef struct {
+    int32_t batch;
+    const int64_t* offsets;               /* [batch + 1] */
+    const double* x0; const double* x1;   /* [total, 2] pixels */
+    const double* xn;                     /* [total, 4] */
+    const uint8_t* mask;                  /* [total] */
+    const double* K;                      /* [batch, 2, 3, 3] */
+    const double* R; const double* t;     /* [batch, 3, 3], [batch, 3] */
+    const uint8_t* ok;                    /* [batch] */
+    double max_error2;
+    double* angle;                        /* [max(total, 1)] scratch */
+    int64_t* num_good; double* median_angle; double* forward;   /* [batch] */
+} rb_twoview_args;
+int romab200_twoview_score(const rb_twoview_args* args, void* stream);
 
 #ifdef __cplusplus
 }

@@ -186,7 +186,7 @@ _FIELD_DTYPES = {
     "rb_verify_args": {"pairs": torch.int64, "kp_offsets": torch.int64, "keypoints": _F32, "match_offsets": torch.int64, "matches": torch.int32,
                        "match_scores": _F32, "info": torch.int64, "x0": _F64, "x1": _F64, "chunk_offsets": torch.int64, "ok": torch.uint8,
                        "mask": torch.uint8, "num_inliers": torch.int64, "accepted": torch.uint8, "tile_scan": torch.int64,
-                       "out_offsets": torch.int64, "out_matches": torch.int32, "out_scores": _F32},
+                       "out_offsets": torch.int64, "out_matches": torch.int32, "out_scores": _F32, "pair_list": torch.int32},
     "rb_tri_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "cameras": _F64,
                     "info": torch.int64, "X": _F64, "ok": torch.uint8, "num_inliers": torch.int32, "error": _F64, "inlier": torch.uint8},
     "rb_ba_args": {"track_offsets": torch.int64, "elements": torch.int32, "kp_offsets": torch.int64, "keypoints": _F32, "track_ok": torch.uint8,
@@ -201,6 +201,8 @@ _FIELD_DTYPES = {
                          "points": _F64, "info": torch.int64, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32,
                          "image_offsets": torch.int64, "elem": torch.int32, "track": torch.int32, "images": torch.int32,
                          "out_offsets": torch.int64, "x": _F64, "X": _F64},
+    "rb_twoview_args": {"offsets": torch.int64, "x0": _F64, "x1": _F64, "xn": _F64, "mask": torch.uint8, "K": _F64, "R": _F64, "t": _F64,
+                        "ok": torch.uint8, "angle": _F64, "num_good": torch.int64, "median_angle": _F64, "forward": _F64},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
                           "valid": torch.uint8},
     "rb_gt_warp_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "grid_x": _F32, "grid_y": _F32,
@@ -284,6 +286,8 @@ def _verify_min_elems(kw):
            "out_matches": 2 * kept, "out_scores": kept}
     if "chunk_offsets" in kw:
         out["chunk_offsets"] = kw["pair_end"] - kw["pair_begin"] + 1
+    if kw.get("pair_list") is not None:
+        out["pair_list"] = kw["pair_end"]
     return out
 
 
@@ -327,12 +331,19 @@ def _register_min_elems(kw):
     return out
 
 
+def _twoview_min_elems(kw):
+    B, total = kw["batch"], kw["mask"].numel()
+    return {"offsets": B + 1, "x0": 2 * total, "x1": 2 * total, "xn": 4 * total, "K": 18 * B, "R": 9 * B, "t": 3 * B, "ok": B,
+            "angle": total, "num_good": B, "median_angle": B, "forward": B}
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
               "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
-              "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems}
+              "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems,
+              "rb_twoview_args": _twoview_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

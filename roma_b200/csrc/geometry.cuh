@@ -175,6 +175,30 @@ __device__ __forceinline__ void jacobi_eig_warp(double (*A)[N], double (*V)[N], 
     }
 }
 
+// Linear (DLT) triangulation of normalised (x0, y0) <-> (x1, y1) with P0 = [I | 0], P1 = [R | t] (R row-major): the eigenvector of
+// the smallest eigenvalue of the 4x4 A^T A (10 Jacobi sweeps), i.e. the right singular vector of the smallest singular value of A,
+// as homogeneous Q.  recoverPose's chirality test (pose.cu) and the two-view statistics (twoview.cu) share it.
+__device__ __forceinline__ void dlt_two_view(const double* R, const double* t, double x0, double y0, double x1, double y1,
+                                             double (&Q)[4]) {
+    const double rows[4][4] = {{-1.0, 0.0, x0, 0.0},
+                               {0.0, -1.0, y0, 0.0},
+                               {x1 * R[6] - R[0], x1 * R[7] - R[1], x1 * R[8] - R[2], x1 * t[2] - t[0]},
+                               {y1 * R[6] - R[3], y1 * R[7] - R[4], y1 * R[8] - R[5], y1 * t[2] - t[1]}};
+    double M[4][4], V[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) M[i][j] = rows[0][i] * rows[0][j] + rows[1][i] * rows[1][j] + rows[2][i] * rows[2][j] + rows[3][i] * rows[3][j];
+    jacobi_eig<4>(M, V, 10);
+    int k = 0;
+    double mn = M[0][0];
+#pragma unroll
+    for (int i = 1; i < 4; ++i)
+        if (M[i][i] < mn) { mn = M[i][i]; k = i; }
+#pragma unroll
+    for (int i = 0; i < 4; ++i) Q[i] = k == 0 ? V[i][0] : (k == 1 ? V[i][1] : (k == 2 ? V[i][2] : V[i][3]));
+}
+
 // 3x3 SVD M = sum_k s_k u_k v_k^T from cyclic Jacobi on M^T M: v[k] is the k-th right singular vector by descending singular
 // value with det [v0 v1 v2] = +1, u[k] = M v_k / s_k and s[k] = |M v_k| for k < 2, u[2] = u[0] x u[1] (M row-major)
 __device__ __forceinline__ void svd3(const double* M, double (&u)[3][3], double (&v)[3][3], double (&s)[2]) {

@@ -555,28 +555,11 @@ __device__ void decompose_essential(const double* E, double (&R1)[9], double (&R
     for (int i = 0; i < 3; ++i) tv[i] = u[2][i];
 }
 
-// cv::recoverPose's test for one candidate P1 = [R | t] (P0 = [I | 0]): DLT triangulation (the right singular vector of the
-// smallest singular value of A, i.e. the smallest eigenvector of A^T A), Q.z Q.w > 0, Q.z / Q.w < dist, 0 < (P1 Q / Q.w).z < dist
+// cv::recoverPose's test for one candidate P1 = [R | t] (P0 = [I | 0]): DLT triangulation (dlt_two_view), Q.z Q.w > 0, Q.z / Q.w < dist, 0 < (P1 Q / Q.w).z < dist
 __device__ __forceinline__ bool chirality(const double* R, const double* t, double x0, double y0, double x1, double y1) {
     constexpr double dist = 1e9;
-    const double rows[4][4] = {{-1.0, 0.0, x0, 0.0},
-                               {0.0, -1.0, y0, 0.0},
-                               {x1 * R[6] - R[0], x1 * R[7] - R[1], x1 * R[8] - R[2], x1 * t[2] - t[0]},
-                               {y1 * R[6] - R[3], y1 * R[7] - R[4], y1 * R[8] - R[5], y1 * t[2] - t[1]}};
-    double M[4][4], V[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) M[i][j] = rows[0][i] * rows[0][j] + rows[1][i] * rows[1][j] + rows[2][i] * rows[2][j] + rows[3][i] * rows[3][j];
-    jacobi_eig<4>(M, V, 10);
-    int k = 0;
-    double mn = M[0][0];
-#pragma unroll
-    for (int i = 1; i < 4; ++i)
-        if (M[i][i] < mn) { mn = M[i][i]; k = i; }
     double Q[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) Q[i] = k == 0 ? V[i][0] : (k == 1 ? V[i][1] : (k == 2 ? V[i][2] : V[i][3]));
+    dlt_two_view(R, t, x0, y0, x1, y1, Q);
     if (!(Q[2] * Q[3] > 0.0)) return false;
     const double X = Q[0] / Q[3], Y = Q[1] / Q[3], Z = Q[2] / Q[3];
     if (!(Z < dist)) return false;

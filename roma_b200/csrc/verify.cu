@@ -2,6 +2,8 @@
 // estimator (fundamental.cu, run chunk by chunk by the caller), then only the inlier matches of accepted pairs kept.
 //   check    a thread per match: its pair by binary search in match_offsets, its ids checked; info[0] |= RB_VERIFY_BAD_ID.
 //   gather   a thread per match of one chunk: x0, x1 widened to float64 at (match - chunk base), and the chunk's offsets.
+//            With a pair_list, one CTA first scans the listed pairs' match counts into the chunk's offsets, then a thread per
+//            packed point finds its list entry by binary search in them.
 //   count    a CTA per pair: num_inliers (integer sum of its mask), accepted, its kept count into out_offsets;
 //            a CTA per RB_VERIFY_TILE matches: the kept matches of the tile into tile_scan; both scanned; info[1] = the total.
 //   emit     the same tiles write the kept matches and scores at the scanned offsets, in match order.
@@ -89,6 +91,54 @@ __global__ void __launch_bounds__(VF_THREADS) vf_gather_kernel(rb_verify_args a)
     }
 }
 
+// the matches of list entry c, or 0 (and RB_VERIFY_BAD_ID) for a pair index outside [0, num_pairs)
+__device__ __forceinline__ int64_t vf_list_count(const rb_verify_args& a, int c) {
+    const int k = a.pair_list[a.pair_begin + c];
+    if (k < 0 || k >= a.num_pairs) {
+        atomicOr((unsigned long long*)a.info, (unsigned long long)RB_VERIFY_BAD_ID);
+        return 0;
+    }
+    return a.match_offsets[k + 1] - a.match_offsets[k];
+}
+
+// one CTA: chunk_offsets = the exclusive scan of the listed pairs' match counts, each thread a contiguous run of entries
+__global__ void __launch_bounds__(VF_THREADS) vf_list_offsets_kernel(rb_verify_args a) {
+    pdl_wait();
+    const int pairs = a.pair_end - a.pair_begin, per = (pairs + VF_THREADS - 1) / VF_THREADS;
+    const int c0 = min(pairs, (int)threadIdx.x * per), c1 = min(pairs, c0 + per);
+    long long run = 0;
+    for (int c = c0; c < c1; ++c) run += vf_list_count(a, c);
+    long long total;
+    long long before = vf_block_scan(run, &total);
+    for (int c = c0; c < c1; ++c) {
+        a.chunk_offsets[c] = before;
+        before += vf_list_count(a, c);
+    }
+    if (threadIdx.x == 0) a.chunk_offsets[pairs] = total;
+}
+
+// a thread per packed point q of the listed pairs: its entry c by binary search in chunk_offsets, its match, x0 and x1
+__global__ void __launch_bounds__(VF_THREADS) vf_gather_list_kernel(rb_verify_args a) {
+    pdl_wait();
+    const int pairs = a.pair_end - a.pair_begin;
+    const int64_t n = a.chunk_offsets[pairs];
+    for (int64_t q = blockIdx.x * (int64_t)VF_THREADS + threadIdx.x; q < n; q += (int64_t)gridDim.x * VF_THREADS) {
+        const int c = vf_pair_of(a.chunk_offsets, 0, pairs - 1, q);
+        const int k = a.pair_list[a.pair_begin + c];          // in range: an entry outside it has no points
+        const int64_t m = a.match_offsets[k] + (q - a.chunk_offsets[c]);
+        int64_t ra, rb;
+        double2 p0 = make_double2(0.0, 0.0), p1 = make_double2(0.0, 0.0);
+        if (vf_rows(a, k, m, &ra, &rb)) {
+            p0 = make_double2(a.keypoints[2 * ra], a.keypoints[2 * ra + 1]);
+            p1 = make_double2(a.keypoints[2 * rb], a.keypoints[2 * rb + 1]);
+        } else {
+            atomicOr((unsigned long long*)a.info, (unsigned long long)RB_VERIFY_BAD_ID);
+        }
+        reinterpret_cast<double2*>(a.x0)[q] = p0;
+        reinterpret_cast<double2*>(a.x1)[q] = p1;
+    }
+}
+
 // CTA k: num_inliers[k] = the integer sum of pair k's mask, accepted[k], out_offsets[k] = its kept count
 __global__ void __launch_bounds__(VF_THREADS) vf_pairs_kernel(rb_verify_args a) {
     pdl_wait();
@@ -162,6 +212,12 @@ extern "C" int romab200_verify_gather(const rb_verify_args* a, void* stream) {
     RB_REQUIRE(a->pair_begin >= 0 && a->pair_begin < a->pair_end && a->pair_end <= a->num_pairs, "verify_gather: bad chunk [%d, %d) of %d pairs",
                a->pair_begin, a->pair_end, a->num_pairs);
     cudaStream_t st = (cudaStream_t)stream;
+    if (a->pair_list) {
+        launch_pdl(vf_list_offsets_kernel, dim3(1), dim3(VF_THREADS), 0, st, *a);
+        if (check_launch("verify_gather(list offsets)")) return 1;
+        launch_pdl(vf_gather_list_kernel, dim3(grid1d(a->num_matches, VF_THREADS, 16 * 1024)), dim3(VF_THREADS), 0, st, *a);
+        return check_launch("verify_gather(list)");
+    }
     launch_pdl(vf_gather_kernel, dim3(grid1d(a->num_matches, VF_THREADS, 16 * 1024)), dim3(VF_THREADS), 0, st, *a);
     return check_launch("verify_gather");
 }
