@@ -1048,7 +1048,27 @@ int romab200_triangulate(const rb_tri_args* args, void* stream);
  *   per element keys 8, keys_alt 8, elem_track 4, obs 4, W 144, inlier 1; per track track_sys 104, X 24, X_trial 24, track_part 24,
  *   error 8, track_offsets 8, track_ok 1; per image cams 168, cams_trial 168, cam_pred 8, free_index 4, obs_offsets 8, kp_offsets 8;
  *   per free camera cam_sys 96, rhs 48, free_cams 4, fixed_tx 1; S 288 F^2; once hist 4, obs_offsets 8, kp_offsets 8, track_offsets
- *   8, info 16, result 32.  W is stored rather than recomputed by the camera kernel: 144 B per element is 576 MB at 4 M elements. */
+ *   8, info 16, result 32.  W is stored rather than recomputed by the camera kernel: 144 B per element is 576 MB at 4 M elements.
+ *
+ * Camera models.  camera_model = 0 is the PINHOLE model above, and a zero-initialised struct means it.  camera_model = 1 is
+ * SIMPLE_RADIAL (see the keypoint undistortion below): cams rows are RB_BA_CAM1 doubles R (9), t (3), f, cx, cy, k, and each camera
+ * also refines its focal length and radial coefficient, with the principal point fixed.  The rules change as follows:
+ * 2'. Residual.  r_e = (f d x + cx, f d y + cy) - x_e with (x, y) = (p0, p1) / p2, p = R_i X_k + t_i, r^2 = x^2 + y^2 and
+ *    d = 1 + k r^2, on the raw (distorted) keypoint widened to float64.
+ * 3'. Parameters.  Camera i has the 8 parameters (d_omega, d_t, d_f, d_k); the update adds f <- f + d_f and k <- k + d_k.  Through
+ *    (x, y): du/dx = f (d + 2 k x^2), du/dy = dv/dx = 2 f k x y, dv/dy = f (d + 2 k y^2).  Intrinsics: d(u, v)/df = d (x, y) and
+ *    d(u, v)/dk = f r^2 (x, y).
+ * 4'. Gauge as pinned rows.  fixed_tx is not read.  A camera is free (enters the reduced system) when any of its 8 parameters is
+ *    free, and pin [num_free, 8] uint8 marks its pinned parameters: rows 0-5 for a camera whose pose is fixed, row 3 for a fixed
+ *    t_x, row 6 for a fixed f, row 7 for a fixed k.  Each pinned row and column of S becomes the identity with a zero right-hand
+ *    side, so its step is exactly 0, and the trial camera copies a pinned parameter (all of R when rows 0-2 are pinned).
+ * 6'. Trial.  result[2] also counts the used observations whose camera's trial f is not > 0, so such a trial is rejected.  A free
+ *    camera without used observations has a zero step.
+ * Shapes for model 1: W [num_elements, 24] (8 x 3), cam_sys [num_free, 16] = g_c (8), D_c (8), S [8 num_free, 8 num_free], rhs
+ * [8 num_free].  Device bytes: RB_BA_ELEMENT_BYTES1 E + RB_BA_TRACK_BYTES T + RB_BA_IMAGE_BYTES1 N + RB_BA_FREE_BYTES1 F + 512 F^2
+ *   + 1024 ceil(E / RB_TRACKS_TILE) + RB_BA_ONCE_BYTES
+ *   per element W 192 (the rest as above); per image cams 128, cams_trial 128; per free camera cam_sys 128, rhs 64, free_cams 4,
+ *   pin 8 (no fixed_tx). */
 #define RB_BA_BAD_ID 1
 #define RB_BA_REPEATED 2
 #define RB_BA_CAM 21
@@ -1060,6 +1080,10 @@ int romab200_triangulate(const rb_tri_args* args, void* stream);
 #define RB_BA_IMAGE_BYTES 364
 #define RB_BA_FREE_BYTES 149
 #define RB_BA_ONCE_BYTES 76
+#define RB_BA_CAM1 16
+#define RB_BA_ELEMENT_BYTES1 217
+#define RB_BA_IMAGE_BYTES1 284
+#define RB_BA_FREE_BYTES1 204
 typedef struct {
     int32_t num_tracks, num_images, num_free;
     const int64_t* track_offsets; const int32_t* elements; int64_t num_elements;
@@ -1075,6 +1099,8 @@ typedef struct {
     double* W; double* track_sys; double* cam_sys; double* S; double* rhs;
     double* cam_pred; double* track_part; double* result;
     double* error;
+    int32_t camera_model;                                               /* 0 PINHOLE, 1 SIMPLE_RADIAL */
+    const uint8_t* pin;                                                 /* [num_free, 8], model 1 */
 } rb_ba_args;
 int romab200_ba_setup(const rb_ba_args* args, void* stream);
 int romab200_ba_linearize(const rb_ba_args* args, void* stream);
@@ -1236,6 +1262,32 @@ typedef struct {
     int64_t* num_good; double* median_angle; double* forward;   /* [batch] */
 } rb_twoview_args;
 int romab200_twoview_score(const rb_twoview_args* args, void* stream);
+
+/* ---- keypoint undistortion under SIMPLE_RADIAL cameras (COLMAP's camera model 2) ----
+ * Not in the reference.  Camera i has intrinsics [num_images, 4] float64 (f, cx, cy, k) and maps a camera-frame point p to
+ * x = p0 / p2, y = p1 / p2, r^2 = x^2 + y^2, d = 1 + k r^2, u = f d x + cx, v = f d y + cy.  Each keypoint (u, v) of image i,
+ * keypoints[kp_offsets[i] .. kp_offsets[i + 1]), is mapped to the pixel of the same camera without distortion.  All arithmetic is
+ * float64 on the keypoint widened from fp32.  The rules:
+ * 1. Normalise.  (dx, dy) = (u - cx, v - cy) and rho_d = sqrt(dx^2 + dy^2) / f.
+ * 2. Solve rho (1 + k rho^2) = rho_d by Newton from rho = rho_d: step = (rho (1 + k rho^2) - rho_d) / (1 + 3 k rho^2), rho -= step,
+ *    at most RB_UNDISTORT_ITERS steps, stopping after a step that is exactly 0.  g(rho) = rho (1 + k rho^2) - rho_d is convex on
+ *    rho > 0 for k > 0 and concave for k < 0, so the iterates move monotonically towards the root from rho_d.
+ * 3. Output (cx + dx s, cy + dy s) with s = rho / rho_d, rounded to fp32.  With k = 0 or rho_d = 0 the keypoint is copied bit for bit.
+ * 4. For k < 0, g has no root at or beyond rho_d >= 2 / (3 sqrt(-3 k)), the image of the turning radius 1 / sqrt(-3 k).  Such a
+ *    keypoint gets rho = 1 / sqrt(-3 k) (clamped in its own direction) and counts in clamped[0].  No output is NaN.
+ * The caller checks on the host that every f is finite and > 0 and every cx, cy, k finite.
+ * romab200_undistort_keypoints: a thread per keypoint; clamped [1] int64 is zeroed and counted with integer atomics. */
+#define RB_UNDISTORT_ITERS 20
+typedef struct {
+    int32_t num_images;
+    int64_t num_rows;
+    const int64_t* kp_offsets;            /* [num_images + 1] */
+    const float* keypoints;               /* [num_rows, 2] */
+    const double* intrinsics;             /* [num_images, 4] */
+    float* out;                           /* [num_rows, 2] */
+    int64_t* clamped;                     /* [1] */
+} rb_undistort_args;
+int romab200_undistort_keypoints(const rb_undistort_args* args, void* stream);
 
 #ifdef __cplusplus
 }

@@ -41,6 +41,9 @@ def __getattr__(name):
     if name in ("register_images", "Registration"):
         from . import register
         return getattr(register, name)
+    if name in ("default_intrinsics", "pinhole_K", "undistort_keypoints", "undistort_graph"):
+        from . import camera
+        return getattr(camera, name)
     if name in ("bundle_adjust", "BundleResult"):
         from . import bundle
         return getattr(bundle, name)

@@ -1,7 +1,8 @@
 """Bundle adjustment of cameras and track points on the device (`bundle_adjust`): Levenberg-Marquardt over the poses of the free
 cameras and the points of the ok tracks, minimising the (optionally Cauchy-robust) reprojection error of the inlier observations
 that `triangulate_tracks` marked.  The normal equations are reduced to the cameras by the Schur complement and factored by dense
-Cholesky on the device; the host only drives the loop.  The exact rules are in include/romab200.h and INTEGRATION.md;
+Cholesky on the device; the host only drives the loop.  With camera_model="SIMPLE_RADIAL" each camera also refines its focal
+length and radial coefficient (`roma_b200.camera`).  The exact rules are in include/romab200.h and INTEGRATION.md;
 `oracle/bundle.py` restates them in numpy."""
 from __future__ import annotations
 
@@ -13,6 +14,7 @@ import numpy as np
 import torch
 
 from . import cabi
+from . import camera as _camera
 from . import triangulate as _tri
 from .match_graph import WORKSPACE_BYTES, MatchGraph
 from .tracks import Tracks
@@ -27,7 +29,8 @@ class BundleResult:
     error recomputed at the final X, R, t (the given points unchanged when no step was kept).  cost: host float64 [n + 1], the
     cost before the first trial and after each (a rejected trial repeats it); accepted: host bool [n]; pred: host float64 [n], each
     trial's predicted decrease 1/2 d^T (lambda D d - g); termination:
-    "function_tolerance", "max_iterations", "no_progress" or "nothing_to_adjust"."""
+    "function_tolerance", "max_iterations", "no_progress" or "nothing_to_adjust".  intrinsics: with camera_model="SIMPLE_RADIAL",
+    the refined float64 [N, 4] (f, cx, cy, k) on the graph's device; None for PINHOLE."""
     R: torch.Tensor
     t: torch.Tensor
     points: Points3D
@@ -35,25 +38,34 @@ class BundleResult:
     accepted: np.ndarray
     pred: np.ndarray
     termination: str
+    intrinsics: torch.Tensor = None
 
 
-def workspace_bytes(num_images: int, num_free: int, num_tracks: int, num_elements: int) -> int:
+CAMERA_MODELS = {"PINHOLE": 0, "SIMPLE_RADIAL": 1}
+
+
+def workspace_bytes(num_images: int, num_free: int, num_tracks: int, num_elements: int, camera_model: str = "PINHOLE") -> int:
     """Device bytes of one call (include/romab200.h): every buffer `_buffers` allocates."""
     tiles = -(-num_elements // cabi.RB_TRACKS_TILE)
+    if camera_model == "SIMPLE_RADIAL":
+        return (cabi.RB_BA_ELEMENT_BYTES1 * num_elements + cabi.RB_BA_TRACK_BYTES * num_tracks + cabi.RB_BA_IMAGE_BYTES1 * num_images
+                + cabi.RB_BA_FREE_BYTES1 * num_free + 512 * num_free * num_free + 1024 * tiles + cabi.RB_BA_ONCE_BYTES)
     return (cabi.RB_BA_ELEMENT_BYTES * num_elements + cabi.RB_BA_TRACK_BYTES * num_tracks + cabi.RB_BA_IMAGE_BYTES * num_images
             + cabi.RB_BA_FREE_BYTES * num_free + 288 * num_free * num_free + 1024 * tiles + cabi.RB_BA_ONCE_BYTES)
 
 
-def _buffers(dev, N, F, T, E) -> dict:
+def _buffers(dev, N, F, T, E, model=0) -> dict:
     """The call's device buffers, named by their rb_ba_args fields (uninitialised; the kernels write them before reading)."""
     f64, i32, i64, u8 = torch.float64, torch.int32, torch.int64, torch.uint8
     tiles = -(-E // cabi.RB_TRACKS_TILE)
+    nc, cam = (8, cabi.RB_BA_CAM1) if model else (6, cabi.RB_BA_CAM)
     shapes = dict(kp_offsets=(N + 1, i64), track_offsets=(T + 1, i64), track_ok=(T, u8), inlier=(E, u8),
-                  free_index=(N, i32), free_cams=(F, i32), fixed_tx=(F, u8), info=(2, i64), elem_track=(E, i32), keys=(E, i64),
-                  keys_alt=(E, i64), hist=(256 * tiles + 1, i32), obs_offsets=(N + 1, i64), obs=(E, i32), cams=(N * cabi.RB_BA_CAM, f64),
-                  X=(3 * T, f64), cams_trial=(N * cabi.RB_BA_CAM, f64), X_trial=(3 * T, f64), W=(18 * E, f64),
-                  track_sys=(T * cabi.RB_BA_TRACK, f64), cam_sys=(12 * F, f64), S=(36 * F * F, f64), rhs=(6 * F, f64), cam_pred=(N, f64),
-                  track_part=(3 * T, f64), result=(cabi.RB_BA_RESULT, f64), error=(T, f64))
+                  free_index=(N, i32), free_cams=(F, i32), info=(2, i64), elem_track=(E, i32), keys=(E, i64),
+                  keys_alt=(E, i64), hist=(256 * tiles + 1, i32), obs_offsets=(N + 1, i64), obs=(E, i32), cams=(N * cam, f64),
+                  X=(3 * T, f64), cams_trial=(N * cam, f64), X_trial=(3 * T, f64), W=(3 * nc * E, f64),
+                  track_sys=(T * cabi.RB_BA_TRACK, f64), cam_sys=(2 * nc * F, f64), S=(nc * nc * F * F, f64), rhs=(nc * F, f64),
+                  cam_pred=(N, f64), track_part=(3 * T, f64), result=(cabi.RB_BA_RESULT, f64), error=(T, f64))
+    shapes.update(pin=(8 * F, u8)) if model else shapes.update(fixed_tx=(F, u8))
     return {k: torch.empty(n, dtype=d, device=dev) for k, (n, d) in shapes.items()}
 
 
@@ -67,12 +79,41 @@ def _indices(name, v, N):
     return sorted(set(out))
 
 
-def _check(graph, tracks, points, K, R, t, fixed_poses, fixed_tx, loss_scale, max_iterations, function_tolerance, workspace_bytes_):
-    """Argument rules, checked before any device work.  Returns (kp_offsets, track_offsets, K, R, t as float64 arrays, fixed
-    poses, fixed_tx, c^2, max_iterations, function_tolerance)."""
-    kp_off, tr_off, *_ = _tri._check(graph, tracks, K, R, t, 1.0, 0.0, 1, 0, what="bundle_adjust", device=False)
+def _free_and_pins(N, fixed_poses, fixed_tx, radial, refine_f, refine_k, fixed_intrinsics):
+    """The free cameras, ascending, and per free camera its pinned rows [F, 8] (rule 4'; all zero for PINHOLE)."""
+    fp, ftx, fin = set(fixed_poses), set(fixed_tx), set(fixed_intrinsics)
+    if not radial:
+        free = [i for i in range(N) if i not in fp]
+        return free, np.zeros((len(free), 8), np.uint8)
+    pins = np.zeros((N, 8), np.uint8)
+    for i in range(N):
+        pins[i, :6] = i in fp
+        pins[i, 3] |= i in ftx
+        pins[i, 6] = not refine_f or i in fin
+        pins[i, 7] = not refine_k or i in fin
+    free = [i for i in range(N) if not (i in fp and pins[i, 6] and pins[i, 7])]
+    return free, pins[free]
+
+
+def _check(graph, tracks, points, K, R, t, fixed_poses, fixed_tx, loss_scale, max_iterations, function_tolerance, workspace_bytes_,
+           camera_model="PINHOLE", refine_focal_length=True, refine_extra_params=True, fixed_intrinsics=()):
+    """Argument rules, checked before any device work.  Returns (kp_offsets, track_offsets, K (or the [N, 4] intrinsics), R, t as
+    float64 arrays, fixed poses, fixed_tx, c^2, max_iterations, function_tolerance, model code, fixed_intrinsics)."""
+    if not isinstance(camera_model, str) or camera_model not in CAMERA_MODELS:
+        raise ValueError(f"bundle_adjust: camera_model must be one of {sorted(CAMERA_MODELS)}, got {camera_model!r}")
+    radial = camera_model == "SIMPLE_RADIAL"
+    for name, v in (("refine_focal_length", refine_focal_length), ("refine_extra_params", refine_extra_params)):
+        if not isinstance(v, bool):
+            raise ValueError(f"bundle_adjust: {name} must be a bool, got {v!r}")
+    N0 = len(graph._kp_off) - 1 if isinstance(graph, MatchGraph) else 0
+    kp_off, tr_off, *_ = _tri._check(graph, tracks, np.broadcast_to(np.eye(3), (max(N0, 0), 3, 3)) if radial else K, R, t, 1.0, 0.0, 1, 0,
+                                     what="bundle_adjust", device=False)
     N, T, E = len(kp_off) - 1, len(tr_off) - 1, tr_off[-1]
-    K, R, t = (_tri._float64(n, v, s, "bundle_adjust") for n, v, s in (("K", K, (N, 3, 3)), ("R", R, (N, 3, 3)), ("t", t, (N, 3))))
+    K = _camera.check_intrinsics(K, N, "bundle_adjust") if radial else _tri._float64("K", K, (N, 3, 3), "bundle_adjust")
+    R, t = (_tri._float64(n, v, s, "bundle_adjust") for n, v, s in (("R", R, (N, 3, 3)), ("t", t, (N, 3))))
+    fixed_intrinsics = _indices("fixed_intrinsics", fixed_intrinsics, N)
+    if fixed_intrinsics and not radial:
+        raise ValueError("bundle_adjust: fixed_intrinsics needs camera_model=\"SIMPLE_RADIAL\" (PINHOLE keeps K fixed)")
     if not isinstance(points, Points3D):
         raise ValueError(f"bundle_adjust: points must be Points3D, got {type(points).__name__}")
     for name, v, dt, shape in (("points.X", points.X, torch.float64, (T, 3)), ("points.ok", points.ok, torch.bool, (T,)),
@@ -93,20 +134,23 @@ def _check(graph, tracks, points, K, R, t, fixed_poses, fixed_tx, loss_scale, ma
         raise ValueError(f"bundle_adjust: function_tolerance must be a number >= 0, got {function_tolerance!r}")
     if isinstance(workspace_bytes_, bool) or not isinstance(workspace_bytes_, int):
         raise ValueError(f"bundle_adjust: workspace_bytes must be an int, got {workspace_bytes_!r}")
-    need = workspace_bytes(N, N - len(fixed_poses), T, E)
+    num_free = len(_free_and_pins(N, fixed_poses, fixed_tx, radial, refine_focal_length, refine_extra_params, fixed_intrinsics)[0])
+    need = workspace_bytes(N, num_free, T, E, camera_model)
     if need > workspace_bytes_:
-        raise ValueError(f"bundle_adjust: the call needs {need} bytes of device memory ({N - len(fixed_poses)} free cameras, {T} tracks, "
+        raise ValueError(f"bundle_adjust: the call needs {need} bytes of device memory ({num_free} free cameras, {T} tracks, "
                          f"{E} elements), more than workspace_bytes = {workspace_bytes_}")
     _tri._check_device([graph.kp_offsets, graph.keypoints, tracks.track_offsets, tracks.elements, points.X, points.ok, points.inlier],
                        "bundle_adjust")
     if not bool(torch.isfinite(points.X).all()):
         raise ValueError("bundle_adjust: points.X has values that are not finite")
     c2 = 0.0 if loss_scale is None else float(loss_scale) ** 2
-    return kp_off, tr_off, K, R, t, fixed_poses, fixed_tx, c2, max_iterations, float(function_tolerance)
+    return (kp_off, tr_off, K, R, t, fixed_poses, fixed_tx, c2, max_iterations, float(function_tolerance), CAMERA_MODELS[camera_model],
+            fixed_intrinsics)
 
 
 def bundle_adjust(graph: MatchGraph, tracks: Tracks, points: Points3D, K, R, t, *, fixed_poses=(0,), fixed_tx=(1,), loss_scale=None,
-                  max_iterations=50, function_tolerance=1e-6, workspace_bytes=WORKSPACE_BYTES) -> BundleResult:
+                  max_iterations=50, function_tolerance=1e-6, workspace_bytes=WORKSPACE_BYTES, camera_model="PINHOLE",
+                  refine_focal_length=True, refine_extra_params=True, fixed_intrinsics=()) -> BundleResult:
     """Refines the cameras x ~ K[i] (R[i] X + t[i]) (the convention of `triangulate_tracks`; K stays fixed) and the points of the ok
     tracks of `points` (from `triangulate_tracks` on the same graph and tracks) to minimise 1/2 sum rho(|r_e|^2) over the inlier
     observations: rho(s) = s, or the Cauchy c^2 log(1 + s / c^2) with c = `loss_scale` px.  K, R [N, 3, 3] and t [N, 3] are tensors or
@@ -118,37 +162,46 @@ def bundle_adjust(graph: MatchGraph, tracks: Tracks, points: Points3D, K, R, t, 
     `function_tolerance` times the cost, or when lambda exceeds 1e32.  A track whose inlier observations repeat an image (tracks
     built with drop_conflicts=False) raises ValueError, as does an element id outside its image's keypoints.
 
+    camera_model="SIMPLE_RADIAL" takes K as the [N, 4] intrinsics (f, cx, cy, k) of `roma_b200.camera` and the raw (distorted)
+    keypoints, and also refines f (with `refine_focal_length`) and k (with `refine_extra_params`) of every image not in
+    `fixed_intrinsics`; the principal point stays fixed.  A camera in fixed_poses keeps its pose while its intrinsics move, which is
+    COLMAP's gauge.  The refined intrinsics are BundleResult.intrinsics.
+
     Bit-identical from run to run.  Arguments are checked before any device work; `workspace_bytes` bounds the device memory of
     the call (`workspace_bytes()` gives it).  Host reads: the offsets, a finiteness flag of X, the setup status and cost, and four
     numbers per trial."""
-    kp_off, tr_off, K, R, t, fixed, ftx, c2, max_iterations, ftol = _check(graph, tracks, points, K, R, t, fixed_poses, fixed_tx,
-                                                                           loss_scale, max_iterations, function_tolerance, workspace_bytes)
+    (kp_off, tr_off, K, R, t, fixed, ftx, c2, max_iterations, ftol, model, fin) = _check(
+        graph, tracks, points, K, R, t, fixed_poses, fixed_tx, loss_scale, max_iterations, function_tolerance, workspace_bytes,
+        camera_model, refine_focal_length, refine_extra_params, fixed_intrinsics)
     N, T, E = len(kp_off) - 1, len(tr_off) - 1, tr_off[-1]
     dev = graph.kp_offsets.device
     with torch.cuda.device(dev):
         R0, t0 = torch.from_numpy(R).to(dev), torch.from_numpy(t).to(dev)
-        inputs = BundleResult(R0, t0, points, np.zeros(1), np.zeros(0, bool), np.zeros(0), "nothing_to_adjust")
+        intr0 = torch.from_numpy(K).to(dev) if model else None
+        inputs = BundleResult(R0, t0, points, np.zeros(1), np.zeros(0, bool), np.zeros(0), "nothing_to_adjust", intr0)
         if T == 0 or E == 0:
             return inputs
-        free_cams = [i for i in range(N) if i not in set(fixed)]
+        free_cams, pins = _free_and_pins(N, fixed, ftx, model == 1, refine_focal_length, refine_extra_params, fin)
         F = len(free_cams)
-        b = _buffers(dev, N, F, T, E)
+        b = _buffers(dev, N, F, T, E, model)
         free_index = np.full(N, -1, np.int32)
         free_index[free_cams] = np.arange(F, dtype=np.int32)
-        cams = np.concatenate((R.reshape(N, 9), t, K.reshape(N, 9)), 1)
+        cams = np.concatenate((R.reshape(N, 9), t, K.reshape(N, -1)), 1)
+        gauge = ("pin", pins.reshape(-1)) if model else ("fixed_tx", np.asarray([i in set(ftx) for i in free_cams], np.uint8))
         # the offsets the host checked, not the tensors' current contents: the device indexes with exactly what was validated
         for name, v in (("kp_offsets", np.asarray(kp_off, np.int64)), ("track_offsets", np.asarray(tr_off, np.int64)),
-                        ("free_index", free_index), ("free_cams", np.asarray(free_cams, np.int32)),
-                        ("fixed_tx", np.asarray([i in set(ftx) for i in free_cams], np.uint8)), ("cams", cams.reshape(-1))):
+                        ("free_index", free_index), ("free_cams", np.asarray(free_cams, np.int32)), gauge, ("cams", cams.reshape(-1))):
             b[name].copy_(torch.from_numpy(v))
         b["track_ok"].copy_(points.ok)
         b["inlier"].copy_(points.inlier)
         b["X"].copy_(points.X.reshape(-1))
         if F == 0:
-            for name in ("free_cams", "fixed_tx", "cam_sys", "S", "rhs"):
+            for name in ("free_cams", gauge[0], "cam_sys", "S", "rhs"):
                 b[name] = None
         args = dict(num_tracks=T, num_images=N, num_free=F, elements=tracks.elements.contiguous(), num_elements=E,
                     keypoints=graph.keypoints.contiguous(), num_rows=kp_off[-1], loss_scale2=c2, **b)
+        if model:
+            args["camera_model"] = model
 
         def call(fn, lam):
             cabi.call(f"romab200_ba_{fn}", "rb_ba_args", **args, **{"lambda": lam})
@@ -200,8 +253,9 @@ def bundle_adjust(graph: MatchGraph, tracks: Tracks, points: Points3D, K, R, t, 
                     break
         cost, accepted, preds = np.asarray(cost, np.float64), np.asarray(accepted, bool), np.asarray(preds, np.float64)
         if not accepted.any():
-            return BundleResult(R0, t0, points, cost, accepted, preds, termination)
+            return BundleResult(R0, t0, points, cost, accepted, preds, termination, intr0)
         call("error", lam)
-        cams_d = args["cams"].view(N, cabi.RB_BA_CAM)
+        cams_d = args["cams"].view(N, cabi.RB_BA_CAM1 if model else cabi.RB_BA_CAM)
         out = Points3D(args["X"].view(T, 3).clone(), points.ok, points.num_inliers, args["error"].clone(), points.inlier)
-        return BundleResult(cams_d[:, :9].reshape(N, 3, 3).clone(), cams_d[:, 9:12].clone(), out, cost, accepted, preds, termination)
+        return BundleResult(cams_d[:, :9].reshape(N, 3, 3).clone(), cams_d[:, 9:12].clone(), out, cost, accepted, preds, termination,
+                            cams_d[:, 12:16].clone() if model else None)

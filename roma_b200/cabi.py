@@ -75,10 +75,11 @@ STRUCT_FIELDS, FUNCTIONS = _parse_header(HEADER)
                  "RB_TRI_CAM", "RB_TRI_BAD_ID"))
 RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEADER).read()).group(1), 16)
 (RB_BA_BAD_ID, RB_BA_REPEATED, RB_BA_CAM, RB_BA_TRACK, RB_BA_RESULT, RB_BA_NB, RB_BA_ELEMENT_BYTES, RB_BA_TRACK_BYTES, RB_BA_IMAGE_BYTES,
- RB_BA_FREE_BYTES, RB_BA_ONCE_BYTES) = (
+ RB_BA_FREE_BYTES, RB_BA_ONCE_BYTES, RB_BA_CAM1, RB_BA_ELEMENT_BYTES1, RB_BA_IMAGE_BYTES1, RB_BA_FREE_BYTES1) = (
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
     for name in ("RB_BA_BAD_ID", "RB_BA_REPEATED", "RB_BA_CAM", "RB_BA_TRACK", "RB_BA_RESULT", "RB_BA_NB", "RB_BA_ELEMENT_BYTES",
-                 "RB_BA_TRACK_BYTES", "RB_BA_IMAGE_BYTES", "RB_BA_FREE_BYTES", "RB_BA_ONCE_BYTES"))
+                 "RB_BA_TRACK_BYTES", "RB_BA_IMAGE_BYTES", "RB_BA_FREE_BYTES", "RB_BA_ONCE_BYTES", "RB_BA_CAM1", "RB_BA_ELEMENT_BYTES1",
+                 "RB_BA_IMAGE_BYTES1", "RB_BA_FREE_BYTES1"))
 (RB_ABS_ROUND, RB_ABS_MAX_SOL, RB_ABS_MAX_SPLITS, RB_ABS_SLICE, RB_ABS_STATE, RB_ABS_MAX_BATCH, RB_REG_BAD_ID, RB_REG_ITEM_BYTES, RB_REG_SLICE_BYTES,
  RB_REG_POINT_BYTES, RB_REG_CHUNK_BYTES) = (
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
@@ -193,7 +194,8 @@ _FIELD_DTYPES = {
                    "inlier": torch.uint8, "free_index": torch.int32, "free_cams": torch.int32, "fixed_tx": torch.uint8, "info": torch.int64,
                    "elem_track": torch.int32, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32, "obs_offsets": torch.int64,
                    "obs": torch.int32, "cams": _F64, "X": _F64, "cams_trial": _F64, "X_trial": _F64, "W": _F64, "track_sys": _F64,
-                   "cam_sys": _F64, "S": _F64, "rhs": _F64, "cam_pred": _F64, "track_part": _F64, "result": _F64, "error": _F64},
+                   "cam_sys": _F64, "S": _F64, "rhs": _F64, "cam_pred": _F64, "track_part": _F64, "result": _F64, "error": _F64,
+                   "pin": torch.uint8},
     "rb_abspose_args": {"x": _F64, "X": _F64, "offsets": torch.int64, "K": _F64, "sample": torch.int32, "models": _F64, "nsol": torch.int32,
                         "counts": torch.int32, "state": torch.int32, "best": _F64, "running": torch.int32, "R": _F64, "t": _F64, "ok": torch.uint8,
                         "num_inliers": torch.int64, "mask": torch.uint8},
@@ -201,6 +203,7 @@ _FIELD_DTYPES = {
                          "points": _F64, "info": torch.int64, "keys": torch.int64, "keys_alt": torch.int64, "hist": torch.int32,
                          "image_offsets": torch.int64, "elem": torch.int32, "track": torch.int32, "images": torch.int32,
                          "out_offsets": torch.int64, "x": _F64, "X": _F64},
+    "rb_undistort_args": {"kp_offsets": torch.int64, "keypoints": _F32, "intrinsics": _F64, "out": _F32, "clamped": torch.int64},
     "rb_twoview_args": {"offsets": torch.int64, "x0": _F64, "x1": _F64, "xn": _F64, "mask": torch.uint8, "K": _F64, "R": _F64, "t": _F64,
                         "ok": torch.uint8, "angle": _F64, "num_good": torch.int64, "median_angle": _F64, "forward": _F64},
     "rb_warp_kpts_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "kpts": "kpts_dtype", "warped": _F64,
@@ -299,12 +302,13 @@ def _tri_min_elems(kw):
 
 def _ba_min_elems(kw):
     T, N, F, E = kw["num_tracks"], kw["num_images"], kw.get("num_free", 0), kw["num_elements"]
-    n = 6 * F
+    nc, cam = (8, RB_BA_CAM1) if kw.get("camera_model", 0) == 1 else (6, RB_BA_CAM)
+    n = nc * F
     return {"track_offsets": T + 1, "elements": 2 * E, "kp_offsets": N + 1, "keypoints": 2 * kw["num_rows"], "track_ok": T, "inlier": E,
             "free_index": N, "free_cams": F, "fixed_tx": F, "info": 2, "elem_track": E, "keys": E, "keys_alt": E,
-            "hist": 256 * ((E + RB_TRACKS_TILE - 1) // RB_TRACKS_TILE) + 1, "obs_offsets": N + 1, "obs": E, "cams": N * RB_BA_CAM,
-            "X": 3 * T, "cams_trial": N * RB_BA_CAM, "X_trial": 3 * T, "W": 18 * E, "track_sys": T * RB_BA_TRACK, "cam_sys": 12 * F,
-            "S": n * n, "rhs": n, "cam_pred": N, "track_part": 3 * T, "result": RB_BA_RESULT, "error": T}
+            "hist": 256 * ((E + RB_TRACKS_TILE - 1) // RB_TRACKS_TILE) + 1, "obs_offsets": N + 1, "obs": E, "cams": N * cam,
+            "X": 3 * T, "cams_trial": N * cam, "X_trial": 3 * T, "W": 3 * nc * E, "track_sys": T * RB_BA_TRACK, "cam_sys": 2 * nc * F,
+            "S": n * n, "rhs": n, "cam_pred": N, "track_part": 3 * T, "result": RB_BA_RESULT, "error": T, "pin": 8 * F}
 
 
 def abspose_splits(max_n) -> int:
@@ -331,6 +335,11 @@ def _register_min_elems(kw):
     return out
 
 
+def _undistort_min_elems(kw):
+    return {"kp_offsets": kw["num_images"] + 1, "keypoints": 2 * kw["num_rows"], "intrinsics": 4 * kw["num_images"], "out": 2 * kw["num_rows"],
+            "clamped": 1}
+
+
 def _twoview_min_elems(kw):
     B, total = kw["batch"], kw["mask"].numel()
     return {"offsets": B + 1, "x0": 2 * total, "x1": 2 * total, "xn": 4 * total, "K": 18 * B, "R": 9 * B, "t": 3 * B, "ok": B,
@@ -343,7 +352,7 @@ _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_ele
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
               "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
               "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems,
-              "rb_twoview_args": _twoview_min_elems}
+              "rb_twoview_args": _twoview_min_elems, "rb_undistort_args": _undistort_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

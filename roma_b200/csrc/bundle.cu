@@ -8,6 +8,8 @@
 //   cholesky   right-looking, RB_BA_NB-wide panels (panel, triangular solve, trailing update), then both substitutions.
 //   step       the trial cameras (Rodrigues), then a warp per track: d_X, the trial cost and the depth check; fixed-order tree sums.
 // No float atomics and a fixed order in every reduction, so the result is bit-identical from run to run.
+// The kernels that touch a camera are templated on the camera model M: 0 = PINHOLE (6 parameters per camera), 1 = SIMPLE_RADIAL
+// (8: the pose, then f and k).
 #include "common.cuh"
 
 namespace rb {
@@ -19,6 +21,11 @@ constexpr int BA_SUM_THREADS = 1024;
 constexpr unsigned BA_FULL = 0xffffffffu;
 constexpr int NB = RB_BA_NB;
 static_assert(NB == 32, "the substitutions give a panel column to each lane of a warp");
+
+// per model: camera parameters NC, the length of a cams row, and the thread that starts the W V^-1 products of the camera kernel
+template <int M> struct BaModel;
+template <> struct BaModel<0> { static constexpr int NC = 6, CAM = RB_BA_CAM, A0 = 32; };
+template <> struct BaModel<1> { static constexpr int NC = 8, CAM = RB_BA_CAM1, A0 = 64; };
 
 template <int N>
 __device__ __forceinline__ void ba_warp_sum(double (&v)[N]) {
@@ -40,38 +47,58 @@ __device__ __forceinline__ double ba_rho(double s, double c2, double* w) {
     return c2 * log1p(s / c2);
 }
 
-// observation of element e (ids checked) under camera c = R (9), t (3), K (9) at X: residual (ru, rv) and depth; with JAC, the
-// Jacobians Jc [2][6] (d_omega, d_t) and JX [2][3]
-template <bool JAC>
+// observation of element e (ids checked) under camera c at X: residual (ru, rv), depth and, with JAC, the Jacobians Jc [2][NC]
+// and JX [2][3].  Model 0: c = R (9), t (3), K (9) and Jc = (d_omega, d_t).  Model 1: c = R (9), t (3), f, cx, cy, k and
+// Jc = (d_omega, d_t, d_f, d_k).
+template <bool JAC, int M>
 __device__ __forceinline__ void ba_project(const double* c, const double (&X)[3], double ox, double oy, double* ru, double* rv,
-                                           double* depth, double (*Jc)[6], double (*JX)[3]) {
-    double A[3], p[3], q[3];
+                                           double* depth, double (*Jc)[BaModel<M>::NC], double (*JX)[3]) {
+    double A[3], p[3];
 #pragma unroll
     for (int j = 0; j < 3; ++j) A[j] = c[3 * j] * X[0] + c[3 * j + 1] * X[1] + c[3 * j + 2] * X[2];
 #pragma unroll
     for (int j = 0; j < 3; ++j) p[j] = A[j] + c[9 + j];
+    double Jp[2][3];
+    if constexpr (M == 0) {
+        double q[3];
 #pragma unroll
-    for (int j = 0; j < 3; ++j) q[j] = c[12 + 3 * j] * p[0] + c[13 + 3 * j] * p[1] + c[14 + 3 * j] * p[2];
-    const double u = q[0] / q[2], v = q[1] / q[2];
-    *ru = u - ox;
-    *rv = v - oy;
-    *depth = p[2];
-    if (!JAC) return;
-    const double iz = 1.0 / q[2];
-    double Jq[2][3] = {{iz, 0.0, -u * iz}, {0.0, iz, -v * iz}};
+        for (int j = 0; j < 3; ++j) q[j] = c[12 + 3 * j] * p[0] + c[13 + 3 * j] * p[1] + c[14 + 3 * j] * p[2];
+        const double u = q[0] / q[2], v = q[1] / q[2];
+        *ru = u - ox;
+        *rv = v - oy;
+        *depth = p[2];
+        if (!JAC) return;
+        const double iz = 1.0 / q[2];
+        double Jq[2][3] = {{iz, 0.0, -u * iz}, {0.0, iz, -v * iz}};
+#pragma unroll
+        for (int r = 0; r < 2; ++r)
+#pragma unroll
+            for (int m = 0; m < 3; ++m) Jp[r][m] = Jq[r][0] * c[12 + m] + Jq[r][1] * c[15 + m] + Jq[r][2] * c[18 + m];
+    } else {
+        const double f = c[12], k = c[15];
+        const double x = p[0] / p[2], y = p[1] / p[2], r2 = x * x + y * y, d = 1.0 + k * r2;
+        *ru = f * d * x + c[13] - ox;
+        *rv = f * d * y + c[14] - oy;
+        *depth = p[2];
+        if (!JAC) return;
+        // d(u, v)/d(x, y), then through (x, y) = (p0, p1) / p2
+        const double iz = 1.0 / p[2];
+        const double uxx = f * (d + 2.0 * k * x * x), uxy = 2.0 * f * k * x * y, uyy = f * (d + 2.0 * k * y * y);
+        Jp[0][0] = uxx * iz; Jp[0][1] = uxy * iz; Jp[0][2] = -(uxx * x + uxy * y) * iz;
+        Jp[1][0] = uxy * iz; Jp[1][1] = uyy * iz; Jp[1][2] = -(uxy * x + uyy * y) * iz;
+        Jc[0][6] = d * x; Jc[1][6] = d * y;
+        Jc[0][7] = f * r2 * x; Jc[1][7] = f * r2 * y;
+    }
 #pragma unroll
     for (int r = 0; r < 2; ++r) {
-        double Jp[3];
-#pragma unroll
-        for (int m = 0; m < 3; ++m) Jp[m] = Jq[r][0] * c[12 + m] + Jq[r][1] * c[15 + m] + Jq[r][2] * c[18 + m];
         // d/d_omega of Exp(d_omega) R X is -[R X]x, so row r is (R X) x Jp
-        Jc[r][0] = A[1] * Jp[2] - A[2] * Jp[1];
-        Jc[r][1] = A[2] * Jp[0] - A[0] * Jp[2];
-        Jc[r][2] = A[0] * Jp[1] - A[1] * Jp[0];
+        Jc[r][0] = A[1] * Jp[r][2] - A[2] * Jp[r][1];
+        Jc[r][1] = A[2] * Jp[r][0] - A[0] * Jp[r][2];
+        Jc[r][2] = A[0] * Jp[r][1] - A[1] * Jp[r][0];
 #pragma unroll
-        for (int m = 0; m < 3; ++m) Jc[r][3 + m] = Jp[m];
+        for (int m = 0; m < 3; ++m) Jc[r][3 + m] = Jp[r][m];
 #pragma unroll
-        for (int m = 0; m < 3; ++m) JX[r][m] = Jp[0] * c[m] + Jp[1] * c[3 + m] + Jp[2] * c[6 + m];
+        for (int m = 0; m < 3; ++m) JX[r][m] = Jp[r][0] * c[m] + Jp[r][1] * c[3 + m] + Jp[r][2] * c[6 + m];
     }
 }
 
@@ -133,7 +160,9 @@ __global__ void __launch_bounds__(256) ba_offsets_kernel(rb_ba_args a, const uin
 }
 
 // ---- linearize --------------------------------------------------------------------------------------------------------------
+template <int M>
 __global__ void __launch_bounds__(BA_THREADS) ba_linearize_kernel(rb_ba_args a) {
+    constexpr int NC = BaModel<M>::NC;
     pdl_wait();
     const int lane = threadIdx.x & 31;
     if (blockIdx.x == 0 && threadIdx.x < RB_BA_RESULT) a.result[threadIdx.x] = 0.0;
@@ -152,9 +181,9 @@ __global__ void __launch_bounds__(BA_THREADS) ba_linearize_kernel(rb_ba_args a) 
         for (int64_t e = base + lane; e < base + L; e += 32) {
             if (!ba_used(a, e)) continue;
             int img;
-            double ox, oy, ru, rv, depth, Jc[2][6], JX[2][3], w;
+            double ox, oy, ru, rv, depth, Jc[2][NC], JX[2][3], w;
             ba_keypoint(a, e, &img, &ox, &oy);
-            ba_project<true>(a.cams + (int64_t)img * RB_BA_CAM, X, ox, oy, &ru, &rv, &depth, Jc, JX);
+            ba_project<true, M>(a.cams + (int64_t)img * BaModel<M>::CAM, X, ox, oy, &ru, &rv, &depth, Jc, JX);
             s[9] += 0.5 * ba_rho(ru * ru + rv * rv, a.loss_scale2, &w);
             s[0] += w * (JX[0][0] * JX[0][0] + JX[1][0] * JX[1][0]);
             s[1] += w * (JX[0][0] * JX[0][1] + JX[1][0] * JX[1][1]);
@@ -164,9 +193,9 @@ __global__ void __launch_bounds__(BA_THREADS) ba_linearize_kernel(rb_ba_args a) 
             s[5] += w * (JX[0][2] * JX[0][2] + JX[1][2] * JX[1][2]);
 #pragma unroll
             for (int m = 0; m < 3; ++m) s[6 + m] += w * (JX[0][m] * ru + JX[1][m] * rv);
-            double* W = a.W + e * 18;
+            double* W = a.W + e * (3 * NC);
 #pragma unroll
-            for (int r = 0; r < 6; ++r)
+            for (int r = 0; r < NC; ++r)
 #pragma unroll
                 for (int m = 0; m < 3; ++m) W[3 * r + m] = w * (Jc[0][r] * JX[0][m] + Jc[1][r] * JX[1][m]);
         }
@@ -184,42 +213,44 @@ __global__ void __launch_bounds__(BA_THREADS) ba_linearize_kernel(rb_ba_args a) 
 }
 
 // ---- camera blocks ------------------------------------------------------------------------------------------------------------
+template <int M>
 __global__ void __launch_bounds__(BA_CAM_THREADS) ba_cameras_kernel(rb_ba_args a) {
+    constexpr int NC = BaModel<M>::NC, NU = NC * (NC + 1) / 2, A0 = BaModel<M>::A0;
     pdl_wait();
-    __shared__ double sJ[15];          // Jc (12), r (2), w of the current observation
-    __shared__ double sA[18];          // W_e V_k^-1 (6 x 3)
-    __shared__ double sW[18], sV[9], sg[3];
+    __shared__ double sJ[2 * NC + 3];  // Jc (2 NC), r (2), w of the current observation
+    __shared__ double sA[3 * NC];      // W_e V_k^-1 (NC x 3)
+    __shared__ double sW[3 * NC], sV[9], sg[3];
     const int fi = blockIdx.x, tid = threadIdx.x;
     const int img = a.free_cams[fi];
-    const int64_t n = 6 * (int64_t)a.num_free;
-    double* Srow = a.S + 6 * (int64_t)fi * n;
-    for (int64_t q = tid; q < 6 * n; q += BA_CAM_THREADS) Srow[q] = 0.0;
-    // thread t < 21 accumulates U entry (p, q), p <= q, in row-major order of the upper triangle; 21 <= t < 27 g_c; 27 <= t < 33
-    // the reduced right-hand side's W V^-1 g_X term
+    const int64_t n = NC * (int64_t)a.num_free;
+    double* Srow = a.S + NC * (int64_t)fi * n;
+    for (int64_t q = tid; q < NC * n; q += BA_CAM_THREADS) Srow[q] = 0.0;
+    // thread t < NU accumulates U entry (p, q), p <= q, in row-major order of the upper triangle; NU <= t < NU + NC g_c;
+    // NU + NC <= t < NU + 2 NC the reduced right-hand side's W V^-1 g_X term
     int up = 0, uq = 0;
-    if (tid < 21) {
+    if (tid < NU) {
         int t = tid;
-        while (t >= 6 - up) { t -= 6 - up; ++up; }
+        while (t >= NC - up) { t -= NC - up; ++up; }
         uq = up + t;
     }
     double acc = 0.0;
-    const double* cam = a.cams + (int64_t)img * RB_BA_CAM;
+    const double* cam = a.cams + (int64_t)img * BaModel<M>::CAM;
     for (int64_t o = a.obs_offsets[img]; o < a.obs_offsets[img + 1]; ++o) {
         const int64_t e = a.obs[o];
         const int64_t k = a.elem_track[e];
         __syncthreads();                                  // the previous observation is done with the shared operands
         if (tid == 0) {
             int im;
-            double ox, oy, ru, rv, depth, Jc[2][6], JX[2][3], w;
+            double ox, oy, ru, rv, depth, Jc[2][NC], JX[2][3], w;
             ba_keypoint(a, e, &im, &ox, &oy);
             const double X[3] = {a.X[3 * k], a.X[3 * k + 1], a.X[3 * k + 2]};
-            ba_project<true>(cam, X, ox, oy, &ru, &rv, &depth, Jc, JX);
+            ba_project<true, M>(cam, X, ox, oy, &ru, &rv, &depth, Jc, JX);
             ba_rho(ru * ru + rv * rv, a.loss_scale2, &w);
 #pragma unroll
-            for (int r = 0; r < 6; ++r) { sJ[r] = Jc[0][r]; sJ[6 + r] = Jc[1][r]; }
-            sJ[12] = ru; sJ[13] = rv; sJ[14] = w;
-        } else if (tid >= 32 && tid < 50) {
-            sW[tid - 32] = a.W[e * 18 + tid - 32];
+            for (int r = 0; r < NC; ++r) { sJ[r] = Jc[0][r]; sJ[NC + r] = Jc[1][r]; }
+            sJ[2 * NC] = ru; sJ[2 * NC + 1] = rv; sJ[2 * NC + 2] = w;
+        } else if (tid >= 32 && tid < 32 + 3 * NC) {
+            sW[tid - 32] = a.W[e * (3 * NC) + tid - 32];
         } else if (tid >= 64 && tid < 73) {
             const int r = (tid - 64) / 3, c = (tid - 64) % 3;
             const int lo = min(r, c), hi = max(r, c);
@@ -228,61 +259,68 @@ __global__ void __launch_bounds__(BA_CAM_THREADS) ba_cameras_kernel(rb_ba_args a
             sg[tid - 96] = a.track_sys[k * RB_BA_TRACK + 6 + tid - 96];
         }
         __syncthreads();
-        if (tid < 21) {
-            acc += sJ[14] * (sJ[up] * sJ[uq] + sJ[6 + up] * sJ[6 + uq]);
-        } else if (tid < 27) {
-            const int p = tid - 21;
-            acc += sJ[14] * (sJ[p] * sJ[12] + sJ[6 + p] * sJ[13]);
-        } else if (tid >= 32 && tid < 50) {
-            const int r = (tid - 32) / 3, c = (tid - 32) % 3;
-            sA[tid - 32] = sW[3 * r] * sV[c] + sW[3 * r + 1] * sV[3 + c] + sW[3 * r + 2] * sV[6 + c];
+        if (tid < NU) {
+            acc += sJ[2 * NC + 2] * (sJ[up] * sJ[uq] + sJ[NC + up] * sJ[NC + uq]);
+        } else if (tid < NU + NC) {
+            const int p = tid - NU;
+            acc += sJ[2 * NC + 2] * (sJ[p] * sJ[2 * NC] + sJ[NC + p] * sJ[2 * NC + 1]);
+        } else if (tid >= A0 && tid < A0 + 3 * NC) {
+            const int r = (tid - A0) / 3, c = (tid - A0) % 3;
+            sA[tid - A0] = sW[3 * r] * sV[c] + sW[3 * r + 1] * sV[3 + c] + sW[3 * r + 2] * sV[6 + c];
         }
         __syncthreads();
-        if (tid >= 27 && tid < 33) {
-            const int p = tid - 27;
+        if (tid >= NU + NC && tid < NU + 2 * NC) {
+            const int p = tid - NU - NC;
             acc += sA[3 * p] * sg[0] + sA[3 * p + 1] * sg[1] + sA[3 * p + 2] * sg[2];
         }
         // block (fi, fj) -= A W_e'^T over the track's used observations in free cameras fj <= fi
         const int64_t base = a.track_offsets[k], L = a.track_offsets[k + 1] - base;
-        for (int64_t q = tid; q < 36 * L; q += BA_CAM_THREADS) {
-            const int64_t f = base + q / 36;
+        for (int64_t q = tid; q < NC * NC * L; q += BA_CAM_THREADS) {
+            const int64_t f = base + q / (NC * NC);
             if (!ba_used(a, f)) continue;
             const int fj = a.free_index[a.elements[2 * f]];
             if (fj < 0 || fj > fi) continue;
-            const int r = (int)(q % 36) / 6, c = (int)(q % 36) % 6;
-            const double* Wf = a.W + f * 18 + 3 * c;
-            Srow[r * n + 6 * (int64_t)fj + c] -= sA[3 * r] * Wf[0] + sA[3 * r + 1] * Wf[1] + sA[3 * r + 2] * Wf[2];
+            const int r = (int)(q % (NC * NC)) / NC, c = (int)(q % (NC * NC)) % NC;
+            const double* Wf = a.W + f * (3 * NC) + 3 * c;
+            Srow[r * n + NC * (int64_t)fj + c] -= sA[3 * r] * Wf[0] + sA[3 * r + 1] * Wf[1] + sA[3 * r + 2] * Wf[2];
         }
     }
     __syncthreads();
     // U and its damping on the diagonal block, the right-hand side, g_c and D_c
-    double* diag = Srow + 6 * (int64_t)fi;
-    if (tid < 21) {
+    double* diag = Srow + NC * (int64_t)fi;
+    if (tid < NU) {
         double u = acc;
         if (up == uq) {
             const double D = ba_clamp_diag(acc);
-            a.cam_sys[12 * (int64_t)fi + 6 + up] = D;
+            a.cam_sys[2 * NC * (int64_t)fi + NC + up] = D;
             u += a.lambda * D;
         }
         diag[up * n + uq] += u;
         if (up != uq) diag[uq * n + up] += acc;
     }
     __syncthreads();
-    __shared__ double sb[6];
-    if (tid >= 21 && tid < 27) sb[tid - 21] = -acc;
+    __shared__ double sb[NC];
+    if (tid >= NU && tid < NU + NC) sb[tid - NU] = -acc;
     __syncthreads();
-    if (tid >= 21 && tid < 27) a.cam_sys[12 * (int64_t)fi + tid - 21] = acc;
-    if (tid >= 27 && tid < 33) a.rhs[6 * (int64_t)fi + tid - 27] = sb[tid - 27] + acc;
+    if (tid >= NU && tid < NU + NC) a.cam_sys[2 * NC * (int64_t)fi + tid - NU] = acc;
+    if (tid >= NU + NC && tid < NU + 2 * NC) a.rhs[NC * (int64_t)fi + tid - NU - NC] = sb[tid - NU - NC] + acc;
     __syncthreads();
-    // rule 4: the t_x row of a camera in fixed_tx becomes e_r with a zero right-hand side, and so do the t_x columns
-    for (int64_t q = tid; q < 6 * n; q += BA_CAM_THREADS) {
+    // rule 4: a pinned row becomes e_r with a zero right-hand side, and so does its column.  Model 0 pins the t_x row of a camera
+    // in fixed_tx; model 1 the rows set in pin.
+    for (int64_t q = tid; q < NC * n; q += BA_CAM_THREADS) {
         const int r = (int)(q / n);
-        const int64_t col = q % n, row = 6 * (int64_t)fi + r;
+        const int64_t col = q % n, row = NC * (int64_t)fi + r;
         if (col > row) continue;
-        const bool row_tx = r == 3 && a.fixed_tx[fi];
-        const bool col_tx = col % 6 == 3 && a.fixed_tx[col / 6];
-        if (row_tx || col_tx) Srow[q] = col == row ? 1.0 : 0.0;
-        if (row_tx && col == row) a.rhs[row] = 0.0;
+        bool row_pin, col_pin;
+        if constexpr (M == 0) {
+            row_pin = r == 3 && a.fixed_tx[fi];
+            col_pin = col % 6 == 3 && a.fixed_tx[col / 6];
+        } else {
+            row_pin = a.pin[row] != 0;
+            col_pin = a.pin[col] != 0;
+        }
+        if (row_pin || col_pin) Srow[q] = col == row ? 1.0 : 0.0;
+        if (row_pin && col == row) a.rhs[row] = 0.0;
     }
 }
 
@@ -405,37 +443,63 @@ __global__ void __launch_bounds__(1024) ba_potrs_kernel(const double* __restrict
 }
 
 // ---- step ---------------------------------------------------------------------------------------------------------------------
+template <int M>
 __global__ void __launch_bounds__(128) ba_step_cameras_kernel(rb_ba_args a) {
+    constexpr int NC = BaModel<M>::NC, CAM = BaModel<M>::CAM;
     pdl_wait();
     const int i = blockIdx.x * 128 + threadIdx.x;
     if (i >= a.num_images) return;
-    const double* c = a.cams + (int64_t)i * RB_BA_CAM;
-    double* o = a.cams_trial + (int64_t)i * RB_BA_CAM;
+    const double* c = a.cams + (int64_t)i * CAM;
+    double* o = a.cams_trial + (int64_t)i * CAM;
     const int fi = a.num_free > 0 ? a.free_index[i] : -1;
     if (fi < 0) {
-        for (int j = 0; j < RB_BA_CAM; ++j) o[j] = c[j];
+        for (int j = 0; j < CAM; ++j) o[j] = c[j];
         a.cam_pred[i] = 0.0;
         return;
     }
-    double d[6], pred = 0.0;
+    double d[NC], pred = 0.0;
 #pragma unroll
-    for (int j = 0; j < 6; ++j) d[j] = a.rhs[6 * (int64_t)fi + j];
+    for (int j = 0; j < NC; ++j) d[j] = a.rhs[NC * (int64_t)fi + j];
 #pragma unroll
-    for (int j = 0; j < 6; ++j) pred += d[j] * (a.lambda * a.cam_sys[12 * (int64_t)fi + 6 + j] * d[j] - a.cam_sys[12 * (int64_t)fi + j]);
-    const double w[3] = {d[0], d[1], d[2]};
-    double E[3][3];
-    so3_exp(w, E);
+    for (int j = 0; j < NC; ++j) pred += d[j] * (a.lambda * a.cam_sys[2 * NC * (int64_t)fi + NC + j] * d[j] - a.cam_sys[2 * NC * (int64_t)fi + j]);
+    if constexpr (M == 0) {
+        const double w[3] = {d[0], d[1], d[2]};
+        double E[3][3];
+        so3_exp(w, E);
 #pragma unroll
-    for (int r = 0; r < 3; ++r)
+        for (int r = 0; r < 3; ++r)
 #pragma unroll
-        for (int m = 0; m < 3; ++m) o[3 * r + m] = E[r][0] * c[m] + E[r][1] * c[3 + m] + E[r][2] * c[6 + m];
+            for (int m = 0; m < 3; ++m) o[3 * r + m] = E[r][0] * c[m] + E[r][1] * c[3 + m] + E[r][2] * c[6 + m];
 #pragma unroll
-    for (int j = 0; j < 3; ++j) o[9 + j] = c[9 + j] + d[3 + j];
-    for (int j = 12; j < RB_BA_CAM; ++j) o[j] = c[j];
+        for (int j = 0; j < 3; ++j) o[9 + j] = c[9 + j] + d[3 + j];
+        for (int j = 12; j < CAM; ++j) o[j] = c[j];
+    } else {
+        // a pinned parameter is copied, so it comes back bit-identical whatever its sign of zero
+        const uint8_t* pin = a.pin + NC * (int64_t)fi;
+        if (pin[0] && pin[1] && pin[2]) {
+            for (int j = 0; j < 9; ++j) o[j] = c[j];
+        } else {
+            const double w[3] = {d[0], d[1], d[2]};
+            double E[3][3];
+            so3_exp(w, E);
+#pragma unroll
+            for (int r = 0; r < 3; ++r)
+#pragma unroll
+                for (int m = 0; m < 3; ++m) o[3 * r + m] = E[r][0] * c[m] + E[r][1] * c[3 + m] + E[r][2] * c[6 + m];
+        }
+#pragma unroll
+        for (int j = 0; j < 3; ++j) o[9 + j] = pin[3 + j] ? c[9 + j] : c[9 + j] + d[3 + j];
+        o[12] = pin[6] ? c[12] : c[12] + d[6];
+        o[13] = c[13];
+        o[14] = c[14];
+        o[15] = pin[7] ? c[15] : c[15] + d[7];
+    }
     a.cam_pred[i] = 0.5 * pred;
 }
 
+template <int M>
 __global__ void __launch_bounds__(BA_THREADS) ba_step_points_kernel(rb_ba_args a) {
+    constexpr int NC = BaModel<M>::NC;
     pdl_wait();
     const int lane = threadIdx.x & 31;
     const int64_t stride = (int64_t)gridDim.x * BA_WARPS;
@@ -456,11 +520,17 @@ __global__ void __launch_bounds__(BA_THREADS) ba_step_points_kernel(rb_ba_args a
                 if (!ba_used(a, e)) continue;
                 const int fj = a.free_index[a.elements[2 * e]];
                 if (fj < 0) continue;
-                const double* W = a.W + e * 18;
-                const double* d = a.rhs + 6 * (int64_t)fj;
+                const double* W = a.W + e * (3 * NC);
+                const double* d = a.rhs + NC * (int64_t)fj;
 #pragma unroll
-                for (int m = 0; m < 3; ++m)
-                    b[m] += W[m] * d[0] + W[3 + m] * d[1] + W[6 + m] * d[2] + W[9 + m] * d[3] + W[12 + m] * d[4] + W[15 + m] * d[5];
+                for (int m = 0; m < 3; ++m) {
+                    if constexpr (M == 0) {
+                        b[m] += W[m] * d[0] + W[3 + m] * d[1] + W[6 + m] * d[2] + W[9 + m] * d[3] + W[12 + m] * d[4] + W[15 + m] * d[5];
+                    } else {
+                        b[m] += W[m] * d[0] + W[3 + m] * d[1] + W[6 + m] * d[2] + W[9 + m] * d[3] + W[12 + m] * d[4] + W[15 + m] * d[5] +
+                                W[18 + m] * d[6] + W[21 + m] * d[7];
+                    }
+                }
             }
             ba_warp_sum(b);
         }
@@ -476,9 +546,11 @@ __global__ void __launch_bounds__(BA_THREADS) ba_step_points_kernel(rb_ba_args a
             int img;
             double ox, oy, ru, rv, depth, w;
             ba_keypoint(a, e, &img, &ox, &oy);
-            ba_project<false>(a.cams_trial + (int64_t)img * RB_BA_CAM, X1, ox, oy, &ru, &rv, &depth, nullptr, nullptr);
+            const double* cam = a.cams_trial + (int64_t)img * BaModel<M>::CAM;
+            ba_project<false, M>(cam, X1, ox, oy, &ru, &rv, &depth, nullptr, nullptr);
             s[0] += 0.5 * ba_rho(ru * ru + rv * rv, a.loss_scale2, &w);
-            s[1] += !(depth > 0.0);
+            if constexpr (M == 0) s[1] += !(depth > 0.0);
+            else s[1] += !(depth > 0.0) || !(cam[12] > 0.0);        // a trial focal length that is not > 0 rejects the step
         }
         ba_warp_sum(s);
         if (lane < 3) a.X_trial[3 * k + lane] = lane == 0 ? X1[0] : (lane == 1 ? X1[1] : X1[2]);
@@ -527,6 +599,7 @@ __global__ void __launch_bounds__(BA_SUM_THREADS) ba_sum_kernel(rb_ba_args a) {
     }
 }
 
+template <int M>
 __global__ void __launch_bounds__(BA_THREADS) ba_error_kernel(rb_ba_args a) {
     pdl_wait();
     const int lane = threadIdx.x & 31;
@@ -541,7 +614,7 @@ __global__ void __launch_bounds__(BA_THREADS) ba_error_kernel(rb_ba_args a) {
                 int img;
                 double ox, oy, ru, rv, depth;
                 ba_keypoint(a, e, &img, &ox, &oy);
-                ba_project<false>(a.cams + (int64_t)img * RB_BA_CAM, X, ox, oy, &ru, &rv, &depth, nullptr, nullptr);
+                ba_project<false, M>(a.cams + (int64_t)img * BaModel<M>::CAM, X, ox, oy, &ru, &rv, &depth, nullptr, nullptr);
                 s[0] += sqrt(ru * ru + rv * rv);
                 s[1] += 1.0;
             }
@@ -559,6 +632,7 @@ static int ba_check(const rb_ba_args* a, const char* what) {
                "num_rows=%lld", what, a->num_tracks, a->num_images, a->num_free, (long long)a->num_elements, (long long)a->num_rows);
     RB_REQUIRE(a->loss_scale2 >= 0.0 && isfinite(a->loss_scale2) && a->lambda > 0.0 && isfinite(a->lambda), "%s: bad loss_scale2=%g or "
                "lambda=%g", what, a->loss_scale2, a->lambda);
+    RB_REQUIRE(a->camera_model == 0 || a->camera_model == 1, "%s: bad camera_model=%d", what, a->camera_model);
     return 0;
 }
 
@@ -585,7 +659,8 @@ extern "C" int romab200_ba_setup(const rb_ba_args* a, void* stream) {
 extern "C" int romab200_ba_linearize(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_linearize")) return 1;
     RB_REQUIRE(a->W && a->track_sys && a->result, "ba_linearize: null argument");
-    launch_pdl(ba_linearize_kernel, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0, (cudaStream_t)stream, *a);
+    launch_pdl(a->camera_model ? ba_linearize_kernel<1> : ba_linearize_kernel<0>, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0,
+               (cudaStream_t)stream, *a);
     return check_launch("ba_linearize");
 }
 
@@ -598,9 +673,11 @@ extern "C" int romab200_ba_cost(const rb_ba_args* a, void* stream) {
 
 extern "C" int romab200_ba_cameras(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_cameras")) return 1;
-    RB_REQUIRE(a->num_free > 0 && a->free_index && a->free_cams && a->fixed_tx && a->elem_track && a->obs_offsets && a->obs && a->W &&
-               a->track_sys && a->cam_sys && a->S && a->rhs, "ba_cameras: null argument or no free camera");
-    launch_pdl(ba_cameras_kernel, dim3(a->num_free), dim3(BA_CAM_THREADS), 0, (cudaStream_t)stream, *a);
+    RB_REQUIRE(a->num_free > 0 && a->free_index && a->free_cams && (a->camera_model ? a->pin != nullptr : a->fixed_tx != nullptr) &&
+               a->elem_track && a->obs_offsets && a->obs && a->W && a->track_sys && a->cam_sys && a->S && a->rhs,
+               "ba_cameras: null argument or no free camera");
+    launch_pdl(a->camera_model ? ba_cameras_kernel<1> : ba_cameras_kernel<0>, dim3(a->num_free), dim3(BA_CAM_THREADS), 0,
+               (cudaStream_t)stream, *a);
     return check_launch("ba_cameras");
 }
 
@@ -608,7 +685,7 @@ extern "C" int romab200_ba_cholesky(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_cholesky")) return 1;
     RB_REQUIRE(a->num_free > 0 && a->S && a->rhs && a->result, "ba_cholesky: null argument or no free camera");
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t n = 6 * (int64_t)a->num_free;
+    const int64_t n = (a->camera_model ? 8 : 6) * (int64_t)a->num_free;
     for (int64_t k0 = 0; k0 < n; k0 += NB) {
         const int nb = (int)(n - k0 < NB ? n - k0 : NB);
         launch_pdl(ba_potrf_panel_kernel, dim3(1), dim3(256), 0, st, a->S, n, k0, nb, a->result);
@@ -628,11 +705,14 @@ extern "C" int romab200_ba_cholesky(const rb_ba_args* a, void* stream) {
 extern "C" int romab200_ba_step(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_step")) return 1;
     RB_REQUIRE(a->cams_trial && a->X_trial && a->track_sys && a->cam_pred && a->track_part && a->result &&
-               (a->num_free == 0 || (a->free_index && a->rhs && a->cam_sys && a->W)), "ba_step: null argument");
+               (a->num_free == 0 || (a->free_index && a->rhs && a->cam_sys && a->W && (!a->camera_model || a->pin))),
+               "ba_step: null argument");
     cudaStream_t st = (cudaStream_t)stream;
-    launch_pdl(ba_step_cameras_kernel, dim3((a->num_images + 127) / 128), dim3(128), 0, st, *a);
+    launch_pdl(a->camera_model ? ba_step_cameras_kernel<1> : ba_step_cameras_kernel<0>, dim3((a->num_images + 127) / 128), dim3(128), 0,
+               st, *a);
     if (check_launch("ba_step(cameras)")) return 1;
-    launch_pdl(ba_step_points_kernel, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0, st, *a);
+    launch_pdl(a->camera_model ? ba_step_points_kernel<1> : ba_step_points_kernel<0>, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0, st,
+               *a);
     if (check_launch("ba_step(points)")) return 1;
     launch_pdl(ba_sum_kernel<true>, dim3(1), dim3(BA_SUM_THREADS), 0, st, *a);
     return check_launch("ba_step(sum)");
@@ -641,6 +721,7 @@ extern "C" int romab200_ba_step(const rb_ba_args* a, void* stream) {
 extern "C" int romab200_ba_error(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_error")) return 1;
     RB_REQUIRE(a->error, "ba_error: null argument");
-    launch_pdl(ba_error_kernel, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0, (cudaStream_t)stream, *a);
+    launch_pdl(a->camera_model ? ba_error_kernel<1> : ba_error_kernel<0>, dim3(ba_track_grid(a)), dim3(BA_THREADS), 0,
+               (cudaStream_t)stream, *a);
     return check_launch("ba_error");
 }

@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from . import cabi, geometry
+from . import camera as _camera
 from . import triangulate as _tri
 from . import verify as _verify
 from .bundle import bundle_adjust
@@ -62,6 +63,7 @@ class Reconstruction:
     init: TwoViewInit
     rounds: list
     termination: str
+    intrinsics: torch.Tensor = None
 
 
 def rank_candidates(match_offsets, min_num_inliers, num_candidates) -> list:
@@ -220,7 +222,7 @@ def initialize_reconstruction(pairs, graph: MatchGraph, K, *, init_pair=None, nu
 def reconstruct(pairs, graph: MatchGraph, tracks: Tracks, K, *, init_pair=None, init_num_candidates=256, init_min_num_inliers=100,
                 init_max_error=4.0, init_min_tri_angle=16.0, init_max_forward_motion=0.95, tri_max_error=4.0, tri_min_angle=1.5,
                 abs_max_error=12.0, abs_min_inliers=30, ba_loss_scale=None, ba_max_iterations=50, seed=0,
-                workspace_bytes=WORKSPACE_BYTES) -> Reconstruction:
+                workspace_bytes=WORKSPACE_BYTES, intrinsics=None, refine_intrinsics=False) -> Reconstruction:
     """A reconstruction of the images of `graph` (verified, built from `pairs`) and `tracks` (built from it) with intrinsics K and no
     known camera.  `initialize_reconstruction` (the init_* arguments) chooses the pair (a, b); a gets [I | 0] and b the unit-baseline
     [R | t], and every other camera is zero.  Then each round:
@@ -237,9 +239,31 @@ def reconstruct(pairs, graph: MatchGraph, tracks: Tracks, K, *, init_pair=None, 
     are held.  Without an accepted initial pair nothing is registered and termination is "no_initial_pair" (no exception).  Every
     image that registration accepts is added in the same round (there is no next-best-view order and no local BA).
 
+    Unknown intrinsics: with `intrinsics` [N, 4] (f, cx, cy, k), SIMPLE_RADIAL priors (`camera.default_intrinsics`, or EXIF values),
+    pass K=None.  The stages that take pinhole cameras (the two-view initialisation, triangulation, registration) run on
+    `undistort_graph(graph, current)` with `pinhole_K(current)`; an unregistered image keeps its prior.  Each round's bundle
+    adjustment runs on the raw graph with camera_model="SIMPLE_RADIAL", refine_focal_length = refine_extra_params =
+    `refine_intrinsics`, and every unregistered image in fixed_intrinsics.  The intrinsics stay fixed while fewer than
+    MIN_REGISTERED_TO_REFINE (3) images are registered: with the initial pair alone, focal lengths trade against the baseline depth
+    almost freely.  After the adjustment the graph is undistorted again under the refined intrinsics before the re-triangulation and
+    the registration.  Reconstruction.intrinsics is the final [N, 4].  intrinsics=None is the pinhole call above, unchanged.
+
     Arguments are checked before any device work (ValueError).  Bit-identical from run to run.  Host reads: those of the stages, and
     the accepted flags of each registration."""
     what = "reconstruct"
+    if not isinstance(refine_intrinsics, bool):
+        raise ValueError(f"{what}: refine_intrinsics must be a bool, got {refine_intrinsics!r}")
+    if intrinsics is not None:
+        if K is not None:
+            raise ValueError(f"{what}: pass K=None with intrinsics (the pinhole K is pinhole_K of the current intrinsics)")
+        if not isinstance(graph, MatchGraph):
+            raise ValueError(f"{what}: graph must be a MatchGraph, got {type(graph).__name__}")
+        cur = _camera.check_intrinsics(intrinsics, len(graph._kp_off) - 1, what)
+        return _reconstruct_radial(pairs, graph, tracks, cur, refine_intrinsics, init_pair, init_num_candidates, init_min_num_inliers,
+                                   init_max_error, init_min_tri_angle, init_max_forward_motion, tri_max_error, tri_min_angle,
+                                   abs_max_error, abs_min_inliers, ba_loss_scale, ba_max_iterations, seed, workspace_bytes)
+    if refine_intrinsics:
+        raise ValueError(f"{what}: refine_intrinsics needs intrinsics")
     _float(what, "abs_max_error", abs_max_error, 0.0, True)
     _int(what, "abs_min_inliers", abs_min_inliers, 0)
     if ba_loss_scale is not None:
@@ -297,6 +321,76 @@ def reconstruct(pairs, graph: MatchGraph, tracks: Tracks, K, *, init_pair=None, 
     return Reconstruction(mask, R, t, pts, init, rounds, termination)
 
 
+MIN_REGISTERED_TO_REFINE = 3
+
+
+def _reconstruct_radial(pairs, graph, tracks, cur, refine, init_pair, init_num_candidates, init_min_num_inliers, init_max_error,
+                        init_min_tri_angle, init_max_forward_motion, tri_max_error, tri_min_angle, abs_max_error, abs_min_inliers,
+                        ba_loss_scale, ba_max_iterations, seed, workspace_bytes) -> Reconstruction:
+    """`reconstruct` with SIMPLE_RADIAL intrinsics `cur` [N, 4] (host float64, checked)."""
+    what = "reconstruct"
+    _float(what, "abs_max_error", abs_max_error, 0.0, True)
+    _int(what, "abs_min_inliers", abs_min_inliers, 0)
+    if ba_loss_scale is not None:
+        _float(what, "ba_loss_scale", ba_loss_scale, 0.0, True)
+    _int(what, "ba_max_iterations", ba_max_iterations, 0)
+    _int(what, "workspace_bytes", workspace_bytes, 1)
+    N = len(graph._kp_off) - 1
+    Kc = _camera.pinhole_K(cur)
+    _tri._check(graph, tracks, Kc, np.tile(np.eye(3), (N, 1, 1)), np.zeros((N, 3)), tri_max_error, tri_min_angle, 1, seed, what=what)
+    _check_init(pairs, graph, Kc, init_pair, init_num_candidates, init_min_num_inliers, init_max_error, init_min_tri_angle,
+                init_max_forward_motion, 0.999, 10000, seed, what=what)
+    ug = _camera.undistort_graph(graph, cur)
+    init = initialize_reconstruction(pairs, ug, Kc, init_pair=init_pair, num_candidates=init_num_candidates,
+                                     min_num_inliers=init_min_num_inliers, max_error=init_max_error, min_tri_angle=init_min_tri_angle,
+                                     max_forward_motion=init_max_forward_motion, seed=seed)
+    dev = graph.kp_offsets.device
+    with torch.cuda.device(dev):
+        R = torch.zeros(N, 3, 3, dtype=torch.float64, device=dev)
+        t = torch.zeros(N, 3, dtype=torch.float64, device=dev)
+        tri = dict(max_error=tri_max_error, min_angle=tri_min_angle, seed=seed)
+        if init.chosen < 0:
+            pts = triangulate_tracks(ug, tracks, Kc, R, t, images=[], **tri)
+            return Reconstruction(torch.zeros(N, dtype=torch.bool, device=dev), R, t, pts, init, [], "no_initial_pair",
+                                  torch.from_numpy(cur).to(dev))
+        a, b = init.images[init.chosen].tolist()
+        R[a] = torch.eye(3, dtype=torch.float64, device=dev)
+        R[b], t[b] = init.R[init.chosen], init.t[init.chosen]
+        registered, rounds = sorted((a, b)), []
+        while True:
+            rest = [i for i in range(N) if i not in registered]
+            pts = triangulate_tracks(ug, tracks, Kc, R, t, images=registered, **tri)
+            free_intr = refine and len(registered) >= MIN_REGISTERED_TO_REFINE
+            ba = bundle_adjust(graph, tracks, pts, cur, R, t, fixed_poses=[a] + rest, fixed_tx=[b], loss_scale=ba_loss_scale,
+                               max_iterations=ba_max_iterations, workspace_bytes=workspace_bytes, camera_model="SIMPLE_RADIAL",
+                               refine_focal_length=free_intr, refine_extra_params=free_intr, fixed_intrinsics=rest)
+            R, t = ba.R.clone(), ba.t.clone()
+            if free_intr:
+                cur = ba.intrinsics.cpu().numpy()
+                Kc = _camera.pinhole_K(cur)
+                ug = _camera.undistort_graph(graph, cur)
+            pts = triangulate_tracks(ug, tracks, Kc, R, t, images=registered, **tri)
+            rnd = dict(registered=list(registered), ba_termination=ba.termination, ba_cost=(float(ba.cost[0]), float(ba.cost[-1])),
+                       ok_tracks=int(pts.ok.sum().item()), added=[])
+            rounds.append(rnd)
+            if not rest:
+                termination = "all_registered"
+                break
+            reg = register_images(ug, tracks, pts, Kc, rest, max_error=abs_max_error, min_inliers=abs_min_inliers, seed=seed)
+            acc = reg.accepted.tolist()
+            rnd["added"] = [i for m, i in enumerate(rest) if acc[m]]
+            if not rnd["added"]:
+                termination = "no_image_added"
+                break
+            rows = torch.tensor([m for m in range(len(rest)) if acc[m]], device=dev)
+            idx = torch.tensor(rnd["added"], device=dev)
+            R[idx], t[idx] = reg.R[rows], reg.t[rows]
+            registered = sorted(registered + rnd["added"])
+        mask = torch.zeros(N, dtype=torch.bool, device=dev)
+        mask[registered] = True
+    return Reconstruction(mask, R, t, pts, init, rounds, termination, torch.from_numpy(cur).to(dev))
+
+
 # ---- COLMAP text model ---------------------------------------------------------------------------------------------------
 def rotation_to_quaternion(R) -> np.ndarray:
     """Hamilton quaternions (qw, qx, qy, qz) with qw >= 0 of rotations R [..., 3, 3], by Shepperd's method: the largest of 1 + tr,
@@ -352,12 +446,21 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
     images.txt lists the registered images: the Hamilton quaternion (QW >= 0) of R and t, then every keypoint of the image (so
     POINT2D_IDX is the keypoint id) with POINT3D_ID k + 1 when it is an inlier element of ok track k and -1 otherwise.  points3D.txt
     has one line per ok track: X, colour 128 128 128, ERROR = points.error and its inlier elements in element order.  image_names
-    default to "image_<i>".  Values are written with 17 significant digits, so they read back exactly."""
+    default to "image_<i>".  Values are written with 17 significant digits, so they read back exactly.
+
+    When recon.intrinsics is set (`reconstruct(..., intrinsics=...)`), K is not read (pass None) and every camera is written as
+    "SIMPLE_RADIAL W H f cx cy k" of recon.intrinsics.  The keypoints of `graph` (the raw, distorted ones) are written as they are,
+    which is what COLMAP expects; ERROR is points.error, the mean reprojection error of the re-triangulation in the undistorted
+    frame."""
     kp_off = np.asarray(graph._kp_off, np.int64)
     N = len(kp_off) - 1
-    K = _tri._float64("K", K, (N, 3, 3), "write_colmap_text")
-    if np.any(K[:, 0, 1] != 0) or np.any(K[:, 1, 0] != 0) or np.any(K[:, 2] != np.array([0.0, 0.0, 1.0])):
-        raise ValueError("write_colmap_text: K must be a pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] (no skew)")
+    radial = recon.intrinsics is not None
+    if radial:
+        intr = _camera.check_intrinsics(recon.intrinsics, N, "write_colmap_text")
+    else:
+        K = _tri._float64("K", K, (N, 3, 3), "write_colmap_text")
+        if np.any(K[:, 0, 1] != 0) or np.any(K[:, 1, 0] != 0) or np.any(K[:, 2] != np.array([0.0, 0.0, 1.0])):
+            raise ValueError("write_colmap_text: K must be a pinhole matrix [[fx, 0, cx], [0, fy, cy], [0, 0, 1]] (no skew)")
     sizes = _host(image_sizes).astype(np.int64).reshape(N, 2)
     names = [f"image_{i}" for i in range(N)] if image_names is None else [str(n) for n in image_names]
     if len(names) != N:
@@ -375,8 +478,12 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
     pid = np.full(kp_off[-1], -1, np.int64)
     pid[kp_off[el[used, 0]] + el[used, 1]] = track[used] + 1
 
-    cam = _join(np.arange(1, N + 1), np.full(N, "PINHOLE"), sizes[:, 1], sizes[:, 0], _fmt(K[:, 0, 0]), _fmt(K[:, 1, 1]),
-                _fmt(K[:, 0, 2]), _fmt(K[:, 1, 2]))
+    if radial:
+        cam = _join(np.arange(1, N + 1), np.full(N, "SIMPLE_RADIAL"), sizes[:, 1], sizes[:, 0], _fmt(intr[:, 0]), _fmt(intr[:, 1]),
+                    _fmt(intr[:, 2]), _fmt(intr[:, 3]))
+    else:
+        cam = _join(np.arange(1, N + 1), np.full(N, "PINHOLE"), sizes[:, 1], sizes[:, 0], _fmt(K[:, 0, 0]), _fmt(K[:, 1, 1]),
+                    _fmt(K[:, 0, 2]), _fmt(K[:, 1, 2]))
     with open(os.path.join(path, "cameras.txt"), "w") as f:
         f.write("# Camera list with one line of data per camera:\n#   CAMERA_ID, MODEL, WIDTH, HEIGHT, PARAMS[]\n"
                 f"# Number of cameras: {N}\n")

@@ -530,7 +530,7 @@ def _planted_samples(g, vis, cells, H, W, cs, outlier_frac, device):
 
 
 def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024), cell_size: int = 1, noise: float = 0.5,
-                    visibility: float = 0.5, outlier_frac: float = 0.0, device="cpu"):
+                    visibility: float = 0.5, outlier_frac: float = 0.0, device="cpu", radial=None, spread: bool = False):
     """Seeded multi-view samples of a real scene, for geometric verification (`verify_matches`): `planted_views` with geometry.  A
     cloud of `n_points` scene points fills a 8 x 6 x 6 box around the origin; `n_images` pinhole cameras of `size` (H, W) with the
     intrinsics of `_scene_intrinsics` stand 8-10 units from the origin at azimuths of -40..40 degrees and heights of -1..1 and look at
@@ -540,7 +540,14 @@ def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024)
     `visibility` fails, or when its cell (the fp32 rule of `consolidate_matches` applied to the normalised coordinates) is already
     taken by a lower-indexed point.  Samples, outliers, certainties and padding are those of `planted_views` for these cells.
     Returns, on `device`: what `planted_views` returns (pairs, matches, certainty, image_sizes, views), then K [N, 3, 3], R [N, 3, 3]
-    and t [N, 3] float64 (x ~ K (R X + t)) and X [n_points, 3] float64."""
+    and t [N, 3] float64 (x ~ K (R X + t)) and X [n_points, 3] float64.
+
+    Options, drawn from a second generator so that the draws above are the same with and without them:
+    - radial=(k_lo, k_hi): SIMPLE_RADIAL cameras (`roma_b200.camera`): each image keeps the f of its pinhole intrinsics, square pixels,
+      the principal point at (W / 2, H / 2) and k uniform in [k_lo, k_hi], applied before the noise and the cell assignment.  K is
+      then the [N, 4] (f, cx, cy, k) float64 intrinsics.
+    - spread=True: look-at targets uniform in a 4 x 3 x 3 box, heights of -3..3 and rolls of -20..20 degrees about the optical
+      axis, so that the optical axes do not all meet near one point (per-image focal lengths are then better determined)."""
     import numpy as np
 
     H, W = size
@@ -553,17 +560,36 @@ def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024)
     r, h = rng.uniform(8.0, 10.0, n_images), rng.uniform(-1.0, 1.0, n_images)
     C = np.stack((r * np.sin(az), h, -r * np.cos(az)), 1)
     target = rng.uniform(-0.5, 0.5, (n_images, 3))
+    extra = np.random.default_rng([seed, 1])
+    roll = np.zeros(n_images)
+    if spread:
+        target = extra.uniform(-1.0, 1.0, (n_images, 3)) * np.array([2.0, 1.5, 1.5])
+        C[:, 1] = extra.uniform(-3.0, 3.0, n_images)
+        roll = np.deg2rad(extra.uniform(-20.0, 20.0, n_images))
     R = np.empty((n_images, 3, 3))
     for c in range(n_images):
         z = (target[c] - C[c]) / np.linalg.norm(target[c] - C[c])
         x = np.cross([0.0, 1.0, 0.0], z)
         x /= np.linalg.norm(x)
         R[c] = np.stack((x, np.cross(z, x), z))
+        if roll[c]:
+            cr, sr = np.cos(roll[c]), np.sin(roll[c])
+            R[c] = np.array([[cr, -sr, 0.0], [sr, cr, 0.0], [0.0, 0.0, 1.0]]) @ R[c]
     t = -np.einsum("cij,cj->ci", R, C)
-    p = np.einsum("cij,cjk,pk->cpi", K, R, X) + np.einsum("cij,cj->ci", K, t)[:, None]        # [N, n_points, 3]
-    depth = p[..., 2]
-    with np.errstate(divide="ignore", invalid="ignore"):
-        xy = p[..., :2] / depth[..., None] + rng.normal(scale=noise, size=(n_images, n_points, 2))
+    if radial is not None:
+        k = extra.uniform(radial[0], radial[1], n_images)
+        K = np.stack((K[:, 0, 0], np.full(n_images, W / 2), np.full(n_images, H / 2), k), 1)
+        pc = np.einsum("cij,pj->cpi", R, X) + t[:, None]
+        depth = pc[..., 2]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xn = pc[..., :2] / depth[..., None]
+            d = 1.0 + K[:, 3, None] * (xn * xn).sum(-1)
+            xy = K[:, None, 0, None] * d[..., None] * xn + K[:, None, 1:3] + rng.normal(scale=noise, size=(n_images, n_points, 2))
+    else:
+        p = np.einsum("cij,cjk,pk->cpi", K, R, X) + np.einsum("cij,cj->ci", K, t)[:, None]        # [N, n_points, 3]
+        depth = p[..., 2]
+        with np.errstate(divide="ignore", invalid="ignore"):
+            xy = p[..., :2] / depth[..., None] + rng.normal(scale=noise, size=(n_images, n_points, 2))
     vis = (depth > 0) & (xy[..., 0] >= 0) & (xy[..., 0] < W) & (xy[..., 1] >= 0) & (xy[..., 1] < H)
     vis &= rng.random((n_images, n_points)) < visibility
     u = np.where(vis, 2 * xy[..., 0] / W - 1, 0.0).astype(np.float32)
