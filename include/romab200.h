@@ -1289,6 +1289,87 @@ typedef struct {
 } rb_undistort_args;
 int romab200_undistort_keypoints(const rb_undistort_args* args, void* stream);
 
+/* ---- dense reconstruction: per-image depth maps triangulated from dense warps, fused into a point cloud ----
+ * Not in the reference.  The input is what match_pairs returns for the rows first_pair .. first_pair + chunk of pairs [num_pairs, 2]
+ * int64: warp [chunk, H, 2W, 4] and certainty [chunk, H, 2W] fp32, symmetric.  Element (r, c) of the left half is grid pixel (r, c)
+ * of image pairs[k][0], matched at warp[..., 2:4] in image pairs[k][1]; element (r, W + c) of the right half is grid pixel (r, c) of
+ * image pairs[k][1], matched at warp[..., 0:2] in image pairs[k][0].  k = first_pair + row is the global pair index, half 0 / 1 the
+ * side, g = 2 k + half names the element's pair-half.  image_sizes [num_images, 2] int32 (H_img, W_img) is the pixel frame of the
+ * cameras; cameras [num_images, RB_DENSE_CAM] float64 per image: K (9, row-major), K^-1 (9, computed on the host), R (9), t (3),
+ * SIMPLE_RADIAL (f, cx, cy, k) (4), 2 unused; x ~ K (R X + t).  All geometry is float64.  The rules of one element:
+ * 1. Grid side.  x = W_img (c + 0.5) / W, y = H_img (r + 0.5) / H in the grid image's frame, evaluated left to right.
+ * 2. Match side.  (u, v) read from the warp; x = (W_img / 2) * (u + 1), y = (H_img / 2) * (v + 1), each operation rounded to fp32
+ *    (consolidate_matches' rule), then widened.
+ * 3. Rejection, in this order, the first failure being the element's reason: 1 certainty <= min_certainty or any of the certainty,
+ *    u, v not finite; 2 u or v outside [-1, 1]; 3 either image not registered; 4 (radial only) either position clamped by the
+ *    undistortion; 5 the point not in front of both cameras (Q_w = 0, or either depth not > 0, NaN included); 6 the squared
+ *    reprojection error in px in either image > max_error2; 7 the triangulation angle < min_angle (radians).  Reason 0 is accepted.
+ * 4. Normalised coordinates.  Pinhole: h = K^-1 (x, y, 1), (h0 / h2, h1 / h2).  radial = 1: (dx, dy) = (x - cx, y - cy), rho_d =
+ *    |(dx, dy)| / f and (dx s / f, dy s / f) with s = rho / rho_d from the Newton loop of the keypoint undistortion below (s = 1 when
+ *    k = 0 or rho_d = 0); clamped positions are reason 4.
+ * 5. Triangulation.  dlt_two_view (geometry.cuh) with the relative pose R_m R_g^T, t_m - R_m R_g^T t_g (g the grid image, m the match
+ *    image) gives Q; X = Q.xyz / Q.w in the grid camera's frame and X_m = R_rel X + t_rel.  Reprojection: pinhole pi(K X), radial
+ *    the forward model (f d x + cx, f d y + cy), each against the position of rule 1 / 2 (the raw, distorted pixel).  Angle:
+ *    atan2(|a x b|, a . b) with a = X and b = X - C_m, C_m = -R_rel^T t_rel.  The depth is X.z rounded to fp32.
+ * 6. Winner.  A grid pixel keeps the accepted element with the largest certainty, ties to the smallest g: the 64-bit integer maximum
+ *    of key = (certainty bits << 32) | ~g (uint32), over every call that accumulates into the same maps, so the maps do not depend on
+ *    chunking, pair order or arrival order.  depth, score [num_images, H, W] fp32 and source [num_images, H, W] int64 hold the winner's
+ *    depth, certainty and g (0, 0, -1 where none).
+ * romab200_dense_triangulate: source and score of the listed images `images` [num_list] int32 (every image the chunk references, each
+ *   once) are packed into keys in place (source holds key, 0 for none); one thread per (pair-half, pixel) with grid.y = 2 row + half
+ *   classifies its element, writes elem_depth [chunk, 2, H, W] (0 unless accepted) and takes the atomicMax of its key; the reason
+ *   counts go through warp reductions into partial [2 chunk, RB_DENSE_MAX_CTAS, RB_DENSE_REASONS] int32, and one more kernel adds them
+ *   per pair in a fixed order to pair_counts [num_pairs, RB_DENSE_REASONS] int64 (row k: accepted, then reasons 1-7).
+ * romab200_dense_resolve (same arguments, after triangulate): every accepted element whose key won writes its depth, then the listed
+ *   images' keys are unpacked back to source and score.  Between the two calls source holds keys.
+ *
+ * Fusion.  Neighbours of image i: nbrs[nbr_offsets[i] .. nbr_offsets[i + 1]) int32, the registered images sharing a pair with i in
+ * ascending order (built on the host).  For grid pixel p = (r, c) of a registered image i with depth d > 0:
+ * F1. X = R_i^T (d (a, b, 1) - t_i) with (a, b) the normalised coordinates (rule 4) of p's position (rule 1); a clamped p is skipped.
+ * F2. Per neighbour j in order: X_j = R_j X + t_j; skip unless X_j.z > 0; (u, v) its pixel, q = (floor(v H / H_j), floor(u W / W_j));
+ *     q agrees when it lies inside the grid, d_q = depth_j(q) > 0, |d_q - X_j.z| <= max_depth_error X_j.z, q's position is not
+ *     clamped, and Y = R_j^T (d_q (a', b', 1) - t_j) (F1 for q) has R_i Y + t_i in front of i and projects within max_reproj_error
+ *     (squared: max_reproj_error2) of p's position.
+ * F3. p is kept when at least min_num_views - 1 neighbours agree, and emitted when also no agreeing neighbour has an index < i.  The
+ *     point is (X + the agreeing Y in neighbour order) / (1 + agreeing), num_views = 1 + agreeing, score = score_i(p), image i,
+ *     pixel r W + c, colour the pixel (((2 r + 1) H_c) / (2 H), ((2 c + 1) W_c) / (2 W)) (integer division) of image i's colour
+ *     image [H_c, W_c, 3] uint8 at colors + color_offsets[i] (color_sizes [num_images, 2] int32, color_bytes the buffer's size), or
+ *     128 grey when colors is null.
+ * romab200_dense_fuse_count: one CTA per tile of RB_DENSE_TILE pixels of one image (tiles = ceil(H W / RB_DENSE_TILE) per image,
+ *   image-major) counts its emitted pixels into tile_scan [num_images tiles + 1] int64, then scans it (exclusive, total last).
+ * romab200_dense_fuse_emit (after the caller has read the total into num_points): the same CTAs write points [num_points, 3] float64,
+ *   rgb [num_points, 3] uint8, image int32, pixel int64, num_views int32 and point_score fp32 at their offsets, pixels in order. */
+#define RB_DENSE_CAM 36
+#define RB_DENSE_REASONS 8
+#define RB_DENSE_MAX_CTAS 256
+#define RB_DENSE_TILE 256
+typedef struct {
+    const int64_t* pairs; int32_t num_pairs, num_images;
+    int32_t first_pair, chunk, H, W;
+    const float* warp; const float* certainty;
+    const int32_t* image_sizes; const double* cameras; const uint8_t* registered; int32_t radial;
+    float min_certainty; double max_error2, min_angle;
+    const int32_t* images; int32_t num_list;
+    float* depth; float* score; int64_t* source;
+    float* elem_depth; int32_t* partial; int64_t* pair_counts;
+} rb_dense_tri_args;
+int romab200_dense_triangulate(const rb_dense_tri_args* args, void* stream);
+int romab200_dense_resolve(const rb_dense_tri_args* args, void* stream);
+
+typedef struct {
+    int32_t num_images, H, W;
+    const int32_t* image_sizes; const double* cameras; const uint8_t* registered; int32_t radial;
+    const int64_t* nbr_offsets; const int32_t* nbrs;
+    const float* depth; const float* score;
+    double max_reproj_error2, max_depth_error; int32_t min_num_views;
+    const uint8_t* colors; const int64_t* color_offsets; const int32_t* color_sizes; int64_t color_bytes;
+    int64_t* tile_scan;
+    int64_t num_points;                                                 /* emit only: */
+    double* points; uint8_t* rgb; int32_t* image; int64_t* pixel; int32_t* num_views; float* point_score;
+} rb_dense_fuse_args;
+int romab200_dense_fuse_count(const rb_dense_fuse_args* args, void* stream);
+int romab200_dense_fuse_emit(const rb_dense_fuse_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -50,6 +50,9 @@ def __getattr__(name):
     if name in ("initialize_reconstruction", "TwoViewInit", "reconstruct", "Reconstruction", "write_colmap_text"):
         from . import mapper
         return getattr(mapper, name)
+    if name in ("triangulate_warps", "fuse_depth_maps", "write_ply", "DepthMaps", "DenseCloud"):
+        from . import dense
+        return getattr(dense, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
         from . import depth_warp
         return getattr(depth_warp, name)

@@ -85,6 +85,9 @@ RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEA
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
     for name in ("RB_ABS_ROUND", "RB_ABS_MAX_SOL", "RB_ABS_MAX_SPLITS", "RB_ABS_SLICE", "RB_ABS_STATE", "RB_ABS_MAX_BATCH", "RB_REG_BAD_ID", "RB_REG_ITEM_BYTES",
                  "RB_REG_SLICE_BYTES", "RB_REG_POINT_BYTES", "RB_REG_CHUNK_BYTES"))
+RB_DENSE_CAM, RB_DENSE_REASONS, RB_DENSE_MAX_CTAS, RB_DENSE_TILE = (
+    int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+    for name in ("RB_DENSE_CAM", "RB_DENSE_REASONS", "RB_DENSE_MAX_CTAS", "RB_DENSE_TILE"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -213,6 +216,13 @@ _FIELD_DTYPES = {
     "rb_dense_geometric_dist_args": {"depth0": "depth_dtype", "depth1": "depth_dtype", "T": _F64, "K0": _F64, "K1": _F64, "dense_matches": _F32,
                                      "gd": _F64, "prob": _F32, "partial_sum": _F64, "partial_cnt": torch.int32, "pair_sum": _F64,
                                      "pair_cnt": torch.int64, "pck": _F32, "epe": _F64},
+    "rb_dense_tri_args": {"pairs": torch.int64, "warp": _F32, "certainty": _F32, "image_sizes": torch.int32, "cameras": _F64,
+                          "registered": torch.uint8, "images": torch.int32, "depth": _F32, "score": _F32, "source": torch.int64,
+                          "elem_depth": _F32, "partial": torch.int32, "pair_counts": torch.int64},
+    "rb_dense_fuse_args": {"image_sizes": torch.int32, "cameras": _F64, "registered": torch.uint8, "nbr_offsets": torch.int64,
+                           "nbrs": torch.int32, "depth": _F32, "score": _F32, "colors": torch.uint8, "color_offsets": torch.int64,
+                           "color_sizes": torch.int32, "tile_scan": torch.int64, "points": _F64, "rgb": torch.uint8, "image": torch.int32,
+                           "pixel": torch.int64, "num_views": torch.int32, "point_score": _F32},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}, "rb_dense_geometric_dist_args": {"dense_matches"}}
@@ -346,13 +356,31 @@ def _twoview_min_elems(kw):
             "angle": total, "num_good": B, "median_angle": B, "forward": B}
 
 
+def _dense_tri_min_elems(kw):
+    P, N, C, n = kw["num_pairs"], kw["num_images"], kw["chunk"], kw["H"] * kw["W"]
+    return {"pairs": 2 * P, "warp": 8 * C * n, "certainty": 2 * C * n, "image_sizes": 2 * N, "cameras": N * RB_DENSE_CAM, "registered": N,
+            "images": kw["num_list"], "depth": N * n, "score": N * n, "source": N * n, "elem_depth": 2 * C * n,
+            "partial": 2 * C * RB_DENSE_MAX_CTAS * RB_DENSE_REASONS, "pair_counts": P * RB_DENSE_REASONS}
+
+
+def _dense_fuse_min_elems(kw):
+    N, n, M = kw["num_images"], kw["H"] * kw["W"], kw.get("num_points", 0)
+    out = {"image_sizes": 2 * N, "cameras": N * RB_DENSE_CAM, "registered": N, "nbr_offsets": N + 1, "depth": N * n, "score": N * n,
+           "color_offsets": N + 1, "color_sizes": 2 * N, "tile_scan": N * (-(-n // RB_DENSE_TILE)) + 1, "points": 3 * M, "rgb": 3 * M,
+           "image": M, "pixel": M, "num_views": M, "point_score": M}
+    if kw.get("colors") is not None:
+        out["colors"] = kw["color_bytes"]
+    return out
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
               "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
               "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems,
-              "rb_twoview_args": _twoview_min_elems, "rb_undistort_args": _undistort_min_elems}
+              "rb_twoview_args": _twoview_min_elems, "rb_undistort_args": _undistort_min_elems,
+              "rb_dense_tri_args": _dense_tri_min_elems, "rb_dense_fuse_args": _dense_fuse_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

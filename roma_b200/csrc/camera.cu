@@ -1,6 +1,6 @@
 // Keypoint undistortion under SIMPLE_RADIAL cameras (include/romab200.h): a thread per keypoint, all in float64.  The image of a
 // keypoint is found by binary search on kp_offsets.  The clamped count is an integer atomic, so it does not depend on the order.
-#include "common.cuh"
+#include "geometry.cuh"
 
 namespace rb {
 
@@ -27,19 +27,9 @@ __global__ void __launch_bounds__(UD_THREADS) undistort_kernel(rb_undistort_args
             a.out[2 * r + 1] = v;
             continue;
         }
-        double rho;
-        if (k < 0.0 && rd >= 2.0 / (3.0 * sqrt(-3.0 * k))) {
-            rho = 1.0 / sqrt(-3.0 * k);                        // the turning radius: no inverse at or beyond it
-            ++clamped;
-        } else {
-            rho = rd;
-#pragma unroll 1
-            for (int it = 0; it < RB_UNDISTORT_ITERS; ++it) {
-                const double step = (rho * (1.0 + k * rho * rho) - rd) / (1.0 + 3.0 * k * rho * rho);
-                if (step == 0.0) break;
-                rho -= step;
-            }
-        }
+        bool at_turn;
+        const double rho = radial_undistort_rho(rd, k, at_turn);
+        clamped += at_turn;
         const double s = rho / rd;
         a.out[2 * r] = (float)(cx + dx * s);
         a.out[2 * r + 1] = (float)(cy + dy * s);

@@ -199,6 +199,25 @@ __device__ __forceinline__ void dlt_two_view(const double* R, const double* t, d
     for (int i = 0; i < 4; ++i) Q[i] = k == 0 ? V[i][0] : (k == 1 ? V[i][1] : (k == 2 ? V[i][2] : V[i][3]));
 }
 
+// SIMPLE_RADIAL undistortion of a radius (include/romab200.h, keypoint undistortion rules 2 and 4): rho with rho (1 + k rho^2) =
+// rd by Newton from rho = rd, or the turning radius 1 / sqrt(-3 k) with clamped set when k < 0 and rd is at or beyond its image.
+// The caller handles k = 0 and rd = 0.  camera.cu (keypoints) and dense.cu (dense warps) share it.
+__device__ __forceinline__ double radial_undistort_rho(double rd, double k, bool& clamped) {
+    if (k < 0.0 && rd >= 2.0 / (3.0 * sqrt(-3.0 * k))) {
+        clamped = true;
+        return 1.0 / sqrt(-3.0 * k);
+    }
+    clamped = false;
+    double rho = rd;
+#pragma unroll 1
+    for (int it = 0; it < RB_UNDISTORT_ITERS; ++it) {
+        const double step = (rho * (1.0 + k * rho * rho) - rd) / (1.0 + 3.0 * k * rho * rho);
+        if (step == 0.0) break;
+        rho -= step;
+    }
+    return rho;
+}
+
 // 3x3 SVD M = sum_k s_k u_k v_k^T from cyclic Jacobi on M^T M: v[k] is the k-th right singular vector by descending singular
 // value with det [v0 v1 v2] = +1, u[k] = M v_k / s_k and s[k] = |M v_k| for k < 2, u[2] = u[0] x u[1] (M row-major)
 __device__ __forceinline__ void svd3(const double* M, double (&u)[3][3], double (&v)[3][3], double (&s)[2]) {

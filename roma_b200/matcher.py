@@ -262,6 +262,48 @@ class RegressionMatcher:
             buf = [torch.empty(0, 0, 4, device=self.engine.device), torch.empty(0, 0, device=self.engine.device)]
         return consolidate_matches(pairs, buf[0], buf[1], image_sizes, cell_size=cell_size)
 
+    @torch.inference_mode()
+    def dense_cloud(self, images, pairs, K, R, t, *, registered=None, intrinsics=None, image_sizes=None, colors=None, max_batch=8,
+                    images_high_res=None, **options):
+        """A dense point cloud of an image set with known cameras, without holding dense warps: runs `match_pairs(images, pairs,
+        max_batch=max_batch)` chunk by chunk, triangulates each chunk into one `DepthMaps` (`triangulate_warps(..., first_pair=k0,
+        depth_maps=...)`), then returns `fuse_depth_maps` of the maps (a `DenseCloud`).  The result equals that loop written out by
+        hand, byte for byte.  The model must be symmetric.
+
+        Cameras as in `triangulate_warps` (K, R, t as `reconstruct` returns them, or SIMPLE_RADIAL intrinsics with K=None).
+        image_sizes [N, 2] (H, W) is the pixel frame of the cameras; it defaults to each file's own size for paths and PIL images,
+        and is required for tensor images (with images_high_res, as in `match_pairs`).  colors: see `fuse_depth_maps`.  options: min_certainty, max_error, min_angle (passed to
+        triangulate_warps) and max_reproj_error, max_depth_error, min_num_views (passed to fuse_depth_maps)."""
+        from .dense import check_cameras, fuse_depth_maps, triangulate_warps
+        if not self.symmetric:
+            raise ValueError("dense_cloud: the model must be symmetric (triangulate_warps takes both halves of the warp)")
+        if isinstance(images, torch.Tensor):
+            if image_sizes is None:
+                raise ValueError("dense_cloud: image_sizes [N, 2] (H, W) is required for tensor images")
+            if images.dim() != 4:
+                raise ValueError(f"images must be [N, 3, h, w], got shape {tuple(images.shape)}")
+            n_images = images.shape[0]
+        else:
+            images = list(images)
+            n_images = len(images)
+            if image_sizes is None:
+                image_sizes = [_image_size(x) for x in images]
+        if len(image_sizes) != n_images:
+            raise ValueError(f"dense_cloud: image_sizes holds {len(image_sizes)} sizes for {n_images} images")
+        cams = dict(registered=registered, intrinsics=intrinsics)
+        tri, fuse = check_cameras("dense_cloud", pairs, K, R, t, image_sizes, **cams, **options)
+        pairs = pair_tensor(pairs, n_images)
+        state = {}
+
+        def on_batch(k0, warp, cert):
+            state["dm"] = triangulate_warps(pairs, warp, cert, K, R, t, image_sizes, first_pair=k0, depth_maps=state.get("dm"), **cams,
+                                            **tri)
+
+        self.match_pairs(images, pairs, images_high_res, max_batch=max_batch, on_batch=on_batch)
+        if "dm" not in state:
+            raise ValueError("dense_cloud: no pairs to match")
+        return fuse_depth_maps(state["dm"], pairs, K, R, t, image_sizes, colors=colors, **cams, **fuse)
+
     def _match_pairs_device(self, images, images_high_res, plan, lo_res, hi_res, out_res, on_batch):
         eng = self.engine
         dev = eng.device

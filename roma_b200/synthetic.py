@@ -685,3 +685,159 @@ def track_points(track_offsets, elements, kp_offsets, keypoints, views, width: i
         if pk.size and pk[0] >= 0 and (pk == pk[0]).all():
             out[k] = pk[0]
     return out
+
+
+def _radial_rays(intr, x, y):
+    """Normalised undistorted coordinates of pixels (x, y) under SIMPLE_RADIAL (f, cx, cy, k): the Newton loop of the keypoint
+    undistortion (include/romab200.h), which converges for the scenes here (no pixel reaches the turning radius)."""
+    import numpy as np
+
+    f, cx, cy, k = intr
+    dx, dy = x - cx, y - cy
+    rd = np.sqrt(dx * dx + dy * dy) / f
+    rho = rd.copy()
+    for _ in range(20):
+        rho = rho - (rho * (1.0 + k * rho * rho) - rd) / (1.0 + 3.0 * k * rho * rho)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        s = np.where(rd > 0, rho / rd, 1.0)
+    return dx * s / f, dy * s / f
+
+
+def depth_views(seed: int, n_images: int, size=(96, 128), radial=None):
+    """Seeded multi-view scenes with exact per-view depth maps, for dense reconstruction (`roma_b200.dense`).  Cameras are laid out as
+    in `planted_cameras` (pinhole intrinsics of `_scene_intrinsics`, 8-10 units from the origin at azimuths of -40..40 degrees and
+    heights of -1..1, looking at a point near the origin).  The scene is `depth_scene`'s: a tilted ground plane n . X = d 1.5-3 units
+    beyond the origin, and two occluding quads 0-2 units in front of it.  View i's depth at pixel (x, y) is the z in its camera frame of
+    the nearest ray-plane intersection through the pixel centre (x + 0.5, y + 0.5), stored as float32; five random rectangles per view
+    are holes of zero depth.  Each view also gets a uint8 colour image, a function of the world point it sees (black where it sees
+    nothing), so the colours of one surface point agree across views.
+    radial=(k_lo, k_hi): SIMPLE_RADIAL cameras with the pinhole f, the principal point at (W / 2, H / 2) and k uniform in the range
+    (from a second generator, so the other draws do not change); the pixel centres are then distorted pixels.
+    Returns a dict of CPU tensors: depth [N, H, W] float32, K [N, 3, 3] float64 (pinhole_K of the intrinsics when radial), intrinsics
+    [N, 4] float64 or None, R [N, 3, 3], t [N, 3] float64 (x ~ K (R X + t)), colors [N, H, W, 3] uint8, image_sizes [N, 2] int64."""
+    import numpy as np
+
+    H, W = size
+    rng = np.random.default_rng(seed)
+    K = np.stack([_scene_intrinsics(rng, W, H) for _ in range(n_images)])
+    az = np.deg2rad(rng.uniform(-40.0, 40.0, n_images))
+    r, h = rng.uniform(8.0, 10.0, n_images), rng.uniform(-1.0, 1.0, n_images)
+    C = np.stack((r * np.sin(az), h, -r * np.cos(az)), 1)
+    target = rng.uniform(-0.5, 0.5, (n_images, 3))
+    R = np.empty((n_images, 3, 3))
+    for c in range(n_images):
+        z = (target[c] - C[c]) / np.linalg.norm(target[c] - C[c])
+        x = np.cross([0.0, 1.0, 0.0], z)
+        x /= np.linalg.norm(x)
+        R[c] = np.stack((x, np.cross(z, x), z))
+    t = -np.einsum("cij,cj->ci", R, C)
+    n = np.array([rng.uniform(-0.15, 0.15), rng.uniform(-0.25, -0.1), -1.0])
+    planes = [(n / np.linalg.norm(n), -rng.uniform(1.5, 3.0), None, None, None)]
+    for _ in range(2):
+        qn = np.array([rng.uniform(-0.3, 0.3), rng.uniform(-0.3, 0.3), -1.0])
+        qn /= np.linalg.norm(qn)
+        centre = np.array([rng.uniform(-1.5, 1.5), rng.uniform(-1.0, 1.0), rng.uniform(-2.0, 0.0)])
+        e1 = np.cross(qn, [0.0, 1.0, 0.0])
+        e1 /= np.linalg.norm(e1)
+        planes.append((qn, qn @ centre, centre, (e1, np.cross(qn, e1)), (rng.uniform(0.8, 1.2), rng.uniform(0.6, 1.0))))
+    intr = None
+    if radial is not None:
+        k = np.random.default_rng([seed, 1]).uniform(radial[0], radial[1], n_images)
+        intr = np.stack((K[:, 0, 0], np.full(n_images, W / 2), np.full(n_images, H / 2), k), 1)
+        K = np.zeros((n_images, 3, 3))
+        K[:, 0, 0] = K[:, 1, 1] = intr[:, 0]
+        K[:, 0, 2], K[:, 1, 2], K[:, 2, 2] = intr[:, 1], intr[:, 2], 1.0
+    ys, xs = np.meshgrid(np.arange(H) + 0.5, np.arange(W) + 0.5, indexing="ij")
+    depth = np.zeros((n_images, H, W), np.float32)
+    colors = np.zeros((n_images, H, W, 3), np.uint8)
+    for c in range(n_images):
+        if intr is None:
+            rays = np.stack((xs, ys, np.ones_like(xs)), -1) @ np.linalg.inv(K[c]).T
+        else:
+            a, b = _radial_rays(intr[c], xs, ys)
+            rays = np.stack((a, b, np.ones_like(a)), -1)
+        dirs = rays @ R[c]                                  # world directions whose camera-frame z is 1
+        z = np.full((H, W), np.inf)
+        for nrm, d, centre, axes, half in planes:
+            with np.errstate(divide="ignore", invalid="ignore"):
+                s = (d - nrm @ C[c]) / (dirs @ nrm)
+            hit = np.isfinite(s) & (s > 0)
+            if centre is not None:
+                Xw = C[c] + dirs * np.where(hit, s, 0.0)[..., None]
+                for e, a in zip(axes, half):
+                    hit &= np.abs((Xw - centre) @ e) < a
+            z = np.where(hit & (s < z), s, z)
+        seen = np.isfinite(z)
+        Xw = C[c] + dirs * np.where(seen, z, 0.0)[..., None]
+        rgb = 128 + 100 * np.sin(np.stack((3.0 * Xw[..., 0], 3.0 * Xw[..., 1], 2.0 * Xw[..., 0] + 2.0 * Xw[..., 2]), -1))
+        colors[c] = np.where(seen[..., None], rgb, 0).astype(np.uint8)
+        z[~seen] = 0.0
+        for _ in range(5):
+            hh, hw = int(H * rng.uniform(0.05, 0.12)), int(W * rng.uniform(0.05, 0.12))
+            y0, x0 = rng.integers(0, H - hh), rng.integers(0, W - hw)
+            z[y0:y0 + hh, x0:x0 + hw] = 0.0
+        depth[c] = z.astype(np.float32)
+    f64 = lambda a: torch.from_numpy(np.ascontiguousarray(a, np.float64))     # noqa: E731
+    return {"depth": torch.from_numpy(depth), "K": f64(K), "intrinsics": None if intr is None else f64(intr), "R": f64(R), "t": f64(t),
+            "colors": torch.from_numpy(colors), "image_sizes": torch.tensor([[H, W]] * n_images, dtype=torch.int64)}
+
+
+def depth_view_warps(views, pairs, device="cuda"):
+    """The symmetric ground-truth warps of `depth_views` for the pairs [P, 2], on the views' own grid: for pair (i, j) the left half
+    is `get_gt_warp(depth_i, depth_j, T_i->j, K_i, K_j)` (grid pixel of i, its match in j), the right half the same from j to i with the
+    two positions swapped, as match_pairs lays out a symmetric warp; certainty is `prob`.  Pinhole views only (get_gt_warp has no
+    distortion): radial views take the same rule in numpy float64 (the match is the distorted projection, and prob is 1 where the
+    point is covisible strictly inside the image less one pixel and within 5 % of the other view's nearest depth).  Returns
+    (warp [P, H, 2W, 4], certainty [P, H, 2W]) fp32 on `device`."""
+    import numpy as np
+    from .depth_warp import get_gt_warp
+
+    pairs = torch.as_tensor(pairs, dtype=torch.int64).reshape(-1, 2)
+    depth, R, t = views["depth"], views["R"], views["t"]
+    N, H, W = depth.shape
+    i, j = pairs[:, 0], pairs[:, 1]
+    halves = []
+    for a, b in ((i, j), (j, i)):
+        Rr = R[b] @ R[a].transpose(1, 2)
+        T = torch.zeros(len(a), 4, 4, dtype=torch.float64)
+        T[:, :3, :3], T[:, :3, 3], T[:, 3, 3] = Rr, t[b] - (Rr @ t[a][..., None])[..., 0], 1.0
+        gy, gx = (torch.linspace(-1 + 1 / n, 1 - 1 / n, n, dtype=torch.float32) for n in (H, W))
+        grid = torch.stack(torch.meshgrid(gy, gx, indexing="ij")[::-1], -1).expand(len(a), H, W, 2)
+        if views["intrinsics"] is None:
+            x2, prob = get_gt_warp(depth[a].to(device), depth[b].to(device), T.to(device), views["K"][a].to(device),
+                                   views["K"][b].to(device))
+            x2 = x2.float()
+        else:
+            x2, prob = _radial_gt_warp(views, a, b, T, H, W)
+            x2, prob = x2.to(device), prob.to(device)
+        halves.append((grid.to(device), x2, prob))
+    (g0, m0, p0), (g1, m1, p1) = halves
+    warp = torch.cat((torch.cat((g0, m0), -1), torch.cat((m1, g1), -1)), 2)
+    return warp.contiguous(), torch.cat((p0, p1), 2).contiguous()
+
+
+def _radial_gt_warp(views, a, b, T, H, W):
+    import numpy as np
+
+    intr, depth, sizes = views["intrinsics"].numpy(), views["depth"].numpy(), views["image_sizes"].numpy()
+    ys, xs = np.meshgrid(np.arange(H) + 0.5, np.arange(W) + 0.5, indexing="ij")
+    x2 = np.zeros((len(a), H, W, 2), np.float32)
+    prob = np.zeros((len(a), H, W), np.float32)
+    for q, (ia, ib) in enumerate(zip(a.tolist(), b.tolist())):
+        fa, ca = intr[ia], intr[ib]
+        ra, rb = _radial_rays(fa, xs, ys)              # the views' images are the size of their grids
+        d = depth[ia].astype(np.float64)
+        P = np.stack((ra * d, rb * d, d), -1) @ T[q, :3, :3].numpy().T + T[q, :3, 3].numpy()
+        with np.errstate(divide="ignore", invalid="ignore"):
+            x, y = P[..., 0] / P[..., 2], P[..., 1] / P[..., 2]
+            dd = 1.0 + ca[3] * (x * x + y * y)
+            u, v = ca[0] * dd * x + ca[1], ca[0] * dd * y + ca[2]
+            Hb, Wb = sizes[ib]
+            cov = (u > 0) & (u < Wb - 1) & (v > 0) & (v < Hb - 1)
+            col = np.clip(np.floor(u * W / Wb), 0, W - 1).astype(np.int64)
+            row = np.clip(np.floor(v * H / Hb), 0, H - 1).astype(np.int64)
+            db = depth[ib][np.where(cov, row, 0), np.where(cov, col, 0)].astype(np.float64)
+            ok = (d > 0) & cov & (np.abs((db - P[..., 2]) / db) < 0.05)
+        x2[q] = np.stack((2 * u / Wb - 1, 2 * v / Hb - 1), -1)
+        prob[q] = ok
+    return torch.from_numpy(np.nan_to_num(x2)), torch.from_numpy(prob)
