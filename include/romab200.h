@@ -1068,7 +1068,33 @@ int romab200_triangulate(const rb_tri_args* args, void* stream);
  * [8 num_free].  Device bytes: RB_BA_ELEMENT_BYTES1 E + RB_BA_TRACK_BYTES T + RB_BA_IMAGE_BYTES1 N + RB_BA_FREE_BYTES1 F + 512 F^2
  *   + 1024 ceil(E / RB_TRACKS_TILE) + RB_BA_ONCE_BYTES
  *   per element W 192 (the rest as above); per image cams 128, cams_trial 128; per free camera cam_sys 128, rhs 64, free_cams 4,
- *   pin 8 (no fixed_tx). */
+ *   pin 8 (no fixed_tx).
+ *
+ * Shared intrinsics (model 1, rb_ba_groups_args).  Each image belongs to a camera group, and the images of a group share f and k;
+ * each keeps its own pose and the principal point stays fixed.  With J the per-image Jacobian above and P the 8F x n' matrix that
+ * maps a free camera's pose rows to its own 6 parameters and its f, k rows to its group's, the shared Jacobian is J P.  Hence:
+ * 4''. Gauge.  A camera is free when its pose is free or its group's intrinsics are.  pin keeps the pose pins of rule 4' and gives
+ *    every member its group's f, k pins; group_pin [num_groups, 2] uint8 pins the group's (f, k) rows after the fold.  A free camera
+ *    without observations (an image whose pose is pinned) gets its group's step.
+ * 5''. Fold.  S' = P^T S P and b' = P^T b of order n' = 6F + 2G: the free cameras' pose rows at 6 fi, then group g's (f, k) rows at
+ *    6F + 2g.  S and b are those of romab200_ba_cameras; the point blocks are unchanged, so the Schur reduction commutes with P.
+ *    The group's damping is the sum of its members' clamped diagonals, sum_i clamp(U_i[f, f]) (Ceres clamps the sum; the two
+ *    differ only for a member whose diagonal is below 1e-6).  A pinned group row and column become the identity with a zero
+ *    right-hand side.  After the Cholesky solve, d = P d' (unfold) and romab200_ba_step runs unchanged; its per-member pred sums
+ *    to the group's term up to rounding.
+ * The G groups are those with a free camera, ascending by id; group_offsets [G + 1] int32 indexes group_members [F] int32, the
+ * free camera indices (fi) of each group, ascending.  The groups path has its own argument struct, rb_ba_groups_args, whose S, rhs
+ * and result are the rb_ba_args buffers of the same call; rb_ba_args is unchanged.  A trial is romab200_ba_cameras,
+ * romab200_ba_fold, romab200_ba_groups_cholesky, romab200_ba_unfold, romab200_ba_step; without groups it is the model-1 trial above
+ * and launches nothing new.
+ * romab200_ba_fold: a thread per entry of S' in a pose column (pose-pose copies, group-pose sums over the members in list order)
+ *   and of b'; then a CTA per group pair (g, h <= g), whose 2 x 2 block sums the |g| |h| member pairs in a fixed-order tree.
+ *   Only the lower triangle of S and S' is read and written.
+ * romab200_ba_groups_cholesky: the Cholesky factorisation and both substitutions of romab200_ba_cholesky (the same kernels), on
+ *   S_groups and rhs_groups of order n'; a pivot that is not > 0 and finite sets result[3].
+ * romab200_ba_unfold: a CTA per group writes rhs [8F] of its members from rhs_groups.
+ * Device bytes of the groups path: those of model 1 plus 8 (6F + 2G)^2 + 8 (6F + 2G) + 4 (G + 1) + 4 F + 2 G (S_groups,
+ *   rhs_groups, group_offsets, group_members, group_pin). */
 #define RB_BA_BAD_ID 1
 #define RB_BA_REPEATED 2
 #define RB_BA_CAM 21
@@ -1109,6 +1135,17 @@ int romab200_ba_cholesky(const rb_ba_args* args, void* stream);
 int romab200_ba_step(const rb_ba_args* args, void* stream);
 int romab200_ba_cost(const rb_ba_args* args, void* stream);
 int romab200_ba_error(const rb_ba_args* args, void* stream);
+typedef struct {
+    int32_t num_free, num_groups;                                       /* F free cameras, G groups with a free camera */
+    const int32_t* group_offsets; const int32_t* group_members;         /* [G + 1], [F] */
+    const uint8_t* group_pin;                                           /* [G, 2] */
+    const double* S; double* rhs;                                       /* rb_ba_args' S [8F, 8F] and rhs [8F] */
+    double* S_groups; double* rhs_groups;                               /* [n', n'], [n'], n' = 6F + 2G */
+    double* result;                                                     /* rb_ba_args' result: [3] is the pivot flag */
+} rb_ba_groups_args;
+int romab200_ba_fold(const rb_ba_groups_args* args, void* stream);
+int romab200_ba_groups_cholesky(const rb_ba_groups_args* args, void* stream);
+int romab200_ba_unfold(const rb_ba_groups_args* args, void* stream);
 
 /* ---- absolute pose: batched P3P RANSAC and Gauss-Newton refinement (COLMAP's EstimateAbsolutePose + RefineAbsolutePose) ----
  * Not in the reference.  B items with ragged point counts, packed: item b owns points [offsets[b], offsets[b+1]), each a pixel x

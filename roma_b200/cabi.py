@@ -199,6 +199,8 @@ _FIELD_DTYPES = {
                    "obs": torch.int32, "cams": _F64, "X": _F64, "cams_trial": _F64, "X_trial": _F64, "W": _F64, "track_sys": _F64,
                    "cam_sys": _F64, "S": _F64, "rhs": _F64, "cam_pred": _F64, "track_part": _F64, "result": _F64, "error": _F64,
                    "pin": torch.uint8},
+    "rb_ba_groups_args": {"group_offsets": torch.int32, "group_members": torch.int32, "group_pin": torch.uint8, "S": _F64, "rhs": _F64,
+                          "S_groups": _F64, "rhs_groups": _F64, "result": _F64},
     "rb_abspose_args": {"x": _F64, "X": _F64, "offsets": torch.int64, "K": _F64, "sample": torch.int32, "models": _F64, "nsol": torch.int32,
                         "counts": torch.int32, "state": torch.int32, "best": _F64, "running": torch.int32, "R": _F64, "t": _F64, "ok": torch.uint8,
                         "num_inliers": torch.int64, "mask": torch.uint8},
@@ -321,6 +323,13 @@ def _ba_min_elems(kw):
             "S": n * n, "rhs": n, "cam_pred": N, "track_part": 3 * T, "result": RB_BA_RESULT, "error": T, "pin": 8 * F}
 
 
+def _ba_groups_min_elems(kw):
+    F, G = kw["num_free"], kw["num_groups"]
+    ng = 6 * F + 2 * G
+    return {"group_offsets": G + 1, "group_members": F, "group_pin": 2 * G, "S": 64 * F * F, "rhs": 8 * F, "S_groups": ng * ng,
+            "rhs_groups": ng, "result": RB_BA_RESULT}
+
+
 def abspose_splits(max_n) -> int:
     """Score slices of an absolute-pose launch whose largest item has max_n points (include/romab200.h)."""
     return max(1, min(RB_ABS_MAX_SPLITS, -(-int(max_n) // RB_ABS_SLICE)))
@@ -378,7 +387,8 @@ _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_ele
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
               "rb_match_graph_keypoints_args": _match_graph_keypoints_min_elems, "rb_match_graph_pairs_args": _match_graph_pairs_min_elems,
               "rb_tracks_args": _tracks_min_elems, "rb_verify_args": _verify_min_elems, "rb_tri_args": _tri_min_elems,
-              "rb_ba_args": _ba_min_elems, "rb_abspose_args": _abspose_min_elems, "rb_register_args": _register_min_elems,
+              "rb_ba_args": _ba_min_elems, "rb_ba_groups_args": _ba_groups_min_elems, "rb_abspose_args": _abspose_min_elems,
+              "rb_register_args": _register_min_elems,
               "rb_twoview_args": _twoview_min_elems, "rb_undistort_args": _undistort_min_elems,
               "rb_dense_tri_args": _dense_tri_min_elems, "rb_dense_fuse_args": _dense_fuse_min_elems}
 

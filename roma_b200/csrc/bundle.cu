@@ -324,6 +324,98 @@ __global__ void __launch_bounds__(BA_CAM_THREADS) ba_cameras_kernel(rb_ba_args a
     }
 }
 
+// ---- shared intrinsics: fold and unfold -------------------------------------------------------------------------------------
+// S' = P^T S P and b' = P^T b of order n' = 6F + 2G: free camera fi's pose rows at 6 fi, group g's (f, k) rows at 6F + 2g.  P maps
+// camera fi's parameter p < 6 to pose row 6 fi + p and its f, k to its group's rows.  S holds its lower triangle (rows of 8F); so
+// does S'.
+__device__ __forceinline__ double ba_lower(const double* S, int64_t n, int64_t r, int64_t c) { return r >= c ? S[r * n + c] : S[c * n + r]; }
+
+// a thread per entry (R, C) of S' with a pose column C <= R: pose-pose entries are copies, group-pose entries sum over the group's
+// members in list order; then b'.  A pinned group row becomes 0 here (its diagonal is in the group-group block).
+__global__ void __launch_bounds__(256) ba_fold_kernel(rb_ba_groups_args a) {
+    pdl_wait();
+    const int64_t F = a.num_free, n = 8 * F, np = 6 * F + 2 * (int64_t)a.num_groups, t0 = blockIdx.x * (int64_t)256 + threadIdx.x;
+    const int64_t step = (int64_t)gridDim.x * 256;
+    for (int64_t q = t0; q < np * 6 * F; q += step) {
+        const int64_t R = q / (6 * F), C = q % (6 * F);
+        if (C > R) continue;
+        const int64_t c8 = 8 * (C / 6) + C % 6;
+        double v;
+        if (R < 6 * F) {
+            v = a.S[(8 * (R / 6) + R % 6) * n + c8];
+        } else {
+            const int g = (int)((R - 6 * F) >> 1), j = (int)((R - 6 * F) & 1);
+            v = 0.0;
+            if (!a.group_pin[2 * g + j])
+                for (int m = a.group_offsets[g]; m < a.group_offsets[g + 1]; ++m) v += ba_lower(a.S, n, 8 * (int64_t)a.group_members[m] + 6 + j, c8);
+        }
+        a.S_groups[R * np + C] = v;
+    }
+    for (int64_t R = t0; R < np; R += step) {
+        double v;
+        if (R < 6 * F) {
+            v = a.rhs[8 * (R / 6) + R % 6];
+        } else {
+            const int g = (int)((R - 6 * F) >> 1), j = (int)((R - 6 * F) & 1);
+            v = 0.0;
+            if (!a.group_pin[2 * g + j])
+                for (int m = a.group_offsets[g]; m < a.group_offsets[g + 1]; ++m) v += a.rhs[8 * (int64_t)a.group_members[m] + 6 + j];
+        }
+        a.rhs_groups[R] = v;
+    }
+}
+
+// a CTA per group pair (g, h), h <= g: the 2 x 2 block of S' at rows 6F + 2g, columns 6F + 2h, each entry the sum over the
+// |g| |h| member pairs (member pair q = (q / |h|, q % |h|)): every thread a strided slice in order, then a fixed tree.  A pinned
+// row or column becomes that of the identity.
+__global__ void __launch_bounds__(256) ba_fold_groups_kernel(rb_ba_groups_args a) {
+    pdl_wait();
+    const int g = blockIdx.y, h = blockIdx.x, tid = threadIdx.x;
+    if (h > g) return;
+    __shared__ double red[4][256];
+    const int64_t F = a.num_free, n = 8 * F, np = 6 * F + 2 * (int64_t)a.num_groups;
+    const int og = a.group_offsets[g], oh = a.group_offsets[h], nh = a.group_offsets[h + 1] - oh;
+    const int64_t terms = (int64_t)(a.group_offsets[g + 1] - og) * nh;
+    double s[4] = {0.0, 0.0, 0.0, 0.0};             // (j, l) = (0, 0), (0, 1), (1, 0), (1, 1)
+    for (int64_t q = tid; q < terms; q += 256) {
+        const int64_t r = 8 * (int64_t)a.group_members[og + q / nh] + 6, c = 8 * (int64_t)a.group_members[oh + q % nh] + 6;
+#pragma unroll
+        for (int k = 0; k < 4; ++k) s[k] += ba_lower(a.S, n, r + (k >> 1), c + (k & 1));
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) red[k][tid] = s[k];
+    __syncthreads();
+    for (int w = 128; w; w >>= 1) {
+        if (tid < w)
+#pragma unroll
+            for (int k = 0; k < 4; ++k) red[k][tid] += red[k][tid + w];
+        __syncthreads();
+    }
+    if (tid < 4) {
+        const int j = tid >> 1, l = tid & 1;
+        const int64_t R = 6 * F + 2 * g + j, C = 6 * F + 2 * h + l;
+        if (C <= R) {
+            const bool pinned = a.group_pin[2 * g + j] || a.group_pin[2 * h + l];
+            a.S_groups[R * np + C] = pinned ? (R == C ? 1.0 : 0.0) : red[tid][0];
+        }
+    }
+}
+
+// d = P d': a CTA per group, a thread per member writes its camera's 8 rows of rhs
+__global__ void __launch_bounds__(128) ba_unfold_kernel(rb_ba_groups_args a) {
+    pdl_wait();
+    const int g = blockIdx.x;
+    const int64_t F = a.num_free;
+    const double* d = a.rhs_groups;
+    for (int m = a.group_offsets[g] + threadIdx.x; m < a.group_offsets[g + 1]; m += 128) {
+        const int64_t fi = a.group_members[m];
+#pragma unroll
+        for (int p = 0; p < 6; ++p) a.rhs[8 * fi + p] = d[6 * fi + p];
+        a.rhs[8 * fi + 6] = d[6 * F + 2 * g];
+        a.rhs[8 * fi + 7] = d[6 * F + 2 * g + 1];
+    }
+}
+
 // ---- Cholesky -----------------------------------------------------------------------------------------------------------------
 // the nb x nb diagonal block at k0 (nb <= NB), unblocked in shared memory; a pivot that is not > 0 and finite sets result[3]
 __global__ void __launch_bounds__(256) ba_potrf_panel_kernel(double* S, int64_t n, int64_t k0, int nb, double* result) {
@@ -636,6 +728,33 @@ static int ba_check(const rb_ba_args* a, const char* what) {
     return 0;
 }
 
+// the folded system's arguments: 1 <= num_groups <= num_free and every buffer
+static int ba_check_groups(const rb_ba_groups_args* a, const char* what) {
+    RB_REQUIRE(a && a->num_free > 0 && a->num_groups > 0 && a->num_groups <= a->num_free && a->num_groups <= 65535, "%s: null argument "
+               "or bad num_groups=%d (num_free=%d)", what, a ? a->num_groups : 0, a ? a->num_free : 0);
+    RB_REQUIRE(a->group_offsets && a->group_members && a->group_pin && a->S && a->rhs && a->S_groups && a->rhs_groups && a->result,
+               "%s: null argument", what);
+    return 0;
+}
+
+// S = L L^T in place (lower triangle, order n), then rhs <- S^-1 rhs; a pivot that is not > 0 and finite sets result[3]
+static int ba_cholesky_solve(double* S, int64_t n, double* rhs, double* result, cudaStream_t st) {
+    for (int64_t k0 = 0; k0 < n; k0 += NB) {
+        const int nb = (int)(n - k0 < NB ? n - k0 : NB);
+        launch_pdl(ba_potrf_panel_kernel, dim3(1), dim3(256), 0, st, S, n, k0, nb, result);
+        if (check_launch("ba_cholesky(panel)")) return 1;
+        const int64_t rest = n - k0 - NB;
+        if (rest <= 0) break;
+        launch_pdl(ba_trsm_kernel, dim3((unsigned)((rest + 127) / 128)), dim3(128), 0, st, S, n, k0);
+        if (check_launch("ba_cholesky(trsm)")) return 1;
+        const unsigned tiles = (unsigned)((rest + NB - 1) / NB);
+        launch_pdl(ba_syrk_kernel, dim3(tiles, tiles), dim3(256), 0, st, S, n, k0);
+        if (check_launch("ba_cholesky(update)")) return 1;
+    }
+    launch_pdl(ba_potrs_kernel, dim3(1), dim3(1024), 0, st, (const double*)S, n, rhs);
+    return check_launch("ba_cholesky(solve)");
+}
+
 static unsigned ba_track_grid(const rb_ba_args* a) { return grid1d(a->num_tracks, BA_WARPS, 64 * 1024); }
 
 }  // namespace rb
@@ -684,22 +803,29 @@ extern "C" int romab200_ba_cameras(const rb_ba_args* a, void* stream) {
 extern "C" int romab200_ba_cholesky(const rb_ba_args* a, void* stream) {
     if (ba_check(a, "ba_cholesky")) return 1;
     RB_REQUIRE(a->num_free > 0 && a->S && a->rhs && a->result, "ba_cholesky: null argument or no free camera");
+    return ba_cholesky_solve(a->S, (a->camera_model ? 8 : 6) * (int64_t)a->num_free, a->rhs, a->result, (cudaStream_t)stream);
+}
+
+extern "C" int romab200_ba_fold(const rb_ba_groups_args* a, void* stream) {
+    if (ba_check_groups(a, "ba_fold")) return 1;
     cudaStream_t st = (cudaStream_t)stream;
-    const int64_t n = (a->camera_model ? 8 : 6) * (int64_t)a->num_free;
-    for (int64_t k0 = 0; k0 < n; k0 += NB) {
-        const int nb = (int)(n - k0 < NB ? n - k0 : NB);
-        launch_pdl(ba_potrf_panel_kernel, dim3(1), dim3(256), 0, st, a->S, n, k0, nb, a->result);
-        if (check_launch("ba_cholesky(panel)")) return 1;
-        const int64_t rest = n - k0 - NB;
-        if (rest <= 0) break;
-        launch_pdl(ba_trsm_kernel, dim3((unsigned)((rest + 127) / 128)), dim3(128), 0, st, a->S, n, k0);
-        if (check_launch("ba_cholesky(trsm)")) return 1;
-        const unsigned tiles = (unsigned)((rest + NB - 1) / NB);
-        launch_pdl(ba_syrk_kernel, dim3(tiles, tiles), dim3(256), 0, st, a->S, n, k0);
-        if (check_launch("ba_cholesky(update)")) return 1;
-    }
-    launch_pdl(ba_potrs_kernel, dim3(1), dim3(1024), 0, st, (const double*)a->S, n, a->rhs);
-    return check_launch("ba_cholesky(solve)");
+    const int64_t F = a->num_free, np = 6 * F + 2 * (int64_t)a->num_groups;
+    launch_pdl(ba_fold_kernel, dim3(grid1d(np * 6 * F, 256, 64 * 1024)), dim3(256), 0, st, *a);
+    if (check_launch("ba_fold(poses)")) return 1;
+    launch_pdl(ba_fold_groups_kernel, dim3(a->num_groups, a->num_groups), dim3(256), 0, st, *a);
+    return check_launch("ba_fold(groups)");
+}
+
+extern "C" int romab200_ba_groups_cholesky(const rb_ba_groups_args* a, void* stream) {
+    if (ba_check_groups(a, "ba_groups_cholesky")) return 1;
+    return ba_cholesky_solve(a->S_groups, 6 * (int64_t)a->num_free + 2 * (int64_t)a->num_groups, a->rhs_groups, a->result,
+                             (cudaStream_t)stream);
+}
+
+extern "C" int romab200_ba_unfold(const rb_ba_groups_args* a, void* stream) {
+    if (ba_check_groups(a, "ba_unfold")) return 1;
+    launch_pdl(ba_unfold_kernel, dim3(a->num_groups), dim3(128), 0, (cudaStream_t)stream, *a);
+    return check_launch("ba_unfold");
 }
 
 extern "C" int romab200_ba_step(const rb_ba_args* a, void* stream) {

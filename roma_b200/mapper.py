@@ -17,7 +17,7 @@ from . import cabi, geometry
 from . import camera as _camera
 from . import triangulate as _tri
 from . import verify as _verify
-from .bundle import bundle_adjust
+from .bundle import _camera_ids, bundle_adjust
 from .match_graph import WORKSPACE_BYTES, MatchGraph
 from .register import register_images
 from .tracks import Tracks
@@ -55,7 +55,8 @@ class Reconstruction:
     final Points3D (triangulated with the registered cameras); init: the TwoViewInit; rounds: one host dict per round (registered:
     the images registered when it started, ba_termination, ba_cost: the cost before and after its bundle adjustment, ok_tracks after
     its re-triangulation, added: the images registration added); termination: "all_registered", "no_image_added" or
-    "no_initial_pair"."""
+    "no_initial_pair".  intrinsics: the final SIMPLE_RADIAL [N, 4] when `reconstruct` was given intrinsics; camera_ids: the int64 [N]
+    camera group of every image when it was given camera_ids (else None)."""
     registered: torch.Tensor
     R: torch.Tensor
     t: torch.Tensor
@@ -64,6 +65,7 @@ class Reconstruction:
     rounds: list
     termination: str
     intrinsics: torch.Tensor = None
+    camera_ids: torch.Tensor = None
 
 
 def rank_candidates(match_offsets, min_num_inliers, num_candidates) -> list:
@@ -222,7 +224,7 @@ def initialize_reconstruction(pairs, graph: MatchGraph, K, *, init_pair=None, nu
 def reconstruct(pairs, graph: MatchGraph, tracks: Tracks, K, *, init_pair=None, init_num_candidates=256, init_min_num_inliers=100,
                 init_max_error=4.0, init_min_tri_angle=16.0, init_max_forward_motion=0.95, tri_max_error=4.0, tri_min_angle=1.5,
                 abs_max_error=12.0, abs_min_inliers=30, ba_loss_scale=None, ba_max_iterations=50, seed=0,
-                workspace_bytes=WORKSPACE_BYTES, intrinsics=None, refine_intrinsics=False) -> Reconstruction:
+                workspace_bytes=WORKSPACE_BYTES, intrinsics=None, refine_intrinsics=False, camera_ids=None) -> Reconstruction:
     """A reconstruction of the images of `graph` (verified, built from `pairs`) and `tracks` (built from it) with intrinsics K and no
     known camera.  `initialize_reconstruction` (the init_* arguments) chooses the pair (a, b); a gets [I | 0] and b the unit-baseline
     [R | t], and every other camera is zero.  Then each round:
@@ -248,20 +250,33 @@ def reconstruct(pairs, graph: MatchGraph, tracks: Tracks, K, *, init_pair=None, 
     almost freely.  After the adjustment the graph is undistorted again under the refined intrinsics before the re-triangulation and
     the registration.  Reconstruction.intrinsics is the final [N, 4].  intrinsics=None is the pinhole call above, unchanged.
 
+    Shared cameras: with `camera_ids` [N] (integers in [0, C); the rows of `intrinsics` within a group equal bit for bit) the
+    images of a group share f and k, as with COLMAP's single_camera options.  Each round's bundle adjustment then passes camera_ids;
+    a group is refined when at least one of its images is registered (and MIN_REGISTERED_TO_REFINE holds), and is fixed otherwise.
+    An unregistered image of a refined group takes the group's new estimate, so it is registered under the group's current
+    intrinsics.  Reconstruction.camera_ids keeps the groups, and `write_colmap_text` writes one camera per group.
+
     Arguments are checked before any device work (ValueError).  Bit-identical from run to run.  Host reads: those of the stages, and
     the accepted flags of each registration."""
     what = "reconstruct"
     if not isinstance(refine_intrinsics, bool):
         raise ValueError(f"{what}: refine_intrinsics must be a bool, got {refine_intrinsics!r}")
+    if camera_ids is not None and intrinsics is None:
+        raise ValueError(f"{what}: camera_ids needs intrinsics (shared cameras are SIMPLE_RADIAL)")
     if intrinsics is not None:
         if K is not None:
             raise ValueError(f"{what}: pass K=None with intrinsics (the pinhole K is pinhole_K of the current intrinsics)")
         if not isinstance(graph, MatchGraph):
             raise ValueError(f"{what}: graph must be a MatchGraph, got {type(graph).__name__}")
         cur = _camera.check_intrinsics(intrinsics, len(graph._kp_off) - 1, what)
+        if camera_ids is not None:
+            try:
+                camera_ids = _camera_ids(camera_ids, len(cur), cur)
+            except ValueError as e:
+                raise ValueError(f"{what}: {str(e).split(': ', 1)[-1]}") from None
         return _reconstruct_radial(pairs, graph, tracks, cur, refine_intrinsics, init_pair, init_num_candidates, init_min_num_inliers,
                                    init_max_error, init_min_tri_angle, init_max_forward_motion, tri_max_error, tri_min_angle,
-                                   abs_max_error, abs_min_inliers, ba_loss_scale, ba_max_iterations, seed, workspace_bytes)
+                                   abs_max_error, abs_min_inliers, ba_loss_scale, ba_max_iterations, seed, workspace_bytes, camera_ids)
     if refine_intrinsics:
         raise ValueError(f"{what}: refine_intrinsics needs intrinsics")
     _float(what, "abs_max_error", abs_max_error, 0.0, True)
@@ -326,8 +341,9 @@ MIN_REGISTERED_TO_REFINE = 3
 
 def _reconstruct_radial(pairs, graph, tracks, cur, refine, init_pair, init_num_candidates, init_min_num_inliers, init_max_error,
                         init_min_tri_angle, init_max_forward_motion, tri_max_error, tri_min_angle, abs_max_error, abs_min_inliers,
-                        ba_loss_scale, ba_max_iterations, seed, workspace_bytes) -> Reconstruction:
-    """`reconstruct` with SIMPLE_RADIAL intrinsics `cur` [N, 4] (host float64, checked)."""
+                        ba_loss_scale, ba_max_iterations, seed, workspace_bytes, ids=None) -> Reconstruction:
+    """`reconstruct` with SIMPLE_RADIAL intrinsics `cur` [N, 4] (host float64, checked) and the checked camera groups `ids` (host
+    int64 [N]) or None."""
     what = "reconstruct"
     _float(what, "abs_max_error", abs_max_error, 0.0, True)
     _int(what, "abs_min_inliers", abs_min_inliers, 0)
@@ -349,10 +365,11 @@ def _reconstruct_radial(pairs, graph, tracks, cur, refine, init_pair, init_num_c
         R = torch.zeros(N, 3, 3, dtype=torch.float64, device=dev)
         t = torch.zeros(N, 3, dtype=torch.float64, device=dev)
         tri = dict(max_error=tri_max_error, min_angle=tri_min_angle, seed=seed)
+        ids_out = None if ids is None else torch.from_numpy(ids).to(dev)
         if init.chosen < 0:
             pts = triangulate_tracks(ug, tracks, Kc, R, t, images=[], **tri)
             return Reconstruction(torch.zeros(N, dtype=torch.bool, device=dev), R, t, pts, init, [], "no_initial_pair",
-                                  torch.from_numpy(cur).to(dev))
+                                  torch.from_numpy(cur).to(dev), ids_out)
         a, b = init.images[init.chosen].tolist()
         R[a] = torch.eye(3, dtype=torch.float64, device=dev)
         R[b], t[b] = init.R[init.chosen], init.t[init.chosen]
@@ -361,9 +378,14 @@ def _reconstruct_radial(pairs, graph, tracks, cur, refine, init_pair, init_num_c
             rest = [i for i in range(N) if i not in registered]
             pts = triangulate_tracks(ug, tracks, Kc, R, t, images=registered, **tri)
             free_intr = refine and len(registered) >= MIN_REGISTERED_TO_REFINE
+            if ids is None:
+                shared = dict(fixed_intrinsics=rest)
+            else:                                       # a group with no registered image keeps its intrinsics
+                seen = set(ids[registered].tolist())
+                shared = dict(camera_ids=ids, fixed_intrinsics=[g for g in range(int(ids.max()) + 1) if g not in seen])
             ba = bundle_adjust(graph, tracks, pts, cur, R, t, fixed_poses=[a] + rest, fixed_tx=[b], loss_scale=ba_loss_scale,
                                max_iterations=ba_max_iterations, workspace_bytes=workspace_bytes, camera_model="SIMPLE_RADIAL",
-                               refine_focal_length=free_intr, refine_extra_params=free_intr, fixed_intrinsics=rest)
+                               refine_focal_length=free_intr, refine_extra_params=free_intr, **shared)
             R, t = ba.R.clone(), ba.t.clone()
             if free_intr:
                 cur = ba.intrinsics.cpu().numpy()
@@ -388,7 +410,7 @@ def _reconstruct_radial(pairs, graph, tracks, cur, refine, init_pair, init_num_c
             registered = sorted(registered + rnd["added"])
         mask = torch.zeros(N, dtype=torch.bool, device=dev)
         mask[registered] = True
-    return Reconstruction(mask, R, t, pts, init, rounds, termination, torch.from_numpy(cur).to(dev))
+    return Reconstruction(mask, R, t, pts, init, rounds, termination, torch.from_numpy(cur).to(dev), ids_out)
 
 
 # ---- COLMAP text model ---------------------------------------------------------------------------------------------------
@@ -451,7 +473,11 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
     When recon.intrinsics is set (`reconstruct(..., intrinsics=...)`), K is not read (pass None) and every camera is written as
     "SIMPLE_RADIAL W H f cx cy k" of recon.intrinsics.  The keypoints of `graph` (the raw, distorted ones) are written as they are,
     which is what COLMAP expects; ERROR is points.error, the mean reprojection error of the re-triangulation in the undistorted
-    frame."""
+    frame.
+
+    When recon.camera_ids is set (shared cameras), cameras.txt has one SIMPLE_RADIAL camera per camera id g that some image uses,
+    CAMERA_ID g + 1, with the intrinsics and size of its images (the images of a camera must have one size), and images.txt
+    references it."""
     kp_off = np.asarray(graph._kp_off, np.int64)
     N = len(kp_off) - 1
     radial = recon.intrinsics is not None
@@ -478,7 +504,20 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
     pid = np.full(kp_off[-1], -1, np.int64)
     pid[kp_off[el[used, 0]] + el[used, 1]] = track[used] + 1
 
-    if radial:
+    cam_of = np.arange(N)                                        # the row of cameras.txt each image references
+    if recon.camera_ids is not None:
+        if not radial:
+            raise ValueError("write_colmap_text: recon.camera_ids needs recon.intrinsics (shared cameras are SIMPLE_RADIAL)")
+        ids = _host(recon.camera_ids).astype(np.int64).reshape(N)
+        groups, first = np.unique(ids, return_index=True)
+        for g, j in zip(groups, first):
+            m = ids == g
+            if (sizes[m] != sizes[j]).any() or (intr[m] != intr[j]).any():
+                raise ValueError(f"write_colmap_text: the images of camera {g} differ in size or intrinsics")
+        cam = _join(groups + 1, np.full(groups.size, "SIMPLE_RADIAL"), sizes[first, 1], sizes[first, 0], _fmt(intr[first, 0]),
+                    _fmt(intr[first, 1]), _fmt(intr[first, 2]), _fmt(intr[first, 3]))
+        cam_of = ids
+    elif radial:
         cam = _join(np.arange(1, N + 1), np.full(N, "SIMPLE_RADIAL"), sizes[:, 1], sizes[:, 0], _fmt(intr[:, 0]), _fmt(intr[:, 1]),
                     _fmt(intr[:, 2]), _fmt(intr[:, 3]))
     else:
@@ -486,7 +525,7 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
                     _fmt(K[:, 0, 2]), _fmt(K[:, 1, 2]))
     with open(os.path.join(path, "cameras.txt"), "w") as f:
         f.write("# Camera list with one line of data per camera:\n#   CAMERA_ID, MODEL, WIDTH, HEIGHT, PARAMS[]\n"
-                f"# Number of cameras: {N}\n")
+                f"# Number of cameras: {len(cam)}\n")
         f.write("\n".join(cam) + "\n")
 
     ids = np.flatnonzero(reg)
@@ -495,7 +534,7 @@ def write_colmap_text(path, recon: Reconstruction, graph: MatchGraph, tracks: Tr
         f.write("# Image list with two lines of data per image:\n#   IMAGE_ID, QW, QX, QY, QZ, TX, TY, TZ, CAMERA_ID, NAME\n"
                 f"#   POINTS2D[] as (X, Y, POINT3D_ID)\n# Number of images: {ids.size}\n")
         for m, i in enumerate(ids):
-            head = " ".join([str(i + 1), *_fmt(q[m]), *_fmt(t[i]), str(i + 1), names[i]])
+            head = " ".join([str(i + 1), *_fmt(q[m]), *_fmt(t[i]), str(cam_of[i] + 1), names[i]])
             b, e = kp_off[i], kp_off[i + 1]
             f.write(head + "\n" + " ".join(_join(_fmt(kps[b:e, 0]), _fmt(kps[b:e, 1]), pid[b:e])) + "\n")
 

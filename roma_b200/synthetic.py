@@ -530,7 +530,7 @@ def _planted_samples(g, vis, cells, H, W, cs, outlier_frac, device):
 
 
 def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024), cell_size: int = 1, noise: float = 0.5,
-                    visibility: float = 0.5, outlier_frac: float = 0.0, device="cpu", radial=None, spread: bool = False):
+                    visibility: float = 0.5, outlier_frac: float = 0.0, device="cpu", radial=None, spread: bool = False, camera_ids=None):
     """Seeded multi-view samples of a real scene, for geometric verification (`verify_matches`): `planted_views` with geometry.  A
     cloud of `n_points` scene points fills a 8 x 6 x 6 box around the origin; `n_images` pinhole cameras of `size` (H, W) with the
     intrinsics of `_scene_intrinsics` stand 8-10 units from the origin at azimuths of -40..40 degrees and heights of -1..1 and look at
@@ -547,7 +547,9 @@ def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024)
       the principal point at (W / 2, H / 2) and k uniform in [k_lo, k_hi], applied before the noise and the cell assignment.  K is
       then the [N, 4] (f, cx, cy, k) float64 intrinsics.
     - spread=True: look-at targets uniform in a 4 x 3 x 3 box, heights of -3..3 and rolls of -20..20 degrees about the optical
-      axis, so that the optical axes do not all meet near one point (per-image focal lengths are then better determined)."""
+      axis, so that the optical axes do not all meet near one point (per-image focal lengths are then better determined).
+    - camera_ids [n_images] (integers >= 0): shared cameras.  Every image of a group takes the intrinsics of the group's first image,
+      and with `radial` the group draws one k (one draw per id in [0, max + 1)), so the rows of K within a group are equal."""
     import numpy as np
 
     H, W = size
@@ -576,8 +578,18 @@ def planted_cameras(seed: int, n_images: int, n_points: int, *, size=(768, 1024)
             cr, sr = np.cos(roll[c]), np.sin(roll[c])
             R[c] = np.array([[cr, -sr, 0.0], [sr, cr, 0.0], [0.0, 0.0, 1.0]]) @ R[c]
     t = -np.einsum("cij,cj->ci", R, C)
+    if camera_ids is not None:
+        ids = np.asarray(camera_ids, np.int64)
+        if ids.shape != (n_images,) or ids.min() < 0:
+            raise ValueError(f"planted_cameras: camera_ids must be [{n_images}] integers >= 0")
+        first = {}
+        for i, g in enumerate(ids.tolist()):
+            first.setdefault(g, i)
+        K = K[[first[g] for g in ids.tolist()]]
     if radial is not None:
-        k = extra.uniform(radial[0], radial[1], n_images)
+        k = extra.uniform(radial[0], radial[1], n_images if camera_ids is None else int(ids.max()) + 1)
+        if camera_ids is not None:
+            k = k[ids]
         K = np.stack((K[:, 0, 0], np.full(n_images, W / 2), np.full(n_images, H / 2), k), 1)
         pc = np.einsum("cij,pj->cpi", R, X) + t[:, None]
         depth = pc[..., 2]
