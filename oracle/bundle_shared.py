@@ -40,7 +40,9 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
     """Returns dict(R, t, intrinsics, X, cost, accepted, termination, trials) as `oracle.bundle_radial.bundle_adjust` does; the
     rows of intrinsics within a group stay equal.  A list `systems` receives one dict per trial: lam, S [n', n'] and b [n'] after
     the pins, d [n'], D [n'] (the damping diagonal: each free camera's clamped pose diagonal, and per group the sum of its free
-    members' clamped f and k diagonals) and gc [n'] (the gradient J'^T W r in the shared parameters), with n' = 6F + 2G."""
+    members' clamped f and k diagonals), gc [n'] (the gradient J'^T W r in the shared parameters), and S_abs, b_abs: the assembly
+    of S and b repeated over the absolute value of every term (0 in pinned rows and columns), the summation scale of their rounding
+    error; with n' = 6F + 2G."""
     kpo, xy = _arr(kp_offsets, np.int64), _arr(keypoints, np.float64)
     off, el = _arr(track_offsets, np.int64), _arr(elements, np.int64).reshape(-1, 2)
     X, okb, inl = _arr(X, np.float64).copy(), _arr(ok, bool), _arr(inlier, bool)
@@ -111,10 +113,24 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
         A = Wk @ Vinv                                   # W_k V_k^-1 [T, n', 3]
         S = U + lam * np.diag(D) - np.tensordot(A, Wk, axes=([0, 2], [0, 2]))
         b = -gc + np.einsum("kai,ki->a", A, gp)
+        if systems is not None:
+            # the same assembly over |term|: folding only adds entries, so this is P^T S_abs P of the per-image system
+            # (in matrix products: this is a scale, so its summation order does not matter)
+            aJ, ar, aJX = np.abs(J), np.abs(r), np.abs(JX)
+            wJ = (w[:, None, None] * aJ).reshape(-1, n)
+            Wabs = np.zeros((T, n, 3))
+            np.add.at(Wabs, trk, wJ.reshape(M, 2, n).transpose(0, 2, 1) @ aJX)
+            gpabs = np.zeros((T, 3))
+            np.add.at(gpabs, trk, np.einsum("m,mai,ma->mi", w, aJX, ar))
+            Aabs = Wabs @ np.abs(Vinv)
+            S_abs = wJ.T @ aJ.reshape(-1, n) + lam * np.diag(D) + np.tensordot(Aabs, Wabs, axes=([0, 2], [0, 2]))
+            b_abs = wJ.T @ ar.reshape(-1) + np.einsum("kai,ki->a", Aabs, gpabs)
         for j in np.flatnonzero(pinned):
             S[j, :] = S[:, j] = 0.0
             S[j, j] = 1.0
             b[j] = 0.0
+            if systems is not None:
+                S_abs[j, :] = S_abs[:, j] = b_abs[j] = 0.0
         d, pivot_ok = np.zeros(n), True
         if n:
             try:
@@ -123,7 +139,7 @@ def bundle_adjust(kp_offsets, keypoints, track_offsets, elements, X, ok, inlier,
             except np.linalg.LinAlgError:
                 pivot_ok = False
         if systems is not None:
-            systems.append(dict(lam=lam, S=S, b=b, d=d, D=D, gc=gc, free=free, groups=groups))
+            systems.append(dict(lam=lam, S=S, b=b, d=d, D=D, gc=gc, free=free, groups=groups, S_abs=S_abs, b_abs=b_abs))
         dX = np.einsum("kij,kj->ki", Vinv, -gp - np.einsum("kai,a->ki", Wk, d))
         dX[~okb] = 0.0
         pred = 0.5 * (d @ (lam * D * d - gc) + np.einsum("ki,ki->", dX[okb], lam * Dp[okb] * dX[okb] - gp[okb]))

@@ -1,5 +1,6 @@
 """Shared cameras (`camera_ids`) on the host: `oracle/bundle_shared.py` (its Jacobian in the shared parameters against central
-differences, its reduced system against P^T (dense damped Hessian) P with pins, singleton groups against oracle/bundle_radial.py),
+differences, its reduced system against P^T (dense damped Hessian) P with pins, its summation scale S'_abs against P^T S_abs P from
+a dense Jacobian written out over |term|, singleton groups against oracle/bundle_radial.py),
 the argument rules of `bundle_adjust` and `reconstruct`, the group layout and workspace formula, `write_colmap_text` with one
 camera per group, and `planted_cameras(camera_ids=...)` leaving existing calls unchanged."""
 import numpy as np
@@ -128,6 +129,67 @@ def test_reduced_system_equals_the_folded_dense_hessian(ids, gauge):
     assert (s["d"][pinned] == 0).all()
 
 
+def _close_scale(a, ref, rtol=1e-12):
+    """Two sums of the same nonnegative terms in different orders: equal to rtol of each entry (0 where ref is 0)."""
+    assert a.shape == ref.shape and (a >= 0).all() and (ref >= 0).all()
+    assert (np.abs(a - ref) <= rtol * ref).all(), np.max(np.abs(a - ref) / np.where(ref > 0, ref, 1.0))
+
+
+@pytest.mark.parametrize("ids, loss_scale, gauge", [
+    ([0, 0, 1, 1, 1, 2], None, dict(fixed_poses=(0,), fixed_tx=(1,))),
+    ([0, 0, 1, 1, 1, 2], 1.0, dict(fixed_poses=(0, 4), fixed_tx=(2,), fixed_intrinsics=(2,))),
+    ([0, 1, 0, 1, 0, 1], None, dict(fixed_poses=(0, 1, 2), fixed_tx=(), refine_extra_params=False)),
+])
+def test_summation_scale_is_the_folded_per_image_scale(ids, loss_scale, gauge):
+    """The oracle's S'_abs and b'_abs bound |S'| and |b'| entry by entry, and equal P^T S_abs P and P^T b_abs, where S_abs and b_abs
+    are assembled here over |term| from an explicit dense Jacobian in the per-image parameters (8 per camera, then 3 per track)."""
+    ids = np.asarray(ids)
+    g, tr, tri, prior, R, t, _ = shared_scene(6, ids, 150)
+    args = _args(g, tr, tri)
+    N, T = ids.size, tri["ok"].size
+    systems = []
+    osh.bundle_adjust(*args, prior, R, t, ids, max_iterations=1, loss_scale=loss_scale, systems=systems, **gauge)
+    s = systems[0]
+    pose_pin, group_pin, free, groups = osh.layout(ids, **gauge)
+    pinned = np.r_[pose_pin[free].reshape(-1), group_pin[groups].reshape(-1)]
+    # a pinned row is e_r in S' and 0 in S'_abs: no rounding reaches it
+    keep = ~pinned
+    assert (np.abs(s["S"])[np.ix_(keep, keep)] <= s["S_abs"][np.ix_(keep, keep)]).all() and (np.abs(s["b"])[keep] <= s["b_abs"][keep]).all()
+    # every used observation's Jacobian in the per-image parameters, written out densely
+    kpo, xy = np.asarray(g["kp_offsets"], np.int64), np.asarray(g["keypoints"], np.float64)
+    off, el = np.asarray(tr["track_offsets"], np.int64), np.asarray(tr["elements"], np.int64).reshape(-1, 2)
+    track = np.repeat(np.arange(T), np.diff(off))
+    e = np.flatnonzero(np.repeat(np.asarray(tri["ok"], bool), np.diff(off)) & np.asarray(tri["inlier"], bool))
+    img, trk = el[e, 0], track[e]
+    X = np.asarray(tri["X"], np.float64)
+    u, _, Jc, JX = orad.project(prior[img], R[img], t[img], X[trk], True)
+    r = u - xy[kpo[img] + el[e, 1]]
+    c2 = 0.0 if loss_scale is None else loss_scale ** 2
+    w = 1.0 / (1.0 + (r * r).sum(1) / c2) if c2 else np.ones(e.size)
+    nc, lam = 8 * N, s["lam"]
+    J = np.zeros((e.size, 2, nc + 3 * T))
+    for q in range(e.size):
+        J[q, :, 8 * img[q]:8 * img[q] + 8] = Jc[q]
+        J[q, :, nc + 3 * trk[q]:nc + 3 * trk[q] + 3] = JX[q]
+    H = np.einsum("m,mai,maj->ij", w, J, J)
+    Habs = np.einsum("m,mai,maj->ij", w, np.abs(J), np.abs(J))
+    gabs = np.einsum("m,mai,ma->i", w, np.abs(J), np.abs(r))
+    Dc = np.clip(np.diag(H)[:nc], 1e-6, 1e32)
+    S_abs, b_abs = Habs[:nc, :nc] + lam * np.diag(Dc), gabs[:nc].copy()
+    for k in np.unique(trk):
+        p = nc + 3 * k + np.arange(3)
+        Vk = H[np.ix_(p, p)]
+        Vinv = np.abs(np.linalg.inv(Vk + lam * np.diag(np.clip(np.diag(Vk), 1e-6, 1e32))))
+        S_abs += Habs[:nc, p] @ Vinv @ Habs[p, :nc]
+        b_abs += Habs[:nc, p] @ Vinv @ gabs[p]
+    n = 6 * len(s["free"]) + 2 * len(s["groups"])
+    P = _P(ids, s["free"], s["groups"], N, T)[:nc, :n]
+    S_ref, b_ref = P.T @ S_abs @ P, P.T @ b_abs
+    S_ref[pinned, :] = S_ref[:, pinned] = b_ref[pinned] = 0.0
+    _close_scale(s["S_abs"], S_ref)
+    _close_scale(s["b_abs"], b_ref)
+
+
 @pytest.mark.parametrize("seed, N, loss_scale, gauge", [(7, 4, None, {}), (8, 6, 1.0, dict(fixed_poses=(0, 3), fixed_intrinsics=(2,)))])
 def test_singleton_groups_equal_the_per_image_oracle(seed, N, loss_scale, gauge):
     g, tr, tri, prior, R, t, _ = shared_scene(seed, np.arange(N), 150)
@@ -139,6 +201,22 @@ def test_singleton_groups_equal_the_per_image_oracle(seed, N, loss_scale, gauge)
     assert np.abs(a["cost"] - b["cost"]).max() <= 1e-10 * b["cost"][0]
     for name in ("R", "t", "intrinsics", "X"):
         assert np.abs(a[name] - b[name]).max() <= 1e-10 * max(1.0, np.abs(b[name]).max()), name
+
+
+@pytest.mark.parametrize("seed, N, loss_scale, gauge", [(7, 4, None, {}), (8, 6, 1.0, dict(fixed_poses=(0, 3), fixed_intrinsics=(2,)))])
+def test_singleton_groups_summation_scale_equals_the_per_image_one(seed, N, loss_scale, gauge):
+    """With singleton groups, S'_abs and b'_abs are oracle/bundle_radial.py's S_abs and b_abs with the rows in the order (poses, then
+    groups)."""
+    g, tr, tri, prior, R, t, _ = shared_scene(seed, np.arange(N), 150)
+    args = _args(g, tr, tri)
+    sa, sb = [], []
+    osh.bundle_adjust(*args, prior, R, t, np.arange(N), loss_scale=loss_scale, max_iterations=1, systems=sa, **gauge)
+    orad.bundle_adjust(*args, prior, R, t, loss_scale=loss_scale, max_iterations=1, systems=sb, **gauge)
+    F = len(sa[0]["free"])
+    assert sa[0]["free"] == sb[0]["free"] and sa[0]["groups"] == sa[0]["free"]
+    perm = np.r_[(8 * np.arange(F)[:, None] + np.arange(6)).reshape(-1), (8 * np.arange(F)[:, None] + np.arange(6, 8)).reshape(-1)]
+    _close_scale(sa[0]["S_abs"], sb[0]["S_abs"][np.ix_(perm, perm)])
+    _close_scale(sa[0]["b_abs"], sb[0]["b_abs"][perm])
 
 
 def test_shared_groups_stay_equal_and_fit_a_single_camera_scene():
