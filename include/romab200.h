@@ -1407,6 +1407,58 @@ typedef struct {
 int romab200_dense_fuse_count(const rb_dense_fuse_args* args, void* stream);
 int romab200_dense_fuse_emit(const rb_dense_fuse_args* args, void* stream);
 
+/* ---- Retrieval: DINOv2 global descriptors and nearest-neighbour pair selection (not in the reference) -------------------------
+ * Chooses the pairs that match_pairs / match_graph run on.  With synthetic weights the retrieval quality (recall of overlapping
+ * pairs) is not measured, and it has not been measured on real DINOv2 weights either.
+ *
+ * romab200_global_descriptor: tokens [batch, n_tokens, dim] in `tokens_dtype` (RB_F32 / RB_F16 / RB_BF16; the final-norm DINOv2 tokens,
+ * row 0 the class token, rows 1 .. n the patch tokens, n = n_tokens - 1), out [batch, 2 dim] fp32.  Every operation is fp32,
+ * round-to-nearest, with no FMA contraction.  Per image and channel ch:
+ *   c[ch] = T[0, ch];  s = 0, then s = s + T[t, ch] for t = 1 .. n in ascending order;  m[ch] = s / (float)n;
+ *   |v| = sqrt_rn(q) where q = 0, then q = q + v[ch] * v[ch] for ch = 0 .. dim - 1 in ascending order (the product rounded first);
+ *   out[0 .. dim) = c[ch] / (fp32(sqrt 2) * |c|),  out[dim .. 2 dim) = m[ch] / (fp32(sqrt 2) * |m|)  (the product rounded first),
+ * fp32(sqrt 2) = 1.41421354f, so |out| ~ 1; a half whose norm is 0 is written as zeros.  One CTA per image, one thread per channel
+ * (dim <= 1024).  The descriptor of an image depends on its own tokens only.
+ *
+ * Pair selection over N images with descriptors X [N, D] fp32, k = min(num_neighbors, N - 1), 2 <= N <= RB_RETRIEVAL_MAX_IMAGES,
+ * 1 <= k <= RB_RETRIEVAL_MAX_K:
+ *   1. Score.  s_ij = the dot product of rows i and j as one fp32 FMA chain over the D components in ascending order, which is what
+ *      romab200_gemm computes for fp32 operands on its default (SIMT) back end with B = X as [N, D]: one register accumulator per
+ *      output, k ascending, no split-K.  So s_ij == s_ji bit for bit (fma(a, b, c) = fma(b, a, c)) for every tile shape.  The
+ *      back end runs the chain over zero-padded k up to a multiple of its k-tile: a zero term changes nothing but -0 into +0, and a
+ *      -0 score counts as +0 below.  The caller makes the scores of rows [row_begin, row_end) against all N rows in a block
+ *      scores [row_end - row_begin, ld_scores] per call.
+ *   2. Neighbours.  neighbors[i] [k] int64 are the k largest s_ij, j != i, ordered by score descending, then j ascending;
+ *      neighbor_scores[i] their scores.  romab200_retrieval_select, one CTA per row: the 48-bit key (order-preserving bit pattern of
+ *      s_ij << 16) | (0xffff - j) is unique per column, so an exact radix select (12-bit digits from the top) finds the k-th largest
+ *      key with no tie pass; the keys at or above the selected digit prefix are collected once they fit a shared list, sorted there,
+ *      and the first k written.  Any non-finite s_ij of the row, s_ii included (a non-finite descriptor has a non-finite self-score),
+ *      sets *status = 1 (it is never cleared).
+ *   3. Pairs.  The set {(min(i, j), max(i, j)) : j in neighbors[i]}, unique, sorted by (i, j).  romab200_retrieval_pairs_count: the
+ *      keys (min N + max) << 32 of the N k entries in keys, sorted by radix_sort_hi32 over keys / keys_alt / hist (RADIX_DIGITS
+ *      ceil(N k / RB_RETRIEVAL_TILE) + 1 int32), then offsets [N k + 1] int64 receives the exclusive scan of "first of a run of equal
+ *      keys" flags, offsets[N k] = the number of pairs P.  romab200_retrieval_pairs_emit (after the caller has read P): pairs [P, 2]
+ *      int64.  Every image is in at least k pairs and P <= N k.
+ * No float atomics: every output is the same bytes from run to run and for every split of the rows into blocks. */
+#define RB_RETRIEVAL_MAX_IMAGES 65535
+#define RB_RETRIEVAL_MAX_K 128
+#define RB_RETRIEVAL_TILE 4096
+typedef struct {
+    const void* tokens; float* out; int32_t batch, n_tokens, dim, tokens_dtype;
+} rb_global_descriptor_args;
+int romab200_global_descriptor(const rb_global_descriptor_args* args, void* stream);
+
+typedef struct {
+    int32_t num_images, k;
+    const float* scores; int64_t ld_scores; int32_t row_begin, row_end;     /* select */
+    int64_t* neighbors; float* neighbor_scores; int32_t* status;
+    int64_t* keys; int64_t* keys_alt; int32_t* hist; int64_t* offsets;     /* pairs */
+    int64_t num_pairs; int64_t* pairs;                                      /* emit only */
+} rb_retrieval_args;
+int romab200_retrieval_select(const rb_retrieval_args* args, void* stream);
+int romab200_retrieval_pairs_count(const rb_retrieval_args* args, void* stream);
+int romab200_retrieval_pairs_emit(const rb_retrieval_args* args, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -53,6 +53,9 @@ def __getattr__(name):
     if name in ("triangulate_warps", "fuse_depth_maps", "write_ply", "DepthMaps", "DenseCloud"):
         from . import dense
         return getattr(dense, name)
+    if name in ("select_pairs", "RetrievalPairs"):
+        from . import retrieval
+        return getattr(retrieval, name)
     if name in ("warp_kpts", "get_gt_warp", "dense_geometric_dist"):
         from . import depth_warp
         return getattr(depth_warp, name)

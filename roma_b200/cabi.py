@@ -88,6 +88,9 @@ RB_TRI_CTR = int(re.search(r"#define\s+RB_TRI_CTR\s+0x([0-9a-fA-F]+)u", open(HEA
 RB_DENSE_CAM, RB_DENSE_REASONS, RB_DENSE_MAX_CTAS, RB_DENSE_TILE = (
     int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
     for name in ("RB_DENSE_CAM", "RB_DENSE_REASONS", "RB_DENSE_MAX_CTAS", "RB_DENSE_TILE"))
+RB_RETRIEVAL_MAX_IMAGES, RB_RETRIEVAL_MAX_K, RB_RETRIEVAL_TILE = (
+    int(re.search(rf"#define\s+{name}\s+(\d+)", open(HEADER).read()).group(1))
+    for name in ("RB_RETRIEVAL_MAX_IMAGES", "RB_RETRIEVAL_MAX_K", "RB_RETRIEVAL_TILE"))
 STRUCTS = {name: type(name, (ctypes.Structure,), {"_fields_": fields}) for name, fields in STRUCT_FIELDS.items()}
 _PTR_FIELDS = {name: {f for f, t in fields if t is ctypes.c_void_p} for name, fields in STRUCT_FIELDS.items()}
 
@@ -225,6 +228,9 @@ _FIELD_DTYPES = {
                            "nbrs": torch.int32, "depth": _F32, "score": _F32, "colors": torch.uint8, "color_offsets": torch.int64,
                            "color_sizes": torch.int32, "tile_scan": torch.int64, "points": _F64, "rgb": torch.uint8, "image": torch.int32,
                            "pixel": torch.int64, "num_views": torch.int32, "point_score": _F32},
+    "rb_global_descriptor_args": {"tokens": "tokens_dtype", "out": _F32},
+    "rb_retrieval_args": {"scores": _F32, "neighbors": torch.int64, "neighbor_scores": _F32, "status": torch.int32, "keys": torch.int64,
+                          "keys_alt": torch.int64, "hist": torch.int32, "offsets": torch.int64, "pairs": torch.int64},
 }
 # tensor fields that the call describes with explicit element strides, so they may be non-contiguous views
 _STRIDED_FIELDS = {"rb_keypoints_sample_args": {"warp", "cert"}, "rb_dense_geometric_dist_args": {"dense_matches"}}
@@ -382,6 +388,19 @@ def _dense_fuse_min_elems(kw):
     return out
 
 
+def _global_descriptor_min_elems(kw):
+    return {"tokens": kw["batch"] * kw["n_tokens"] * kw["dim"], "out": 2 * kw["batch"] * kw["dim"]}
+
+
+def _retrieval_min_elems(kw):
+    total = kw["num_images"] * kw["k"]
+    out = {"neighbors": total, "neighbor_scores": total, "status": 1, "keys": total, "keys_alt": total,
+           "hist": 256 * (-(-total // RB_RETRIEVAL_TILE)) + 1, "offsets": total + 1, "pairs": 2 * kw.get("num_pairs", 0)}
+    if "row_end" in kw:
+        out["scores"] = (kw["row_end"] - kw["row_begin"] - 1) * kw["ld_scores"] + kw["num_images"]
+    return out
+
+
 # struct -> function of the call's arguments giving {field: minimum number of elements} for the described geometry
 _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_elems, "rb_gather_rows_args": _gather_rows_min_elems,
               "rb_sample_args": _sample_min_elems, "rb_sample_gather_args": _sample_gather_min_elems,
@@ -390,7 +409,8 @@ _MIN_ELEMS = {"rb_gemm_args": _gemm_min_elems, "rb_copy2d_args": _copy2d_min_ele
               "rb_ba_args": _ba_min_elems, "rb_ba_groups_args": _ba_groups_min_elems, "rb_abspose_args": _abspose_min_elems,
               "rb_register_args": _register_min_elems,
               "rb_twoview_args": _twoview_min_elems, "rb_undistort_args": _undistort_min_elems,
-              "rb_dense_tri_args": _dense_tri_min_elems, "rb_dense_fuse_args": _dense_fuse_min_elems}
+              "rb_dense_tri_args": _dense_tri_min_elems, "rb_dense_fuse_args": _dense_fuse_min_elems,
+              "rb_global_descriptor_args": _global_descriptor_min_elems, "rb_retrieval_args": _retrieval_min_elems}
 
 
 def _validate(fn_name, struct_name, kw):

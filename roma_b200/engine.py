@@ -294,6 +294,20 @@ class Engine(BufferArena):
     # ------------------------------------------------------------------ DINOv2 ViT-L/14 (encoders.py:60-67)
     def dinov2(self, image: torch.Tensor):
         """image [E,3,H,W] fp32 -> patch tokens [E, hp*wp, 1024] in the compute dtype (channels-last stride-14 map)."""
+        out, hp, wp = self.dinov2_tokens(image)
+        E, npatch, dim = image.shape[0], hp * wp, arch.VIT_DIM
+        N = npatch + 1
+        feats = self.buf("vit.feat16", (E, npatch, dim))
+        # drop the cls token: rows 1..N of every image
+        for e in range(E):
+            self.copy2d(at(out, (e * N + 1) * dim), feats[e], npatch, dim, dim, dim, self.dt, self.dt)
+        if self.debug is not None:
+            self.debug["vit.feat16"] = feats.float().clone()
+        return feats, hp, wp
+
+    def dinov2_tokens(self, image: torch.Tensor):
+        """image [E,3,H,W] fp32 -> (the final-norm tokens [E * (1 + hp*wp), 1024] in the compute dtype, the class token first in
+        every image's rows, hp, wp)."""
         E, _, H, W = image.shape
         hp, wp = H // arch.VIT_PATCH, W // arch.VIT_PATCH
         npatch, dim = hp * wp, arch.VIT_DIM
@@ -312,13 +326,19 @@ class Engine(BufferArena):
             self.block(x, blk, E, N, dim, arch.VIT_HEADS, arch.VIT_MLP, arch.VIT_LN_EPS, "vit")
         out = self.buf("vit.out", (E * N, dim))
         self.layernorm(x, out, self.w.vit_norm, E * N, dim, arch.VIT_LN_EPS)
-        feats = self.buf("vit.feat16", (E, npatch, dim))
-        # drop the cls token: rows 1..N of every image
-        for e in range(E):
-            self.copy2d(at(out, (e * N + 1) * dim), feats[e], npatch, dim, dim, dim, self.dt, self.dt)
+        return out, hp, wp
+
+    def global_descriptors(self, images: torch.Tensor, out: torch.Tensor):
+        """Global descriptors of E images [E, 3, H, W] fp32 into out [E, 2048] fp32: DINOv2's final-norm class token and the mean of
+        its patch tokens, each scaled to norm 1/sqrt(2) (`romab200_global_descriptor`, rules in include/romab200.h).  Neither the
+        CNN branch nor the GP runs.  No allocation beyond the arena, no host sync."""
+        with self.stage("dinov2"):
+            tokens, hp, wp = self.dinov2_tokens(images)
         if self.debug is not None:
-            self.debug["vit.feat16"] = feats.float().clone()
-        return feats, hp, wp
+            self.debug["vit.out"] = tokens.view(images.shape[0], hp * wp + 1, arch.VIT_DIM).float().clone()
+        with self.stage("descriptor"):
+            call("romab200_global_descriptor", "rb_global_descriptor_args", tokens=tokens, out=out, batch=images.shape[0], n_tokens=hp * wp + 1,
+                 dim=arch.VIT_DIM, tokens_dtype=self.dt)
 
     # ------------------------------------------------------------------ proj (roma_models.py:156-169)
     def proj_from_padded(self, s, tap, E, h, w, tag):

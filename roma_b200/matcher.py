@@ -18,7 +18,7 @@ import torch
 import torch.nn.functional as F
 from PIL import Image
 
-from . import cabi
+from . import arch, cabi
 from .cache import GraphCache
 from .engine import Engine
 from .preprocess import DeviceImage, DevicePreprocessor, open_inputs
@@ -137,22 +137,7 @@ class RegressionMatcher:
         in error messages.  Returns ([coarse-resolution tensor [b, 3, h, w] per input], [upsample-resolution tensor per input] when
         upsample_preds, else None).  JPEG paths are decoded on the device in one launch set; path and PIL inputs are resized
         there (Pillow-exact bicubic, csrc/preprocess.cu) to (h_resized, w_resized) and to upsample_res."""
-        opened = open_inputs(inputs, self.engine.device)
-        hs, ws = self.h_resized, self.w_resized
-        pil_route = all(isinstance(im, (Image.Image, DeviceImage)) for im in opened)
-        if pil_route:
-            # raw RGB bytes go up once per image (or were decoded there)
-            pre = self._preprocessor()
-            raws = [im.raw if isinstance(im, DeviceImage) else pre.upload(im) for im in opened]
-            lo = [pre.resize_normalize(raw, (hs, ws))[None] for raw in raws]
-        elif all(isinstance(im, torch.Tensor) for im in opened):
-            h, w = opened[0].shape[-2:]
-            assert all(im.shape[-2:] == (h, w) for im in opened), "For batched images we assume same size"
-            if h != self.h_resized or self.w_resized != w:
-                warn("Model resolution and batch resolution differ, may produce unexpected results")
-            lo = list(opened)
-        else:
-            raise ValueError("Unsupported input type: " + " and ".join(f"type({nm})={type(im)!r}" for nm, im in zip(names, opened)))
+        lo, raws, opened = self._coarse_inputs(inputs, names)
         if not self.upsample_preds:
             return lo, None
         hs, ws = self.upsample_res
@@ -161,12 +146,75 @@ class RegressionMatcher:
             if not isinstance(inputs[0], (str, os.PathLike)):
                 for nm, x in zip(names, inputs):
                     assert isinstance(x, Image.Image), f"Unsupported input type: type({nm}_input)={type(x)!r}"
-            assert pil_route, "upsample_preds without high-res tensors needs path or PIL inputs"
+            assert raws is not None, "upsample_preds without high-res tensors needs path or PIL inputs"
+            pre = self._preprocessor()
             return lo, [pre.resize_normalize(raw, (hs, ws))[None] for raw in raws]
         if all(h is not None for h in high_res):
             return lo, list(high_res)
         parts = [p for nm, im, h in zip(names, opened, high_res) for p in (f"{nm}={im!r}", f"{nm}_high_res={h!r}")]
         raise ValueError(f"Invalid upsample_preds and high_res inputs with {','.join(parts[:-1])} and {parts[-1]}")
+
+    def _coarse_inputs(self, inputs, names):
+        """The coarse-resolution half of `_device_inputs`: ([tensor [b, 3, h, w] per input], the raw device RGB bytes of path / PIL
+        inputs or None for tensor inputs, the opened inputs)."""
+        opened = open_inputs(inputs, self.engine.device)
+        hs, ws = self.h_resized, self.w_resized
+        if all(isinstance(im, (Image.Image, DeviceImage)) for im in opened):
+            # raw RGB bytes go up once per image (or were decoded there)
+            pre = self._preprocessor()
+            raws = [im.raw if isinstance(im, DeviceImage) else pre.upload(im) for im in opened]
+            return [pre.resize_normalize(raw, (hs, ws))[None] for raw in raws], raws, opened
+        if all(isinstance(im, torch.Tensor) for im in opened):
+            h, w = opened[0].shape[-2:]
+            assert all(im.shape[-2:] == (h, w) for im in opened), "For batched images we assume same size"
+            if h != self.h_resized or self.w_resized != w:
+                warn("Model resolution and batch resolution differ, may produce unexpected results")
+            return list(opened), None, opened
+        raise ValueError("Unsupported input type: " + " and ".join(f"type({nm})={type(im)!r}" for nm, im in zip(names, opened)))
+
+    @torch.inference_mode()
+    def global_descriptors(self, images, *, max_batch=8):
+        """Global image descriptors for retrieval (`roma_b200.select_pairs`): float32 [N, 2048] on the model's device, row i the
+        final-norm DINOv2 class token of images[i] and the mean of its patch tokens, each half scaled to norm 1/sqrt(2) (rules in
+        include/romab200.h).
+
+        images: as in `match_pairs`, a sequence of paths / PIL images (decoded and resized on the device to (h_resized, w_resized))
+        or a tensor [N, 3, h, w].  Only the ViT runs (not the CNN branch or the GP), on batches of at most `max_batch` images, each
+        batch replayed as a CUDA graph.  Row i depends on images[i] only, bit for bit: not on the other images or on max_batch."""
+        eng = self.engine
+        if int(max_batch) < 1:
+            raise ValueError(f"max_batch must be positive, got {max_batch}")
+        max_batch = int(max_batch)
+        if isinstance(images, torch.Tensor):
+            if images.dim() != 4:
+                raise ValueError(f"images must be [N, 3, h, w], got shape {tuple(images.shape)}")
+            self._coarse_inputs([images], ("images",))         # match()'s checks of tensor inputs; no device work
+            hs, ws = images.shape[-2:]
+        else:
+            images = list(images)
+            bad = [type(x) for x in images if not isinstance(x, (str, os.PathLike, Image.Image))]
+            if bad:
+                raise ValueError(f"Unsupported input type: images mixes paths / PIL images with {bad[0]!r}")
+            hs, ws = self.h_resized, self.w_resized
+        n_images, dev = len(images), eng.device
+        out = torch.empty(n_images, 2 * arch.VIT_DIM, dtype=torch.float32, device=dev)
+        use_graph = self.use_cuda_graph and eng.debug is None and eng.profile is None and eng.gemm_profile is None
+        with torch.cuda.device(dev):
+            for e0 in range(0, n_images, max_batch):
+                E = min(max_batch, n_images - e0)
+                entry = self._pair_graphs.entry(("descriptors", E, hs, ws), lambda: dict(
+                    images=torch.empty(E, 3, hs, ws, dtype=torch.float32, device=dev),
+                    out=torch.empty(E, out.shape[1], dtype=torch.float32, device=dev)), use_graph, eng.generation)
+                bufs = entry["bufs"]
+                if isinstance(images, torch.Tensor):
+                    bufs["images"].copy_(images[e0:e0 + E], non_blocking=True)
+                else:
+                    lo = self._coarse_inputs(images[e0:e0 + E], [f"images[{i}]" for i in range(e0, e0 + E)])[0]
+                    for k, t in enumerate(lo):
+                        bufs["images"][k:k + 1].copy_(t, non_blocking=True)
+                self._pair_graphs.run(entry, lambda: eng.global_descriptors(bufs["images"], bufs["out"]))
+                out[e0:e0 + E].copy_(bufs["out"])
+        return out
 
     @torch.inference_mode()
     def match_pairs(self, images, pairs, images_high_res=None, *, max_batch=8, on_batch=None):
